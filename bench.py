@@ -2,6 +2,7 @@
 """bench.py — headline benchmark of the sylph_b200 hot paths (contract: see DESIGN.md §Measurement).
 
   python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--workload sketch|profile]
+                  [--dump-outputs DIR]
 
 Primary line (default --workload sketch) = BASELINE.json configs[1]:
   sketch 1 Gbp of synthetic 150 bp single-end reads, k=31 c=200, per GPU (weak scaling: every
@@ -76,13 +77,15 @@ def parse():
     ap.add_argument("--no-pairs", action="store_true", help="skip the secondary containment measurement")
     ap.add_argument("--no-cpu", action="store_true", help="skip the cpu_baseline leg")
     ap.add_argument("--fixed-warmup", action="store_true",
-                    help="exactly --warmup untimed steps (no settle loop): for runs under ncu, whose numbers are never bench values")
+                    help="exactly --warmup untimed steps (no settle loop): for runs under a profiler, whose numbers are never bench values")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write what the timed paths returned in their last step to DIR/<name>.npy (float64, at most 64 MB)")
     return ap.parse_args()
 
 
 # ------------------------------------------------------------------------------------------------
 class ClockSampler:
-    """SM clock + throttle reasons of THIS rank's GPU during the timed region (B200_PROFILING.md's clocks line).
+    """SM clock + throttle reasons of THIS rank's GPU during the timed region.
     In-process NVML from a background thread (20 samples/s: two driver calls of a few microseconds each) — a polling
     `nvidia-smi -lms` process that watches all N GPUs takes driver locks on every one of them per sample, and a
     sample that lands inside a 40 ms timed region costs the slowest rank milliseconds (seen as 1.9 vs 2.4 ms per
@@ -181,7 +184,39 @@ def measured_peak_hbm():
             return float(json.load(open(p))["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
         except Exception:
             pass
-    return 6650.0, "fallback (B200_PROFILING.md 6.65 TB/s)"
+    return 3350.0, "H100 SXM data sheet (3.35 TB/s), not measured"
+
+
+DUMP_MAX_BYTES = 64 << 20
+DUMP_MAX_ROWS = 1 << 20
+
+
+class OutputDump:
+    """--dump-outputs DIR: the arrays a caller of each timed path received in its last timed step, as DIR/<name>.npy in
+    float64.  A u64 array (hashes) is written exactly as its 32-bit halves <name>_hi / <name>_lo.  An array longer than
+    `rows` is replaced by the same fixed, seeded sample of its rows for the same length, so that two builds of the
+    project can be compared output for output."""
+
+    def __init__(self, outdir):
+        self.dir, self.bytes = outdir, 0
+        if outdir:
+            os.makedirs(outdir, exist_ok=True)
+
+    def __bool__(self):
+        return bool(self.dir)
+
+    def add(self, name, a, rows=DUMP_MAX_ROWS, seed=0):
+        import numpy as np
+        a = np.asarray(a)
+        if len(a) > rows:
+            a = a[np.sort(np.random.default_rng(seed).choice(len(a), rows, replace=False))]
+        parts = {name + "_hi": a >> np.uint64(32), name + "_lo": a & np.uint64(0xFFFFFFFF)} if a.dtype == np.uint64 else {name: a}
+        for n, x in parts.items():
+            x = np.ascontiguousarray(x, dtype=np.float64)
+            self.bytes += x.nbytes
+            if self.bytes > DUMP_MAX_BYTES:
+                raise SystemExit("bench: --dump-outputs would exceed %d bytes at %s" % (DUMP_MAX_BYTES, n))
+            np.save(os.path.join(self.dir, n + ".npy"), x)
 
 
 def dist_setup(n):
@@ -328,7 +363,7 @@ def run_reference(args):
 
 
 # ------------------------------------------------------------------------------------------------
-def bench_sketch(args, ctx, rank, world, local):
+def bench_sketch(args, ctx, rank, world, local, dump):
     import numpy as np
     import torch
     from sylph_b200 import synth
@@ -339,9 +374,11 @@ def bench_sketch(args, ctx, rank, world, local):
     state = {}
 
     def step_resident():
+        if "s" in state:  # the previous step's sample; the last one is kept for --dump-outputs
+            state.pop("s").free()
         s = ctx.sketch_sequences(bases, off, k=K, c=C)
         state["n"] = len(s)
-        s.free()
+        state["s"] = s
 
     # clocks are sampled from before the warm-up to the end of the timed region: nvidia-smi needs ~100 ms to
     # start and its first query can stall the GPU, so neither may fall inside the (tens of ms) timed region;
@@ -384,6 +421,13 @@ def bench_sketch(args, ctx, rank, world, local):
     launches = ctx.launches - l0
     kms, klaunch, kbases = ctx.seed_kernel_time(reset=True)
     ctx.enable_timing(False)
+    s = state.pop("s")
+    if dump:
+        h, c = s.download()
+        dump.add("sketch_hash", h)
+        dump.add("sketch_count", c)
+        dump.add("sketch_meta", [len(h), s.num_dup_removed, s.mean_read_length])
+    s.free()
     total_bases = sum_over_ranks(float(n_bases), world)
     value = total_bases * args.steps / (ms * 1e-3)
 
@@ -396,17 +440,12 @@ def bench_sketch(args, ctx, rank, world, local):
     peak, peak_src = measured_peak_hbm()
     k_ms = kms / max(klaunch, 1)
     achieved = alg_bytes / (k_ms * 1e-3) / 1e9
-    traffic = None
-    tpath = os.path.join(ROOT, "profiles", "r01_k_seed_traffic.json")
-    if os.path.exists(tpath):  # dram__bytes_read+write of one ncu --set full capture, scaled by bases per launch
-        traffic = json.load(open(tpath))["dram_bytes_per_base"] * n_bases
     roofline = {"kernel": "k_seed<31, events, W=30>", "bound": "hbm", "achieved": achieved, "peak": peak, "unit": "GB/s",
-                "frac": achieved / peak, "traffic": traffic, "peak_source": peak_src,
+                "frac": achieved / peak, "traffic": None, "peak_source": peak_src,
                 "kernel_ms": k_ms, "kernel_share_of_step": kms / ms if ms else None,
                 "algorithmic_bytes_per_launch": alg_bytes, "traffic_model_bytes_per_launch": model_bytes,
-                "note": "integer-issue bound: ~33 SASS instructions per window, 18.4 of them on the ALU pipe (1 warp "
-                        "instruction / 2 cycles) and 12.4 IMADs on the FMA pipe; ncu: ALU pipe 75 % active, fmaheavy 59 %, "
-                        "DRAM 9 %; see DESIGN.md 4.1 and profiles/"}
+                "note": "integer-issue bound: every window costs a 64-bit hash on the ALU and FMA pipes while it reads "
+                        "one byte; see DESIGN.md 4.1"}
 
     # ---- e2e: pinned host buffers through the C ABI, H2D + D2H inside the timed region
     hb = torch.empty(n_bases, dtype=torch.uint8, pin_memory=True)
@@ -433,7 +472,7 @@ def bench_sketch(args, ctx, rank, world, local):
 
     for _ in range(max(1, args.warmup // 2)):
         step_e2e()
-    e2e_steps = max(1, min(args.steps, 10))
+    e2e_steps = args.steps
     e2e_state["t"] = []
     ctx.enable_timing(True)
     ctx.seed_kernel_time(reset=True)
@@ -478,7 +517,7 @@ def genomes_config(args):
             "l2": "inputs (%.2f GB per step) are larger than L2; no flush needed" % (args.batch_genomes * GENOME_LEN / 1e9)}
 
 
-def bench_genomes(args, ctx, rank, world, local):
+def bench_genomes(args, ctx, rank, world, local, dump):
     """Genome (database) sketching, device-resident synthetic genomes generated on the device (config 5: 452 GB of bases
     cannot cross PCIe in useful time).  step = one batch of genomes -> CSR genome_kmers + tracked, resident."""
     import numpy as np
@@ -491,31 +530,28 @@ def bench_genomes(args, ctx, rank, world, local):
     st = {}
 
     def step():
-        g = ctx.sketch_genomes(bases, off, goff, k=K, c=C)
-        st["g"] = g
+        if "g" in st:  # the previous step's sketches; the last one is kept for the parity check and --dump-outputs
+            st.pop("g").free()
+        st["g"] = ctx.sketch_genomes(bases, off, goff, k=K, c=C)
 
     for _ in range(max(args.warmup, 3)):
         step()
-        st["g"].free()
     ctx.enable_timing(True)
     ctx.seed_kernel_time(reset=True)
     ctx.kernel_time("genome_post", reset=True)
     l0 = ctx.launches
-
-    def tstep():
-        step()
-        st["g"].free()
-
-    ms, _ = timed(tstep, args.steps, world)
+    ms, _ = timed(step, args.steps, world)
     launches = ctx.launches - l0
     kms = ctx.seed_kernel_time(reset=True)[0] / args.steps
     pms = ctx.kernel_time("genome_post", reset=True)[0] / args.steps
     ctx.enable_timing(False)
     n_bases = float(bases.numel())
     value = sum_over_ranks(n_bases, world) * args.steps / (ms * 1e-3)
-    step()
-    g = st["g"]
+    g = st.pop("g")
     d = g.download()
+    if dump:
+        for name in ("kmers", "kmer_off", "tracked", "tracked_off", "gn_size"):
+            dump.add("genomes_" + name, d[name], rows=DUMP_MAX_ROWS // 2)
     peak, peak_src = measured_peak_hbm()
     n_surv_est = int(d["kmer_off"][-1] + d["tracked_off"][-1])
     alg = n_bases + 16.0 * n_surv_est   # SURVEY §8(d), positions variant: 1 B/base + 16 B per survivor
@@ -574,13 +610,13 @@ def rows_equal_oracle(rows, exp, tol=1e-6):
 
 
 PAIR_KERNELS = {"join": "k_join_hist<pass 1> (+ k_range_bounds)", "join2": "k_join2_order (+ k_local_best)", "stats": "k_stats_hist", "boot": "k_boot_iter_p"}
-PAIR_LIMITER = {"join": "DRAM: random sectors of the db index (ncu: 0.32 GB per sample at 4.9 TB/s)",
+PAIR_LIMITER = {"join": "DRAM: random sectors of the db index",
                 "join2": "DRAM / latency: genome ids of the recorded equal ranges",
                 "stats": "latency (one warp per touched pair)",
-                "boot": "integer issue: 39 instructions per 32 bootstrap draws on the main path (11 of them the 128-bit multiply), ~50 all-in; issue slots ~70 % busy, no DRAM traffic"}
+                "boot": "integer issue: the 128-bit multiplies of the bootstrap draws; no DRAM traffic"}
 
 
-def bench_pairs(args, ctx, rank, world, local, reads):
+def bench_pairs(args, ctx, rank, world, local, reads, dump):
     """BASELINE.json configs[2] (1 sample x G genomes, 1 GPU) and configs[3] (16 samples x G genomes PER GPU, db sharded
     by genome, weak scaling: --samples 16 runs the same 16-sample workload on 1 GPU).  Multi-sample runs draw a
     different community for every sample (seeds 0x5EED0010 + s) from the WHOLE genome range, so pass-1 survivors,
@@ -637,6 +673,10 @@ def bench_pairs(args, ctx, rank, world, local, reads):
     pairs = float(n_samples) * G_total
     value = pairs * args.steps / (ms * 1e-3)
     rows = st["rows"]
+    if dump:
+        for f in rows.dtype.names:
+            if f != "reserved":
+                dump.add("profile_" + f, rows[f])
     out = {"metric": "(sample x genome) containment pairs/s", "value": value, "unit": "pairs/s", "ms_per_step": ms / args.steps,
            "wall_ms_per_step": wall / args.steps, "steps": args.steps, "gpu_launches": int(launches),
            "config": profile_config(args, world),
@@ -665,7 +705,7 @@ def bench_pairs(args, ctx, rank, world, local, reads):
                        "algorithmic_bytes_per_launch": alg_bytes,
                        "note": "SURVEY §8(d) byte model of a genome-streaming probe loop; this implementation probes a sorted db "
                                "index with the sample keys and never streams the db, so this is an EQUIVALENT bandwidth (DESIGN.md "
-                               "4.4); ncu --set full of the kernels: profiles/r02_contain_kernels_ncu_full_selected.csv"}
+                               "4.4)"}
     # ---- parity: sample 0's rows against the CPU oracle on the WHOLE db (N>1: shards gathered on every rank)
     if not args.no_cpu:
         if world > 1:
@@ -716,18 +756,19 @@ def main():
     rank, world, local = dist_setup(args.gpus)
     import sylph_b200
     ctx = sylph_b200.Context(local, stream=torch.cuda.current_stream().cuda_stream)
+    dump = OutputDump(args.dump_outputs if rank == 0 else None)
     if args.workload == "sketch":
-        line, reads = bench_sketch(args, ctx, rank, world, local)
+        line, reads = bench_sketch(args, ctx, rank, world, local, dump)
         if not args.no_pairs:
-            line["pairs"] = bench_pairs(args, ctx, rank, world, local, reads)
+            line["pairs"] = bench_pairs(args, ctx, rank, world, local, reads, dump)
             del reads
-            line["genomes"] = bench_genomes(args, ctx, rank, world, local)
+            line["genomes"] = bench_genomes(args, ctx, rank, world, local, dump)
     elif args.workload == "genomes":
-        line = bench_genomes(args, ctx, rank, world, local)
+        line = bench_genomes(args, ctx, rank, world, local, dump)
     else:
         from sylph_b200 import synth
         reads = synth.reads(args.reads, READ_LEN, seed=synth.SEED_READS + 0x10 * rank, device="cuda")
-        p = bench_pairs(args, ctx, rank, world, local, reads)
+        p = bench_pairs(args, ctx, rank, world, local, reads, dump)
         line = {"metric": p["metric"], "value": p["value"], "unit": p["unit"], "n_gpus": world, "steps": args.steps,
                 "warmup": args.warmup, "ms_per_step": p["ms_per_step"], "higher_is_better": True, "scaling": "weak",
                 "vs_baseline": None, "dtype": "u64", "data": "synthetic", "config": p["config"],

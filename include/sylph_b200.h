@@ -1,5 +1,5 @@
 /*
- * sylph_b200.h — C ABI of the B200-native (sm_100a) implementation of sylph's two hot paths:
+ * sylph_b200.h — C ABI of the H100-native (sm_90a) implementation of sylph's two hot paths:
  * FracMinHash sketching and containment query/profile.
  *
  * The reference (bluenote-1577/sylph v0.8.1, Rust) has no FFI or plugin interface; its backend
@@ -17,7 +17,7 @@
  *     says otherwise.  `mem` tells where caller pointers live (SYL_MEM_HOST / SYL_MEM_DEVICE).
  *   - a syl_ctx owns one CUDA device + one stream; calls on one ctx are serialised by the
  *     caller (one ctx per rayon worker / per rank).  No global mutable state.
- *   - there is NO CPU fallback: if no sm_100-class device / kernel image is available, calls
+ *   - there is NO CPU fallback: if no compute capability 9.0 device / kernel image is available, calls
  *     fail with SYL_ERR_CUDA.
  *   - hard limits (reported as SYL_ERR_ARG, never silently wrapped): fewer than 2^32-2 records per batch,
  *     fewer than 2^32-2 survivor events per sample, fewer than 2^32-2 index entries (genome_kmers + tracked)

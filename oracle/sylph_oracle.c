@@ -1,7 +1,7 @@
 /*
  * sylph_oracle.c — CPU restatement of sylph v0.8.1's sketch + containment hot paths.
  * TEST INFRASTRUCTURE ONLY (see sylph_oracle.h for the usage rule and the parity-pin status).
- * Every function cites the reference file:line (relative to /root/reference) it follows.
+ * Every function cites the reference file:line (relative to the root of the reference repository) it follows.
  */
 #include "sylph_oracle.h"
 

@@ -2,7 +2,7 @@
  * sylph_oracle.h — CPU restatement of sylph's two hot paths (TEST INFRASTRUCTURE ONLY).
  *
  * This is the parity oracle for sylph_b200.  It restates, in plain C, the algorithm of
- * bluenote-1577/sylph v0.8.1 (reference tree at /root/reference, cited file:line below).
+ * bluenote-1577/sylph v0.8.1 (cited file:line relative to the root of the reference repository).
  * Nothing in the product path (sylph_b200/, include/) may include, link or call this file;
  * only tests/, __graft_entry__.smoke() and bench.py's cpu_baseline / --impl reference legs do.
  *

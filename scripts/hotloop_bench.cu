@@ -1,6 +1,6 @@
 // Scratch microbenchmark: the seeding hot loop alone (no staging, packing, tables or output) at several
 // occupancies, to separate "what the instruction mix can sustain" from "what the phases around it cost".
-//   nvcc -gencode arch=compute_100a,code=sm_100a -O3 -std=c++17 --expt-relaxed-constexpr -o exp/hotloop_bench scripts/hotloop_bench.cu
+//   nvcc -gencode arch=compute_90a,code=sm_90a -O3 -std=c++17 --expt-relaxed-constexpr -o exp/hotloop_bench scripts/hotloop_bench.cu
 #include <cstdio>
 #include <vector>
 #include "../sylph_b200/csrc/seed_warp.cuh"
@@ -79,7 +79,7 @@ __global__ void __launch_bounds__(256) k_hot(uint32_t *out, int iters, ShiftMul 
 int main() {
     cudaDeviceProp prop; cudaGetDeviceProperties(&prop, 0);
     const int sms = prop.multiProcessorCount;
-    uint32_t *out; cudaMalloc(&out, 148 * 8 * 256 * 4 * 2);
+    uint32_t *out; cudaMalloc(&out, (size_t)sms * 8 * 256 * 4 * 2);
     const ShiftMul smul = {1u << 8, 1u << 18, 1u << 4, 1u, 0u};
     const uint32_t thr_hi = 0x0147AE14u;
     const int iters = 2000;

@@ -1,4 +1,4 @@
-"""sylph_b200 — B200-native (sm_100a) FracMinHash sketching + containment for sylph.
+"""sylph_b200 — H100-native (sm_90a) FracMinHash sketching + containment for sylph.
 
 The product is the CUDA shared library behind include/sylph_b200.h; this package is the thin
 host-side mirror used by the tests, bench.py and Python callers.  Importing it never touches

@@ -95,9 +95,9 @@ int syl_ctx_create(int device, void *stream, syl_ctx **out) {
     SYL_CUDA(cudaSetDevice(device));
     cudaDeviceProp prop;
     SYL_CUDA(cudaGetDeviceProperties(&prop, device));
-    if (prop.major < 10) {
+    if (prop.major != 9 || prop.minor != 0) {  // sm_90a code runs on compute capability 9.0 only
         set_error(std::string("device ") + prop.name + " is sm_" + std::to_string(prop.major) +
-                  std::to_string(prop.minor) + "; this library only carries sm_100a code");
+                  std::to_string(prop.minor) + "; this library only carries sm_90a code");
         return SYL_ERR_CUDA;
     }
     syl_ctx *ctx = new (std::nothrow) syl_ctx();

@@ -1,4 +1,4 @@
-// common.cuh — shared device/host helpers for the sylph_b200 kernels (sm_100a only).
+// common.cuh — shared device/host helpers for the sylph_b200 kernels (sm_90a only).
 #pragma once
 
 #include <cuda_runtime.h>
@@ -48,7 +48,7 @@ struct syl_ctx {
     int device = 0;
     cudaStream_t stream = nullptr;
     bool own_stream = false;
-    int num_sms = 148;
+    int num_sms = 132;
     uint64_t launches = 0;
     // small persistent scratch: device counters + pinned host mirror
     uint64_t *d_counters = nullptr;  // 32 x u64

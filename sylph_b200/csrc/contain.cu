@@ -1,4 +1,4 @@
-// contain.cu — containment query / profile on sm_100a.
+// contain.cu — containment query / profile on sm_90a.
 //
 // Replaces, for every (sample, genome) pair at once, the get_stats loops of contain()
 // (src/contain.rs:284-292 pass 1, :297-327 pass 2) including

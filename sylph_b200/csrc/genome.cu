@@ -328,7 +328,7 @@ __global__ void k_genome_ranges(const uint64_t *__restrict__ poskey, const uint3
 }
 
 // ---- duplicates (src/sketch.rs:594-600,605: a hash seen twice in one genome drops all its occurrences) ----
-// One open-addressing table for the whole batch in global memory (it stays in the 126 MB L2): genome g owns the
+// One open-addressing table for the whole batch in global memory (blocks touch only their genomes' regions): genome g owns the
 // slots [2 * gs[g], 2 * gs[g+1]) — load factor 1/2 whatever the genome's size or its share of repeats, so there is
 // no table-overflow case.  A key is the 64-bit hash (< 2^63 for every c >= 2); bit 63 of a stored key is the
 // "seen again" mark, set with an atomic OR by every later occurrence; the empty key is all ones.

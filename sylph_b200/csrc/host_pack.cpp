@@ -16,7 +16,7 @@ namespace syl {
 
 namespace {
 
-constexpr uint64_t PACK_PREFETCH_DEFAULT = 2048;  // measured on the B200 hosts: 1 GB in 13.3 ms (off), 12.3 (1024), 11.3 (4096), 11.9 (8192) with 15 threads
+constexpr uint64_t PACK_PREFETCH_DEFAULT = 2048;  // bytes the packer prefetches ahead of its read position
 
 struct Lut {
     uint8_t t[256];
@@ -174,8 +174,7 @@ int default_pack_threads() {
             return (int)std::max(1u, std::min(std::min(hc, 32u), mine));
         }
     }
-    // the packer is memory-bound well before all cores of a big host are busy (measured on a 2 x 32-core
-    // host: 16 threads 68 GB/s, 32 threads 85 GB/s, 64 threads 90 GB/s of ASCII input)
+    // the packer is memory-bound well before all cores of a big host are busy
     return (int)std::max(1u, std::min(hc > 2 ? hc / 2u : hc, 32u));
 }
 

@@ -1,4 +1,4 @@
-// seed.cu — FracMinHash seeding on sm_100a.
+// seed.cu — FracMinHash seeding on sm_90a.
 //
 // Replaces, for a whole batch of records at once, the reference's per-record
 //   extract_markers            (src/sketch.rs:53-69  -> src/avx2_seeding.rs:33-148 / src/seeding.rs:86-146)

@@ -1,4 +1,4 @@
-"""CPU suite: the C-ABI library builds for sm_100a, loads, exports every symbol the header
+"""CPU suite: the C-ABI library builds for sm_90a, loads, exports every symbol the header
 declares, and refuses to work without a GPU (no CPU fallback)."""
 import ctypes as C
 import os
@@ -60,8 +60,8 @@ def test_product_never_imports_oracle():
                 assert not re.search(r"(from|import)\s+oracle\b|#include\s+[\"<].*oracle|liboracle", code), os.path.join(root, f)
 
 
-def test_sass_is_blackwell_native():
-    """cuobjdump evidence: sm_100a cubin, TMA bulk copy (UBLKCP) + mbarrier (SYNCS) in the seeding kernel."""
+def test_sass_is_hopper_native():
+    """cuobjdump evidence: sm_90a cubin, TMA bulk copy (UBLKCP) + mbarrier (SYNCS) in the seeding kernel."""
     import shutil
     import subprocess
     from sylph_b200 import build
@@ -71,5 +71,5 @@ def test_sass_is_blackwell_native():
     build.build()
     obj = os.path.join(build.OBJ, "seed_k31_ev.o")  # k_seed<31, events> for the three run lengths
     out = subprocess.run([cuobjdump, "-sass", obj], stdout=subprocess.PIPE, text=True).stdout
-    assert "sm_100a" in out or "SM100" in out.upper()
+    assert "sm_90a" in out or "SM90A" in out.upper()
     assert "UBLKCP" in out and "SYNCS" in out

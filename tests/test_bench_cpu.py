@@ -44,6 +44,32 @@ def test_both_arms_share_the_config_object():
     assert bench.profile_config(A, 1)["samples"] == 1 and bench.profile_config(A, 8)["samples"] == 16
 
 
+def test_output_dump_is_exact_seeded_and_bounded(tmp_path):
+    """--dump-outputs: u64 hashes survive as float64 halves, long arrays are sampled at the same rows every time."""
+    import numpy as np
+    sys.path.insert(0, REPO)
+    import bench
+    h = np.sort(np.random.default_rng(7).integers(0, 2**63, bench.DUMP_MAX_ROWS + 5, dtype=np.uint64))
+    for d in (tmp_path / "a", tmp_path / "b"):
+        dump = bench.OutputDump(str(d))
+        dump.add("hash", h)
+        dump.add("count", np.arange(10, dtype=np.uint32))
+    a = {p.name: np.load(p) for p in (tmp_path / "a").iterdir()}
+    assert set(a) == {"hash_hi.npy", "hash_lo.npy", "count.npy"} and all(x.dtype == np.float64 for x in a.values())
+    back = (a["hash_hi.npy"].astype(np.uint64) << np.uint64(32)) | a["hash_lo.npy"].astype(np.uint64)
+    assert len(back) == bench.DUMP_MAX_ROWS and np.all(np.isin(back, h)) and np.all(back[1:] > back[:-1])
+    assert all(np.array_equal(x, np.load(tmp_path / "b" / n)) for n, x in a.items())
+    assert a["count.npy"].tolist() == list(range(10))
+    big = bench.OutputDump(str(tmp_path / "c"))
+    try:
+        for i in range(9):
+            big.add("x%d" % i, np.zeros(bench.DUMP_MAX_ROWS, np.uint32))
+        raise AssertionError("the 64 MB bound was not enforced")
+    except SystemExit:
+        pass
+    assert not bench.OutputDump(None)
+
+
 def test_clock_sampler_degrades_without_a_gpu():
     sys.path.insert(0, REPO)
     import bench
