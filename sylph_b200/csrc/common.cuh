@@ -152,6 +152,8 @@ static_assert(sizeof(EventRec) == 32, "EventRec is one 32-byte sector");
 constexpr uint64_t NO_PAIR = 1ull;
 constexpr uint64_t EV_PENDING = 1ull << 63;
 
+constexpr uint32_t GRP_BPG = 32;  // hash buckets per read-sketch post-pass group (GroupOut in seed_kernel.cuh)
+
 // One batch for the seeding kernel (seed.cu: seed_enqueue).  Exactly one of d_bases (ASCII) / d_packed
 // (2-bit words: base 16w+j of the batch in bits [30-2j, 31-2j] of word w) is set.
 struct SeedJob {
@@ -163,15 +165,15 @@ struct SeedJob {
     int k = 31;
     uint64_t c = 200;
     int sem = SYL_SEM_AVX2, with_pos = 0;
-    void *d_out = nullptr;                // syl_survivor[cap], or EventRec[cap] when emit_events
+    void *d_out = nullptr;                // syl_survivor[cap], or EventRec[ng * slot + cap] when emit_events
     uint64_t cap = 0;
     int emit_events = 0;
     uint64_t rec_base = 0;                // index of the batch's first read (events)
     int no_dedup = 0;
     uint32_t *d_pend = nullptr;           // indices of events whose pair keys are still missing
-    uint32_t *d_bucket_cnt = nullptr;     // post-pass bucket histogram (events)
+    uint32_t *d_group_cnt = nullptr;      // events: post-pass group counters (GroupOut in seed_kernel.cuh); nullptr = append
     uint64_t Mb = 0;
-    uint32_t nbk = 0;
+    uint32_t nbk = 0, ng = 0, slot = 0;
     unsigned long long *d_count = nullptr, *d_pend_count = nullptr;  // running device counters
     // slotted survivor output (genome sketching, CTA kernel only): see SlotOut in seed_kernel.cuh
     uint32_t slot_cap = 0;

@@ -273,84 +273,33 @@ __global__ void k_copy_len(const uint32_t *__restrict__ len, uint32_t *__restric
 
 
 // ------------------------------------------------------------------------------------------------
-// Post-pass, primary path: MSD bucket partition + CTA-local sort + fused run-length / dedup.
-//   k_bucket_hist / k_scan_u32 / k_scatter_events : partition the events by bucket =
-//       mulhi(hash, Mb) (monotone in the hash, uniform because hashes are uniform below thr)
-//   k_group_dedup : one CTA takes the consecutive buckets whose start offset falls into
-//       [g*T, (g+1)*T) (<= GRP_CAP events), bitonic-sorts them by (hash, read) in shared memory,
-//       finds the k-mer segments and replays dup_removal_lsh_full_exact per segment
+// Post-pass, primary path: MSD bucket partition + CTA-local grouping + fused run-length / dedup.
+//   the seeding kernel's flush (GroupOut, seed_kernel.cuh) : writes every event into the slot of its
+//       group g = bucket / GRP_BPG, bucket = min(mulhi(hash, Mb), nbk - 1) (monotone in the hash, uniform
+//       because hashes are uniform below thr); the groups are fixed in begin() at ~GRP_T expected events
+//   k_group_dedup : one CTA per group (<= slot events) groups the events by k-mer in shared memory
+//       and replays dup_removal_lsh_full_exact per k-mer
 //   k_compact_uniq : staged (hash,count) pairs -> dense arrays; buckets are monotone in the hash
 //       and every group is sorted, so the result is globally sorted without a merge.
-// Groups that do not fit (heavy-hitter k-mers, > GRP_CAP events) or whose dedup set outgrows
-// the per-thread buffer are handed to the generic radix-sort path below and merged at the end.
+// Groups that do not fit (heavy-hitter k-mers: more events than the slot, the rest in the overflow list)
+// or whose dedup set outgrows the per-thread buffer are handed to the generic radix-sort path below and
+// merged at the end.
 constexpr int GRP_THREADS = 256;
-constexpr int GRP_CAP = 1024;   // most events one CTA handles in shared memory
-constexpr int GRP_T = 768;      // group span in event offsets: typical n ~ 800, leaving room for k-mers with ~200 events
-
-__global__ void k_bucket_hist(const EventRec *__restrict__ ev, uint64_t n, uint64_t Mb, uint32_t nbk,
-                              uint32_t *__restrict__ cnt) {
-    uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= n) return;
-    uint32_t b = (uint32_t)__umul64hi(ev[i].hash, Mb);
-    atomicAdd(&cnt[b < nbk ? b : nbk - 1], 1u);
-}
-
-// n events (device-side count, clamped to the array capacity) -> bucket order
-__global__ void k_scatter_events(const EventRec *__restrict__ ev, const unsigned long long *__restrict__ d_n, uint64_t ev_cap,
-                                 uint64_t Mb, uint32_t nbk, const uint32_t *__restrict__ boff,
-                                 uint32_t *__restrict__ cursor, EventRec *__restrict__ part) {
-    const uint64_t n = *d_n < ev_cap ? *d_n : ev_cap;
-    for (uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (uint64_t)gridDim.x * blockDim.x) {
-        const uint4 *src = reinterpret_cast<const uint4 *>(ev + i);
-        const uint4 lo = __ldcs(src), hi = __ldcs(src + 1);  // read once: keep L2 for the scattered writes
-        const uint64_t h = ((uint64_t)lo.y << 32) | lo.x;
-        uint32_t b = (uint32_t)__umul64hi(h, Mb);
-        if (b >= nbk) b = nbk - 1;
-        const uint64_t pos = (uint64_t)boff[b] + atomicAdd(&cursor[b], 1u);
-        if (pos >= ev_cap) continue;  // only after an overflow (the whole sample is redone then)
-        uint4 *dst = reinterpret_cast<uint4 *>(part + pos);
-        dst[0] = lo;
-        dst[1] = hi;
-    }
-}
-
-__device__ __forceinline__ uint32_t lower_bound_u32(const uint32_t *a, uint32_t n, uint64_t v) {
-    uint32_t lo = 0, hi = n;
-    while (lo < hi) {
-        uint32_t mid = (lo + hi) >> 1;
-        if ((uint64_t)a[mid] < v) lo = mid + 1; else hi = mid;
-    }
-    return lo;
-}
-
-// group g = the consecutive buckets whose start offset lies in [g*T, (g+1)*T): bucket range -> g_bf / g_be
-__global__ void k_group_ranges(const uint32_t *__restrict__ boff, uint32_t nbk, uint32_t ng, uint32_t *__restrict__ g_bf,
-                               uint32_t *__restrict__ g_be) {
-    const uint32_t g = blockIdx.x * blockDim.x + threadIdx.x;
-    if (g >= ng) return;
-    uint32_t bf = lower_bound_u32(boff, nbk + 1, (uint64_t)g * GRP_T);
-    uint32_t be = lower_bound_u32(boff, nbk + 1, (uint64_t)(g + 1) * GRP_T);
-    if (bf > nbk) bf = nbk;
-    if (be > nbk) be = nbk;
-    if (be < bf) be = bf;
-    g_bf[g] = bf;
-    g_be[g] = be;
-}
+constexpr int GRP_CAP = 1024;   // most events one CTA handles in shared memory (= slot per group)
+constexpr int GRP_T = 640;      // expected events per group: room in the slot for the spread of duplicate-heavy k-mers
 
 __device__ __forceinline__ uint32_t bucket_of(uint64_t h, uint64_t Mb, uint32_t nbk) {
     const uint32_t b = (uint32_t)__umul64hi(h, Mb);
     return b < nbk ? b : nbk - 1;
 }
 
-// One CTA per group (<= GRP_CAP events, consecutive buckets). Shared-memory traffic is what
+// One CTA per group (<= slot events, GRP_BPG consecutive buckets). Shared-memory traffic is what
 // bounds this kernel, so instead of sorting all events (a 128-bit-key bitonic sort was 4x slower)
 // it (1) groups equal hashes with an open-addressing table, (2) replays
 // dup_removal_lsh_full_exact on each k-mer's first events in read order, (3) orders the resulting
 // unique (hash, count) pairs: the group's buckets are already monotone in the hash, so a pair's
-// position is its bucket's offset plus its rank among the ~10 pairs of the same bucket (a bitonic
-// sort of the pairs remains for groups spanning more than GRP_LB buckets).
+// position is its bucket's offset plus its rank among the ~10 pairs of the same bucket.
 constexpr int GRP_SLOTS = 2048;  // table slots (load factor <= 0.5)
-constexpr int GRP_LB = 512;      // most buckets per group for the bucket-rank output ordering (else bitonic sort)
 constexpr int GRP_SELECT_STEPS = 64;  // selection steps before a duplicate-heavy k-mer goes to the generic path
 
 struct GroupSmem {
@@ -360,44 +309,37 @@ struct GroupSmem {
     uint64_t p1[GRP_CAP];              //  8 KB  second pair key per event
     uint16_t scnt[GRP_SLOTS];          //  4 KB  events per slot, then fill cursor, then the k-mer's count
     uint16_t soff[GRP_SLOTS + 2];      //  4 KB  exclusive scan of scnt
-    uint16_t ev_slot[GRP_CAP];         //  2 KB  slot per event | after the member fill: 2 x GRP_LB bucket counters / offsets
+    uint16_t ev_slot[GRP_CAP];         //  2 KB  slot per event | after the member fill: 2 x GRP_BPG bucket counters / offsets
     uint16_t member[GRP_CAP];          //  2 KB  event indices grouped by slot
     uint16_t occ[GRP_CAP];             //  2 KB  occupied slots, compacted
     uint32_t wtot[GRP_THREADS / 32], wocc[GRP_THREADS / 32];
-    uint32_t e0, e1, overflow, dups, nuniq, nlong, lb_n, bf;
+    uint32_t overflow, dups, nlong;
     uint16_t longs[GRP_CAP / 2];      //  1 KB  slots of k-mers that need the warp-cooperative replay
 };
 
 __global__ void __launch_bounds__(GRP_THREADS)
-k_group_dedup(const EventRec *__restrict__ part, const uint32_t *__restrict__ boff, const uint32_t *__restrict__ g_bf,
-              const uint32_t *__restrict__ g_be, uint32_t cap, uint32_t ev_cap, uint64_t Mb, uint32_t nbk,
+k_group_dedup(const EventRec *__restrict__ ev, const uint32_t *__restrict__ g_cnt, uint32_t slot, uint64_t Mb, uint32_t nbk,
               int no_dedup, uint64_t *__restrict__ st_hash, uint32_t *__restrict__ st_cnt,
-              uint32_t *__restrict__ g_nuniq, uint32_t *__restrict__ g_e0, uint32_t *__restrict__ g_n,
+              uint32_t *__restrict__ g_nuniq, uint32_t *__restrict__ g_n,
               uint8_t *__restrict__ g_fallback, unsigned long long *__restrict__ n_dup) {
     extern __shared__ __align__(16) uint8_t grp_smem_raw[];
     GroupSmem &S = *reinterpret_cast<GroupSmem *>(grp_smem_raw);
     const int tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
     const uint32_t g = blockIdx.x;
     if (tid == 0) {
-        S.e0 = boff[g_bf[g]];  // boff[nbk] = N
-        S.e1 = boff[g_be[g]];
-        S.bf = g_bf[g];
-        S.lb_n = g_be[g] - g_bf[g];
         S.overflow = 0;
         S.dups = 0;
         S.nlong = 0;
     }
-    __syncthreads();
-    const uint32_t e0 = S.e0, bf = S.bf;
-    const uint32_t n = S.e1 <= ev_cap ? S.e1 - S.e0 : 0u;  // past the capacity only after an overflow (sample is redone)
-    if (tid == 0) { g_e0[g] = e0; g_n[g] = n; g_nuniq[g] = 0; g_fallback[g] = 0; }
-    if (n == 0) return;  // the grid is sized for the event capacity: most surplus groups leave here
+    const uint32_t e0 = g * slot, bf = g * GRP_BPG;
+    const uint32_t n_all = g_cnt[g], n = min(n_all, slot);  // events past the slot are in the overflow list
+    if (tid == 0) { g_n[g] = n; g_nuniq[g] = 0; g_fallback[g] = n_all > slot; }
+    if (n == 0 || n_all > slot) return;
     for (int i = tid; i < GRP_SLOTS; i += GRP_THREADS) { S.ht[i] = 0xFFFFFFFFFFFFFFFFull; S.scnt[i] = 0; }
     __syncthreads();
-    if (n > cap) { if (tid == 0) g_fallback[g] = 1; return; }
     // (1) stage the events, group equal hashes: slot per event, events per slot
     for (uint32_t i = tid; i < n; i += GRP_THREADS) {
-        const uint4 *src = reinterpret_cast<const uint4 *>(part + e0 + i);
+        const uint4 *src = reinterpret_cast<const uint4 *>(ev + e0 + i);
         const uint4 a = __ldcs(src), b = __ldcs(src + 1);  // read once
         const unsigned long long h = ((unsigned long long)a.y << 32) | a.x;
         S.rf[i] = ((uint64_t)a.w << 32) | a.z;
@@ -460,17 +402,14 @@ k_group_dedup(const EventRec *__restrict__ part, const uint32_t *__restrict__ bo
     //     has more than four events AND a duplicate among the first four needs more; it is queued
     //     for the warp-cooperative path below.
     //     The thread also counts its k-mer into its bucket (local index) for the output ordering.
-    const uint32_t lb_n = S.lb_n;
-    uint16_t *lb_cnt = S.ev_slot, *lb_off = S.ev_slot + GRP_LB;  // ev_slot is dead: 2 x GRP_LB u16
-    if (lb_n <= (uint32_t)GRP_LB) {
-        for (int i = tid; i < GRP_LB; i += GRP_THREADS) { lb_cnt[i] = 0; }
-        __syncthreads();
-    }
+    uint16_t *lb_cnt = S.ev_slot, *lb_off = S.ev_slot + GRP_BPG;  // ev_slot is dead: 2 x GRP_BPG u16
+    if (tid < (int)GRP_BPG) lb_cnt[tid] = 0;
+    __syncthreads();
     uint32_t my_dups = 0;
     for (uint32_t u = tid; u < nu; u += GRP_THREADS) {
         const uint32_t sl = S.occ[u];
         const uint32_t a0 = S.soff[sl], len = S.soff[sl + 1] - a0;
-        if (lb_n <= (uint32_t)GRP_LB) {
+        {
             const uint32_t lb = bucket_of(S.ht[sl], Mb, nbk) - bf;
             atomicAdd(reinterpret_cast<unsigned int *>(lb_cnt) + (lb >> 1), (lb & 1) ? 0x10000u : 1u);
         }
@@ -566,26 +505,19 @@ k_group_dedup(const EventRec *__restrict__ part, const uint32_t *__restrict__ bo
     if (my_dups) atomicAdd(&S.dups, my_dups);
     __syncthreads();
     if (S.overflow) { if (tid == 0) g_fallback[g] = 1; return; }
-    // (3) output order.  Bucket-rank path: lb_cnt holds the k-mers per bucket (counted in (2)).
-    if (lb_n <= (uint32_t)GRP_LB) {
+    // (3) output order: lb_cnt holds the k-mers per bucket (counted in (2)).
+    {
         uint16_t *list = S.member;  // event grouping is dead: k-mer slots ordered by bucket
-        {   // exclusive scan of lb_cnt (GRP_LB = 2 per thread) -> lb_off, counters reset as cursors
-            constexpr int PER = GRP_LB / GRP_THREADS;
-            uint32_t loc[PER], tot = 0;
-#pragma unroll
-            for (int e = 0; e < PER; e++) { loc[e] = lb_cnt[tid * PER + e]; tot += loc[e]; }
-            uint32_t inc = tot;
+        static_assert(GRP_BPG == 32, "one lane per bucket");
+        if (wid == 0) {  // exclusive scan of lb_cnt -> lb_off, counters reset as cursors
+            const uint32_t v = lb_cnt[lane];
+            uint32_t inc = v;
 #pragma unroll
             for (int d = 1; d < 32; d <<= 1) { const uint32_t t = __shfl_up_sync(0xffffffffu, inc, d); if (lane >= d) inc += t; }
-            if (lane == 31) S.wtot[wid] = inc;
-            __syncthreads();
-            uint32_t base = inc - tot;
-#pragma unroll
-            for (int w = 0; w < GRP_THREADS / 32; w++) if (w < wid) base += S.wtot[w];
-#pragma unroll
-            for (int e = 0; e < PER; e++) { lb_off[tid * PER + e] = (uint16_t)base; base += loc[e]; lb_cnt[tid * PER + e] = 0; }
-            __syncthreads();
+            lb_off[lane] = (uint16_t)(inc - v);
+            lb_cnt[lane] = 0;
         }
+        __syncthreads();
         for (uint32_t u = tid; u < nu; u += GRP_THREADS) {
             const uint32_t sl = S.occ[u];
             const uint32_t lb = bucket_of(S.ht[sl], Mb, nbk) - bf;
@@ -604,49 +536,21 @@ k_group_dedup(const EventRec *__restrict__ part, const uint32_t *__restrict__ bo
             st_hash[e0 + q0 + r] = h;
             st_cnt[e0 + q0 + r] = S.scnt[sl];
         }
-        if (tid == 0) { g_nuniq[g] = nu; if (S.dups) atomicAdd(n_dup, (unsigned long long)S.dups); }
-        return;
     }
-    // Bitonic path: unique pairs into the (now dead) rf / p0 arrays, sorted by hash
-    uint64_t *uh = S.rf;
-    uint32_t *uc = reinterpret_cast<uint32_t *>(S.p0);
-    uint32_t P = 32;
-    while (P < nu) P <<= 1;
-    for (uint32_t i = tid; i < P; i += GRP_THREADS) {
-        if (i < nu) { const uint32_t sl = S.occ[i]; uh[i] = S.ht[sl]; uc[i] = S.scnt[sl]; }
-        else { uh[i] = 0xFFFFFFFFFFFFFFFFull; uc[i] = 0; }
-    }
-    __syncthreads();
-    for (uint32_t k = 2; k <= P; k <<= 1) {
-        for (uint32_t j = k >> 1; j > 0; j >>= 1) {
-            for (uint32_t t = tid; t < (P >> 1); t += GRP_THREADS) {
-                const uint32_t i = ((t & ~(j - 1)) << 1) | (t & (j - 1));
-                const uint32_t l = i | j;
-                const bool up = (i & k) == 0;
-                const uint64_t ha = uh[i], hb = uh[l];
-                if ((ha > hb) == up) {
-                    uh[i] = hb; uh[l] = ha;
-                    const uint32_t x = uc[i]; uc[i] = uc[l]; uc[l] = x;
-                }
-            }
-            __syncthreads();
-        }
-    }
-    for (uint32_t i = tid; i < nu; i += GRP_THREADS) { st_hash[e0 + i] = uh[i]; st_cnt[e0 + i] = uc[i]; }
     if (tid == 0) { g_nuniq[g] = nu; if (S.dups) atomicAdd(n_dup, (unsigned long long)S.dups); }
 }
 
-// staged pairs of group g live at [e0, e0 + nuniq); dense destination starts at uoff[g]
+// staged pairs of group g live at [g * slot, g * slot + nuniq); dense destination starts at uoff[g]
 __global__ void k_compact_uniq(const uint64_t *__restrict__ st_hash, const uint32_t *__restrict__ st_cnt,
-                               const uint32_t *__restrict__ g_e0, const uint32_t *__restrict__ g_nuniq,
+                               uint32_t slot, const uint32_t *__restrict__ g_nuniq,
                                const uint32_t *__restrict__ uoff, const uint8_t *__restrict__ g_fallback,
                                const uint32_t *__restrict__ g_src, const uint64_t *__restrict__ f_hash,
                                const uint32_t *__restrict__ f_cnt, uint64_t *__restrict__ out_hash,
                                uint32_t *__restrict__ out_cnt) {
     const uint32_t g = blockIdx.x, nu = g_nuniq[g], u0 = uoff[g];
     const bool fb = g_fallback[g] != 0;
-    const uint64_t *sh = fb ? f_hash + g_src[g] : st_hash + g_e0[g];
-    const uint32_t *sc = fb ? f_cnt + g_src[g] : st_cnt + g_e0[g];
+    const uint64_t *sh = fb ? f_hash + g_src[g] : st_hash + (uint64_t)g * slot;
+    const uint32_t *sc = fb ? f_cnt + g_src[g] : st_cnt + (uint64_t)g * slot;
     for (uint32_t i = threadIdx.x; i < nu; i += blockDim.x) {
         out_hash[u0 + i] = sh[i];
         out_cnt[u0 + i] = sc[i];
@@ -656,8 +560,7 @@ __global__ void k_compact_uniq(const uint64_t *__restrict__ st_hash, const uint3
 // The generic path returns the fallback groups' unique pairs as ONE list sorted by hash.  Groups own
 // disjoint, increasing hash ranges (bucket = mulhi(hash, Mb) is monotone), so group g's slice is
 // [lower_bound(hash >= first hash of bucket bf), lower_bound(hash >= first hash of bucket be)).
-__global__ void k_fallback_place(const uint8_t *__restrict__ g_fallback, const uint32_t *__restrict__ g_bf,
-                                 const uint32_t *__restrict__ g_be, uint32_t ng, uint32_t nbk, uint64_t Mb,
+__global__ void k_fallback_place(const uint8_t *__restrict__ g_fallback, uint32_t ng, uint32_t nbk, uint64_t Mb,
                                  const uint64_t *__restrict__ f_hash, uint64_t fu, uint32_t *__restrict__ g_nuniq,
                                  uint32_t *__restrict__ g_src) {
     const uint32_t g = blockIdx.x * blockDim.x + threadIdx.x;
@@ -671,23 +574,24 @@ __global__ void k_fallback_place(const uint8_t *__restrict__ g_fallback, const u
         while (lo < hi) { uint64_t mid = (lo + hi) >> 1; if (f_hash[mid] < v) lo = mid + 1; else hi = mid; }
         return lo;
     };
-    const uint32_t bf = g_bf[g], be = g_be[g];
+    const uint32_t bf = g * GRP_BPG, be = bf + GRP_BPG;
     const uint64_t a = bf == 0 ? 0 : lb(first_hash_of(bf));
     const uint64_t b = be >= nbk ? fu : lb(first_hash_of(be));
     g_src[g] = (uint32_t)a;
     g_nuniq[g] = (uint32_t)(b - a);
 }
 
-// events of fallback groups -> compact SoA arrays for the generic path
-__global__ void k_gather_fallback(const EventRec *__restrict__ part, const uint32_t *__restrict__ g_e0,
+// slotted events of fallback groups -> compact SoA arrays for the generic path
+__global__ void k_gather_fallback(const EventRec *__restrict__ ev, uint32_t slot,
                                   const uint32_t *__restrict__ g_n, const uint8_t *__restrict__ g_fallback,
                                   const uint32_t *__restrict__ foff, uint64_t *__restrict__ hash,
                                   uint64_t *__restrict__ recflag, uint64_t *__restrict__ p0, uint64_t *__restrict__ p1) {
     const uint32_t g = blockIdx.x;
     if (!g_fallback[g]) return;
-    const uint32_t e0 = g_e0[g], n = g_n[g], f0 = foff[g];
+    const uint64_t e0 = (uint64_t)g * slot;
+    const uint32_t n = g_n[g], f0 = foff[g];
     for (uint32_t i = threadIdx.x; i < n; i += blockDim.x) {
-        const EventRec r = part[e0 + i];
+        const EventRec r = ev[e0 + i];
         hash[f0 + i] = r.hash; recflag[f0 + i] = r.recflag; p0[f0 + i] = r.p0; p1[f0 + i] = r.p1;
     }
 }
@@ -719,34 +623,50 @@ struct SampleBuilder {
     int no_dedup, sem;
     uint64_t n_reads = 0, n_bases = 0, cap = 0;
     bool paired = false;     // read pairs (syl_sketch_read_pairs): events wait for k_events_fix_paired, generic post-pass only
-    DevBuf<EventRec> b_ev;   // event array (a scratch block of the ctx cache)
+    bool generic_postpass() const {
+        static const bool env_sort = []() { const char *e = getenv("SYL_SAMPLE_POSTPASS"); return e && std::string(e) == "sort"; }();
+        return env_sort || paired;
+    }
+    // Event array: ng group slots of `slot` events each, then the overflow list of cap events (everything
+    // in the overflow list without groups).  A scratch block of the ctx cache.
+    DevBuf<EventRec> b_ev;
     DevBuf<uint32_t> b_pend; // indices of events whose pair keys are filled in by k_events_fix
-    // Post-pass buckets: fixed before the first batch from the expected number of events, so that
-    // the seeding kernel can fill the bucket histogram while it flushes the events.
+    // Post-pass groups: fixed before the first batch from the expected number of events, so that the
+    // seeding kernel can write every event into its group while it flushes them.
     uint64_t expect_bases = 0, expect_reads = 0;
-    uint32_t nbk = 0;
+    uint32_t nbk = 0, ng = 0, slot = 0;
     uint64_t Mb = 0;
-    DevBuf<uint32_t> cnt;
-    // ctx->d_counters slots: [0] events, [1] pending events, [2] duplicates removed, [3] pending snapshot
+    DevBuf<uint32_t> g_cnt;  // events per group
+    // ctx->d_counters slots: [0] events in the overflow list, [1] pending events, [2] duplicates removed, [3] pending snapshot
     unsigned long long *d_count() const { return reinterpret_cast<unsigned long long *>(ctx->d_counters); }
+    uint64_t ev_total() const { return (uint64_t)ng * slot + cap; }
 
     int begin(uint64_t cap_override) {
         cudaStream_t st = ctx->stream;
         const uint64_t win = expect_bases > expect_reads * (uint64_t)(k - 1) ? expect_bases - expect_reads * (uint64_t)(k - 1) : 0;
         const uint64_t n_exp = win / c;
-        nbk = 4096;
-        while (nbk < n_exp / 32 && nbk < (1u << 22)) nbk <<= 1;
-        const uint64_t thr = fmh_threshold(c);
-        unsigned __int128 mb = ((unsigned __int128)nbk << 64) / ((unsigned __int128)thr + 1);
-        Mb = mb > (unsigned __int128)UINT64_MAX ? UINT64_MAX : (uint64_t)mb;
-        SYL_TRY(cnt.alloc(nbk, st));
-        SYL_CUDA(cudaMemsetAsync(cnt.p, 0, (size_t)nbk * 4, st));
+        if (!generic_postpass()) {
+            static const uint32_t grp_cap = []() { const char *e = getenv("SYL_GROUP_CAP"); int v = e ? atoi(e) : GRP_CAP; return (uint32_t)std::min(std::max(v, 32), GRP_CAP); }();
+            slot = grp_cap;
+            const uint64_t g = n_exp / GRP_T + 1;
+            if (g * GRP_BPG >= 0xFFFFFFFFull) { set_error("more than 2^32-2 survivor events in one sample"); return SYL_ERR_ARG; }
+            ng = (uint32_t)g;
+            nbk = ng * GRP_BPG;
+            const uint64_t thr = fmh_threshold(c);
+            unsigned __int128 mb = ((unsigned __int128)nbk << 64) / ((unsigned __int128)thr + 1);
+            Mb = mb > (unsigned __int128)UINT64_MAX ? UINT64_MAX : (uint64_t)mb;
+            SYL_TRY(g_cnt.alloc(ng, st));
+            SYL_CUDA(cudaMemsetAsync(g_cnt.p, 0, (size_t)ng * 4, st));
+        }
         cap = expect_bases / c + expect_bases / (4 * c) + 65536;
         if (cap > expect_bases) cap = expect_bases + 16;
+        // with groups cap is the overflow list, almost always empty: 1/16 of the estimate; a sample that
+        // needs more (duplicate-heavy, homopolymers) is redone with the exact length
+        if (ng) cap = cap / 16 + 65536;
         if (cap_override) cap = cap_override;
-        if (cap >= 0xFFFFFFFEull) { set_error("more than 2^32-2 survivor events in one sample"); return SYL_ERR_ARG; }
-        SYL_TRY(b_ev.alloc(cap, st));
-        SYL_TRY(b_pend.alloc(cap, st));
+        if (ev_total() >= 0xFFFFFFFEull) { set_error("more than 2^32-2 survivor events in one sample"); return SYL_ERR_ARG; }
+        SYL_TRY(b_ev.alloc(ev_total(), st));
+        SYL_TRY(b_pend.alloc(ev_total(), st));
         SYL_CUDA(cudaMemsetAsync(ctx->d_counters, 0, 4 * sizeof(uint64_t), st));
         return SYL_OK;
     }
@@ -764,12 +684,12 @@ struct SampleBuilder {
         job.d_bases = d_bases; job.d_packed = d_packed; job.n_bases = nb; job.d_rec_off = d_off; job.off_bias = off_bias;
         job.n_rec = nr; job.k = k; job.c = c; job.sem = sem; job.with_pos = 0; job.d_out = b_ev.p; job.cap = cap;
         job.emit_events = 1; job.rec_base = rec_base; job.no_dedup = paired ? 2 : no_dedup; job.d_pend = b_pend.p;
-        job.d_bucket_cnt = cnt.p; job.Mb = Mb; job.nbk = nbk; job.d_count = dc; job.d_pend_count = dc + 1;
+        job.d_group_cnt = g_cnt.p; job.Mb = Mb; job.nbk = nbk; job.ng = ng; job.slot = slot; job.d_count = dc; job.d_pend_count = dc + 1;
         SYL_TRY(seed_enqueue(ctx, job));
         if (!no_dedup && !paired && nb) {  // reads cut by a tile edge: their pair keys come from global memory
             const uint64_t n_words = (nb + 15) / 16;
-            if (d_packed) k_events_fix<true><<<ctx->num_sms * 2, EV_THREADS, 0, st>>>(b_ev.p, b_pend.p, dc + 3, dc + 1, cap, nullptr, d_packed, n_words, d_off, off_bias, rec_base);
-            else k_events_fix<false><<<ctx->num_sms * 2, EV_THREADS, 0, st>>>(b_ev.p, b_pend.p, dc + 3, dc + 1, cap, d_bases, nullptr, 0, d_off, off_bias, rec_base);
+            if (d_packed) k_events_fix<true><<<ctx->num_sms * 2, EV_THREADS, 0, st>>>(b_ev.p, b_pend.p, dc + 3, dc + 1, ev_total(), nullptr, d_packed, n_words, d_off, off_bias, rec_base);
+            else k_events_fix<false><<<ctx->num_sms * 2, EV_THREADS, 0, st>>>(b_ev.p, b_pend.p, dc + 3, dc + 1, ev_total(), d_bases, nullptr, 0, d_off, off_bias, rec_base);
             ctx->launches++;
             SYL_CUDA(cudaGetLastError());
         }
@@ -870,13 +790,10 @@ struct SampleBuilder {
         auto fail = [&](int rc) { syl_sample_free(s); return rc; };
 #define SB_CUDA(x) do { cudaError_t _e = (x); if (_e != cudaSuccess) { set_error(std::string(#x) + ": " + cudaGetErrorString(_e)); return fail(_e == cudaErrorMemoryAllocation ? SYL_ERR_OOM : SYL_ERR_CUDA); } } while (0)
         if (n_reads == 0 || n_bases == 0) { *out = s; return SYL_OK; }
-        static const bool env_sort = []() { const char *e = getenv("SYL_SAMPLE_POSTPASS"); return e && std::string(e) == "sort"; }();
-        const bool force_sort = env_sort || paired;
-        static const uint32_t grp_cap = []() { const char *e = getenv("SYL_GROUP_CAP"); int v = e ? atoi(e) : GRP_CAP; return (uint32_t)std::min(std::max(v, 32), GRP_CAP); }();
         unsigned long long *dc = d_count();
         EventRec *ev = b_ev.p;
         int rc;
-        if (force_sort) {
+        if (generic_postpass()) {
             SB_CUDA(cudaMemcpyAsync(ctx->h_counters, dc, 8, cudaMemcpyDeviceToHost, st));
             SB_CUDA(cudaStreamSynchronize(st));
             const uint64_t N = ctx->h_counters[0];
@@ -900,58 +817,45 @@ struct SampleBuilder {
             *out = s;
             return SYL_OK;
         }
-        // ---- primary path: bucket partition + CTA-local grouping / dedup (nbk, Mb, cnt: begin()).
-        // Every grid is sized for the capacity; the kernels read the event count from device memory.
-        const uint32_t ng = (uint32_t)(cap / GRP_T + 1);
-        DevBuf<uint32_t> boff, cursor, st_cnt, g_nuniq, g_e0, g_n, uoff, fsz, foff, g_bf, g_be, g_src, tmp_c;
+        // ---- primary path: CTA-local grouping / dedup of the group slots (ng, slot, Mb, g_cnt: begin()).
+        // The kernels read the group counts from device memory.
+        const uint64_t n_slots = (uint64_t)ng * slot;
+        DevBuf<uint32_t> st_cnt, g_nuniq, g_n, uoff, fsz, foff, g_src, tmp_c;
         DevBuf<uint64_t> st_hash, tmp_h;
         DevBuf<uint8_t> g_fb;
-        DevBuf<EventRec> part;
-        if ((rc = boff.alloc((uint64_t)nbk + 1, st)) || (rc = cursor.alloc(nbk, st)) ||
-            (rc = part.alloc(cap, st)) || (rc = st_hash.alloc(cap, st)) || (rc = st_cnt.alloc(cap, st)) ||
-            (rc = tmp_h.alloc(cap, st)) || (rc = tmp_c.alloc(cap, st)) ||
-            (rc = g_nuniq.alloc(ng, st)) || (rc = g_e0.alloc(ng, st)) || (rc = g_n.alloc(ng, st)) ||
+        if ((rc = st_hash.alloc(n_slots, st)) || (rc = st_cnt.alloc(n_slots, st)) ||
+            (rc = tmp_h.alloc(n_slots, st)) || (rc = tmp_c.alloc(n_slots, st)) ||  // in-kernel uniques: <= the slotted events
+            (rc = g_nuniq.alloc(ng, st)) || (rc = g_n.alloc(ng, st)) ||
             (rc = g_fb.alloc(ng, st)) || (rc = uoff.alloc((uint64_t)ng + 1, st)) || (rc = fsz.alloc(ng, st)) ||
-            (rc = foff.alloc((uint64_t)ng + 1, st)) || (rc = g_bf.alloc(ng, st)) || (rc = g_be.alloc(ng, st)) ||
-            (rc = g_src.alloc(ng, st)))
+            (rc = foff.alloc((uint64_t)ng + 1, st)) || (rc = g_src.alloc(ng, st)))
             return fail(rc);
         unsigned long long *d_ndup = dc + 2;
-        SB_CUDA(cudaMemsetAsync(cursor.p, 0, (size_t)nbk * 4, st));
-        {   // boff = exclusive scan of cnt (nbk >= 4096 entries): local scans, scan of block totals, add back
-            const uint32_t nblk1 = nbk / 1024;
-            DevBuf<uint32_t> btot, boff2;
-            if ((rc = btot.alloc(nblk1, st)) || (rc = boff2.alloc((uint64_t)nblk1 + 1, st))) return fail(rc);
-            k_scan_local<<<nblk1, 1024, 0, st>>>(cnt.p, nbk, boff.p, btot.p);
-            k_scan_u32<<<1, 1024, 0, st>>>(btot.p, nblk1, boff2.p);
-            k_scan_add<<<nblk1, 1024, 0, st>>>(boff.p, nbk, boff2.p);
-            ctx->launches += 3;
-        }
-        k_scatter_events<<<ctx->num_sms * 8, 256, 0, st>>>(ev, dc, cap, Mb, nbk, boff.p, cursor.p, part.p);
         SB_CUDA(cudaFuncSetAttribute(k_group_dedup, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(GroupSmem)));
-        k_group_ranges<<<nblk(ng, 256), 256, 0, st>>>(boff.p, nbk, ng, g_bf.p, g_be.p);
         {
             KernelTimer kt(ctx, SYL_KERNEL_GROUP_DEDUP);
-            k_group_dedup<<<ng, GRP_THREADS, sizeof(GroupSmem), st>>>(part.p, boff.p, g_bf.p, g_be.p, grp_cap, (uint32_t)cap, Mb, nbk, no_dedup,
-                                                                       st_hash.p, st_cnt.p, g_nuniq.p, g_e0.p, g_n.p, g_fb.p, d_ndup);
+            k_group_dedup<<<ng, GRP_THREADS, sizeof(GroupSmem), st>>>(ev, g_cnt.p, slot, Mb, nbk, no_dedup,
+                                                                       st_hash.p, st_cnt.p, g_nuniq.p, g_n.p, g_fb.p, d_ndup);
         }
         k_scan_u32<<<1, 1024, 0, st>>>(g_nuniq.p, ng, uoff.p);
         k_fallback_sizes<<<nblk(ng, 256), 256, 0, st>>>(g_n.p, g_fb.p, ng, fsz.p);
         k_scan_u32<<<1, 1024, 0, st>>>(fsz.p, ng, foff.p);
-        k_compact_uniq<<<ng, 128, 0, st>>>(st_hash.p, st_cnt.p, g_e0.p, g_nuniq.p, uoff.p, g_fb.p, g_src.p, nullptr, nullptr,
+        k_compact_uniq<<<ng, 128, 0, st>>>(st_hash.p, st_cnt.p, slot, g_nuniq.p, uoff.p, g_fb.p, g_src.p, nullptr, nullptr,
                                             tmp_h.p, tmp_c.p);
-        ctx->launches += 7;
+        ctx->launches += 5;
         SB_CUDA(cudaGetLastError());
         SB_CUDA(cudaMemcpyAsync(ctx->h_counters, dc, 24, cudaMemcpyDeviceToHost, st));  // events, pending, duplicates
         SB_CUDA(cudaMemcpyAsync(ctx->h_counters + 4, uoff.p + ng, 4, cudaMemcpyDeviceToHost, st));
         SB_CUDA(cudaMemcpyAsync(ctx->h_counters + 5, foff.p + ng, 4, cudaMemcpyDeviceToHost, st));
         SB_CUDA(cudaStreamSynchronize(st));  // the one synchronisation of a sketch
-        const uint64_t N = ctx->h_counters[0];
-        if (N > cap) { *need_cap = N; syl_sample_free(s); return SYL_ERR_CAPACITY; }
-        const uint64_t U1 = (uint32_t)ctx->h_counters[4], NF = (uint32_t)ctx->h_counters[5];
+        const uint64_t N_ovf = ctx->h_counters[0];
+        if (N_ovf > cap) { *need_cap = N_ovf; syl_sample_free(s); return SYL_ERR_CAPACITY; }
+        // the overflow list holds only events of groups past their slot, all of which are fallback groups
+        const uint64_t U1 = (uint32_t)ctx->h_counters[4], NF_slots = (uint32_t)ctx->h_counters[5], NF = NF_slots + N_ovf;
         uint64_t ndup = ctx->h_counters[2];
         static const bool dbg = getenv("SYL_DEBUG_TIMING") != nullptr;
-        if (dbg) fprintf(stderr, "[sample post-pass] events %llu (cap %llu) buckets %u groups %u: in-kernel uniques %llu, events handed to the generic path %llu (%.1f %%)\n",
-                         (unsigned long long)N, (unsigned long long)cap, nbk, ng, (unsigned long long)U1, (unsigned long long)NF, N ? 100.0 * NF / N : 0.);
+        if (dbg) fprintf(stderr, "[sample post-pass] groups %u of %u slots, overflow list %llu (cap %llu): in-kernel uniques %llu, events handed to the generic path %llu (%.2f %% of the slotted events)\n",
+                         ng, slot, (unsigned long long)N_ovf, (unsigned long long)cap, (unsigned long long)U1, (unsigned long long)NF,
+                         n_slots ? 100.0 * (double)NF_slots / (double)n_slots : 0.);
         uint64_t U = U1;
         if (NF) {  // fallback groups through the generic path (heavy-hitter k-mers, duplicate-heavy replays)
             DevBuf<uint64_t> fh, f_rf, f_p0, f_p1, f_uq;
@@ -959,23 +863,29 @@ struct SampleBuilder {
             uint64_t U2 = 0, nd2 = 0;
             if ((rc = fh.alloc(NF, st)) || (rc = f_rf.alloc(NF, st)) || (rc = f_p0.alloc(NF, st)) || (rc = f_p1.alloc(NF, st)))
                 return fail(rc);
-            k_gather_fallback<<<ng, 256, 0, st>>>(part.p, g_e0.p, g_n.p, g_fb.p, foff.p, fh.p, f_rf.p, f_p0.p, f_p1.p);
+            k_gather_fallback<<<ng, 256, 0, st>>>(ev, slot, g_n.p, g_fb.p, foff.p, fh.p, f_rf.p, f_p0.p, f_p1.p);
             ctx->launches++;
+            if (N_ovf) {
+                k_unpack_events<<<nblk(N_ovf, 256), 256, 0, st>>>(ev + n_slots, N_ovf, fh.p + NF_slots, f_rf.p + NF_slots,
+                                                                  f_p0.p + NF_slots, f_p1.p + NF_slots);
+                ctx->launches++;
+            }
             if ((rc = dedup_sorted(fh.p, f_rf.p, f_p0.p, f_p1.p, NF, f_uq, f_ct, &U2, &nd2)) != SYL_OK) return fail(rc);
             ndup += nd2;
             U = U1 + U2;
-            if (U2) {  // slot the generic path's pairs into their groups' positions and redo the output offsets
-                k_fallback_place<<<nblk(ng, 128), 128, 0, st>>>(g_fb.p, g_bf.p, g_be.p, ng, nbk, Mb, f_uq.p, U2, g_nuniq.p, g_src.p);
-                k_scan_u32<<<1, 1024, 0, st>>>(g_nuniq.p, ng, uoff.p);
-                k_compact_uniq<<<ng, 128, 0, st>>>(st_hash.p, st_cnt.p, g_e0.p, g_nuniq.p, uoff.p, g_fb.p, g_src.p, f_uq.p, f_ct.p,
-                                                    tmp_h.p, tmp_c.p);
-                ctx->launches += 3;
-                SB_CUDA(cudaGetLastError());
-            }
             if ((rc = hblock_alloc(ctx, (void **)&s->hash, std::max<uint64_t>(U, 1) * 8))) return fail(rc);
             if ((rc = hblock_alloc(ctx, (void **)&s->count, std::max<uint64_t>(U, 1) * 4))) return fail(rc);
-            SB_CUDA(cudaMemcpyAsync(s->hash, tmp_h.p, U * 8, cudaMemcpyDeviceToDevice, st));
-            SB_CUDA(cudaMemcpyAsync(s->count, tmp_c.p, U * 4, cudaMemcpyDeviceToDevice, st));
+            if (U2) {  // slot the generic path's pairs into their groups' positions, compact straight into the result
+                k_fallback_place<<<nblk(ng, 128), 128, 0, st>>>(g_fb.p, ng, nbk, Mb, f_uq.p, U2, g_nuniq.p, g_src.p);
+                k_scan_u32<<<1, 1024, 0, st>>>(g_nuniq.p, ng, uoff.p);
+                k_compact_uniq<<<ng, 128, 0, st>>>(st_hash.p, st_cnt.p, slot, g_nuniq.p, uoff.p, g_fb.p, g_src.p, f_uq.p, f_ct.p,
+                                                    s->hash, s->count);
+                ctx->launches += 3;
+                SB_CUDA(cudaGetLastError());
+            } else if (U) {
+                SB_CUDA(cudaMemcpyAsync(s->hash, tmp_h.p, U * 8, cudaMemcpyDeviceToDevice, st));
+                SB_CUDA(cudaMemcpyAsync(s->count, tmp_c.p, U * 4, cudaMemcpyDeviceToDevice, st));
+            }
             SB_CUDA(cudaStreamSynchronize(st));  // f_uq / f_ct go out of scope
         } else {
             // exact-size result arrays; the copies are ordered on the ctx stream like every later use of the handle

@@ -88,9 +88,9 @@ static uint32_t pick_warp_tile(uint64_t mean_len, int k, int sem, int with_pos, 
 // Two formulations of the kernel (same arithmetic, same results):
 //   cta  (default for ASCII input): one 32K tile per CTA, phases separated by CTA-wide barriers (seed_kernel.cuh)
 //   warp (SYL_SEED_IMPL=warp; always for 2-bit packed input): warp-autonomous persistent kernel (seed_warp.cuh)
-// Measured on 1 Gbp of 150 bp reads: cta 1.44 ms, warp 1.50 ms — the hot loop alone (scripts/hotloop_bench.cu)
-// sustains 0.74 T windows/s = 1.08 ms for the same windows with its two pipes (ALU 18.5, FMA-heavy 13
-// instructions per window) each ~73 % busy, so what the phases around it can still give back is small.
+// Measured on 1 Gbp of 150 bp reads (one H100 SXM, 400 W): cta 1.6-1.9 ms, warp 2.58 ms; the hot loop alone
+// (scripts/hotloop_bench.cu) sustains 0.66 T windows/s = 1.22 ms for the same windows, so the phases around
+// the loop cost about 0.4-0.5 ms of the CTA kernel.
 static bool use_warp_kernel() {
     const char *e = getenv("SYL_SEED_IMPL");  // read per call: the tests switch it at run time
     return e && strcmp(e, "warp") == 0;
@@ -139,7 +139,7 @@ int seed_enqueue(syl_ctx *ctx, const SeedJob &job) {
     }
     const uint64_t thr = fmh_threshold(job.c);
     const ShiftMul smul = {1u << 8, 1u << 18, 1u << 4, 1u, 0u};
-    const BucketHist bh{job.emit_events ? job.d_bucket_cnt : nullptr, job.Mb, job.nbk};
+    const GroupOut go{job.emit_events ? job.d_group_cnt : nullptr, job.Mb, job.nbk, job.ng, job.slot};
     if (!warp) {
         if (job.d_pend_count != job.d_count + 1) { set_error("internal: cta kernel expects adjacent counters"); return SYL_ERR_ARG; }
         const size_t smem = sizeof(SeedSmem);
@@ -150,7 +150,7 @@ int seed_enqueue(syl_ctx *ctx, const SeedJob &job) {
         const SlotOut slot{job.emit_events ? 0u : job.slot_cap, job.d_tile_cnt, job.d_slot_overflow};
         kern<<<(unsigned)n_tiles, SEED_THREADS, smem, st>>>(
             job.d_bases, job.n_bases, job.d_rec_off, job.off_bias, tile_rec.p, thr, job.sem, job.with_pos, job.d_out,
-            slot.cap ? 0 : job.cap, job.d_count, smul, job.rec_base, job.no_dedup, job.d_pend, bh, slot);
+            slot.cap ? 0 : job.cap, job.d_count, smul, job.rec_base, job.no_dedup, job.d_pend, go, slot);
         kt.stop();
     } else {
         const bool pk = job.d_packed != nullptr;
@@ -174,7 +174,7 @@ int seed_enqueue(syl_ctx *ctx, const SeedJob &job) {
         A.bases = job.d_bases; A.packed = job.d_packed; A.n_bases = job.n_bases; A.rec_off = job.d_rec_off;
         A.off_bias = job.off_bias; A.tile_rec = tile_rec.p; A.n_tiles = n_tiles; A.tw = (uint32_t)tile; A.thr = thr; A.sem = job.sem;
         A.with_pos = job.with_pos; A.out = job.d_out; A.cap = job.cap; A.g_count = job.d_count; A.g_pend = job.d_pend_count;
-        A.g_tile = d_tile; A.smul = smul; A.rec_base = job.rec_base; A.no_dedup = job.no_dedup; A.pend = job.d_pend; A.bh = bh;
+        A.g_tile = d_tile; A.smul = smul; A.rec_base = job.rec_base; A.no_dedup = job.no_dedup; A.pend = job.d_pend; A.go = go;
         KernelTimer kt(ctx, SYL_KERNEL_SEED);
         kern<<<(unsigned)grid, SW_THREADS, smem, st>>>(A);
         kt.stop();

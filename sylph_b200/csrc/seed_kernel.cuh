@@ -60,22 +60,32 @@ __device__ __forceinline__ uint16_t *seed_stage_pos(SeedMeta &M) {
     return reinterpret_cast<uint16_t *>(reinterpret_cast<syl_survivor *>(M.stage) + SEED_STAGE);
 }
 
-// Multipliers 2^(32-s) for the three xor-shift distances, passed as kernel parameters so that
-// ptxas cannot strength-reduce "mul.hi by a power of two" back into an ALU-pipe shift.
-// Histogram of the emitted events over the post-pass's hash buckets (sample.cu), filled while the
-// events are flushed so that the post-pass does not have to re-read them for it.
-struct BucketHist {
-    uint32_t *cnt;  // nullptr: off
-    uint64_t Mb;    // bucket = min(mulhi(hash, Mb), nbk - 1)
-    uint32_t nbk;
-    __device__ __forceinline__ void add(uint64_t h) const {
+// Where an emitted event goes (read-sketch post-pass, sample.cu).  Group g of the post-pass owns the
+// GRP_BPG consecutive hash buckets [g * GRP_BPG, (g + 1) * GRP_BPG), bucket = min(mulhi(hash, Mb), nbk - 1),
+// and the fixed slot out[g * slot, (g + 1) * slot): the flush writes every event straight into its group.
+// An event past its slot's capacity is appended to the overflow list out[ng * slot ..) at the running
+// counter *g_count; its group then takes the post-pass's generic path.  cnt == nullptr: no groups, every
+// event is appended at *g_count (read pairs, SYL_SAMPLE_POSTPASS=sort).  Appends past cap are counted
+// but dropped; the caller compares the final count with cap and redoes the sample.
+struct GroupOut {
+    uint32_t *cnt;  // events per group (can exceed slot)
+    uint64_t Mb;
+    uint32_t nbk, ng, slot;
+    // position of the event in out, or ~0ull when it is dropped
+    __device__ __forceinline__ uint64_t place(uint64_t h, unsigned long long *g_count, uint64_t cap) const {
         if (cnt) {
-            const uint32_t b = (uint32_t)__umul64hi(h, Mb);
-            atomicAdd(&cnt[b < nbk ? b : nbk - 1], 1u);
+            uint32_t g = (uint32_t)__umul64hi(h, Mb);
+            g = (g < nbk ? g : nbk - 1) / GRP_BPG;
+            const uint32_t i = atomicAdd(&cnt[g], 1u);
+            if (i < slot) return (uint64_t)g * slot + i;
         }
+        const unsigned long long gi = atomicAdd(g_count, 1ull);
+        return gi < cap ? (uint64_t)ng * slot + gi : ~0ull;  // ng * slot == 0 without groups
     }
 };
 
+// Multipliers 2^(32-s) for the three xor-shift distances, passed as kernel parameters so that
+// ptxas cannot strength-reduce "mul.hi by a power of two" back into an ALU-pipe shift.
 struct ShiftMul { uint32_t m24, m14, m28, one, zero; };
 
 // Slotted survivor output (genome sketching): tile t writes its survivors to out[t * cap ..) and their
@@ -143,7 +153,7 @@ template <int K, int EMIT>
 __device__ __forceinline__ void seed_resolve(const SeedSmem &S, SeedMeta &M, uint32_t pw, int j, uint64_t rc, uint64_t thr,
                                              void *__restrict__ out, uint64_t cap,
                                              unsigned long long *__restrict__ g_count, uint64_t rec_base, int no_dedup,
-                                             uint32_t *__restrict__ pend, const BucketHist bh) {
+                                             uint32_t *__restrict__ pend, const GroupOut go) {
     constexpr uint32_t PAD = 64 - 2 * K;
     constexpr uint32_t HI_MASK = (1u << (32 - PAD)) - 1u;
     const uint32_t bitpos = 32u + 2u * pw - PAD;
@@ -193,11 +203,10 @@ __device__ __forceinline__ void seed_resolve(const SeedSmem &S, SeedMeta &M, uin
         if (idx < (unsigned)SEED_STAGE) {
             M.stage[idx] = ev;
         } else {
-            const unsigned long long gi = atomicAdd(g_count, 1ull);
-            if (gi < cap) {
-                reinterpret_cast<EventRec *>(out)[gi] = ev;
-                if (ev.recflag & EV_PENDING) pend[atomicAdd(g_count + 1, 1ull)] = (uint32_t)gi;
-                bh.add(ev.hash);
+            const uint64_t pos = go.place(ev.hash, g_count, cap);
+            if (pos != ~0ull) {
+                reinterpret_cast<EventRec *>(out)[pos] = ev;
+                if (ev.recflag & EV_PENDING) pend[atomicAdd(g_count + 1, 1ull)] = (uint32_t)pos;
             }
         }
     }
@@ -208,7 +217,7 @@ __global__ void __launch_bounds__(SEED_THREADS, SEED_MINB_CFG)
 k_seed(const uint8_t *__restrict__ bases, uint64_t n_bases, const uint64_t *__restrict__ rec_off, uint64_t off_bias,
        const uint32_t *__restrict__ tile_rec, uint64_t thr, int sem, int with_pos,
        void *__restrict__ out, uint64_t cap, unsigned long long *__restrict__ g_count,
-       const ShiftMul smul, uint64_t rec_base, int no_dedup, uint32_t *__restrict__ pend, const BucketHist bh, const SlotOut slot) {
+       const ShiftMul smul, uint64_t rec_base, int no_dedup, uint32_t *__restrict__ pend, const GroupOut go, const SlotOut slot) {
     static_assert(W >= SEED_W_MIN && W <= SEED_W_MAX, "run length");
     extern __shared__ __align__(128) uint8_t smem_raw[];
     SeedSmem &S = *reinterpret_cast<SeedSmem *>(smem_raw);
@@ -438,7 +447,7 @@ k_seed(const uint8_t *__restrict__ bases, uint64_t n_bases, const uint64_t *__re
                 if (ci < (unsigned)SEED_CAND) {
                     M.cand[ci] = ((uint32_t)(p + i) << 8) | (uint32_t)j;
                 } else {  // list full (tiny c): resolve inline
-                    seed_resolve<K, EMIT>(S, M, (uint32_t)(p + i), j, rc, thr, out, cap, g_count, rec_base, no_dedup, pend, bh);
+                    seed_resolve<K, EMIT>(S, M, (uint32_t)(p + i), j, rc, thr, out, cap, g_count, rec_base, no_dedup, pend, go);
                 }
             }
         }
@@ -447,7 +456,7 @@ k_seed(const uint8_t *__restrict__ bases, uint64_t n_bases, const uint64_t *__re
             const unsigned int nc = min(M.cand_count, (unsigned)SEED_CAND);
             for (unsigned int ci = tid; ci < nc; ci += SEED_THREADS) {
                 const uint32_t e = M.cand[ci];
-                seed_resolve<K, EMIT>(S, M, e >> 8, (int)(e & 255u), rc, thr, out, cap, g_count, rec_base, no_dedup, pend, bh);
+                seed_resolve<K, EMIT>(S, M, e >> 8, (int)(e & 255u), rc, thr, out, cap, g_count, rec_base, no_dedup, pend, go);
             }
         }
         __syncthreads();  // table is rewritten by the next chunk
@@ -496,6 +505,17 @@ k_seed(const uint8_t *__restrict__ bases, uint64_t n_bases, const uint64_t *__re
         return;
     }
     const unsigned int staged = min(M.stage_count, (unsigned)SEED_STAGE);
+    if (EMIT == 1 && go.cnt) {  // events straight into their post-pass groups
+        for (unsigned int i = tid; i < staged; i += SEED_THREADS) {
+            const EventRec ev = M.stage[i];
+            const uint64_t pos = go.place(ev.hash, g_count, cap);
+            if (pos == ~0ull) continue;
+            reinterpret_cast<EventRec *>(out)[pos] = ev;
+            // reads cut by the tile edge: pair keys are filled in by k_events_fix
+            if (ev.recflag & EV_PENDING) pend[atomicAdd(g_count + 1, 1ull)] = (uint32_t)pos;
+        }
+        return;
+    }
     if (tid == 0 && staged) M.flush_base = atomicAdd(g_count, (unsigned long long)staged);
     __syncthreads();
     if (staged) {
@@ -508,7 +528,6 @@ k_seed(const uint8_t *__restrict__ bases, uint64_t n_bases, const uint64_t *__re
                 reinterpret_cast<EventRec *>(out)[base + i] = ev;
                 // reads cut by the tile edge: pair keys are filled in by k_events_fix
                 if (ev.recflag & EV_PENDING) pend[atomicAdd(g_count + 1, 1ull)] = (uint32_t)(base + i);
-                bh.add(ev.hash);
             }
         }
     }
@@ -516,7 +535,7 @@ k_seed(const uint8_t *__restrict__ bases, uint64_t n_bases, const uint64_t *__re
 
 
 using seed_kern_t = void (*)(const uint8_t *, uint64_t, const uint64_t *, uint64_t, const uint32_t *, uint64_t, int, int,
-                             void *, uint64_t, unsigned long long *, const ShiftMul, uint64_t, int, uint32_t *, const BucketHist, const SlotOut);
+                             void *, uint64_t, unsigned long long *, const ShiftMul, uint64_t, int, uint32_t *, const GroupOut, const SlotOut);
 
 // One translation unit per (K, EMIT) instantiates the three run lengths and exports a getter, so
 // the twelve kernels compile in parallel.

@@ -77,7 +77,7 @@ struct SeedWArgs {
     uint64_t rec_base;
     int no_dedup;
     uint32_t *pend;
-    BucketHist bh;
+    GroupOut go;               // events: post-pass groups (see seed_kernel.cuh)
 };
 
 // one run of W windows starting at tile-relative window start p: candidate bit mask (bit i: high word of
@@ -184,11 +184,10 @@ __device__ __forceinline__ void seedw_resolve(SeedWSlab<PACKED> &S, const SeedWA
         if (idx < (unsigned)SW_STAGE) {
             S.stage[idx] = ev;
         } else {
-            const unsigned long long gi = atomicAdd(A.g_count, 1ull);
-            if (gi < A.cap) {
-                reinterpret_cast<EventRec *>(A.out)[gi] = ev;
-                if (ev.recflag & EV_PENDING) A.pend[atomicAdd(A.g_pend, 1ull)] = (uint32_t)gi;
-                A.bh.add(ev.hash);
+            const uint64_t pos = A.go.place(ev.hash, A.g_count, A.cap);
+            if (pos != ~0ull) {
+                reinterpret_cast<EventRec *>(A.out)[pos] = ev;
+                if (ev.recflag & EV_PENDING) A.pend[atomicAdd(A.g_pend, 1ull)] = (uint32_t)pos;
             }
         }
     }
@@ -398,7 +397,15 @@ k_seed_w(const SeedWArgs A) {
 
         // ---- flush the staged survivors: one global atomic per warp-tile
         const unsigned int staged = min(S.stage_count, (unsigned)SW_STAGE);
-        if (staged) {
+        if (EMIT == 1 && A.go.cnt) {  // events straight into their post-pass groups
+            for (unsigned int i = lane; i < staged; i += 32) {
+                const EventRec ev = S.stage[i];
+                const uint64_t pos = A.go.place(ev.hash, A.g_count, A.cap);
+                if (pos == ~0ull) continue;
+                reinterpret_cast<EventRec *>(A.out)[pos] = ev;
+                if (ev.recflag & EV_PENDING) A.pend[atomicAdd(A.g_pend, 1ull)] = (uint32_t)pos;
+            }
+        } else if (staged) {
             unsigned long long base = 0;
             if (lane == 0) base = atomicAdd(A.g_count, (unsigned long long)staged);
             base = __shfl_sync(0xffffffffu, base, 0);
@@ -409,7 +416,6 @@ k_seed_w(const SeedWArgs A) {
                     const EventRec ev = S.stage[i];
                     reinterpret_cast<EventRec *>(A.out)[base + i] = ev;
                     if (ev.recflag & EV_PENDING) A.pend[atomicAdd(A.g_pend, 1ull)] = (uint32_t)(base + i);
-                    A.bh.add(ev.hash);
                 }
             }
         }
