@@ -21,8 +21,10 @@
  *     fail with SYL_ERR_CUDA.
  *   - hard limits (reported as SYL_ERR_ARG, never silently wrapped): fewer than 2^32-2 records per batch,
  *     fewer than 2^32-2 survivor events per sample, fewer than 2^32-2 index entries (genome_kmers + tracked)
- *     and 2^31 genomes per db shard, fewer than 2^31 (sample, genome) pairs and at most 8 GB of per-pair
- *     histograms (2^23 pairs) per syl_query / syl_profile call — split the sample batch above that.
+ *     and 2^31 genomes per db shard, fewer than 2^31 (sample, genome) pairs per syl_query / syl_profile call.
+ *     Above 2^23 pairs per call the 256-bin per-pair histograms would exceed 8 GB: syl_query / syl_profile
+ *     then run in the CSR formulation (slower, one more host synchronisation), the sharded profile (5)
+ *     reports SYL_ERR_UNSUPPORTED.
  *   - handles (syl_sample / syl_genomes / syl_db / syl_profile_job) borrow device blocks from the ctx that
  *     created them: free them before their ctx, and use them with that ctx.
  */
@@ -82,10 +84,10 @@ int syl_ctx_seed_kernel_time(syl_ctx *ctx, double *total_ms, uint64_t *launches,
 enum {
     SYL_KERNEL_SEED = 0,        /* k_seed (all variants) */
     SYL_KERNEL_GROUP_DEDUP = 1, /* read-sketch post-pass: k_group_dedup */
-    SYL_KERNEL_JOIN = 2,        /* containment pass 1 probe: k_join_hist<pass 1> */
-    SYL_KERNEL_JOIN2 = 3,       /* containment pass 2: k_join2_hits / k_join_hist<pass 2> */
+    SYL_KERNEL_JOIN = 2,        /* containment pass 1: k_join_hist (+ k_range_bounds, CSR formulation: k_join_csr) */
+    SYL_KERNEL_JOIN2 = 3,       /* containment pass 2: k_join2_order (+ k_local_best when sharded) */
     SYL_KERNEL_STATS = 4,       /* k_stats_hist / k_stats */
-    SYL_KERNEL_BOOT = 5,        /* bootstrap: k_boot_iter (+ k_boot_seq, k_boot_final) */
+    SYL_KERNEL_BOOT = 5,        /* bootstrap: k_boot_iter_p (+ k_boot_seq, k_boot_final) */
     SYL_KERNEL_GENOME_POST = 6, /* genome-sketch post-pass (everything after k_seed) */
     SYL_KERNEL_PACK = 7,        /* ASCII -> 2-bit packing on the device (unused by the host-packed path) */
     SYL_KERNEL_COUNT = 8

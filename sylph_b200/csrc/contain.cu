@@ -19,10 +19,12 @@
 // genomes the database holds, and the database is never streamed.  The per-genome statistics
 // are functions of the multiset of hit counts: the join accumulates a 256-bin histogram of the
 // counts per (sample, genome) pair and one warp per pair derives everything from it (a count
-// >= 256 anywhere sends the pass through the CSR formulation instead: count, scan, scatter,
-// exact radix select for the median — no range limit).  In pass 2 the winner of a k-mer is the
-// best pass-1 ANI inside that k-mer's equal range — a purely local decision, so no global
-// k-mer -> winner map is ever materialised.
+// >= 256 anywhere, or histograms beyond 8 GB, send the call through the CSR formulation instead:
+// count, scan, scatter, exact radix select for the median — no range limit).  In pass 2 the
+// winner of a k-mer is the pass-1 survivor that comes first in its sample's order (ANI
+// descending, genome ascending) inside that k-mer's equal range — a purely local decision, so no
+// global k-mer -> winner map is ever materialised.  Both formulations run through one staged
+// driver (contain_fast below).
 #include <cub/cub.cuh>
 
 #include <algorithm>
@@ -115,73 +117,11 @@ __global__ void k_bucket_starts(const uint64_t *__restrict__ keys, uint64_t N, u
 }
 
 // ---- the join -------------------------------------------------------------------------------
-// PASS2 == false: count / fill hits of genome_kmers entries (pass 1).
-// PASS2 == true : only entries of pass-1 survivors take part; the winner of a k-mer is the
-//                 survivor with the best pass-1 ANI in the equal range (lowest genome on ties);
-//                 a genome_kmers hit whose genome is not the winner is "lost" (:641-646).
-// FILL == false : per-genome hit counters only;  FILL == true: scatter the counts into CSR.
 struct SampleView {
     const uint64_t *hash;
     const uint32_t *count;
     uint64_t n;
 };
-
-template <bool PASS2, bool FILL>
-__global__ void k_join(const SampleView *__restrict__ views, uint64_t G,
-                       const uint64_t *__restrict__ keys, const uint32_t *__restrict__ gid,
-                       const uint32_t *__restrict__ bstart, uint64_t M, uint64_t NB, uint64_t maxkey,
-                       const uint8_t *__restrict__ survivor, const double *__restrict__ ani1,
-                       uint32_t *__restrict__ cnt, const uint64_t *__restrict__ off, uint32_t *__restrict__ cursor,
-                       uint32_t *__restrict__ covs, uint32_t *__restrict__ lost) {
-    const SampleView sv = views[blockIdx.y];
-    uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= sv.n) return;
-    // per-(sample, genome) arrays: this sample's row
-    const uint64_t row = (uint64_t)blockIdx.y * G;
-    if (PASS2) { survivor += row; ani1 += row; }
-    if (cnt) cnt += row;
-    if (off) off += row;
-    if (cursor) cursor += row;
-    if (lost) lost += row;
-    const uint64_t key = sv.hash[i];
-    const uint32_t c = sv.count[i];
-    if (key > maxkey || c == 0) return;  // count 0: src/contain.rs:634-636
-    const uint64_t b = bucket_of(key, M, NB);
-    uint32_t lo = bstart[b];
-    const uint32_t hi = bstart[b + 1];
-    while (lo < hi && keys[lo] < key) lo++;
-    if (lo >= hi || keys[lo] != key) return;
-    // the equal range may run past the bucket end only if keys are equal, which maps to the same bucket
-    uint32_t e = lo;
-    uint32_t winner = 0xFFFFFFFFu;
-    if (PASS2) {
-        double best = -1.0;
-        for (uint32_t j = lo; j < hi && keys[j] == key; j++) {
-            const uint32_t g = gid[j] >> 1;
-            if (!survivor[g]) continue;
-            const double a = ani1[g];
-            if (a > best || (a == best && g < winner)) { best = a; winner = g; }
-        }
-    }
-    for (; e < hi && keys[e] == key; e++) {
-        const uint32_t gv = gid[e];
-        if (gv & 1u) continue;  // tracked k-mers only take part in the winner decision
-        const uint32_t g = gv >> 1;
-        if (PASS2) {
-            if (!survivor[g]) continue;
-            if (g != winner) {
-                if (!FILL) atomicAdd(&lost[g], 1u);
-                continue;
-            }
-        }
-        if (!FILL) {
-            atomicAdd(&cnt[g], 1u);
-        } else {
-            const uint32_t p = atomicAdd(&cursor[g], 1u);
-            covs[off[g] + p] = c;
-        }
-    }
-}
 
 // ---- per-genome statistics: one warp per genome ---------------------------------------------
 
@@ -279,12 +219,13 @@ __device__ __forceinline__ void stats_emit(uint32_t sample_idx, uint64_t g, uint
 
 constexpr int STAT_WARPS = 4;
 
+// CSR formulation: one warp per (sample, genome) over the pair's hit values covs[off[pair], off[pair] + cnt[pair])
 __global__ void __launch_bounds__(STAT_WARPS * 32)
 k_stats(const uint32_t *__restrict__ cnt, const uint64_t *__restrict__ off, const uint32_t *__restrict__ covs,
         const uint32_t *__restrict__ glen, const uint32_t *__restrict__ lost, uint64_t n_genomes, uint64_t n_pairs,
         uint32_t genome_base, StatParams P, int pass2, syl_ani_row *__restrict__ rows, uint64_t rows_cap,
         uint32_t *__restrict__ boot_rows, uint32_t *__restrict__ hist_out, uint64_t boot_cap,
-        unsigned long long *__restrict__ n_rows, unsigned long long *__restrict__ n_boot) {
+        unsigned long long *__restrict__ n_rows, unsigned long long *__restrict__ n_boot, const StatExtra X) {
     __shared__ uint32_t s_hist[STAT_WARPS][256];
     const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
     const uint64_t pair = (uint64_t)blockIdx.x * STAT_WARPS + w;
@@ -364,7 +305,7 @@ k_stats(const uint32_t *__restrict__ cnt, const uint64_t *__restrict__ off, cons
     if (lane != 0) return;
 
     stats_emit(sample_idx, g, n, gl, median, sum, nz, hist, lost, genome_base, P, pass2, rows, rows_cap, boot_rows, hist_out,
-               boot_cap, n_rows, n_boot);
+               boot_cap, n_rows, n_boot, X);
 }
 
 
@@ -375,7 +316,7 @@ k_stats(const uint32_t *__restrict__ cnt, const uint64_t *__restrict__ off, cons
 // ONE probe pass per get_stats pass (the CSR formulation probes twice: count, then fill) and a
 // k_stats that reads 1 KB per pair instead of selecting a median from a value list.  Values
 // >= COV_BINS (a genome covered 256x or deeper) are only counted in `ovf`; if there are any, the
-// caller falls back to the CSR formulation for this pass.
+// call is redone in the CSR formulation.
 constexpr uint32_t COV_BINS = 256;
 
 // ---- thread -> (sample, key) mapping of the join kernels ---------------------------------------------------------
@@ -416,31 +357,10 @@ __global__ void k_range_bounds(const SampleView *__restrict__ views, uint32_t S,
     rb[t] = (uint32_t)lo;
 }
 
-// The genome ids of one k-mer's equal range [lo, e) -> hit counters / count histograms of one sample.
-// PASS2: the k-mer belongs to the pass-1 survivor with the best pass-1 ANI (lowest genome on ties,
-// tracked k-mers take part in the decision); other survivors lose it (src/contain.rs:410-430, :641-646).
-template <bool PASS2>
+// Pass 1, histogram formulation: the genome ids of one k-mer's equal range [lo, e) -> count histograms of one sample.
 __device__ __forceinline__ void join_range(const uint32_t *__restrict__ gid, uint32_t lo, uint32_t e, uint32_t c,
-                                           const uint8_t *__restrict__ survivor, const double *__restrict__ ani1,
-                                           uint8_t *__restrict__ touched, uint32_t *__restrict__ lost,
-                                           uint32_t *__restrict__ chist, unsigned long long *__restrict__ ovf) {
-    uint32_t winner = 0xFFFFFFFFu;
-    if (PASS2) {
-        double best = -1.0;
-        for (uint32_t j = lo; j < e; j += 4) {
-            uint32_t gq[4];
-#pragma unroll
-            for (int q = 0; q < 4; q++) gq[q] = j + q < e ? gid[j + q] : 0xFFFFFFFFu;
-#pragma unroll
-            for (int q = 0; q < 4; q++) {
-                if (j + q >= e) continue;
-                const uint32_t g = gq[q] >> 1;
-                if (!survivor[g]) continue;
-                const double a = ani1[g];
-                if (a > best || (a == best && g < winner)) { best = a; winner = g; }
-            }
-        }
-    }
+                                           uint8_t *__restrict__ touched, uint32_t *__restrict__ chist,
+                                           unsigned long long *__restrict__ ovf) {
     for (uint32_t j = lo; j < e; j += 4) {
         uint32_t gq[4];
 #pragma unroll
@@ -451,10 +371,6 @@ __device__ __forceinline__ void join_range(const uint32_t *__restrict__ gid, uin
             const uint32_t gv = gq[q];
             if (gv & 1u) continue;  // tracked k-mers only take part in the winner decision
             const uint32_t g = gv >> 1;
-            if (PASS2) {
-                if (!survivor[g]) continue;
-                if (g != winner) { atomicAdd(&lost[g], 1u); continue; }
-            }
             // no per-genome hit counter: the sample's k-mers concentrate on the few genomes that are
             // present, and a million atomics on a handful of adjacent counters serialise in one L2
             // slice (measured: 2/3 of this kernel's time).  The hit count is the histogram's total.
@@ -465,21 +381,16 @@ __device__ __forceinline__ void join_range(const uint32_t *__restrict__ gid, uin
     }
 }
 
-template <bool PASS2>
+// Pass-1 probe: every sample key looks up its equal range in the db index and records it in `hits` (for pass 2 and,
+// in the CSR formulation, for pass 1's count / fill walks).  PROBE_ONLY == false also accumulates the count histograms.
+template <bool PROBE_ONLY>
 __global__ void k_join_hist(const SampleView *__restrict__ views, uint64_t G,
                             const uint64_t *__restrict__ keys, const uint32_t *__restrict__ gid, uint64_t N,
                             const uint32_t *__restrict__ bstart, uint64_t M, uint64_t NB, uint64_t maxkey,
-                            const uint8_t *__restrict__ survivor, const double *__restrict__ ani1,
-                            uint8_t *__restrict__ touched, uint32_t *__restrict__ lost, uint32_t *__restrict__ chist,
+                            uint8_t *__restrict__ touched, uint32_t *__restrict__ chist,
                             unsigned long long *__restrict__ ovf, uint2 *__restrict__ hits, uint64_t hits_stride, const KeyMap km) {
   for_each_key(km, views, [&](const uint32_t smp, const uint64_t i) {
     const SampleView sv = views[smp];
-    const uint64_t row = (uint64_t)smp * G;
-    const uint8_t *survivor_r = PASS2 ? survivor + row : survivor;
-    const double *ani1_r = PASS2 ? ani1 + row : ani1;
-    uint32_t *lost_r = PASS2 ? lost + row : lost;
-    uint8_t *touched_r = touched + row;
-    uint32_t *chist_r = chist + row * COV_BINS;
     const uint64_t key = sv.hash[i];
     const uint32_t c = sv.count[i];
     if (key > maxkey || c == 0) return;  // count 0: src/contain.rs:634-636
@@ -514,25 +425,12 @@ __global__ void k_join_hist(const SampleView *__restrict__ views, uint64_t G,
         e += adv;
         if (adv < 4) break;
     }
-    if (hits) hits[(uint64_t)smp * hits_stride + i] = make_uint2(lo, e - lo);  // equal range in the db, for pass 2
-    join_range<PASS2>(gid, lo, e, c, survivor_r, ani1_r, touched_r, lost_r, chist_r, ovf);
+    if (hits) hits[(uint64_t)smp * hits_stride + i] = make_uint2(lo, e - lo);  // equal range in the db
+    if (!PROBE_ONLY) {
+        const uint64_t row = (uint64_t)smp * G;
+        join_range(gid, lo, e, c, touched + row, chist + row * COV_BINS, ovf);
+    }
   });
-}
-
-// Pass 2 over the equal ranges recorded by pass 1: no directory / key look-ups, only the genome ids.
-__global__ void k_join2_hits(const SampleView *__restrict__ views, uint64_t G, const uint32_t *__restrict__ gid,
-                             const uint2 *__restrict__ hits, uint64_t hits_stride,
-                             const uint8_t *__restrict__ survivor, const double *__restrict__ ani1,
-                             uint8_t *__restrict__ touched, uint32_t *__restrict__ lost, uint32_t *__restrict__ chist,
-                             unsigned long long *__restrict__ ovf) {
-    const SampleView sv = views[blockIdx.y];
-    const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= sv.n) return;
-    const uint2 h = hits[(uint64_t)blockIdx.y * hits_stride + i];
-    if (h.y == 0) return;
-    const uint64_t row = (uint64_t)blockIdx.y * G;
-    join_range<true>(gid, h.x, h.x + h.y, sv.count[i], survivor + row, ani1 + row, touched + row, lost + row,
-                     chist + row * COV_BINS, ovf);
 }
 
 // one warp per (sample, genome); lane l owns the bins [8l, 8l+8)
@@ -741,18 +639,7 @@ __device__ __forceinline__ void boot_one(uint32_t row, uint32_t it, const uint32
     }
 }
 
-// grid (BOOT_ITERS, n_boot): host-side row count
-__global__ void __launch_bounds__(BOOT_THREADS)
-k_boot_iter(const uint32_t *__restrict__ hist_in, StatParams P,
-            double *__restrict__ res_ani, double *__restrict__ res_lambda, uint8_t *__restrict__ res_ok,
-            uint32_t *__restrict__ reject_flag) {
-    __shared__ uint32_t Hb[17];
-    __shared__ uint64_t cum[17];
-    __shared__ uint64_t thr[16], nthr[16];
-    boot_one(blockIdx.y, blockIdx.x, hist_in, P, res_ani, res_lambda, res_ok, reject_flag, Hb, cum, thr, nthr);
-}
-
-// persistent form: the number of bootstrapped rows is read from device memory (no host round trip
+// Persistent kernel: the number of bootstrapped rows is read from device memory (no host round trip
 // between the statistics kernel and the bootstrap).  One CTA per resident slot; the (row, iteration)
 // items are handed out through a device counter, because their cost follows |genome_kmers| of the
 // row and a fixed stride leaves the CTAs that drew the large rows running alone at the end.
@@ -864,32 +751,6 @@ k_boot_final(const uint32_t *__restrict__ boot_rows, uint32_t n_boot, const doub
     if (t == 0) r.ci_valid = 1;
 }
 
-// mark the pass-1 survivors (rows of the compact list) in the dense (sample, genome) tables
-__global__ void k_mark_survivors(const syl_ani_row *__restrict__ rows, uint64_t n, uint64_t G, uint32_t genome_base,
-                                 uint8_t *__restrict__ survivor, double *__restrict__ ani1) {
-    uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= n) return;
-    const uint64_t p = (uint64_t)rows[i].sample * G + (rows[i].genome - genome_base);
-    survivor[p] = 1;
-    ani1[p] = rows[i].final_est_ani;
-}
-
-// Scratch for one syl_query / syl_profile call: dense per-(sample, genome) tables + compact outputs
-struct ContainScratch {
-    DevBuf<SampleView> views;
-    DevBuf<uint32_t> cnt, cursor, lost, boot_rows, hist, covs, reject, chist;
-    bool use_hist = false;  // per-pair coverage histograms fit (COV_BINS x 4 B per pair)
-    DevBuf<uint2> hits;     // [sample][max_n] equal range of every sample key in the db (recorded by pass 1 for pass 2)
-    bool hits_valid = false;
-    DevBuf<uint64_t> off;
-    DevBuf<uint8_t> survivor, tmp, res_ok, touched;
-    DevBuf<double> ani1, res_ani, res_lambda;
-    DevBuf<syl_ani_row> rows;
-    size_t tmp_bytes = 0;
-    uint64_t S = 0, G = 0, P = 0, max_n = 0;
-    uint64_t rows_cap = 0, boot_cap = 0;
-};
-
 static StatParams make_params(const syl_contain_params *p) {
     StatParams P;
     P.k = p->k;
@@ -902,185 +763,10 @@ static StatParams make_params(const syl_contain_params *p) {
     return P;
 }
 
-static int scratch_init(syl_ctx *ctx, const syl_db *db, const syl_sample *const *samples, uint32_t n_samples,
-                        bool need_pass2, ContainScratch &S) {
-    cudaStream_t st = ctx->stream;
-    S.S = n_samples;
-    S.G = db->n_genomes;
-    S.P = S.S * S.G;
-    if (S.P >= 0x7FFFFFFFull) { set_error("samples x genomes exceeds 2^31 pairs per call; split the sample batch"); return SYL_ERR_ARG; }
-    std::vector<SampleView> hv(n_samples);
-    for (uint32_t i = 0; i < n_samples; i++) {
-        hv[i] = {samples[i]->hash, samples[i]->count, samples[i]->n};
-        S.max_n = std::max<uint64_t>(S.max_n, samples[i]->n);
-    }
-    SYL_TRY(S.views.alloc(n_samples, st));
-    SYL_CUDA(cudaMemcpyAsync(S.views.p, hv.data(), n_samples * sizeof(SampleView), cudaMemcpyHostToDevice, st));
-    SYL_CUDA(cudaStreamSynchronize(st));  // hv goes out of scope
-    SYL_TRY(S.cnt.alloc(S.P, st)); SYL_TRY(S.cursor.alloc(S.P, st)); SYL_TRY(S.off.alloc(S.P + 1, st));
-    if (need_pass2) {
-        SYL_TRY(S.lost.alloc(S.P, st)); SYL_TRY(S.survivor.alloc(S.P, st)); SYL_TRY(S.ani1.alloc(S.P, st));
-    }
-    S.rows_cap = std::min<uint64_t>(S.P, 1u << 16);
-    S.boot_cap = S.rows_cap;
-    SYL_TRY(S.rows.alloc(S.rows_cap, st));
-    SYL_TRY(S.boot_rows.alloc(S.boot_cap, st));
-    SYL_TRY(S.hist.alloc(S.boot_cap * 17, st));
-    SYL_TRY(S.covs.alloc(1 << 16, st));
-    const bool force_csr = getenv("SYL_CONTAIN_CSR") != nullptr;  // testing: always take the CSR formulation (read per call)
-    S.use_hist = !force_csr && S.P * COV_BINS * 4 <= (8ull << 30);
-    if (S.use_hist) { SYL_TRY(S.chist.alloc(S.P * COV_BINS, st)); SYL_TRY(S.touched.alloc(S.P, st)); }
-    if (S.use_hist && need_pass2 && S.max_n) SYL_TRY(S.hits.alloc(S.S * S.max_n, st));
-    cub::DeviceScan::ExclusiveSum(nullptr, S.tmp_bytes, S.cnt.p, S.off.p, (int)S.P, st);
-    SYL_TRY(S.tmp.alloc(S.tmp_bytes, st));
-    return SYL_OK;
-}
-
-// One get_stats pass of ALL samples over the whole db (batched: one set of launches, two host
-// syncs).  pass2: S.survivor / S.ani1 must be filled.  Output rows ordered by (sample, genome).
-static int contain_pass(syl_ctx *ctx, const syl_db *db, const StatParams &P, bool pass2, ContainScratch &S,
-                        std::vector<syl_ani_row> &rows_out, bool keep_device_rows, uint64_t *n_dev_rows) {
-    cudaStream_t st = ctx->stream;
-    const uint64_t G = S.G, NP = S.P;
-    rows_out.clear();
-    const dim3 jgrid(nblk(std::max<uint64_t>(S.max_n, 1), 128), (unsigned)S.S);
-    const bool have = S.max_n && db->N;
-    unsigned long long *d_n = reinterpret_cast<unsigned long long *>(ctx->d_counters + 12);  // [12] rows, [13] boot rows, [15] overflow
-    unsigned long long *d_ovf = reinterpret_cast<unsigned long long *>(ctx->d_counters + 15);
-    uint64_t n_rows = 0, n_boot = 0;
-    bool done = false;
-    auto grow_rows = [&]() -> int {  // rare: more rows than the first guess, redo the statistics with room
-        S.rows_cap = std::max(S.rows_cap, n_rows);
-        S.boot_cap = std::max(S.boot_cap, n_boot);
-        SYL_TRY(S.rows.alloc(S.rows_cap, st));
-        SYL_TRY(S.boot_rows.alloc(S.boot_cap, st));
-        SYL_TRY(S.hist.alloc(S.boot_cap * 17, st));
-        return SYL_OK;
-    };
-    if (S.use_hist) {
-        // histogram formulation: one probe pass, statistics from the per-pair count histograms
-        SYL_CUDA(cudaMemsetAsync(S.touched.p, 0, NP, st));
-        if (pass2) SYL_CUDA(cudaMemsetAsync(S.lost.p, 0, NP * 4, st));
-        SYL_CUDA(cudaMemsetAsync(S.chist.p, 0, NP * COV_BINS * 4, st));
-        SYL_CUDA(cudaMemsetAsync(d_ovf, 0, 8, st));
-        if (have) {
-            if (!pass2 && S.hits.p) SYL_CUDA(cudaMemsetAsync(S.hits.p, 0, S.S * S.max_n * sizeof(uint2), st));
-            KernelTimer kt(ctx, pass2 ? SYL_KERNEL_JOIN2 : SYL_KERNEL_JOIN);
-            if (!pass2)
-                k_join_hist<false><<<jgrid, 128, 0, st>>>(S.views.p, G, db->keys, db->gid, db->N, db->bstart, db->M, db->NB, db->maxkey,
-                                                          nullptr, nullptr, S.touched.p, nullptr, S.chist.p, d_ovf, S.hits.p, S.max_n, KeyMap{nullptr, 0, 0});
-            else if (S.hits_valid)
-                k_join2_hits<<<jgrid, 128, 0, st>>>(S.views.p, G, db->gid, S.hits.p, S.max_n, S.survivor.p, S.ani1.p, S.touched.p,
-                                                    S.lost.p, S.chist.p, d_ovf);
-            else
-                k_join_hist<true><<<jgrid, 128, 0, st>>>(S.views.p, G, db->keys, db->gid, db->N, db->bstart, db->M, db->NB, db->maxkey,
-                                                         S.survivor.p, S.ani1.p, S.touched.p, S.lost.p, S.chist.p, d_ovf, nullptr, 0, KeyMap{nullptr, 0, 0});
-            if (!pass2) S.hits_valid = S.hits.p != nullptr;
-            ctx->launches++;
-        }
-        for (;;) {
-            SYL_CUDA(cudaMemsetAsync(d_n, 0, 16, st));
-            KernelTimer kt(ctx, SYL_KERNEL_STATS);
-            k_stats_hist<<<nblk(NP, STAT_WARPS), STAT_WARPS * 32, 0, st>>>(S.touched.p, S.chist.p, db->glen, pass2 ? S.lost.p : nullptr,
-                                                                           G, NP, db->genome_base, P, pass2 ? 1 : 0, S.rows.p, S.rows_cap,
-                                                                           S.boot_rows.p, S.hist.p, S.boot_cap, d_n, d_n + 1);
-            kt.stop();
-            ctx->launches++;
-            SYL_CUDA(cudaGetLastError());
-            SYL_CUDA(cudaMemcpyAsync(ctx->h_counters + 12, d_n, 32, cudaMemcpyDeviceToHost, st));
-            SYL_CUDA(cudaStreamSynchronize(st));
-            if (ctx->h_counters[15]) break;  // coverage >= COV_BINS somewhere: CSR formulation below
-            n_rows = ctx->h_counters[12];
-            n_boot = ctx->h_counters[13];
-            if (n_rows <= S.rows_cap && n_boot <= S.boot_cap) { done = true; break; }
-            SYL_TRY(grow_rows());
-        }
-    }
-    if (!done) {
-        // CSR formulation: count the hits per pair, scan, scatter the counts, select the median
-        SYL_CUDA(cudaMemsetAsync(S.cnt.p, 0, NP * 4, st));
-        SYL_CUDA(cudaMemsetAsync(S.cursor.p, 0, NP * 4, st));
-        if (pass2) SYL_CUDA(cudaMemsetAsync(S.lost.p, 0, NP * 4, st));
-        if (have) {
-            if (!pass2)
-                k_join<false, false><<<jgrid, 128, 0, st>>>(S.views.p, G, db->keys, db->gid, db->bstart, db->M, db->NB, db->maxkey,
-                                                            nullptr, nullptr, S.cnt.p, nullptr, nullptr, nullptr, nullptr);
-            else
-                k_join<true, false><<<jgrid, 128, 0, st>>>(S.views.p, G, db->keys, db->gid, db->bstart, db->M, db->NB, db->maxkey,
-                                                           S.survivor.p, S.ani1.p, S.cnt.p, nullptr, nullptr, nullptr, S.lost.p);
-            ctx->launches++;
-        }
-        size_t tb = S.tmp_bytes;
-        SYL_CUDA(cub::DeviceScan::ExclusiveSum(S.tmp.p, tb, S.cnt.p, S.off.p, (int)NP, st));
-        SYL_CUDA(cudaMemcpyAsync(ctx->h_counters + 10, S.off.p + (NP - 1), 8, cudaMemcpyDeviceToHost, st));
-        SYL_CUDA(cudaMemcpyAsync(ctx->h_counters + 11, S.cnt.p + (NP - 1), 4, cudaMemcpyDeviceToHost, st));
-        SYL_CUDA(cudaStreamSynchronize(st));
-        const uint64_t H = ctx->h_counters[10] + (uint32_t)ctx->h_counters[11];
-        if (H > S.covs.n) SYL_TRY(S.covs.alloc(H + H / 2 + 1024, st));
-        if (H) {
-            if (!pass2)
-                k_join<false, true><<<jgrid, 128, 0, st>>>(S.views.p, G, db->keys, db->gid, db->bstart, db->M, db->NB, db->maxkey,
-                                                           nullptr, nullptr, nullptr, S.off.p, S.cursor.p, S.covs.p, nullptr);
-            else
-                k_join<true, true><<<jgrid, 128, 0, st>>>(S.views.p, G, db->keys, db->gid, db->bstart, db->M, db->NB, db->maxkey,
-                                                          S.survivor.p, S.ani1.p, nullptr, S.off.p, S.cursor.p, S.covs.p, nullptr);
-            ctx->launches++;
-        }
-        for (;;) {
-            SYL_CUDA(cudaMemsetAsync(d_n, 0, 16, st));
-            k_stats<<<nblk(NP, STAT_WARPS), STAT_WARPS * 32, 0, st>>>(S.cnt.p, S.off.p, S.covs.p, db->glen, pass2 ? S.lost.p : nullptr,
-                                                                      G, NP, db->genome_base, P, pass2 ? 1 : 0, S.rows.p, S.rows_cap,
-                                                                      S.boot_rows.p, S.hist.p, S.boot_cap, d_n, d_n + 1);
-            ctx->launches++;
-            SYL_CUDA(cudaGetLastError());
-            SYL_CUDA(cudaMemcpyAsync(ctx->h_counters + 12, d_n, 16, cudaMemcpyDeviceToHost, st));
-            SYL_CUDA(cudaStreamSynchronize(st));
-            n_rows = ctx->h_counters[12];
-            n_boot = ctx->h_counters[13];
-            if (n_rows <= S.rows_cap && n_boot <= S.boot_cap) break;
-            SYL_TRY(grow_rows());
-        }
-    }
-    if (n_boot) {
-        const uint64_t nb = n_boot * BOOT_ITERS;
-        if (nb > S.res_ani.n) {
-            SYL_TRY(S.res_ani.alloc(nb, st));
-            SYL_TRY(S.res_lambda.alloc(nb, st));
-            SYL_TRY(S.res_ok.alloc(nb, st));
-            SYL_TRY(S.reject.alloc(n_boot, st));
-        }
-        SYL_CUDA(cudaMemsetAsync(S.reject.p, 0, (size_t)n_boot * 4, st));
-        KernelTimer kt(ctx, SYL_KERNEL_BOOT);
-        for (uint64_t r0 = 0; r0 < n_boot; r0 += 32768) {  // gridDim.y limit
-            const uint32_t nr = (uint32_t)std::min<uint64_t>(32768, n_boot - r0);
-            k_boot_iter<<<dim3(BOOT_ITERS, nr), BOOT_THREADS, 0, st>>>(S.hist.p + r0 * 17, P, S.res_ani.p + r0 * BOOT_ITERS,
-                                                                       S.res_lambda.p + r0 * BOOT_ITERS,
-                                                                       S.res_ok.p + r0 * BOOT_ITERS, S.reject.p + r0);
-            ctx->launches++;
-        }
-        k_boot_seq<<<nblk(n_boot, 32), 32, 0, st>>>(S.hist.p, (uint32_t)n_boot, P, S.reject.p, S.res_ani.p, S.res_lambda.p, S.res_ok.p);
-        k_boot_final<<<(unsigned)n_boot, 128, 0, st>>>(S.boot_rows.p, (uint32_t)n_boot, S.res_ani.p, S.res_lambda.p, S.res_ok.p, S.rows.p);
-        kt.stop();
-        ctx->launches += 2;
-        SYL_CUDA(cudaGetLastError());
-    }
-    if (n_rows) {
-        rows_out.resize(n_rows);
-        SYL_CUDA(cudaMemcpyAsync(rows_out.data(), S.rows.p, n_rows * sizeof(syl_ani_row), cudaMemcpyDeviceToHost, st));
-        SYL_CUDA(cudaStreamSynchronize(st));
-        std::sort(rows_out.begin(), rows_out.end(), [](const syl_ani_row &a, const syl_ani_row &b) {
-            return a.sample != b.sample ? a.sample < b.sample : a.genome < b.genome;
-        });
-    }
-    (void)keep_device_rows;
-    if (n_dev_rows) *n_dev_rows = n_rows;
-    return SYL_OK;
-}
-
 // ------------------------------------------------------------------------------------------------
-// Device-driven query / profile ("fast path"): both get_stats passes, the winner decision and the
-// bootstrap are enqueued back to back; the host synchronises ONCE, when it reads the final rows.
-//   pass 1      k_join_hist<pass 1> + k_stats_hist -> rows appended to a per-rank ROW TABLE
+// Staged query / profile: both get_stats passes, the winner decision and the bootstrap are enqueued
+// back to back; the host synchronises ONCE, when it reads the final rows.
+//   pass 1      k_join_hist + k_stats_hist -> rows appended to a per-rank ROW TABLE
 //               (header {n_rows, n_boot, overflow} + R rows of 144 bytes, R fixed per call)
 //   [N ranks: the caller all-gathers the row tables — collective 1]
 //   ranking     k_rank_rows: every pass-1 survivor gets its position in the per-sample order
@@ -1094,8 +780,13 @@ static int contain_pass(syl_ctx *ctx, const syl_db *db, const StatParams &P, boo
 //   [N ranks: the caller all-gathers the pass-2 row tables — collective 3]
 //   finish      D2H of the table(s), derep_if_reassign_threshold (:353-375), abundances (:319-326), sort
 // Single GPU: the winner minimum is taken inside k_join2_order and nothing is gathered.  A coverage
-// count >= COV_BINS or more rows than the table holds is reported in the header; the caller then
-// redoes the call on the synchronous path above (CSR formulation) or with a larger table.
+// count >= COV_BINS or more rows than the table holds is reported in the header; contain_fast then
+// redoes the call in the CSR formulation or with a larger table.
+// CSR formulation (single GPU only): k_join_hist<probe only> records the equal ranges, k_join_csr /
+// k_join2_order<.., CSR_*> walk them twice per pass (count hits per pair, CUB scan, scatter the hits'
+// sample counts) and k_stats replaces k_stats_hist; ranking, bootstrap and finish are shared.  Sizing
+// the value array after the pass-1 scan costs a second host synchronisation; pass 2 needs none, because
+// its hits are a subset of pass 1's (same ranges, winners only).
 constexpr uint32_t ORD_NONE = 0x7F7F7F7Fu;  // memset-able; valid as int32 for the MIN all-reduce
 
 struct ShardTable { unsigned long long n_rows, n_boot, ovf, pad; };
@@ -1159,13 +850,42 @@ __global__ void k_local_best(const SampleView *__restrict__ views, uint64_t G, c
   });
 }
 
+// CSR formulation of a pass: the count walk adds up the hits per pair in cnt; after the scan of cnt into off, the
+// fill walk writes each hit's sample count to covs[off[pair] + cursor[pair]++].
+struct CsrBufs { uint32_t *cnt; const uint64_t *off; uint32_t *cursor; uint32_t *covs; };
+
+template <bool FILL>
+__device__ __forceinline__ void csr_hit(const CsrBufs &b, uint64_t pair, uint32_t c) {
+    if (FILL) b.covs[b.off[pair] + atomicAdd(&b.cursor[pair], 1u)] = c;
+    else atomicAdd(&b.cnt[pair], 1u);
+}
+
+// pass 1 of the CSR formulation over the equal ranges recorded by k_join_hist<true>: every genome_kmers hit counts
+template <bool FILL>
+__global__ void k_join_csr(const SampleView *__restrict__ views, uint64_t G, const uint32_t *__restrict__ gid,
+                           const uint2 *__restrict__ hits, uint64_t hits_stride, const CsrBufs csr, const KeyMap km) {
+  for_each_key(km, views, [&](const uint32_t smp, const uint64_t i) {
+    const uint2 h = hits[(uint64_t)smp * hits_stride + i];
+    const uint64_t row = (uint64_t)smp * G;
+    const uint32_t c = views[smp].count[i];
+    for (uint32_t j = h.x; j < h.x + h.y; j++) {
+        const uint32_t gv = gid[j];
+        if (!(gv & 1u)) csr_hit<FILL>(csr, row + (gv >> 1), c);  // tracked k-mers only take part in pass 2's winner decision
+    }
+  });
+}
+
+// What a pass-2 walk produces: count histograms (touched / chist / ovf), or the CSR formulation's count walk
+// (cnt, and lost) or fill walk (covs).
+enum JoinOut { JOIN_HIST, JOIN_CSR_COUNT, JOIN_CSR_FILL };
+
 // pass 2 over the equal ranges recorded by pass 1.  FUSED: the winner (smallest order in the range) is
 // taken here (single GPU); else it comes from wbest (all-reduced over the shards).
-template <bool FUSED>
+template <bool FUSED, JoinOut OUT = JOIN_HIST>
 __global__ void k_join2_order(const SampleView *__restrict__ views, uint64_t G, const uint32_t *__restrict__ gid,
                               const uint2 *__restrict__ hits, uint64_t hits_stride, const uint32_t *__restrict__ order_tbl,
                               const uint32_t *__restrict__ wbest, uint8_t *__restrict__ touched, uint32_t *__restrict__ lost,
-                              uint32_t *__restrict__ chist, unsigned long long *__restrict__ ovf, const KeyMap km) {
+                              uint32_t *__restrict__ chist, unsigned long long *__restrict__ ovf, const CsrBufs csr, const KeyMap km) {
   for_each_key(km, views, [&](const uint32_t smp, const uint64_t i) {
     const uint2 h = hits[(uint64_t)smp * hits_stride + i];
     if (h.y == 0) return;
@@ -1198,7 +918,11 @@ __global__ void k_join2_order(const SampleView *__restrict__ views, uint64_t G, 
             const uint32_t g = gv >> 1;
             const uint32_t o = ord[g];
             if (o == ORD_NONE) continue;                       // not a pass-1 survivor
-            if (o != winner) { atomicAdd(&lost[row + g], 1u); continue; }  // src/contain.rs:641-646
+            if (o != winner) {                                 // src/contain.rs:641-646
+                if (OUT != JOIN_CSR_FILL) atomicAdd(&lost[row + g], 1u);
+                continue;
+            }
+            if (OUT != JOIN_HIST) { csr_hit<OUT == JOIN_CSR_FILL>(csr, row + g, c); continue; }
             if (!touched[row + g]) touched[row + g] = 1;
             if (c < COV_BINS) atomicAdd(&chist[(row + g) * COV_BINS + c], 1u);
             else atomicAdd(ovf, 1ull);
@@ -1226,9 +950,13 @@ struct syl_profile_job {
     uint32_t S = 0, world = 1, rank = 0;
     uint64_t G = 0, R = 0, max_n = 0, tbytes = 0;
     int stage = 0;           // 1 pass 1 enqueued, 2 ranked, 3 pass 2 enqueued
+    bool csr = false;        // CSR formulation (single GPU) instead of the per-pair count histograms
     syl::DevBuf<syl::SampleView> views;
-    syl::DevBuf<uint8_t> touched, tab1, gat1, tab2, gat2, res_ok;
+    syl::DevBuf<uint8_t> touched, tab1, gat1, tab2, gat2, res_ok, scan_tmp;
     syl::DevBuf<uint32_t> chist, lost, order, contain1, wbest, boot_rows, hist, reject, range_bounds;
+    syl::DevBuf<uint32_t> cnt, cursor, covs;   // CSR formulation
+    syl::DevBuf<uint64_t> off;
+    size_t scan_bytes = 0;
     syl::KeyMap km{nullptr, 0, 0};   // tiled (range, sample) mapping of the join kernels when there are several samples
     dim3 jgrid;
     syl::DevBuf<uint2> hits;
@@ -1287,16 +1015,82 @@ static uint64_t default_rows_per_rank(uint32_t S, uint64_t G) {
     return (std::max<uint64_t>(R, 256) + 255) & ~255ull;
 }
 
-// stage 1: allocate, pass 1 (P1 = the pass-1 parameters: profile skips the bootstrap there)
+static bool histograms_fit(uint64_t n_pairs) { return n_pairs * COV_BINS * 4 <= (8ull << 30); }
+
+// CSR formulation of one pass over the equal ranges in j->hits: count walk, scan, fill walk.  Pass 1 sizes covs,
+// which needs a host synchronisation; pass 2's hits are a subset of pass 1's, so that size bounds them as well.
+static int csr_walks(syl_profile_job *j, bool pass2) {
+    syl_ctx *ctx = j->ctx;
+    cudaStream_t st = ctx->stream;
+    const syl_db *db = j->db;
+    const uint64_t NP = (uint64_t)j->S * j->G;
+    const bool walk = j->max_n && db->N;
+    SYL_CUDA(cudaMemsetAsync(j->cnt.p, 0, (NP + 1) * 4, st));  // cnt[NP] = 0: off[NP] is the total
+    SYL_CUDA(cudaMemsetAsync(j->cursor.p, 0, NP * 4, st));
+    CsrBufs b{j->cnt.p, j->off.p, j->cursor.p, j->covs.p};
+    if (walk) {
+        KernelTimer kt(ctx, pass2 ? SYL_KERNEL_JOIN2 : SYL_KERNEL_JOIN);
+        if (pass2)
+            k_join2_order<true, JOIN_CSR_COUNT><<<j->jgrid, 128, 0, st>>>(j->views.p, j->G, db->gid, j->hits.p, j->max_n, j->order.p, nullptr,
+                                                                          nullptr, j->lost.p, nullptr, nullptr, b, j->km);
+        else
+            k_join_csr<false><<<j->jgrid, 128, 0, st>>>(j->views.p, j->G, db->gid, j->hits.p, j->max_n, b, j->km);
+        ctx->launches++;
+    }
+    size_t tb = j->scan_bytes;
+    SYL_CUDA(cub::DeviceScan::ExclusiveSum(j->scan_tmp.p, tb, j->cnt.p, j->off.p, (int)(NP + 1), st));
+    if (!pass2) {
+        SYL_CUDA(cudaMemcpyAsync(ctx->h_counters + 10, j->off.p + NP, 8, cudaMemcpyDeviceToHost, st));
+        SYL_CUDA(cudaStreamSynchronize(st));
+        SYL_TRY(j->covs.alloc(std::max<uint64_t>(ctx->h_counters[10], 1), st));
+        b.covs = j->covs.p;
+    }
+    if (walk) {
+        KernelTimer kt(ctx, pass2 ? SYL_KERNEL_JOIN2 : SYL_KERNEL_JOIN);
+        if (pass2)
+            k_join2_order<true, JOIN_CSR_FILL><<<j->jgrid, 128, 0, st>>>(j->views.p, j->G, db->gid, j->hits.p, j->max_n, j->order.p, nullptr,
+                                                                         nullptr, j->lost.p, nullptr, nullptr, b, j->km);
+        else
+            k_join_csr<true><<<j->jgrid, 128, 0, st>>>(j->views.p, j->G, db->gid, j->hits.p, j->max_n, b, j->km);
+        ctx->launches++;
+    }
+    SYL_CUDA(cudaGetLastError());
+    return SYL_OK;
+}
+
+// statistics of one pass (either formulation) into the row table `tab`
+static int enqueue_stats(syl_profile_job *j, const StatParams &P, bool pass2, void *tab, const StatExtra &X) {
+    syl_ctx *ctx = j->ctx;
+    const syl_db *db = j->db;
+    const uint64_t NP = (uint64_t)j->S * j->G;
+    ShardTable *t = reinterpret_cast<ShardTable *>(tab);
+    uint32_t *lost = pass2 ? j->lost.p : nullptr;
+    KernelTimer kt(ctx, SYL_KERNEL_STATS);
+    if (j->csr)
+        k_stats<<<nblk(NP, STAT_WARPS), STAT_WARPS * 32, 0, ctx->stream>>>(j->cnt.p, j->off.p, j->covs.p, db->glen, lost, j->G, NP, db->genome_base,
+                                                                          P, pass2 ? 1 : 0, table_rows(tab), j->R, j->boot_rows.p, j->hist.p, j->R,
+                                                                          &t->n_rows, &t->n_boot, X);
+    else
+        k_stats_hist<<<nblk(NP, STAT_WARPS), STAT_WARPS * 32, 0, ctx->stream>>>(j->touched.p, j->chist.p, db->glen, lost, j->G, NP, db->genome_base,
+                                                                               P, pass2 ? 1 : 0, table_rows(tab), j->R, j->boot_rows.p, j->hist.p, j->R,
+                                                                               &t->n_rows, &t->n_boot, X);
+    ctx->launches++;
+    SYL_CUDA(cudaGetLastError());
+    return SYL_OK;
+}
+
+// stage 1: allocate, pass 1 (P1 = the pass-1 parameters: profile skips the bootstrap there).  csr: the CSR formulation
+// (single GPU only); otherwise histograms beyond 8 GB are SYL_ERR_UNSUPPORTED.
 static int job_begin(syl_ctx *ctx, const syl_db *db, const syl_sample *const *samples, uint32_t n_samples,
-                     const syl_contain_params *p, bool profile, uint32_t world, uint32_t rank, uint64_t R, syl_profile_job **out) {
+                     const syl_contain_params *p, bool profile, bool csr, uint32_t world, uint32_t rank, uint64_t R,
+                     syl_profile_job **out) {
     cudaStream_t st = ctx->stream;
     syl_profile_job *j = new (std::nothrow) syl_profile_job();
     if (!j) return SYL_ERR_OOM;
     auto fail = [&](int rc) { job_release(j); return rc; };
 #define JOB_CUDA(x) do { cudaError_t _e = (x); if (_e != cudaSuccess) { set_error(std::string(#x) + ": " + cudaGetErrorString(_e)); return fail(_e == cudaErrorMemoryAllocation ? SYL_ERR_OOM : SYL_ERR_CUDA); } } while (0)
 #define JOB_TRY(x) do { int _r = (x); if (_r != SYL_OK) return fail(_r); } while (0)
-    j->ctx = ctx; j->db = db; j->profile = profile; j->S = n_samples; j->G = db->n_genomes; j->world = world; j->rank = rank;
+    j->ctx = ctx; j->db = db; j->profile = profile; j->csr = csr; j->S = n_samples; j->G = db->n_genomes; j->world = world; j->rank = rank;
     syl_contain_params pp = *p;
     pp.pseudotax = profile ? 1 : 0;
     j->P = make_params(&pp);
@@ -1308,7 +1102,7 @@ static int job_begin(syl_ctx *ctx, const syl_db *db, const syl_sample *const *sa
     if (j->R * BOOT_ITERS >= 0xFFFF0000ull) { set_error("row capacity too large for the bootstrap work counter"); return fail(SYL_ERR_ARG); }
     const uint64_t NP = (uint64_t)j->S * j->G;
     if (NP >= 0x7FFFFFFFull) { set_error("samples x genomes exceeds 2^31 pairs per call; split the sample batch"); return fail(SYL_ERR_ARG); }
-    if (NP * COV_BINS * 4 > (8ull << 30)) { set_error("pair histograms exceed 8 GB; split the sample batch"); return fail(SYL_ERR_UNSUPPORTED); }
+    if (!csr && !histograms_fit(NP)) { set_error("pair histograms exceed 8 GB; split the sample batch"); return fail(SYL_ERR_UNSUPPORTED); }
     std::vector<SampleView> hv(n_samples);
     for (uint32_t i = 0; i < n_samples; i++) {
         hv[i] = {samples[i]->hash, samples[i]->count, samples[i]->n};
@@ -1316,7 +1110,14 @@ static int job_begin(syl_ctx *ctx, const syl_db *db, const syl_sample *const *sa
     }
     const uint64_t HN = std::max<uint64_t>((uint64_t)j->S * j->max_n, 1);
     JOB_TRY(j->views.alloc(n_samples, st));
-    JOB_TRY(j->touched.alloc(NP, st)); JOB_TRY(j->chist.alloc(NP * COV_BINS, st)); JOB_TRY(j->hits.alloc(HN, st));
+    if (csr) {
+        JOB_TRY(j->cnt.alloc(NP + 1, st)); JOB_TRY(j->cursor.alloc(NP, st)); JOB_TRY(j->off.alloc(NP + 1, st));
+        cub::DeviceScan::ExclusiveSum(nullptr, j->scan_bytes, j->cnt.p, j->off.p, (int)(NP + 1), st);
+        JOB_TRY(j->scan_tmp.alloc(j->scan_bytes, st));
+    } else {
+        JOB_TRY(j->touched.alloc(NP, st)); JOB_TRY(j->chist.alloc(NP * COV_BINS, st));
+    }
+    JOB_TRY(j->hits.alloc(HN, st));
     JOB_TRY(j->tab1.alloc(j->tbytes, st));
     JOB_TRY(j->boot_rows.alloc(j->R, st)); JOB_TRY(j->hist.alloc(j->R * 17, st));
     JOB_TRY(j->res_ani.alloc(j->R * BOOT_ITERS, st)); JOB_TRY(j->res_lambda.alloc(j->R * BOOT_ITERS, st));
@@ -1330,8 +1131,10 @@ static int job_begin(syl_ctx *ctx, const syl_db *db, const syl_sample *const *sa
     // a pageable source is staged by the driver before cudaMemcpyAsync returns: hv may go out of scope
     JOB_CUDA(cudaMemcpyAsync(j->views.p, hv.data(), n_samples * sizeof(SampleView), cudaMemcpyHostToDevice, st));
     if (profile && j->G) JOB_CUDA(cudaMemcpyAsync(j->gn_size.p, db->h_gn_size.data(), j->G * 8, cudaMemcpyHostToDevice, st));
-    JOB_CUDA(cudaMemsetAsync(j->touched.p, 0, NP, st));
-    JOB_CUDA(cudaMemsetAsync(j->chist.p, 0, NP * COV_BINS * 4, st));
+    if (!csr) {
+        JOB_CUDA(cudaMemsetAsync(j->touched.p, 0, NP, st));
+        JOB_CUDA(cudaMemsetAsync(j->chist.p, 0, NP * COV_BINS * 4, st));
+    }
     JOB_CUDA(cudaMemsetAsync(j->hits.p, 0, HN * sizeof(uint2), st));
     JOB_CUDA(cudaMemsetAsync(j->tab1.p, 0, sizeof(ShardTable), st));
     ShardTable *t1 = reinterpret_cast<ShardTable *>(j->tab1.p);
@@ -1353,23 +1156,21 @@ static int job_begin(syl_ctx *ctx, const syl_db *db, const syl_sample *const *sa
     const dim3 jgrid = j->jgrid;
     if (j->max_n && db->N) {
         KernelTimer kt(ctx, SYL_KERNEL_JOIN);
-        k_join_hist<false><<<jgrid, 128, 0, st>>>(j->views.p, j->G, db->keys, db->gid, db->N, db->bstart, db->M, db->NB, db->maxkey,
-                                                  nullptr, nullptr, j->touched.p, nullptr, j->chist.p, &t1->ovf, j->hits.p, j->max_n, j->km);
+        if (csr)
+            k_join_hist<true><<<jgrid, 128, 0, st>>>(j->views.p, j->G, db->keys, db->gid, db->N, db->bstart, db->M, db->NB, db->maxkey,
+                                                     nullptr, nullptr, nullptr, j->hits.p, j->max_n, j->km);
+        else
+            k_join_hist<false><<<jgrid, 128, 0, st>>>(j->views.p, j->G, db->keys, db->gid, db->N, db->bstart, db->M, db->NB, db->maxkey,
+                                                      j->touched.p, j->chist.p, &t1->ovf, j->hits.p, j->max_n, j->km);
         ctx->launches++;
     }
+    if (csr) JOB_TRY(csr_walks(j, false));
     StatParams P1 = j->P;
     if (profile) P1.no_ci = 1;  // pass-1 confidence intervals are never reported (pass-2 rows replace them)
     StatExtra X;
     X.pair_stride = j->G;
     if (profile) X.contain1_out = j->contain1.p;
-    {
-        KernelTimer kt(ctx, SYL_KERNEL_STATS);
-        k_stats_hist<<<nblk(NP, STAT_WARPS), STAT_WARPS * 32, 0, st>>>(j->touched.p, j->chist.p, db->glen, nullptr, j->G, NP, db->genome_base, P1, 0,
-                                                                       table_rows(j->tab1.p), j->R, j->boot_rows.p, j->hist.p, j->R,
-                                                                       &t1->n_rows, &t1->n_boot, X);
-        ctx->launches++;
-    }
-    JOB_CUDA(cudaGetLastError());
+    JOB_TRY(enqueue_stats(j, P1, false, j->tab1.p, X));
     j->stage = 1;
     *out = j;
     return SYL_OK;
@@ -1420,37 +1221,33 @@ static int job_pass2(syl_profile_job *j) {
     cudaStream_t st = ctx->stream;
     const syl_db *db = j->db;
     const uint64_t NP = (uint64_t)j->S * j->G;
-    ShardTable *t1 = reinterpret_cast<ShardTable *>(j->tab1.p), *t2 = reinterpret_cast<ShardTable *>(j->tab2.p);
-    SYL_CUDA(cudaMemsetAsync(j->touched.p, 0, NP, st));
+    ShardTable *t2 = reinterpret_cast<ShardTable *>(j->tab2.p);
     SYL_CUDA(cudaMemsetAsync(j->lost.p, 0, NP * 4, st));
-    SYL_CUDA(cudaMemsetAsync(j->chist.p, 0, NP * COV_BINS * 4, st));
     SYL_CUDA(cudaMemsetAsync(j->tab2.p, 0, sizeof(ShardTable), st));
-    const dim3 jgrid = j->jgrid;
-    if (j->max_n && db->N) {
-        KernelTimer kt(ctx, SYL_KERNEL_JOIN2);
-        if (j->world > 1)
-            k_join2_order<false><<<jgrid, 128, 0, st>>>(j->views.p, j->G, db->gid, j->hits.p, j->max_n, j->order.p, j->wbest.p, j->touched.p,
-                                                        j->lost.p, j->chist.p, &t2->ovf, j->km);
-        else
-            k_join2_order<true><<<jgrid, 128, 0, st>>>(j->views.p, j->G, db->gid, j->hits.p, j->max_n, j->order.p, nullptr, j->touched.p,
-                                                       j->lost.p, j->chist.p, &t2->ovf, j->km);
-        ctx->launches++;
+    if (j->csr) {
+        SYL_TRY(csr_walks(j, true));
+    } else {
+        SYL_CUDA(cudaMemsetAsync(j->touched.p, 0, NP, st));
+        SYL_CUDA(cudaMemsetAsync(j->chist.p, 0, NP * COV_BINS * 4, st));
+        const dim3 jgrid = j->jgrid;
+        const CsrBufs no_csr{nullptr, nullptr, nullptr, nullptr};
+        if (j->max_n && db->N) {
+            KernelTimer kt(ctx, SYL_KERNEL_JOIN2);
+            if (j->world > 1)
+                k_join2_order<false><<<jgrid, 128, 0, st>>>(j->views.p, j->G, db->gid, j->hits.p, j->max_n, j->order.p, j->wbest.p, j->touched.p,
+                                                            j->lost.p, j->chist.p, &t2->ovf, no_csr, j->km);
+            else
+                k_join2_order<true><<<jgrid, 128, 0, st>>>(j->views.p, j->G, db->gid, j->hits.p, j->max_n, j->order.p, nullptr, j->touched.p,
+                                                           j->lost.p, j->chist.p, &t2->ovf, no_csr, j->km);
+            ctx->launches++;
+        }
     }
     StatExtra X;
     X.pair_stride = j->G;
     X.contain1_in = j->contain1.p;
     X.gn_size = j->gn_size.p;
-    {
-        KernelTimer kt(ctx, SYL_KERNEL_STATS);
-        k_stats_hist<<<nblk(NP, STAT_WARPS), STAT_WARPS * 32, 0, st>>>(j->touched.p, j->chist.p, db->glen, j->lost.p, j->G, NP, db->genome_base, j->P, 1,
-                                                                       table_rows(j->tab2.p), j->R, j->boot_rows.p, j->hist.p, j->R,
-                                                                       &t2->n_rows, &t2->n_boot, X);
-        ctx->launches++;
-    }
-    SYL_CUDA(cudaGetLastError());
+    SYL_TRY(enqueue_stats(j, j->P, true, j->tab2.p, X));
     SYL_TRY(job_bootstrap(j, j->tab2.p));
-    // carry pass 1's overflow / row counts along, so that the final table tells the whole story
-    (void)t1;
     j->stage = 3;
     return SYL_OK;
 }
@@ -1502,7 +1299,7 @@ static void profile_finalize(std::vector<syl_ani_row> &r2, uint32_t n_samples, i
 }
 
 // last stage: read the final table(s); SYL_ERR_CAPACITY: *need_R rows per rank are needed;
-// SYL_ERR_UNSUPPORTED: a coverage count >= COV_BINS somewhere (the caller takes the synchronous CSR path)
+// SYL_ERR_UNSUPPORTED: a coverage count >= COV_BINS somewhere (the call needs the CSR formulation)
 static int job_finish(syl_profile_job *j, std::vector<syl_ani_row> &out, uint64_t *need_R) {
     syl_ctx *ctx = j->ctx;
     cudaStream_t st = ctx->stream;
@@ -1549,13 +1346,16 @@ static int job_finish(syl_profile_job *j, std::vector<syl_ani_row> &out, uint64_
     return SYL_OK;
 }
 
-// single-GPU driver of the stages; rc SYL_ERR_UNSUPPORTED = take the synchronous path
+// single-GPU driver of the stages for syl_query / syl_profile.  The CSR formulation is taken up front when
+// SYL_CONTAIN_CSR is set (read per call) or the per-pair histograms would exceed 8 GB, and after a histogram
+// run that met a count >= COV_BINS; a row table that is too small is redone with the size it needed.
 static int contain_fast(syl_ctx *ctx, const syl_db *db, const syl_sample *const *samples, uint32_t n_samples,
                         const syl_contain_params *p, bool profile, std::vector<syl_ani_row> &out) {
     uint64_t R = 0;
-    for (int attempt = 0; attempt < 3; attempt++) {
+    bool csr = getenv("SYL_CONTAIN_CSR") != nullptr || !histograms_fit((uint64_t)n_samples * db->n_genomes);
+    for (int attempt = 0; attempt < 4; attempt++) {  // one formulation switch + capacity retries
         syl_profile_job *j = nullptr;
-        SYL_TRY(job_begin(ctx, db, samples, n_samples, p, profile, 1, 0, R, &j));
+        SYL_TRY(job_begin(ctx, db, samples, n_samples, p, profile, csr, 1, 0, R, &j));
         int rc = SYL_OK;
         if (profile) {
             rc = job_rank(j);
@@ -1567,13 +1367,11 @@ static int contain_fast(syl_ctx *ctx, const syl_db *db, const syl_sample *const 
         if (rc == SYL_OK) rc = job_finish(j, out, &need);
         job_release(j);
         if (rc == SYL_ERR_CAPACITY) { R = need + 256; out.clear(); continue; }
+        if (rc == SYL_ERR_UNSUPPORTED && !csr) { csr = true; out.clear(); continue; }  // a count >= COV_BINS
         return rc;
     }
     return SYL_ERR_CAPACITY;
 }
-
-// SYL_CONTAIN_CSR / SYL_CONTAIN_SYNC force the synchronous two-pass implementation (tests)
-static bool fast_path_enabled() { return getenv("SYL_CONTAIN_CSR") == nullptr && getenv("SYL_CONTAIN_SYNC") == nullptr; }
 
 static int check_pair_args(syl_ctx *ctx, const syl_db *db, const syl_sample *const *samples, uint32_t n_samples,
                            const syl_contain_params *p, syl_ani_row *rows, uint64_t cap, uint64_t *n_rows) {
@@ -1700,27 +1498,7 @@ int syl_query(syl_ctx *ctx, const syl_db *db, const syl_sample *const *samples, 
     syl::tl_ctx = ctx;
     if (db->n_genomes == 0 || n_samples == 0) return SYL_OK;
     std::vector<syl_ani_row> out;
-    if (fast_path_enabled()) {
-        const int frc = contain_fast(ctx, db, samples, n_samples, p, false, out);
-        if (frc == SYL_OK) {
-            *n_rows = out.size();
-            if (out.size() > cap) { set_error("row buffer too small"); return SYL_ERR_CAPACITY; }
-            std::copy(out.begin(), out.end(), rows);
-            return SYL_OK;
-        }
-        if (frc != SYL_ERR_UNSUPPORTED) return frc;
-        out.clear();
-    }
-    ContainScratch S;
-    SYL_TRY(scratch_init(ctx, db, samples, n_samples, false, S));
-    const StatParams P = make_params(p);
-    SYL_TRY(contain_pass(ctx, db, P, false, S, out, false, nullptr));
-    if (p->estimate_unknown) {  // estimate_true_cov (src/contain.rs:295)
-        std::vector<SampleMeta> metas;
-        SYL_TRY(sample_metas(ctx, samples, n_samples, metas));
-        for (syl_ani_row &r : out)
-            r.final_est_cov = r.final_est_cov / std::pow(p->read_seq_id / 100., (double)p->k) * unknown_multiplier(metas[r.sample], p->k);
-    }
+    SYL_TRY(contain_fast(ctx, db, samples, n_samples, p, false, out));
     *n_rows = out.size();
     if (out.size() > cap) { set_error("row buffer too small"); return SYL_ERR_CAPACITY; }
     std::copy(out.begin(), out.end(), rows);
@@ -1741,7 +1519,7 @@ int syl_profile_shard_begin(syl_ctx *ctx, const syl_db *db, const syl_sample *co
     }
     SYL_CUDA(cudaSetDevice(ctx->device));
     syl::tl_ctx = ctx;
-    return job_begin(ctx, db, samples, n_samples, p, true, world, rank, rows_per_rank, out);
+    return job_begin(ctx, db, samples, n_samples, p, true, false, world, rank, rows_per_rank, out);
 }
 
 int syl_profile_job_buffers(const syl_profile_job *j, void **d_table1, void **d_gathered1, uint64_t *table_bytes,
@@ -1800,51 +1578,11 @@ int syl_profile(syl_ctx *ctx, const syl_db *db, const syl_sample *const *samples
     SYL_CUDA(cudaSetDevice(ctx->device));
     syl::tl_ctx = ctx;
     if (db->n_genomes == 0 || n_samples == 0) return SYL_OK;
-    if (fast_path_enabled()) {
-        std::vector<syl_ani_row> fout;
-        const int frc = contain_fast(ctx, db, samples, n_samples, p, true, fout);
-        if (frc == SYL_OK) {
-            *n_rows = fout.size();
-            if (fout.size() > cap) { set_error("row buffer too small"); return SYL_ERR_CAPACITY; }
-            std::copy(fout.begin(), fout.end(), rows);
-            return SYL_OK;
-        }
-        if (frc != SYL_ERR_UNSUPPORTED) return frc;
-    }
-    cudaStream_t st = ctx->stream;
-    ContainScratch S;
-    SYL_TRY(scratch_init(ctx, db, samples, n_samples, true, S));
-    syl_contain_params pp = *p;
-    pp.pseudotax = 1;
-    const StatParams P = make_params(&pp);
-    std::vector<syl_ani_row> r1, r2, all;
-    uint64_t n1 = 0;
-    StatParams P1 = P;
-    P1.no_ci = 1;  // pass-1 confidence intervals are never reported (pass-2 rows replace them): skip the bootstrap
-    SYL_TRY(contain_pass(ctx, db, P1, false, S, r1, true, &n1));
-    if (r1.empty()) return SYL_OK;
-    // the pass-1 rows (still on the device) define the winner table of every sample
-    SYL_CUDA(cudaMemsetAsync(S.survivor.p, 0, S.P, st));
-    SYL_CUDA(cudaMemsetAsync(S.ani1.p, 0, S.P * 8, st));
-    k_mark_survivors<<<nblk(n1, 256), 256, 0, st>>>(S.rows.p, n1, S.G, db->genome_base, S.survivor.p, S.ani1.p);
-    ctx->launches++;
-    SYL_TRY(contain_pass(ctx, db, P, true, S, r2, false, nullptr));
-    // stash pass 1's containment count and the genome size in the pass-2 rows, then the common host finish
-    // (derep, -u, abundances, order)
-    {
-        size_t j = 0;
-        for (syl_ani_row &n2 : r2) {  // both lists are ordered by (sample, genome); r2's pairs are a subset of r1's
-            while (j < r1.size() && (r1[j].sample < n2.sample || (r1[j].sample == n2.sample && r1[j].genome < n2.genome))) j++;
-            n2.reserved = (double)r1[j].contain;
-            n2.seq_abund = (double)db->h_gn_size[n2.genome - db->genome_base];
-        }
-    }
-    std::vector<SampleMeta> metas;
-    if (pp.estimate_unknown) SYL_TRY(sample_metas(ctx, samples, n_samples, metas));
-    profile_finalize(r2, n_samples, pp.k, pp.redundant_ani, all, pp.estimate_unknown ? &metas : nullptr, pp.estimate_unknown ? pp.read_seq_id : -1.);
-    *n_rows = all.size();
-    if (all.size() > cap) { set_error("row buffer too small"); return SYL_ERR_CAPACITY; }
-    std::copy(all.begin(), all.end(), rows);
+    std::vector<syl_ani_row> out;
+    SYL_TRY(contain_fast(ctx, db, samples, n_samples, p, true, out));
+    *n_rows = out.size();
+    if (out.size() > cap) { set_error("row buffer too small"); return SYL_ERR_CAPACITY; }
+    std::copy(out.begin(), out.end(), rows);
     return SYL_OK;
 }
 

@@ -13,6 +13,19 @@ pytestmark = [pytest.mark.gpu, pytest.mark.usefixtures("contain_mode")]
 FLOAT_TOL = 1e-6
 
 
+@pytest.fixture(params=["device-driven", "synchronous"])
+def contain_mode(request, monkeypatch):
+    """syl_query / syl_profile in both formulations of the staged driver (the library reads SYL_CONTAIN_CSR per call):
+    "device-driven" = the per-pair count histograms, one host synchronisation per call (the CSR formulation only where
+    a count >= 256 or the size asks for it); "synchronous" = the CSR formulation throughout, which synchronises once
+    more to size its value array.  The ids are those of the former device-driven / synchronous paths, so test ids stay
+    stable."""
+    monkeypatch.delenv("SYL_CONTAIN_CSR", raising=False)
+    if request.param == "synchronous":
+        monkeypatch.setenv("SYL_CONTAIN_CSR", "1")
+    return request.param
+
+
 def oracle_rows(db, sample_hc, pseudotax, **kw):
     from oracle import oracle as O
     p = O.default_params(pseudotax=pseudotax, **kw)
@@ -183,11 +196,8 @@ def test_uploaded_sketches_and_zero_counts(ctx):
     compare(ctx.profile(db, [smp]), oracle_rows(d, (sh, sc), True), True)
 
 
-@pytest.mark.parametrize("depth", [40, 250, 255, 256, 700])
-def test_deep_coverage_uploaded_sample(ctx, depth):
-    """Coverage around the 256-bin limit of the per-pair count histograms: up to 255 the histogram
-    formulation of get_stats answers, from 256 on the call falls back to the CSR formulation
-    (contain.cu COV_BINS); medians >= 30 take the no-cutoff branch (src/contain.rs:664)."""
+def deep_coverage_case(ctx, depth):
+    """Three uploaded genomes (genome 0 covered `depth` deep, genome 1 shallow, genome 2 absent) and one sample."""
     rng = np.random.default_rng(1000 + depth)
     kmers = np.unique(rng.integers(1, 2**57, size=9000, dtype=np.uint64))[:8000]
     koff = np.array([0, 3000, 5500, 8000], dtype=np.uint64)
@@ -201,8 +211,17 @@ def test_deep_coverage_uploaded_sample(ctx, depth):
     if depth >= 250:
         sc[:5] = [255, 256, 257, 100000, 255]
     smp = ctx.upload_sample(sh, sc)
-    db = ctx.build_db(g)
     d = dict(kmers=kmers, kmer_off=koff, tracked=tracked, tracked_off=toff, gn_size=gs)
+    return g, d, (sh, sc), smp
+
+
+@pytest.mark.parametrize("depth", [40, 250, 255, 256, 700])
+def test_deep_coverage_uploaded_sample(ctx, depth):
+    """Coverage around the 256-bin limit of the per-pair count histograms: up to 255 the histogram
+    formulation of get_stats answers, from 256 on the call is redone in the CSR formulation
+    (contain.cu COV_BINS); medians >= 30 take the no-cutoff branch (src/contain.rs:664)."""
+    g, d, (sh, sc), smp = deep_coverage_case(ctx, depth)
+    db = ctx.build_db(g)
     exp = oracle_rows(d, (sh, sc), False)
     assert len(exp) >= 1 and exp[0].median_cov >= 30
     compare(sort_query_rows(ctx.query(db, [smp])), exp, False)
@@ -275,3 +294,97 @@ def test_estimate_unknown_with_read_seq_id(ctx, pseudotax):
     with pytest.raises(sylph_b200.SylphError) as e:
         ctx.query(db, [smp], contain_params(pseudotax=False, estimate_unknown=1))
     assert e.value.code == 5                                          # SYL_ERR_UNSUPPORTED
+
+
+def test_sharded_profile_deep_coverage_on_one_gpu(ctx):
+    """A count >= 256 makes the three-collective sharded profile (world = 1) report SYL_ERR_UNSUPPORTED;
+    profile_sharded then takes profile_sharded_gather, whose query / profile calls run the CSR formulation.
+    The result must equal syl_profile field for field."""
+    from sylph_b200 import _lib
+    from sylph_b200 import dist as D
+    from sylph_b200.api import contain_params
+    g, _, _, smp = deep_coverage_case(ctx, 700)
+    db = ctx.build_db(g)
+    P = contain_params(pseudotax=True)
+    job = ctx.profile_shard_begin(db, [smp], P, 1, 0, 0)
+    try:
+        job.rank()
+        job.pass2()
+        _, rc, _ = job.finish()
+    finally:
+        job.free()
+    assert rc == _lib.SYL_ERR_UNSUPPORTED
+    exp = ctx.profile(db, [smp], P)
+    rows = D.profile_sharded(ctx, g, db, [smp], 0, P)
+    assert len(exp) >= 1 and len(rows) == len(exp)
+    for f in rows.dtype.names:
+        assert np.array_equal(rows[f], exp[f]), f
+
+
+@pytest.mark.parametrize("pseudotax", [False, True])
+def test_pass2_tie_goes_to_lowest_genome(ctx, pseudotax):
+    """Two genomes with the same statistics share half of their k-mers: their pass-1 ANIs are equal, and in pass 2
+    every shared k-mer goes to the lower genome index (the other one counts them as lost).  Both genome orders."""
+    rng = np.random.default_rng(77)
+    keys = rng.permutation(np.unique(rng.integers(1, 2**57, size=700, dtype=np.uint64)))[:600]
+    shared, ea, eb = keys[:200], keys[200:400], keys[400:600]
+    c_shared = rng.poisson(2.0, size=200).astype(np.uint32) + 1
+    c_own = rng.poisson(2.0, size=200).astype(np.uint32) + 1
+    sh = np.concatenate([shared, ea, eb])
+    sc = np.concatenate([c_shared, c_own, c_own])                 # the same count multiset for both genomes
+    smp = ctx.upload_sample(sh, sc)
+    for first, second in ((ea, eb), (eb, ea)):
+        kmers = np.concatenate([shared, first, shared, second])
+        koff = np.array([0, 400, 800], dtype=np.uint64)
+        d = dict(kmers=kmers, kmer_off=koff, tracked=np.zeros(0, np.uint64), tracked_off=np.zeros(3, np.uint64),
+                 gn_size=np.array([4000000, 4000000], dtype=np.uint64))
+        g = ctx.upload_genomes(d["kmers"], koff, d["tracked"], d["tracked_off"], d["gn_size"])
+        db = ctx.build_db(g)
+        exp = oracle_rows(d, (sh, sc), pseudotax)
+        rows = ctx.profile(db, [smp]) if pseudotax else sort_query_rows(ctx.query(db, [smp]))
+        compare(rows, exp, pseudotax)
+        if pseudotax:
+            assert [(e.genome, e.kmers_lost) for e in sorted(exp, key=lambda e: e.genome)] == [(0, 0), (1, 200)]
+
+
+def test_more_pairs_than_histograms_hold(ctx):
+    """More than 2^23 (sample, genome) pairs in one call: the per-pair count histograms would exceed 8 GB, so the
+    call runs in the CSR formulation from the start.  3 samples x 3 M genomes of 3 k-mers each; every genome a
+    sample hits yields a row (min_number_kmers = 1).  Rows == the oracle on the genomes that were hit."""
+    from sylph_b200.api import contain_params
+    rng = np.random.default_rng(23)
+    G, K = 3_000_000, 3
+    assert 3 * G > 2**23
+    kmers = rng.permutation(np.unique(rng.integers(1, 2**57, size=G * K + 100000, dtype=np.uint64)))[: G * K]
+    koff = np.arange(0, G * K + 1, K, dtype=np.uint64)
+    gs = np.full(G, 1000000, dtype=np.uint64)
+    g = ctx.upload_genomes(kmers, koff, np.zeros(0, np.uint64), np.zeros(G + 1, np.uint64), gs)
+    db = ctx.build_db(g)
+    hit = [np.sort(rng.choice(G, size=40, replace=False)) for _ in range(3)]
+    hit[1][:10] = hit[0][:10]                                        # genomes hit by two samples
+    samples = []
+    for h in hit:
+        take = [kmers[K * gi: K * gi + 1 + gi % K] for gi in h]     # 1..3 of the genome's k-mers
+        sh = np.concatenate(take + [rng.integers(2**57, 2**58, size=100, dtype=np.uint64)])
+        sc = rng.integers(1, 6, size=len(sh)).astype(np.uint32)
+        samples.append((sh, sc, ctx.upload_sample(sh, sc)))
+    hit_all = np.unique(np.concatenate(hit))
+    sub = dict(kmers=np.concatenate([kmers[K * gi: K * gi + K] for gi in hit_all]),
+               kmer_off=np.arange(0, K * len(hit_all) + 1, K, dtype=np.uint64),
+               tracked=np.zeros(0, np.uint64), tracked_off=np.zeros(len(hit_all) + 1, np.uint64), gn_size=gs[hit_all])
+    for pseudotax in (False, True):
+        P = contain_params(pseudotax=pseudotax, min_number_kmers=1.0)
+        handles = [s for _, _, s in samples]
+        rows = ctx.profile(db, handles, P) if pseudotax else ctx.query(db, handles, P)
+        assert np.isin(rows["genome"], hit_all).all()
+        n_rows = 0
+        for si, (sh, sc, _) in enumerate(samples):
+            sub_rows = rows[rows["sample"] == si].copy()
+            sub_rows["genome"] = np.searchsorted(hit_all, sub_rows["genome"])
+            if not pseudotax:
+                sub_rows = sort_query_rows(sub_rows)
+            exp = oracle_rows(sub, (sh, sc), pseudotax, min_number_kmers=1.0)
+            assert len(exp) == 40
+            compare(sub_rows, exp, pseudotax)
+            n_rows += len(exp)
+        assert n_rows == len(rows)
