@@ -3,17 +3,17 @@
 //   nvcc -gencode arch=compute_90a,code=sm_90a -O3 -std=c++17 --expt-relaxed-constexpr -o exp/hotloop_bench scripts/hotloop_bench.cu
 #include <cstdio>
 #include <vector>
-#include "../sylph_b200/csrc/seed_warp.cuh"
+#include "../sylph_b200/csrc/seed_kernel.cuh"
 
 using namespace syl;
 namespace syl { void set_error(const std::string &) {} thread_local syl_ctx *tl_ctx = nullptr; }
 
 // diagnostic variants of the loop body: which part of the per-window work costs what
-//   MODE 0 full (seedw_run)   1 hash only (operands from registers)   2 extraction + hash of the forward k-mer (no canonical)
+//   MODE 0 full (seed_run, the loop k_seed runs)   1 hash only (operands from registers)   2 extraction + hash of the forward k-mer (no canonical)
 //   3 full, canonical by 64-bit integer compare   4 full, FP64 compare + SEL instead of predicated IMAD
 template <int K, int W, int MODE>
-__device__ __forceinline__ uint32_t run_variant(const uint32_t *fw, const uint32_t *cwp, int p, uint32_t thr_hi, const ShiftMul smul) {
-    if (MODE == 0) return seedw_run<K, 0, W>(fw, cwp, p, thr_hi, smul);
+__device__ __forceinline__ uint32_t run_variant(const uint32_t *fw, const uint32_t *cwp, int p, uint32_t thr_hi, const ImadConst ic) {
+    if (MODE == 0) return seed_run<K, W>(fw, cwp, p, thr_hi, ic);
     constexpr uint32_t PAD = 64 - 2 * K;
     constexpr uint32_t HI_MASK = (1u << (32 - PAD)) - 1u;
     uint32_t F[4], G[4];
@@ -52,15 +52,15 @@ __device__ __forceinline__ uint32_t run_variant(const uint32_t *fw, const uint32
                 }
             }
         }
-        const uint32_t hh = hash_hi32<0>(c_lo, c_hi, smul);
+        const uint32_t hh = hash_hi32(c_lo, c_hi);
         asm("{\n\t.reg .pred p;\n\tsetp.le.u32 p, %1, %2;\n\t@p mad.lo.u32 %0, %3, %4, %0;\n\t}"
-            : "+r"(cand) : "r"(hh), "r"(thr_hi), "r"(smul.one), "r"(1u << i));
+            : "+r"(cand) : "r"(hh), "r"(thr_hi), "r"(ic.one), "r"(1u << i));
     }
     return cand;
 }
 
 template <int W, int MODE>
-__global__ void __launch_bounds__(256) k_hot(uint32_t *out, int iters, ShiftMul smul, uint32_t thr_hi) {
+__global__ void __launch_bounds__(256) k_hot(uint32_t *out, int iters, ImadConst ic, uint32_t thr_hi) {
     extern __shared__ uint32_t sm[];
     const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
     uint32_t *fw = sm + wid * 640, *cw = fw + 320;   // 320 words = 5120 bases per stream per warp
@@ -69,7 +69,7 @@ __global__ void __launch_bounds__(256) k_hot(uint32_t *out, int iters, ShiftMul 
     uint32_t acc = 0;
     int p = lane * W;
     for (int it = 0; it < iters; it++) {
-        acc ^= run_variant<31, W, MODE>(fw, cw, p, thr_hi, smul);
+        acc ^= run_variant<31, W, MODE>(fw, cw, p, thr_hi, ic);
         p += 32 * W;
         if (p > 4096) p -= 4096;
     }
@@ -80,12 +80,12 @@ int main() {
     cudaDeviceProp prop; cudaGetDeviceProperties(&prop, 0);
     const int sms = prop.multiProcessorCount;
     uint32_t *out; cudaMalloc(&out, (size_t)sms * 8 * 256 * 4 * 2);
-    const ShiftMul smul = {1u << 8, 1u << 18, 1u << 4, 1u, 0u};
+    const ImadConst ic = {{0u, 0u, 0u}, 1u, 0u};
     const uint32_t thr_hi = 0x0147AE14u;
     const int iters = 2000;
     cudaEvent_t e0, e1; cudaEventCreate(&e0); cudaEventCreate(&e1);
     printf("device %s, %d SMs\n", prop.name, sms);
-    typedef void (*kern_t)(uint32_t *, int, ShiftMul, uint32_t);
+    typedef void (*kern_t)(uint32_t *, int, ImadConst, uint32_t);
     struct V { const char *name; kern_t k; int W; };
     const V vs[] = {{"W=30 full", k_hot<30, 0>, 30}, {"W=32 full", k_hot<32, 0>, 32}, {"W=30 hash only", k_hot<30, 1>, 30},
                     {"W=30 extract fwd + hash (no canonical)", k_hot<30, 2>, 30}, {"W=30 full, integer compare", k_hot<30, 3>, 30},
@@ -99,7 +99,7 @@ int main() {
             float best = 1e9f;
             for (int rep = 0; rep < 4; rep++) {
                 cudaEventRecord(e0);
-                v.k<<<grid, 256, smem>>>(out, iters, smul, thr_hi);
+                v.k<<<grid, 256, smem>>>(out, iters, ic, thr_hi);
                 cudaEventRecord(e1);
                 cudaEventSynchronize(e1);
                 float ms; cudaEventElapsedTime(&ms, e0, e1);

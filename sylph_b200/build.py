@@ -16,8 +16,6 @@ OBJ = os.path.join(HERE, "build")
 SO = os.path.join(HERE, "libsylph_b200.so")
 HEADER = os.path.join(HERE, "..", "include", "sylph_b200.h")
 SOURCES = ["api.cu", "seed.cu", "seed_k31_sv.cu", "seed_k31_ev.cu", "seed_k21_sv.cu", "seed_k21_ev.cu",
-           "seedw_k31_sv.cu", "seedw_k31_ev.cu", "seedw_k21_sv.cu", "seedw_k21_ev.cu",
-           "seedw_k31_sv_p.cu", "seedw_k31_ev_p.cu", "seedw_k21_sv_p.cu", "seedw_k21_ev_p.cu",
            "sample.cu", "genome.cu", "contain.cu", "host_pack.cpp"]
 CXX_FLAGS = ["-O3", "-std=c++17", "-fPIC", "-pthread"]
 NVCC_FLAGS = [
@@ -26,8 +24,8 @@ NVCC_FLAGS = [
 ]
 
 
-# tuning experiments: extra -D flags and an alternative output name (SYL_BUILD_DEFS="-DSEEDW_TW=2048 -DSEEDW_MINB=4"
-# SYL_BUILD_TAG=tw2048 -> libsylph_b200_tw2048.so, objects under build_tw2048/), loaded with SYLPH_B200_LIB
+# tuning experiments: extra -D flags and an alternative output name (SYL_BUILD_DEFS="-DSEED_MINB_CFG=3"
+# SYL_BUILD_TAG=minb3 -> libsylph_b200_minb3.so, objects under build_minb3/), loaded with SYLPH_B200_LIB
 EXTRA_NVCC = os.environ.get("SYL_BUILD_DEFS", "").split()
 _TAG = os.environ.get("SYL_BUILD_TAG", "")
 if _TAG:

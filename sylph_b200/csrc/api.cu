@@ -237,7 +237,6 @@ static int seed_batch_impl(syl_ctx *ctx, int mem, const uint8_t *bases, const ui
     job.d_rec_off = so.p; job.off_bias = 0; job.n_rec = n_rec; job.k = k; job.c = c; job.sem = sem; job.with_pos = with_pos;
     job.d_out = dst; job.cap = cap;
     job.d_count = reinterpret_cast<unsigned long long *>(ctx->d_counters);
-    job.d_pend_count = job.d_count + 1;
     SYL_CUDA(cudaMemsetAsync(ctx->d_counters, 0, 2 * sizeof(uint64_t), st));
     SYL_TRY(seed_enqueue(ctx, job));
     SYL_CUDA(cudaMemcpyAsync(ctx->h_counters, ctx->d_counters, sizeof(uint64_t), cudaMemcpyDeviceToHost, st));

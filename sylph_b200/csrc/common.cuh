@@ -174,14 +174,13 @@ struct SeedJob {
     uint32_t *d_group_cnt = nullptr;      // events: post-pass group counters (GroupOut in seed_kernel.cuh); nullptr = append
     uint64_t Mb = 0;
     uint32_t nbk = 0, ng = 0, slot = 0;
-    unsigned long long *d_count = nullptr, *d_pend_count = nullptr;  // running device counters
-    // slotted survivor output (genome sketching, CTA kernel only): see SlotOut in seed_kernel.cuh
+    unsigned long long *d_count = nullptr;  // running device counters: [0] survivors / events, [1] pending events
+    // slotted survivor output (genome sketching): see SlotOut in seed_kernel.cuh
     uint32_t slot_cap = 0;
     uint32_t *d_tile_cnt = nullptr, *d_slot_overflow = nullptr;
 };
-uint64_t seed_cta_tiles(uint64_t n_bases);  // number of tiles of the CTA kernel
-uint64_t seed_cta_tile_bases();             // window starts per tile of the CTA kernel
-bool seed_cta_kernel_selected();            // false when SYL_SEED_IMPL=warp forces the warp kernel
+uint64_t seed_cta_tiles(uint64_t n_bases);  // number of tiles of the seeding kernel
+uint64_t seed_cta_tile_bases();             // window starts per tile of the seeding kernel
 int seed_enqueue(syl_ctx *ctx, const SeedJob &job);
 void ingest_destroy(syl_ctx *ctx);
 

@@ -199,7 +199,7 @@ static int genomes_alloc(syl_genomes *g, cudaStream_t st, uint64_t n_genomes, ui
 }
 
 // Generic post-pass: two library radix sorts (position, then hash).  Handles every input; used when the
-// slotted path below does not apply (tiny c, SYL_SEED_IMPL=warp, SYL_GENOME_POSTPASS=sort) or reports an overflow.
+// slotted path below does not apply (tiny c, SYL_GENOME_POSTPASS=sort) or reports an overflow.
 static int sketch_genomes_device_sort(syl_ctx *ctx, const uint8_t *d_bases, uint64_t n_bases, const uint64_t *d_contig_off,
                                       uint64_t n_contigs, const uint64_t *d_genome_off, uint64_t n_genomes, int k, uint64_t c,
                                       uint64_t min_spacing, int pseudotax, int sem, syl_genomes *out) {
@@ -477,7 +477,6 @@ static int sketch_genomes_device_slots(syl_ctx *ctx, const uint8_t *d_bases, uin
     job.d_bases = d_bases; job.n_bases = n_bases; job.d_rec_off = d_contig_off; job.off_bias = 0; job.n_rec = n_contigs;
     job.k = k; job.c = c; job.sem = sem; job.with_pos = 1; job.d_out = slots.p; job.cap = n_tiles * GEN_SLOT;
     job.d_count = reinterpret_cast<unsigned long long *>(ctx->d_counters);
-    job.d_pend_count = job.d_count + 1;
     job.slot_cap = GEN_SLOT; job.d_tile_cnt = tile_cnt.p; job.d_slot_overflow = flags32.p;
     SYL_TRY(seed_enqueue(ctx, job));
     KernelTimer kt_post(ctx, SYL_KERNEL_GENOME_POST);
@@ -540,7 +539,7 @@ int sketch_genomes_device(syl_ctx *ctx, const uint8_t *d_bases, uint64_t n_bases
     const char *e = getenv("SYL_GENOME_POSTPASS");  // "sort" forces the generic path (tests); read per call
     const bool force_sort = e && std::string(e) == "sort";
     // slots hold 512 survivors per 32K-base tile: c >= 96 keeps the expected number below 350
-    if (!force_sort && c >= 96 && seed_cta_kernel_selected() && n_bases && n_contigs && n_genomes) {
+    if (!force_sort && c >= 96 && n_bases && n_contigs && n_genomes) {
         const int rc = sketch_genomes_device_slots(ctx, d_bases, n_bases, d_contig_off, n_contigs, d_genome_off, n_genomes, k, c,
                                                    min_spacing, pseudotax, sem, out);
         if (rc != SYL_ERR_UNSUPPORTED) return rc;

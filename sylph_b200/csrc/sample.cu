@@ -684,7 +684,7 @@ struct SampleBuilder {
         job.d_bases = d_bases; job.d_packed = d_packed; job.n_bases = nb; job.d_rec_off = d_off; job.off_bias = off_bias;
         job.n_rec = nr; job.k = k; job.c = c; job.sem = sem; job.with_pos = 0; job.d_out = b_ev.p; job.cap = cap;
         job.emit_events = 1; job.rec_base = rec_base; job.no_dedup = paired ? 2 : no_dedup; job.d_pend = b_pend.p;
-        job.d_group_cnt = g_cnt.p; job.Mb = Mb; job.nbk = nbk; job.ng = ng; job.slot = slot; job.d_count = dc; job.d_pend_count = dc + 1;
+        job.d_group_cnt = g_cnt.p; job.Mb = Mb; job.nbk = nbk; job.ng = ng; job.slot = slot; job.d_count = dc;
         SYL_TRY(seed_enqueue(ctx, job));
         if (!no_dedup && !paired && nb) {  // reads cut by a tile edge: their pair keys come from global memory
             const uint64_t n_words = (nb + 15) / 16;

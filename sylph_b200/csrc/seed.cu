@@ -5,9 +5,11 @@
 //   extract_markers_positions  (src/sketch.rs:71-93  -> src/avx2_seeding.rs:151-266 / src/seeding.rs:148-209)
 //
 // Formulation (nothing here mirrors the AVX2 traversal; only its window *set* is kept):
-//   * the batch is one flat ASCII buffer; a CTA owns a tile of SEED_TILE window-start positions
+//   * the batch is one flat buffer, ASCII or 2-bit packed; a CTA owns a tile of SEED_TILE window-start
+//     positions (seed_kernel.cuh, k_seed)
 //   * the tile (+halo) is staged HBM -> shared memory with one TMA bulk copy (cp.async.bulk +
-//     mbarrier complete_tx), then packed ONCE into two 2-bit streams:
+//     mbarrier complete_tx), then packed ONCE into two 2-bit streams (2-bit input: the forward
+//     stream is the staged words):
 //        fw: forward codes, MSB-first     -> forward k-mer of any window = one 64-bit funnel extract
 //        cw: complement codes, LSB-first  -> reverse-complement k-mer  = one 64-bit funnel extract
 //     so windows are independent (no serial roll, no per-window byte loads)
@@ -19,11 +21,9 @@
 //     3 ALU-pipe xor-shifts), one compare of the high word against the threshold
 //   * survivors (1/c of windows) are staged in shared memory and flushed with one global
 //     atomic per CTA
-#include <algorithm>
 #include <cstdlib>
-#include <cstring>
 
-#include "seed_warp.cuh"
+#include "seed_kernel.cuh"
 
 namespace syl {
 
@@ -65,45 +65,16 @@ static int pick_run_length(uint64_t mean_len, int k, int sem, int with_pos) {
     return best;
 }
 
-// Tile length of the warp kernel.  A warp processes a tile's runs 32 at a time, and a partially filled
-// round costs as many issue slots as a full one, so the tile is sized to hold just under 32 r runs
-// (r rounds): runs per base follow from the mean record length; two runs of slack absorb the partial
-// runs of the records cut by the tile's two edges.  SYL_SEED_TW forces a length (tests, tuning).
-static uint32_t pick_warp_tile(uint64_t mean_len, int k, int sem, int with_pos, int W) {
-    const char *fe = getenv("SYL_SEED_TW");  // read per call: the tests switch it at run time
-    const int forced = fe ? atoi(fe) : 0;
-    if (forced >= 64) return (uint32_t)std::min(forced & ~63, SW_TW & ~63);  // multiples of 64 bases: 16-byte aligned 2-bit tiles
-    const uint64_t w = valid_windows(mean_len, (uint32_t)k, sem, with_pos);
-    if (mean_len == 0 || w == 0) return (uint32_t)(SW_TW & ~63);
-    double runs_per_base;
-    if (mean_len > 2048) runs_per_base = 1.0 / W;                       // long records: windows ~ bases
-    else runs_per_base = (double)((w + W - 1) / W) / (double)mean_len;  // short reads: whole runs per read
-    for (int r = 8; r >= 1; r--) {
-        const double tw = (32.0 * r - 2.0) / runs_per_base;
-        if (tw <= (double)SW_TW) return (uint32_t)std::max(64, (int)tw & ~63);
-    }
-    return (uint32_t)(SW_TW & ~63);
-}
-
-// Two formulations of the kernel (same arithmetic, same results):
-//   cta  (default for ASCII input): one 32K tile per CTA, phases separated by CTA-wide barriers (seed_kernel.cuh)
-//   warp (SYL_SEED_IMPL=warp; always for 2-bit packed input): warp-autonomous persistent kernel (seed_warp.cuh)
-// Measured on 1 Gbp of 150 bp reads (one H100 SXM, 400 W): cta 1.6-1.9 ms, warp 2.58 ms; the hot loop alone
+// Measured on 1 Gbp of 150 bp reads (one H100 SXM, 400 W): k_seed 1.6-1.9 ms; the hot loop alone
 // (scripts/hotloop_bench.cu) sustains 0.66 T windows/s = 1.22 ms for the same windows, so the phases around
-// the loop cost about 0.4-0.5 ms of the CTA kernel.
-static bool use_warp_kernel() {
-    const char *e = getenv("SYL_SEED_IMPL");  // read per call: the tests switch it at run time
-    return e && strcmp(e, "warp") == 0;
-}
-
+// the loop cost about 0.4-0.5 ms of the kernel.
 uint64_t seed_cta_tiles(uint64_t n_bases) { return (n_bases + SEED_TILE - 1) / SEED_TILE; }
 uint64_t seed_cta_tile_bases() { return SEED_TILE; }
-bool seed_cta_kernel_selected() { return !use_warp_kernel(); }
 
 // Enqueue the seeding of one batch on the ctx stream.  No host synchronisation and no counter reset:
-// survivors / events are appended to job.d_out at the running device counter *job.d_count (entries
+// survivors / events are appended to job.d_out at the running device counter job.d_count[0] (entries
 // past job.cap are counted but dropped; the caller compares the final count with cap), pending
-// event indices at *job.d_pend_count.
+// event indices at job.d_count[1].
 int seed_enqueue(syl_ctx *ctx, const SeedJob &job) {
     if (job.emit_events && (!job.d_pend || job.cap >= 0xFFFFFFFFull)) { set_error("event emission needs a pending list and cap < 2^32"); return SYL_ERR_ARG; }
     if (job.c == 0) { set_error("c must be >= 1"); return SYL_ERR_ARG; }
@@ -119,66 +90,34 @@ int seed_enqueue(syl_ctx *ctx, const SeedJob &job) {
         set_error("device base buffer must be 16-byte aligned (TMA bulk copy)");
         return SYL_ERR_ARG;
     }
-    const bool warp = use_warp_kernel() || job.d_packed != nullptr;
-    if (job.slot_cap && warp) { set_error("internal: slotted output needs the CTA kernel"); return SYL_ERR_ARG; }
+    const bool packed = job.d_packed != nullptr;
     cudaStream_t st = ctx->stream;
     // Run length: every record is cut into runs of W windows and a thread always pays for a full
     // run, so for fixed-length reads W should divide the per-read window count (150 bp, k=31:
     // 120 windows = 4 x 30).  Chosen from the mean record length; long records get 32.
-    const uint64_t mean_len = job.n_bases / job.n_rec;
-    const int W = pick_run_length(mean_len, job.k, job.sem, job.with_pos);
-    const uint64_t tile = warp ? (uint64_t)pick_warp_tile(mean_len, job.k, job.sem, job.with_pos, W) : (uint64_t)SEED_TILE;
-    const uint64_t n_tiles = (job.n_bases + tile - 1) / tile;
+    const int W = pick_run_length(job.n_bases / job.n_rec, job.k, job.sem, job.with_pos);
+    const uint64_t n_tiles = seed_cta_tiles(job.n_bases);
     DevBuf<uint32_t> tile_rec;
     SYL_TRY(tile_rec.alloc(n_tiles + 1, st));
     {
         const int bs = 256;
         const uint64_t nb = (n_tiles + 1 + bs - 1) / bs;
-        k_tile_first_rec<<<(unsigned)nb, bs, 0, st>>>(job.d_rec_off, job.off_bias, job.n_rec, n_tiles, tile, tile_rec.p);
+        k_tile_first_rec<<<(unsigned)nb, bs, 0, st>>>(job.d_rec_off, job.off_bias, job.n_rec, n_tiles, SEED_TILE, tile_rec.p);
         ctx->launches++;
     }
     const uint64_t thr = fmh_threshold(job.c);
-    const ShiftMul smul = {1u << 8, 1u << 18, 1u << 4, 1u, 0u};
+    const ImadConst ic = {{0u, 0u, 0u}, 1u, 0u};
     const GroupOut go{job.emit_events ? job.d_group_cnt : nullptr, job.Mb, job.nbk, job.ng, job.slot};
-    if (!warp) {
-        if (job.d_pend_count != job.d_count + 1) { set_error("internal: cta kernel expects adjacent counters"); return SYL_ERR_ARG; }
-        const size_t smem = sizeof(SeedSmem);
-        const seed_kern_t kern = job.emit_events ? (job.k == 31 ? seed_kernels_k31_ev(W) : seed_kernels_k21_ev(W))
-                                                 : (job.k == 31 ? seed_kernels_k31_sv(W) : seed_kernels_k21_sv(W));
-        SYL_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        KernelTimer kt(ctx, SYL_KERNEL_SEED);
-        const SlotOut slot{job.emit_events ? 0u : job.slot_cap, job.d_tile_cnt, job.d_slot_overflow};
-        kern<<<(unsigned)n_tiles, SEED_THREADS, smem, st>>>(
-            job.d_bases, job.n_bases, job.d_rec_off, job.off_bias, tile_rec.p, thr, job.sem, job.with_pos, job.d_out,
-            slot.cap ? 0 : job.cap, job.d_count, smul, job.rec_base, job.no_dedup, job.d_pend, go, slot);
-        kt.stop();
-    } else {
-        const bool pk = job.d_packed != nullptr;
-        seedw_kern_t kern;
-        if (pk) kern = job.emit_events ? (job.k == 31 ? seedw_kernels_k31_ev_p(W) : seedw_kernels_k21_ev_p(W))
-                                       : (job.k == 31 ? seedw_kernels_k31_sv_p(W) : seedw_kernels_k21_sv_p(W));
-        else kern = job.emit_events ? (job.k == 31 ? seedw_kernels_k31_ev(W) : seedw_kernels_k21_ev(W))
-                                    : (job.k == 31 ? seedw_kernels_k31_sv(W) : seedw_kernels_k21_sv(W));
-        const size_t smem = pk ? seedw_smem_bytes<true>() : seedw_smem_bytes<false>();
-        SYL_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        int per_sm = 0;
-        SYL_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, SW_THREADS, smem));
-        if (per_sm < 1) { set_error("seeding kernel does not fit on an SM"); return SYL_ERR_CUDA; }
-        static const int force_ctas = []() { const char *e = getenv("SYL_SEED_CTAS_PER_SM"); return e ? atoi(e) : 0; }();
-        if (force_ctas > 0) per_sm = std::min(per_sm, force_ctas);
-        uint64_t grid = (uint64_t)per_sm * ctx->num_sms;
-        grid = std::min<uint64_t>(grid, (n_tiles + SW_WARPS - 1) / SW_WARPS);
-        unsigned long long *d_tile = reinterpret_cast<unsigned long long *>(ctx->d_counters + 16);
-        SYL_CUDA(cudaMemsetAsync(d_tile, 0, 8, st));
-        SeedWArgs A;
-        A.bases = job.d_bases; A.packed = job.d_packed; A.n_bases = job.n_bases; A.rec_off = job.d_rec_off;
-        A.off_bias = job.off_bias; A.tile_rec = tile_rec.p; A.n_tiles = n_tiles; A.tw = (uint32_t)tile; A.thr = thr; A.sem = job.sem;
-        A.with_pos = job.with_pos; A.out = job.d_out; A.cap = job.cap; A.g_count = job.d_count; A.g_pend = job.d_pend_count;
-        A.g_tile = d_tile; A.smul = smul; A.rec_base = job.rec_base; A.no_dedup = job.no_dedup; A.pend = job.d_pend; A.go = go;
-        KernelTimer kt(ctx, SYL_KERNEL_SEED);
-        kern<<<(unsigned)grid, SW_THREADS, smem, st>>>(A);
-        kt.stop();
-    }
+    const SlotOut slot{job.emit_events ? 0u : job.slot_cap, job.d_tile_cnt, job.d_slot_overflow};
+    const size_t smem = sizeof(SeedSmem);
+    const seed_kern_t kern = job.emit_events ? (job.k == 31 ? seed_kernels_k31_ev(W, packed) : seed_kernels_k21_ev(W, packed))
+                                             : (job.k == 31 ? seed_kernels_k31_sv(W, packed) : seed_kernels_k21_sv(W, packed));
+    SYL_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    KernelTimer kt(ctx, SYL_KERNEL_SEED);
+    kern<<<(unsigned)n_tiles, SEED_THREADS, smem, st>>>(
+        reinterpret_cast<const uint8_t *>(in), job.n_bases, job.d_rec_off, job.off_bias, tile_rec.p, thr, job.sem, job.with_pos,
+        job.d_out, slot.cap ? 0 : job.cap, job.d_count, ic, job.rec_base, job.no_dedup, job.d_pend, go, slot);
+    kt.stop();
     if (ctx->timing) ctx->seed_bases += job.n_bases;
     ctx->launches++;
     SYL_CUDA(cudaGetLastError());
@@ -198,7 +137,6 @@ int seed_device(syl_ctx *ctx, const uint8_t *d_bases, uint64_t n_bases, const ui
     job.d_bases = d_bases; job.n_bases = n_bases; job.d_rec_off = d_rec_off; job.off_bias = off_bias; job.n_rec = n_rec;
     job.k = k; job.c = c; job.sem = sem; job.with_pos = with_pos; job.d_out = d_out; job.cap = cap;
     job.d_count = reinterpret_cast<unsigned long long *>(ctx->d_counters);
-    job.d_pend_count = job.d_count + 1;
     SYL_CUDA(cudaMemsetAsync(ctx->d_counters, 0, 2 * sizeof(uint64_t), st));
     SYL_TRY(seed_enqueue(ctx, job));
     SYL_CUDA(cudaMemcpyAsync(ctx->h_counters, ctx->d_counters, sizeof(uint64_t), cudaMemcpyDeviceToHost, st));

@@ -1,4 +1,4 @@
-// k_seed<K=31, EMIT=1> for run lengths 24 / 30 / 32 (EMIT 0: 16-byte survivors, 1: 32-byte read-sketch events)
+// k_seed<K=31, EMIT=1> for run lengths 24 / 30 / 32, ASCII and 2-bit input (EMIT 0: 16-byte survivors, 1: 32-byte read-sketch events)
 #include "seed_kernel.cuh"
 
 namespace syl {

@@ -8,9 +8,6 @@ constexpr int SEED_THREADS = 256;
 #ifndef SEED_TILE_CFG
 #define SEED_TILE_CFG 32768
 #endif
-#ifndef SEED_CANON_MODE
-#define SEED_CANON_MODE 3  // 0 integer compare; 1 FP64 compare + SEL; 2 FP64 compare + predicated IMAD moves; 3 = 2 + candidate bit by predicated IMAD
-#endif
 #ifndef SEED_MINB_CFG
 #define SEED_MINB_CFG 4
 #endif
@@ -27,10 +24,12 @@ constexpr int SEED_ASC_BYTES = SEED_TILE + SEED_HALO;  // 32816, multiple of 16
 constexpr int SEED_NCHUNK16 = SEED_ASC_BYTES / 16;     // 2051 16-base words per stream
 constexpr int SEED_FW_WORDS = SEED_NCHUNK16 + 1 + 8;   // +1 leading pad word, +8 slack for run loads
 constexpr int SEED_CW_WORDS = SEED_NCHUNK16 + 8;
+constexpr int SEED_PK_WORDS = (SEED_NCHUNK16 + 3) & ~3;  // 2-bit input: words staged per tile (whole 16-byte groups)
+static_assert(SEED_TILE % 64 == 0, "2-bit tiles must start on 16-byte boundaries");
 
 struct SeedSmem {
-    // region A: ASCII staging; after packing it is reused for the per-chunk record table and
-    // the survivor staging buffer (see offsets below)
+    // region A: staging of the ASCII bytes (or, for 2-bit input, of the packed words); after packing
+    // it is reused for the per-chunk record table and the survivor staging buffer (see offsets below)
     alignas(128) uint8_t asc[SEED_ASC_BYTES + 16];
     alignas(16) uint32_t fw[SEED_FW_WORDS];
     alignas(16) uint32_t cw[SEED_CW_WORDS];
@@ -84,15 +83,17 @@ struct GroupOut {
     }
 };
 
-// Multipliers 2^(32-s) for the three xor-shift distances, passed as kernel parameters so that
-// ptxas cannot strength-reduce "mul.hi by a power of two" back into an ALU-pipe shift.
-struct ShiftMul { uint32_t m24, m14, m28, one, zero; };
+// The constants 1 and 0, passed as kernel parameters so that ptxas cannot fold the hot loop's
+// predicated IMADs (x * one + zero) back into ALU-pipe moves.  The padding keeps k_seed's parameter
+// offsets where its register allocation was tuned: ptxas allocates differently without it, and the
+// W = 24 kernels then spill 8-12 bytes.
+struct ImadConst { uint32_t pad_[3], one, zero; };
 
 // Slotted survivor output (genome sketching): tile t writes its survivors to out[t * cap ..) and their
 // number to tile_cnt[t] instead of appending at a global counter, so that the output is already in tile
 // (= position) order and no global sort is needed.  cap == 0: off.  A tile with more survivors than the
 // slot (or the CTA's staging buffer) holds raises *overflow; the caller then takes the generic path.
-struct SlotOut { uint32_t cap; uint32_t *tile_cnt; uint32_t *overflow; };  // = 1<<8, 1<<18, 1<<4, 1, 0 (opaque to ptxas)
+struct SlotOut { uint32_t cap; uint32_t *tile_cnt; uint32_t *overflow; };
 
 // 64-bit multiply by a 32-bit constant as IMAD.WIDE + IMAD (2 FMA-pipe instructions)
 __device__ __forceinline__ void mul64c(uint32_t lo, uint32_t hi, uint32_t c, uint32_t &plo, uint32_t &phi) {
@@ -102,14 +103,10 @@ __device__ __forceinline__ void mul64c(uint32_t lo, uint32_t hi, uint32_t c, uin
     asm("mad.lo.u32 %0, %1, %2, %3;" : "=r"(phi) : "r"(hi), "r"(c), "r"((uint32_t)(t >> 32)));
 }
 
-// x ^= x >> s on halves. VAR 0: 2 SHF + 2 LOP3 (ALU pipe). VAR 1: the high-word shift is an
-// IMAD.HI (FMA pipe). VAR 2: the funnel shift of the low word also goes to the FMA pipe
-// (IMAD.HI + IMAD). The ALU pipe issues one warp instruction every 2 cycles and is the limiter.
-template <int VAR, int SH>
-__device__ __forceinline__ void xorshift(uint32_t &lo, uint32_t &hi, uint32_t mul, uint32_t extra_hi) {
-    uint32_t sl, sh;
-    if (VAR >= 1) sh = __umulhi(hi, mul); else sh = hi >> SH;
-    if (VAR >= 2) sl = __umulhi(lo, mul) + hi * mul; else sl = __funnelshift_r(lo, hi, SH);
+// x ^= x >> s on halves: 2 SHF + 2 LOP3 (ALU pipe)
+template <int SH>
+__device__ __forceinline__ void xorshift(uint32_t &lo, uint32_t &hi, uint32_t extra_hi) {
+    const uint32_t sh = hi >> SH, sl = __funnelshift_r(lo, hi, SH);
     lo ^= sl;
     hi = hi ^ sh ^ extra_hi;
 }
@@ -119,15 +116,14 @@ __device__ __forceinline__ void xorshift(uint32_t &lo, uint32_t &hi, uint32_t mu
 //       (X ^ X>>24).lo = x.lo ^ (x>>24).lo            (the complements cancel)
 //       (X ^ X>>24).hi = x.hi ^ (x.hi>>24) ^ 0xFFFFFF00
 //   * only the high word of the last multiply is formed; survivors re-derive the full hash
-template <int VAR>
-__device__ __forceinline__ uint32_t hash_hi32(uint32_t lo, uint32_t hi, const ShiftMul sm) {
+__device__ __forceinline__ uint32_t hash_hi32(uint32_t lo, uint32_t hi) {
     uint32_t a, b;
     mul64c(lo, hi, 0x200001u, a, b);
-    xorshift<VAR, 24>(a, b, sm.m24, 0xFFFFFF00u);
+    xorshift<24>(a, b, 0xFFFFFF00u);
     mul64c(a, b, 265u, lo, hi);
-    xorshift<VAR, 14>(lo, hi, sm.m14, 0u);
+    xorshift<14>(lo, hi, 0u);
     mul64c(lo, hi, 21u, a, b);
-    xorshift<VAR, 28>(a, b, sm.m28, 0u);
+    xorshift<28>(a, b, 0u);
     return __umulhi(a, 0x80000001u) + b * 0x80000001u;
 }
 
@@ -140,6 +136,57 @@ __device__ __forceinline__ uint64_t fw64(const SeedSmem &S, uint32_t q) {
     const uint32_t bitpos = 32u + 2u * q, w = bitpos >> 5, sh = bitpos & 31u;
     const uint32_t a = S.fw[w], b = S.fw[w + 1], c = S.fw[w + 2];
     return ((uint64_t)__funnelshift_l(b, a, sh) << 32) | __funnelshift_l(c, b, sh);
+}
+
+// The hot loop: one run of W windows starting at tile-relative window start p of the streams fw / cw.
+// Returns the candidate mask (bit i: the high word of window p+i's hash is <= thr_hi).  Only the high
+// word of the hash is formed; candidates (1/c of windows) are collected in a bit mask, so the loop
+// has no divergent code.
+template <int K, int W>
+__device__ __forceinline__ uint32_t seed_run(const uint32_t *fw, const uint32_t *cw, int p, uint32_t thr_hi, const ImadConst ic) {
+    constexpr uint32_t PAD = 64 - 2 * K;                     // unused high bits of a k-mer word
+    constexpr uint32_t HI_MASK = (1u << (32 - PAD)) - 1u;    // K=31: 0x3FFFFFFF, K=21: 0x3FF
+    // realign the two streams so that window i of this run starts at bit 2i
+    uint32_t F[4], G[4];
+    {
+        const uint32_t bitpos = 32u + 2u * (uint32_t)p - PAD;
+        const uint32_t q0 = bitpos >> 5, sh = bitpos & 31u;
+        uint32_t w0 = fw[q0], w1 = fw[q0 + 1], w2 = fw[q0 + 2], w3 = fw[q0 + 3], w4 = fw[q0 + 4];
+        F[0] = __funnelshift_l(w1, w0, sh);
+        F[1] = __funnelshift_l(w2, w1, sh);
+        F[2] = __funnelshift_l(w3, w2, sh);
+        F[3] = __funnelshift_l(w4, w3, sh);
+        const uint32_t cq = (uint32_t)p >> 4, csh = ((uint32_t)p & 15u) * 2u;
+        uint32_t c0 = cw[cq], c1 = cw[cq + 1], c2 = cw[cq + 2], c3 = cw[cq + 3], c4 = cw[cq + 4];
+        G[0] = __funnelshift_r(c0, c1, csh);
+        G[1] = __funnelshift_r(c1, c2, csh);
+        G[2] = __funnelshift_r(c2, c3, csh);
+        G[3] = __funnelshift_r(c3, c4, csh);
+    }
+    uint32_t cand = 0u;
+#pragma unroll
+    for (int i = 0; i < W; i++) {
+        const int jb = (2 * i) >> 5;
+        const uint32_t sft = (uint32_t)((2 * i) & 31);
+        const uint32_t f_hi = __funnelshift_l(F[jb + 1], F[jb], sft) & HI_MASK;
+        const uint32_t f_lo = __funnelshift_l(F[jb + 2], F[jb + 1], sft);
+        const uint32_t r_lo = __funnelshift_r(G[jb], G[jb + 1], sft);
+        const uint32_t r_hi = __funnelshift_r(G[jb + 1], G[jb + 2], sft) & HI_MASK;
+        // canonical k-mer = min(forward, reverse complement), src/seeding.rs:131-136.  Both are
+        // < 2^62, so as IEEE doubles they are finite, non-negative and ordered like the
+        // integers: ONE compare on the FP64 pipe replaces the two-instruction 64-bit integer
+        // compare on the ALU pipe, which is this loop's limiter.  The select is a pair of
+        // predicated IMADs (FMA pipe).
+        uint32_t c_lo = r_lo, c_hi = r_hi;
+        asm("{\n\t.reg .pred p;\n\t.reg .f64 a, b;\n\tmov.b64 a, {%2, %3};\n\tmov.b64 b, {%4, %5};\n\t"
+            "setp.lt.f64 p, a, b;\n\t@p mad.lo.u32 %0, %2, %6, %7;\n\t@p mad.lo.u32 %1, %3, %6, %7;\n\t}"
+            : "+r"(c_lo), "+r"(c_hi) : "r"(f_lo), "r"(f_hi), "r"(r_lo), "r"(r_hi), "r"(ic.one), "r"(ic.zero));
+        const uint32_t hh = hash_hi32(c_lo, c_hi);
+        // candidate bit set by a predicated IMAD (FMA pipe): the bits are distinct, so add == or
+        asm("{\n\t.reg .pred p;\n\tsetp.le.u32 p, %1, %2;\n\t@p mad.lo.u32 %0, %3, %4, %0;\n\t}"
+            : "+r"(cand) : "r"(hh), "r"(thr_hi), "r"(ic.one), "r"(1u << i));
+    }
+    return cand;
 }
 
 // Exact re-derivation of one candidate window: k-mer halves from the packed streams at an arbitrary
@@ -212,28 +259,34 @@ __device__ __forceinline__ void seed_resolve(const SeedSmem &S, SeedMeta &M, uin
     }
 }
 
-template <int K, int VAR, int EMIT, int W>
+// PACKED: the input is 2-bit codes (16 bases per little-endian u32, base 16w+j in bits [30-2j, 31-2j],
+// i.e. exactly the forward stream), made by the host packer (host_pack.cpp) from the reference's
+// BYTE_TO_SEQ table.  The staging copies a quarter of the bytes and the pack phase shrinks to the
+// complement stream; everything after it is the same as for ASCII input.
+template <int K, int EMIT, int W, bool PACKED>
 __global__ void __launch_bounds__(SEED_THREADS, SEED_MINB_CFG)
 k_seed(const uint8_t *__restrict__ bases, uint64_t n_bases, const uint64_t *__restrict__ rec_off, uint64_t off_bias,
        const uint32_t *__restrict__ tile_rec, uint64_t thr, int sem, int with_pos,
        void *__restrict__ out, uint64_t cap, unsigned long long *__restrict__ g_count,
-       const ShiftMul smul, uint64_t rec_base, int no_dedup, uint32_t *__restrict__ pend, const GroupOut go, const SlotOut slot) {
+       const ImadConst ic, uint64_t rec_base, int no_dedup, uint32_t *__restrict__ pend, const GroupOut go, const SlotOut slot) {
     static_assert(W >= SEED_W_MIN && W <= SEED_W_MAX, "run length");
     extern __shared__ __align__(128) uint8_t smem_raw[];
     SeedSmem &S = *reinterpret_cast<SeedSmem *>(smem_raw);
     SeedMeta &M = *reinterpret_cast<SeedMeta *>(S.asc);
 
-    constexpr uint32_t PAD = 64 - 2 * K;                     // unused high bits of a k-mer word
-    constexpr uint32_t HI_MASK = (1u << (32 - PAD)) - 1u;    // K=31: 0x3FFFFFFF, K=21: 0x3FF
     const int tid = threadIdx.x;
     const uint64_t T0 = (uint64_t)blockIdx.x * SEED_TILE;
     const uint64_t T1 = T0 + SEED_TILE;
     const uint32_t thr_hi = (uint32_t)(thr >> 32);
 
-    // ---- stage the tile: TMA bulk copy for the 16-byte-aligned body, plain loads for the tail
-    const uint64_t remain = n_bases - T0;
-    const uint32_t avail = remain < (uint64_t)SEED_ASC_BYTES ? (uint32_t)remain : (uint32_t)SEED_ASC_BYTES;
-    const uint32_t nbulk = avail & ~15u;
+    // ---- stage the tile: TMA bulk copy for the 16-byte-aligned body, plain loads for the tail.
+    //      ASCII: SEED_ASC_BYTES bytes from bases + T0; PACKED: SEED_PK_WORDS words from word T0 / 16.
+    constexpr uint32_t UNIT = PACKED ? 4u : 1u;                    // bytes per staged element
+    constexpr uint32_t NSTAGE = PACKED ? SEED_PK_WORDS : SEED_ASC_BYTES;
+    const uint64_t e0 = PACKED ? T0 / 16 : T0;
+    const uint64_t remain = (PACKED ? (n_bases + 15) / 16 : n_bases) - e0;
+    const uint32_t avail = remain < (uint64_t)NSTAGE ? (uint32_t)remain : NSTAGE;
+    const uint32_t nbulk = avail & ~(16u / UNIT - 1u);             // elements in whole 16-byte groups
     const uint32_t mbar = smem_u32(&S.mbar);
     if (tid == 0) {
         asm volatile("mbarrier.init.shared::cta.b64 [%0], 1;" ::"r"(mbar));
@@ -241,18 +294,22 @@ k_seed(const uint8_t *__restrict__ bases, uint64_t n_bases, const uint64_t *__re
     }
     __syncthreads();
     if (tid == 0 && nbulk) {
-        asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(mbar), "r"(nbulk)
+        asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(mbar), "r"(nbulk * UNIT)
                      : "memory");
         asm volatile(
             "cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(
                 smem_u32(S.asc)),
-            "l"(bases + T0), "r"(nbulk), "r"(mbar)
+            "l"(bases + e0 * UNIT), "r"(nbulk * UNIT), "r"(mbar)
             : "memory");
     }
     // tail (< 16 bytes) and zero fill of everything past the end of the buffer
-    for (uint32_t i = nbulk + tid; i < (uint32_t)SEED_ASC_BYTES + 16; i += SEED_THREADS)
-        S.asc[i] = (i < avail) ? bases[T0 + i] : (uint8_t)0;
-    {
+    if (PACKED) {
+        const uint32_t *words = reinterpret_cast<const uint32_t *>(bases);
+        for (uint32_t i = nbulk + tid; i < NSTAGE; i += SEED_THREADS)
+            reinterpret_cast<uint32_t *>(S.asc)[i] = (i < avail) ? words[e0 + i] : 0u;
+    } else {
+        for (uint32_t i = nbulk + tid; i < (uint32_t)SEED_ASC_BYTES + 16; i += SEED_THREADS)
+            S.asc[i] = (i < avail) ? bases[T0 + i] : (uint8_t)0;
         const uint32_t code = byte_to_seq((uint32_t)tid);
         S.lut[0][tid] = (uint8_t)(code << 6);
         S.lut[1][tid] = (uint8_t)(code << 4);
@@ -278,27 +335,33 @@ k_seed(const uint8_t *__restrict__ bases, uint64_t n_bases, const uint64_t *__re
     }
     __syncthreads();
 
-    // ---- pack: 16 ASCII bytes -> one forward word (MSB-first) + one complement word (LSB-first)
-    // per byte: one PRMT (extract) + one LDS.U8 from the pre-shifted table; per 4 bytes two 3-input ORs
+    // ---- pack: 16 bases -> one forward word (MSB-first) + one complement word (LSB-first).
+    // ASCII, per byte: one PRMT (extract) + one LDS.U8 from the pre-shifted table; per 4 bytes two 3-input
+    // ORs.  PACKED: the staged word is the forward word.
     for (int ch = tid; ch < SEED_NCHUNK16; ch += SEED_THREADS) {
-        const uint4 v = *reinterpret_cast<const uint4 *>(S.asc + 16 * ch);
-        const uint32_t w[4] = {v.x, v.y, v.z, v.w};
-        uint32_t g[4];
+        uint32_t f;
+        if (PACKED) {
+            f = reinterpret_cast<const uint32_t *>(S.asc)[ch];
+        } else {
+            const uint4 v = *reinterpret_cast<const uint4 *>(S.asc + 16 * ch);
+            const uint32_t w[4] = {v.x, v.y, v.z, v.w};
+            uint32_t g[4];
 #pragma unroll
-        for (int q = 0; q < 4; q++) {
-            const uint32_t b0 = __byte_perm(w[q], 0u, 0x4440), b1 = __byte_perm(w[q], 0u, 0x4441);
-            const uint32_t b2 = __byte_perm(w[q], 0u, 0x4442), b3 = __byte_perm(w[q], 0u, 0x4443);
-            g[q] = ((uint32_t)S.lut[0][b0] | (uint32_t)S.lut[1][b1] | (uint32_t)S.lut[2][b2]) | (uint32_t)S.lut[3][b3];
+            for (int q = 0; q < 4; q++) {
+                const uint32_t b0 = __byte_perm(w[q], 0u, 0x4440), b1 = __byte_perm(w[q], 0u, 0x4441);
+                const uint32_t b2 = __byte_perm(w[q], 0u, 0x4442), b3 = __byte_perm(w[q], 0u, 0x4443);
+                g[q] = ((uint32_t)S.lut[0][b0] | (uint32_t)S.lut[1][b1] | (uint32_t)S.lut[2][b2]) | (uint32_t)S.lut[3][b3];
+            }
+            const uint32_t lo16 = __byte_perm(g[3], g[2], 0x0040), hi16 = __byte_perm(g[1], g[0], 0x0040);
+            f = __byte_perm(lo16, hi16, 0x5410);
         }
-        const uint32_t lo16 = __byte_perm(g[3], g[2], 0x0040), hi16 = __byte_perm(g[1], g[0], 0x0040);
-        const uint32_t f = __byte_perm(lo16, hi16, 0x5410);
         // complement stream: base j's (3 - code) at bits [2j, 2j+2): reverse the 16 fields of f
         uint32_t x = __brev(f);                                        // fields reversed, bits swapped in each
         x = ((x >> 1) & 0x55555555u) | ((x & 0x55555555u) << 1);       // swap bits back inside each field
         S.fw[1 + ch] = f;
         S.cw[ch] = ~x;
     }
-    __syncthreads();  // ASCII bytes are dead from here on; region A becomes SeedMeta
+    __syncthreads();  // the staged input is dead from here on; region A becomes SeedMeta
 
     if (tid == 0) M.stage_count = 0u;
 
@@ -378,66 +441,7 @@ k_seed(const uint8_t *__restrict__ bases, uint64_t n_bases, const uint64_t *__re
             const int ridx = q - M.rbase[j];
             const int p = M.s0[j] + ridx * W;            // tile-relative first window start
             const int n = min(W, M.cnt[j] - ridx * W);
-
-            // realign the two streams so that window i of this run starts at bit 2i
-            uint32_t F[4], G[4];
-            {
-                const uint32_t bitpos = 32u + 2u * (uint32_t)p - PAD;
-                const uint32_t q0 = bitpos >> 5, sh = bitpos & 31u;
-                uint32_t w0 = S.fw[q0], w1 = S.fw[q0 + 1], w2 = S.fw[q0 + 2], w3 = S.fw[q0 + 3],
-                         w4 = S.fw[q0 + 4];
-                F[0] = __funnelshift_l(w1, w0, sh);
-                F[1] = __funnelshift_l(w2, w1, sh);
-                F[2] = __funnelshift_l(w3, w2, sh);
-                F[3] = __funnelshift_l(w4, w3, sh);
-                const uint32_t cq = (uint32_t)p >> 4, csh = ((uint32_t)p & 15u) * 2u;
-                uint32_t c0 = S.cw[cq], c1 = S.cw[cq + 1], c2 = S.cw[cq + 2], c3 = S.cw[cq + 3],
-                         c4 = S.cw[cq + 4];
-                G[0] = __funnelshift_r(c0, c1, csh);
-                G[1] = __funnelshift_r(c1, c2, csh);
-                G[2] = __funnelshift_r(c2, c3, csh);
-                G[3] = __funnelshift_r(c3, c4, csh);
-            }
-            // hot loop: high word of the hash only; candidates (1/c of windows) are collected in a
-            // bit mask, so the loop has no divergent code
-            uint32_t cand = 0u;
-#pragma unroll
-            for (int i = 0; i < W; i++) {
-                const int jb = (2 * i) >> 5;
-                const uint32_t sft = (uint32_t)((2 * i) & 31);
-                const uint32_t f_hi = __funnelshift_l(F[jb + 1], F[jb], sft) & HI_MASK;
-                const uint32_t f_lo = __funnelshift_l(F[jb + 2], F[jb + 1], sft);
-                const uint32_t r_lo = __funnelshift_r(G[jb], G[jb + 1], sft);
-                const uint32_t r_hi = __funnelshift_r(G[jb + 1], G[jb + 2], sft) & HI_MASK;
-                // canonical k-mer = min(forward, reverse complement), src/seeding.rs:131-136.  Both are
-                // < 2^62, so as IEEE doubles they are finite, non-negative and ordered like the
-                // integers: ONE compare on the FP64 pipe replaces the two-instruction 64-bit integer
-                // compare on the ALU pipe, which is this loop's limiter.
-                uint32_t c_lo, c_hi;
-#if SEED_CANON_MODE == 0
-                const uint64_t f = ((uint64_t)f_hi << 32) | f_lo, rr = ((uint64_t)r_hi << 32) | r_lo;
-                const uint64_t canon = f < rr ? f : rr;
-                c_lo = (uint32_t)canon; c_hi = (uint32_t)(canon >> 32);
-#elif SEED_CANON_MODE == 1  // FP64 compare, SEL on the ALU pipe
-                asm("{\n\t.reg .pred p;\n\t.reg .f64 a, b;\n\tmov.b64 a, {%2, %3};\n\tmov.b64 b, {%4, %5};\n\t"
-                    "setp.lt.f64 p, a, b;\n\tselp.b32 %0, %2, %4, p;\n\tselp.b32 %1, %3, %5, p;\n\t}"
-                    : "=r"(c_lo), "=r"(c_hi) : "r"(f_lo), "r"(f_hi), "r"(r_lo), "r"(r_hi));
-#else
-                c_lo = r_lo; c_hi = r_hi;
-                asm("{\n\t.reg .pred p;\n\t.reg .f64 a, b;\n\tmov.b64 a, {%2, %3};\n\tmov.b64 b, {%4, %5};\n\t"
-                    "setp.lt.f64 p, a, b;\n\t@p mad.lo.u32 %0, %2, %6, %7;\n\t@p mad.lo.u32 %1, %3, %6, %7;\n\t}"
-                    : "+r"(c_lo), "+r"(c_hi) : "r"(f_lo), "r"(f_hi), "r"(r_lo), "r"(r_hi), "r"(smul.one), "r"(smul.zero));
-#endif
-                const uint32_t hh = hash_hi32<VAR>(c_lo, c_hi, smul);
-#if SEED_CANON_MODE >= 3
-                // candidate bit set by a predicated IMAD (FMA pipe): the bits are distinct, so add == or
-                asm("{\n\t.reg .pred p;\n\tsetp.le.u32 p, %1, %2;\n\t@p mad.lo.u32 %0, %3, %4, %0;\n\t}"
-                    : "+r"(cand) : "r"(hh), "r"(thr_hi), "r"(smul.one), "r"(1u << i));
-#else
-                asm("{\n\t.reg .pred p;\n\tsetp.le.u32 p, %1, %2;\n\t@p or.b32 %0, %0, %3;\n\t}"
-                    : "+r"(cand) : "r"(hh), "r"(thr_hi), "r"(1u << i));
-#endif
-            }
+            uint32_t cand = seed_run<K, W>(S.fw, S.cw, p, thr_hi, ic);
             if (n < W) cand &= (1u << n) - 1u;  // n >= 1 (windows past n belong to the next run / record)
             // candidates go to a CTA-wide list and are re-derived exactly by all threads afterwards
             while (cand) {
@@ -535,22 +539,22 @@ k_seed(const uint8_t *__restrict__ bases, uint64_t n_bases, const uint64_t *__re
 
 
 using seed_kern_t = void (*)(const uint8_t *, uint64_t, const uint64_t *, uint64_t, const uint32_t *, uint64_t, int, int,
-                             void *, uint64_t, unsigned long long *, const ShiftMul, uint64_t, int, uint32_t *, const GroupOut, const SlotOut);
+                             void *, uint64_t, unsigned long long *, const ImadConst, uint64_t, int, uint32_t *, const GroupOut, const SlotOut);
 
-// One translation unit per (K, EMIT) instantiates the three run lengths and exports a getter, so
-// the twelve kernels compile in parallel.
-#define SEED_DEFINE_KERNELS(NAME, K, EMIT)                            \
-    seed_kern_t NAME(int W) {                                         \
-        switch (W) {                                                  \
-            case 24: return k_seed<K, 0, EMIT, 24>;                   \
-            case 30: return k_seed<K, 0, EMIT, 30>;                   \
-            default: return k_seed<K, 0, EMIT, 32>;                   \
-        }                                                             \
+// One translation unit per (K, EMIT) instantiates the three run lengths for ASCII and 2-bit input and
+// exports a getter, so the 24 kernels compile in parallel.
+#define SEED_DEFINE_KERNELS(NAME, K, EMIT)                                              \
+    seed_kern_t NAME(int W, bool packed) {                                              \
+        switch (W) {                                                                    \
+            case 24: return packed ? k_seed<K, EMIT, 24, true> : k_seed<K, EMIT, 24, false>; \
+            case 30: return packed ? k_seed<K, EMIT, 30, true> : k_seed<K, EMIT, 30, false>; \
+            default: return packed ? k_seed<K, EMIT, 32, true> : k_seed<K, EMIT, 32, false>; \
+        }                                                                               \
     }
 
-seed_kern_t seed_kernels_k31_sv(int W);
-seed_kern_t seed_kernels_k31_ev(int W);
-seed_kern_t seed_kernels_k21_sv(int W);
-seed_kern_t seed_kernels_k21_ev(int W);
+seed_kern_t seed_kernels_k31_sv(int W, bool packed);
+seed_kern_t seed_kernels_k31_ev(int W, bool packed);
+seed_kern_t seed_kernels_k21_sv(int W, bool packed);
+seed_kern_t seed_kernels_k21_ev(int W, bool packed);
 
 }  // namespace syl

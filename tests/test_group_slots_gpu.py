@@ -1,6 +1,6 @@
 """GPU parity: read sketches whose post-pass group slots overflow on an ordinary sample.
 
-SYL_GROUP_CAP shrinks every group's slot, so the events the seeding kernels flush past it land in the
+SYL_GROUP_CAP shrinks every group's slot, so the events the seeding kernel flushes past it land in the
 overflow list and their groups take the generic path.  The library reads the variable once per process,
 hence the subprocess."""
 import os
@@ -22,23 +22,24 @@ ctx = sylph_b200.Context(0)
 b, o = synth.reads(40000, n_comm=4, genome_len=200000)
 b, o = b.numpy(), o.numpy().astype(np.uint64)
 db, do = synth.reads(40000, n_comm=4, genome_len=200000, device="cuda")
+src = (b, o) if SOURCE == "host" else (db, do)  # host memory: packed ingest, 2-bit k_seed; device memory: ASCII k_seed
 for k, c in ((31, 200), (21, 50)):
     eh, ec, _, nd = O.sketch_reads(b, o, k=k, c=c)
-    for src in ((b, o), (db, do)):  # host memory (packed ingest), device memory (ASCII seeding kernel)
-        s = ctx.sketch_sequences(*src, k=k, c=c)
-        h, cnt = s.download()
-        assert len(h) > 1000 and np.array_equal(h, eh) and np.array_equal(cnt, ec), (k, c, len(h), len(eh))
-        assert s.num_dup_removed == nd, (s.num_dup_removed, nd)
-        s.free()
+    s = ctx.sketch_sequences(*src, k=k, c=c)
+    h, cnt = s.download()
+    assert len(h) > 1000 and np.array_equal(h, eh) and np.array_equal(cnt, ec), (k, c, len(h), len(eh))
+    assert s.num_dup_removed == nd, (s.num_dup_removed, nd)
+    s.free()
 print("ok")
 """
 
 
 # 32: nearly every group overflows; 700: just above the expected group size, so in-kernel groups and
 # overflowing groups alternate along the hash range and the generic path's pairs are slotted between them
-@pytest.mark.parametrize("impl", ["cta", "warp"])
+@pytest.mark.parametrize("source", ["host", "device"])
 @pytest.mark.parametrize("group_cap", ["32", "700"])
-def test_reads_overflowing_group_slots(impl, group_cap):
-    env = dict(os.environ, SYL_GROUP_CAP=group_cap, SYL_SEED_IMPL=impl)
-    r = subprocess.run([sys.executable, "-c", SCRIPT], cwd=ROOT, env=env, capture_output=True, text=True, timeout=600)
+def test_reads_overflowing_group_slots(source, group_cap):
+    env = dict(os.environ, SYL_GROUP_CAP=group_cap)
+    r = subprocess.run([sys.executable, "-c", "SOURCE = %r\n" % source + SCRIPT], cwd=ROOT, env=env, capture_output=True,
+                       text=True, timeout=600)
     assert r.returncode == 0 and r.stdout.strip().endswith("ok"), r.stdout + r.stderr

@@ -1,6 +1,7 @@
 """GPU parity of the 2-bit packed ingest path (SURVEY §8 f3): packed == ASCII == oracle.
 syl_pack2 (host packer, exact BYTE_TO_SEQ) -> syl_seed_batch_packed2 / syl_sketch_reads_packed2, host and
-device memory, every byte value, ragged records, tile edges of the warp-tile (4096) and the chunk ring."""
+device memory, every byte value, ragged records, the seeding kernel's tile edges (32 768 bases) inside reads and
+the chunk ring."""
 import numpy as np
 import pytest
 
@@ -42,7 +43,7 @@ def test_seeding_packed_equals_oracle_all_byte_values(ctx, k, sem, device):
 @pytest.mark.parametrize("device", [False, True])
 @pytest.mark.parametrize("no_dedup", [False, True])
 def test_read_sketch_packed_equals_ascii_equals_oracle(ctx, device, no_dedup):
-    """Pair keys come from the packed stream (in-tile) or from packed global memory (reads cut by a warp-tile
+    """Pair keys come from the packed stream (in-tile) or from packed global memory (reads cut by a tile
     edge: k_events_fix<packed>); duplicates make the dedup state machine depend on them."""
     from oracle import oracle as O
     from sylph_b200.api import pack2
@@ -95,25 +96,56 @@ def test_host_ingest_chunk_ring(ctx, monkeypatch):
         assert np.array_equal(h, eh) and np.array_equal(c, ec) and s.num_dup_removed == nd, chunk
 
 
-@pytest.mark.parametrize("tw", [64, 128, 1024, 3072])
-def test_warp_tile_lengths(ctx, monkeypatch, tw):
-    """The launcher sizes the warp-tile from the mean record length; force odd lengths so that tile edges fall
-    everywhere inside records, halos and pair-key windows (ASCII and packed input, survivors and read sketches)."""
+TILE = 32768   # window starts per CTA tile of the seeding kernel (seed_kernel.cuh SEED_TILE)
+HALO = 48      # bases staged past the tile
+
+
+@pytest.mark.parametrize("device", [False, True])
+@pytest.mark.parametrize("L", [66, 150, 400])
+def test_tile_edges_inside_reads(ctx, monkeypatch, L, device):
+    """Tile edges at chosen offsets of reads of length L: the first and last windows, the pair keys' first 32
+    bases and the 32 from the middle, and the edge of the staged halo (the middle window ending exactly at, or
+    one base past, tile + HALO).  Short random filler reads put one such read across every tile edge.  The edge
+    reads are copies of reads elsewhere in the sample, so deduplication compares keys taken from the staged tile
+    with keys filled in from global memory.  ASCII and packed input: survivors with positions and read sketches."""
+    import torch
     from oracle import oracle as O
     from sylph_b200.api import pack2
-    monkeypatch.setenv("SYL_SEED_TW", str(tw))
-    monkeypatch.setenv("SYL_SEED_IMPL", "warp")
-    rng = np.random.default_rng(100 + tw)
-    lengths = list(rng.integers(0, 420, size=1500)) + [5000, 31, 32, 61, 62, 66]
-    buf, off = random_records(rng, [lengths[i] for i in rng.permutation(len(lengths))], alphabet=b"ACGTNacgt\x00\x03")
-    exp = sorted(oracle_survivors(buf, off, 31, 7, 1, True))
-    for packed in (False, True):
-        sv = survivors_packed(ctx, buf, off, 31, 7, 1, True, False) if packed else ctx.extract_markers_batch(buf, off, k=31, c=7, with_pos=True)
-        assert sorted((int(a), int(b), int(h)) for h, a, b in zip(sv["hash"], sv["rec"], sv["pos"])) == exp
+    monkeypatch.delenv("SYL_INGEST_CHUNK", raising=False)   # host input: one chunk, so tile edges sit at multiples of TILE
+    k = 31
+    h = L // 2
+    # h - 16: the middle 32 bases end exactly at TILE + HALO (keys from the tile); h - 17: one base past (from global memory)
+    offsets = [0, 1, k - 2, k - 1, k, h - 1, h, h + 31, h + 32, L - k, L - 1, h - 16, h - 17]
+    rng = np.random.default_rng(1000 + L)
+    bases = list(b"ACGT")
+    proto = [bytes(rng.choice(bases, size=L).astype(np.uint8)) for _ in range(3)]
+    seqs, pos = [], 0
+    for t, d in enumerate(offsets, start=1):
+        start = t * TILE - d                      # the edge read covers tile edge t * TILE at its offset d
+        while start - pos > 450:
+            dup = rng.random() < 0.03
+            seqs.append(proto[t % 3] if dup else bytes(rng.choice(bases, size=int(rng.integers(0, 420))).astype(np.uint8)))
+            pos += len(seqs[-1])
+        seqs.append(bytes(rng.choice(bases, size=start - pos).astype(np.uint8)))
+        seqs.append(proto[t % 3])
+        pos = start + L
+    seqs += proto
+    buf, off = flatten(seqs)
+    words = pack2(buf)
+    if device:
+        o = torch.from_numpy(off.astype(np.int64)).cuda()
+        inputs = [(torch.from_numpy(buf).cuda(), o, {}), (torch.from_numpy(words.view(np.int32)).cuda(), o, {"packed_bases": len(buf)})]
+    else:
+        inputs = [(buf, off, {}), (words, off, {"packed_bases": len(buf)})]
+    exp = sorted(oracle_survivors(buf, off, k, 7, 1, True))
     eh, ec, _, nd = O.sketch_reads(buf, off, c=7)
-    for s in (ctx.sketch_sequences(buf, off, c=7), ctx.sketch_sequences(pack2(buf), off, c=7, packed_bases=len(buf))):
-        h, c = s.download()
-        assert np.array_equal(h, eh) and np.array_equal(c, ec) and s.num_dup_removed == nd
+    assert nd > 0
+    for b, o, kw in inputs:
+        sv = ctx.extract_markers_batch(b, o, k=k, c=7, with_pos=True, **kw)
+        assert sorted((int(a), int(p), int(x)) for x, a, p in zip(sv["hash"], sv["rec"], sv["pos"])) == exp, kw
+        s = ctx.sketch_sequences(b, o, c=7, **kw)
+        hh, cc = s.download()
+        assert np.array_equal(hh, eh) and np.array_equal(cc, ec) and s.num_dup_removed == nd, kw
 
 
 def test_host_ingest_mixed_packed_and_ascii_chunks(ctx, monkeypatch):

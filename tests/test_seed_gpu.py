@@ -4,7 +4,7 @@ import os
 import numpy as np
 import pytest
 
-from tests.util import DATA, flatten, read_fastx
+from tests.util import DATA, flatten, read_fastx, seed_mode  # noqa: F401  (seed_mode: fixture)
 
 pytestmark = [pytest.mark.gpu, pytest.mark.usefixtures("seed_mode")]
 
