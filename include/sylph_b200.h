@@ -152,6 +152,13 @@ int syl_sketch_reads_packed2(syl_ctx *ctx, int mem, const uint32_t *packed, uint
 int syl_sketch_read_pairs(syl_ctx *ctx, int mem, const uint8_t *bases1, uint64_t n_bases1, const uint64_t *rec_off1,
                           const uint8_t *bases2, uint64_t n_bases2, const uint64_t *rec_off2, uint64_t n_pairs,
                           int k, uint64_t c, int no_dedup, int sem, syl_sample **out);
+/* The same for mates that are already 2-bit packed (layout: see syl_sketch_reads_packed2; one word buffer per mate file,
+ * ceil(n_bases_i/16) words, rec_off_i in bases).  Same result as syl_sketch_read_pairs on the ASCII it was packed from.
+ * SYL_MEM_HOST copies each word buffer and each offset array to the device once (4x fewer bytes than ASCII);
+ * SYL_MEM_DEVICE word buffers must be 16-byte aligned (else SYL_ERR_ARG). */
+int syl_sketch_read_pairs_packed2(syl_ctx *ctx, int mem, const uint32_t *packed1, uint64_t n_bases1, const uint64_t *rec_off1,
+                                  const uint32_t *packed2, uint64_t n_bases2, const uint64_t *rec_off2, uint64_t n_pairs,
+                                  int k, uint64_t c, int no_dedup, int sem, syl_sample **out);
 /* Host-side packer used by the above: exact BYTE_TO_SEQ codes, n_threads <= 0 = default. */
 int syl_pack2(const uint8_t *bases, uint64_t n_bases, uint32_t *words, int n_threads);
 /* Worker threads the host-memory path of syl_sketch_reads packs with (for bench.py's e2e record). */
@@ -188,6 +195,14 @@ int syl_sketch_genomes(syl_ctx *ctx, int mem, const uint8_t *bases, uint64_t n_b
                        const uint64_t *contig_off, uint64_t n_contigs, const uint64_t *genome_off,
                        uint64_t n_genomes, int k, uint64_t c, uint64_t min_spacing, int pseudotax,
                        int individual, int sem, syl_genomes **out);
+/* The same for contigs that are already 2-bit packed (layout: see syl_sketch_reads_packed2; ceil(n_bases/16) words,
+ * contig_off in bases): e.g. a 2-bit genome store.  Same result as syl_sketch_genomes on the ASCII it was packed
+ * from (gn_size comes from contig_off).  SYL_MEM_HOST copies the words once (4x fewer bytes than ASCII);
+ * SYL_MEM_DEVICE words must be 16-byte aligned (else SYL_ERR_ARG). */
+int syl_sketch_genomes_packed2(syl_ctx *ctx, int mem, const uint32_t *packed, uint64_t n_bases,
+                               const uint64_t *contig_off, uint64_t n_contigs, const uint64_t *genome_off,
+                               uint64_t n_genomes, int k, uint64_t c, uint64_t min_spacing, int pseudotax,
+                               int individual, int sem, syl_genomes **out);
 /* Wrap existing sketches (e.g. a deserialised .syldb). tracked/tracked_off may be NULL. */
 int syl_genomes_upload(syl_ctx *ctx, int mem, const uint64_t *kmers, const uint64_t *kmer_off,
                        const uint64_t *tracked, const uint64_t *tracked_off, const uint64_t *gn_size,

@@ -58,6 +58,7 @@ SIGNATURES = {
     "syl_sketch_reads": (_i, [_vp, _i, _vp, _u64, _vp, _u64, _i, _u64, _i, _i, _pp]),
     "syl_sketch_reads_packed2": (_i, [_vp, _i, _vp, _u64, _vp, _u64, _i, _u64, _i, _i, _pp]),
     "syl_sketch_read_pairs": (_i, [_vp, _i, _vp, _u64, _vp, _vp, _u64, _vp, _u64, _i, _u64, _i, _i, _pp]),
+    "syl_sketch_read_pairs_packed2": (_i, [_vp, _i, _vp, _u64, _vp, _vp, _u64, _vp, _u64, _i, _u64, _i, _i, _pp]),
     "syl_pack2": (_i, [_vp, _u64, _vp, _i]),
     "syl_pack_threads": (_i, []),
     "syl_ctx_ingest_stats": (_i, [_vp, _vp, _vp, _vp]),
@@ -70,6 +71,7 @@ SIGNATURES = {
     "syl_sample_device_ptrs": (_i, [_vp, _pp, _pp]),
     "syl_sample_free": (None, [_vp]),
     "syl_sketch_genomes": (_i, [_vp, _i, _vp, _u64, _vp, _u64, _vp, _u64, _i, _u64, _u64, _i, _i, _i, _pp]),
+    "syl_sketch_genomes_packed2": (_i, [_vp, _i, _vp, _u64, _vp, _u64, _vp, _u64, _i, _u64, _u64, _i, _i, _i, _pp]),
     "syl_genomes_upload": (_i, [_vp, _i, _vp, _vp, _vp, _vp, _vp, _u64, _i, _u64, _pp]),
     "syl_genomes_concat": (_i, [_vp, _pp, _u32, _pp]),
     "syl_genomes_select": (_i, [_vp, _vp, _vp, _u32, _pp]),

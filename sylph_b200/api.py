@@ -173,21 +173,26 @@ class Context:
         _lib.check(L.syl_sketch_reads(self._h, mem_b, pb, nb, po, no - 1, k, c, int(no_dedup), sem, C.byref(h)))
         return Sample(self, h)
 
-    def sketch_pair_sequences(self, bases1, rec_off1, bases2, rec_off2, k=31, c=200, no_dedup=False, sem=SEM_AVX2):
+    def sketch_pair_sequences(self, bases1, rec_off1, bases2, rec_off2, k=31, c=200, no_dedup=False, sem=SEM_AVX2,
+                              packed=False):
         """Batched body of sketch_pair_sequences with --fpr 0 (src/sketch.rs:771-895): mate i of pair p is record p of
-        buffer i; pairs = min(records) of the two buffers -> Sample."""
+        buffer i; pairs = min(records) of the two buffers -> Sample.
+        packed: `bases1` / `bases2` hold 2-bit words (see pack2) (syl_sketch_read_pairs_packed2)."""
         _CTX_STREAM[0] = self._stream
         L = _lib.lib()
-        m1, p1, n1, k1 = _arg(bases1, np.uint8)
+        dt, fn = (np.uint32, L.syl_sketch_read_pairs_packed2) if packed else (np.uint8, L.syl_sketch_read_pairs)
+        m1, p1, n1, k1 = _arg(bases1, dt)
         mo1, po1, no1, k2 = _arg(rec_off1, np.uint64)
-        m2, p2, n2, k3 = _arg(bases2, np.uint8)
+        m2, p2, n2, k3 = _arg(bases2, dt)
         mo2, po2, no2, k4 = _arg(rec_off2, np.uint64)
         if len({m1, mo1, m2, mo2}) != 1:
             raise ValueError("all four buffers must live in the same memory space")
         n_pairs = min(no1, no2) - 1
-        n1, n2 = int(k2[n_pairs]), int(k4[n_pairs])   # bases of the zipped records only (a longer file's tail is ignored)
+        nb1, nb2 = int(k2[n_pairs]), int(k4[n_pairs])   # bases of the zipped records only (a longer file's tail is ignored)
+        if packed and (n1 < (nb1 + 15) // 16 or n2 < (nb2 + 15) // 16):
+            raise ValueError("packed buffer too short")
         h = C.c_void_p()
-        _lib.check(L.syl_sketch_read_pairs(self._h, m1, p1, n1, po1, p2, n2, po2, n_pairs, k, c, int(no_dedup), sem, C.byref(h)))
+        _lib.check(fn(self._h, m1, p1, nb1, po1, p2, nb2, po2, n_pairs, k, c, int(no_dedup), sem, C.byref(h)))
         return Sample(self, h)
 
     def upload_sample(self, hashes, counts, k=31, c=200):
@@ -202,12 +207,22 @@ class Context:
 
     # ---- (3) genome sketches -----------------------------------------------------------------
     def sketch_genomes(self, bases, contig_off, genome_off=None, k=31, c=200, min_spacing=30, pseudotax=True,
-                       individual=False, sem=SEM_AVX2):
-        """Batched sketch_genome / sketch_genome_individual (src/sketch.rs:550-622, 481-548)."""
+                       individual=False, sem=SEM_AVX2, packed_bases=None):
+        """Batched sketch_genome / sketch_genome_individual (src/sketch.rs:550-622, 481-548).
+        packed_bases: `bases` holds 2-bit words (see pack2) for this many bases (syl_sketch_genomes_packed2)."""
         _CTX_STREAM[0] = self._stream
         L = _lib.lib()
-        mem_b, pb, nb, kb = _arg(bases, np.uint8)
         mem_o, po, no, ko = _arg(contig_off, np.uint64)
+        fn = L.syl_sketch_genomes
+        if packed_bases is not None:
+            mem_b, pb, nw, kb = _arg(bases, np.uint32)
+            if nw < (packed_bases + 15) // 16:
+                raise ValueError("packed buffer too short")
+            if mem_b != mem_o:
+                raise ValueError("bases and contig_off must live in the same memory space")
+            nb, fn = int(packed_bases), L.syl_sketch_genomes_packed2
+        else:
+            mem_b, pb, nb, kb = _arg(bases, np.uint8)
         n_genomes = 0
         pg = None
         if not individual:
@@ -215,8 +230,8 @@ class Context:
             assert mem_g == mem_b
             n_genomes = ng - 1
         h = C.c_void_p()
-        _lib.check(L.syl_sketch_genomes(self._h, mem_b, pb, nb, po, no - 1, pg, n_genomes, k, c, min_spacing,
-                                        int(pseudotax), int(individual), sem, C.byref(h)))
+        _lib.check(fn(self._h, mem_b, pb, nb, po, no - 1, pg, n_genomes, k, c, min_spacing,
+                      int(pseudotax), int(individual), sem, C.byref(h)))
         return Genomes(self, h)
 
     def upload_genomes(self, kmers, kmer_off, tracked=None, tracked_off=None, gn_size=None, k=31, c=200):

@@ -19,8 +19,8 @@
 #include "scan.cuh"
 
 namespace syl {
-int seed_device(syl_ctx *ctx, const uint8_t *d_bases, uint64_t n_bases, const uint64_t *d_rec_off, uint64_t off_bias,
-                uint64_t n_rec, int k, uint64_t c, int sem, int with_pos, syl_survivor *d_out,
+int seed_device(syl_ctx *ctx, const uint8_t *d_bases, const uint32_t *d_packed, uint64_t n_bases, const uint64_t *d_rec_off,
+                uint64_t off_bias, uint64_t n_rec, int k, uint64_t c, int sem, int with_pos, syl_survivor *d_out,
                 uint64_t cap, uint64_t *n_out);
 }
 
@@ -200,9 +200,11 @@ static int genomes_alloc(syl_genomes *g, cudaStream_t st, uint64_t n_genomes, ui
 
 // Generic post-pass: two library radix sorts (position, then hash).  Handles every input; used when the
 // slotted path below does not apply (tiny c, SYL_GENOME_POSTPASS=sort) or reports an overflow.
-static int sketch_genomes_device_sort(syl_ctx *ctx, const uint8_t *d_bases, uint64_t n_bases, const uint64_t *d_contig_off,
-                                      uint64_t n_contigs, const uint64_t *d_genome_off, uint64_t n_genomes, int k, uint64_t c,
-                                      uint64_t min_spacing, int pseudotax, int sem, syl_genomes *out) {
+// Exactly one of d_bases (ASCII) / d_packed (2-bit words) is set, here and in the two functions below.
+static int sketch_genomes_device_sort(syl_ctx *ctx, const uint8_t *d_bases, const uint32_t *d_packed, uint64_t n_bases,
+                                      const uint64_t *d_contig_off, uint64_t n_contigs, const uint64_t *d_genome_off,
+                                      uint64_t n_genomes, int k, uint64_t c, uint64_t min_spacing, int pseudotax, int sem,
+                                      syl_genomes *out) {
     cudaStream_t st = ctx->stream;
     // 1. survivors with positions
     uint64_t scap = n_bases / c + n_bases / (4 * c) + 65536;
@@ -211,7 +213,7 @@ static int sketch_genomes_device_sort(syl_ctx *ctx, const uint8_t *d_bases, uint
     uint64_t N = 0;
     for (;;) {
         SYL_TRY(sv.alloc(scap, st));
-        int rc = seed_device(ctx, d_bases, n_bases, d_contig_off, 0, n_contigs, k, c, sem, /*with_pos=*/1, sv.p, scap, &N);
+        int rc = seed_device(ctx, d_bases, d_packed, n_bases, d_contig_off, 0, n_contigs, k, c, sem, /*with_pos=*/1, sv.p, scap, &N);
         if (rc == SYL_ERR_CAPACITY) { scap = N + 16; continue; }
         if (rc != SYL_OK) return rc;
         break;
@@ -456,9 +458,10 @@ __global__ void k_genome_offsets32(const uint32_t *__restrict__ gs, const uint32
 }
 
 // rc SYL_ERR_UNSUPPORTED: a slot / table overflowed — the caller takes the generic path
-static int sketch_genomes_device_slots(syl_ctx *ctx, const uint8_t *d_bases, uint64_t n_bases, const uint64_t *d_contig_off,
-                                       uint64_t n_contigs, const uint64_t *d_genome_off, uint64_t n_genomes, int k, uint64_t c,
-                                       uint64_t min_spacing, int pseudotax, int sem, syl_genomes *out) {
+static int sketch_genomes_device_slots(syl_ctx *ctx, const uint8_t *d_bases, const uint32_t *d_packed, uint64_t n_bases,
+                                       const uint64_t *d_contig_off, uint64_t n_contigs, const uint64_t *d_genome_off,
+                                       uint64_t n_genomes, int k, uint64_t c, uint64_t min_spacing, int pseudotax, int sem,
+                                       syl_genomes *out) {
     cudaStream_t st = ctx->stream;
     const uint64_t n_tiles = seed_cta_tiles(n_bases);
     if (n_tiles * GEN_SLOT >= 0xFFFFFFFFull) { set_error("genome batch too large; split the batch"); return SYL_ERR_ARG; }
@@ -474,7 +477,7 @@ static int sketch_genomes_device_slots(syl_ctx *ctx, const uint8_t *d_bases, uin
     SYL_CUDA(cudaMemsetAsync(flags32.p, 0, 8, st));
     SYL_CUDA(cudaMemsetAsync(ctx->d_counters, 0, 2 * sizeof(uint64_t), st));
     SeedJob job;
-    job.d_bases = d_bases; job.n_bases = n_bases; job.d_rec_off = d_contig_off; job.off_bias = 0; job.n_rec = n_contigs;
+    job.d_bases = d_bases; job.d_packed = d_packed; job.n_bases = n_bases; job.d_rec_off = d_contig_off; job.off_bias = 0; job.n_rec = n_contigs;
     job.k = k; job.c = c; job.sem = sem; job.with_pos = 1; job.d_out = slots.p; job.cap = n_tiles * GEN_SLOT;
     job.d_count = reinterpret_cast<unsigned long long *>(ctx->d_counters);
     job.slot_cap = GEN_SLOT; job.d_tile_cnt = tile_cnt.p; job.d_slot_overflow = flags32.p;
@@ -533,35 +536,30 @@ static int sketch_genomes_device_slots(syl_ctx *ctx, const uint8_t *d_bases, uin
     return SYL_OK;
 }
 
-int sketch_genomes_device(syl_ctx *ctx, const uint8_t *d_bases, uint64_t n_bases, const uint64_t *d_contig_off,
-                          uint64_t n_contigs, const uint64_t *d_genome_off, uint64_t n_genomes, int k, uint64_t c,
-                          uint64_t min_spacing, int pseudotax, int sem, syl_genomes *out) {
+int sketch_genomes_device(syl_ctx *ctx, const uint8_t *d_bases, const uint32_t *d_packed, uint64_t n_bases,
+                          const uint64_t *d_contig_off, uint64_t n_contigs, const uint64_t *d_genome_off, uint64_t n_genomes,
+                          int k, uint64_t c, uint64_t min_spacing, int pseudotax, int sem, syl_genomes *out) {
     const char *e = getenv("SYL_GENOME_POSTPASS");  // "sort" forces the generic path (tests); read per call
     const bool force_sort = e && std::string(e) == "sort";
     // slots hold 512 survivors per 32K-base tile: c >= 96 keeps the expected number below 350
     if (!force_sort && c >= 96 && n_bases && n_contigs && n_genomes) {
-        const int rc = sketch_genomes_device_slots(ctx, d_bases, n_bases, d_contig_off, n_contigs, d_genome_off, n_genomes, k, c,
-                                                   min_spacing, pseudotax, sem, out);
+        const int rc = sketch_genomes_device_slots(ctx, d_bases, d_packed, n_bases, d_contig_off, n_contigs, d_genome_off,
+                                                   n_genomes, k, c, min_spacing, pseudotax, sem, out);
         if (rc != SYL_ERR_UNSUPPORTED) return rc;
         // a slot or table overflowed (low-complexity sequence): release what was allocated and take the generic path
         hblock_free(out->owner, out->kmer_off); hblock_free(out->owner, out->tracked_off); hblock_free(out->owner, out->gn_size);
         out->kmer_off = out->tracked_off = out->gn_size = nullptr;
     }
-    return sketch_genomes_device_sort(ctx, d_bases, n_bases, d_contig_off, n_contigs, d_genome_off, n_genomes, k, c, min_spacing,
-                                      pseudotax, sem, out);
+    return sketch_genomes_device_sort(ctx, d_bases, d_packed, n_bases, d_contig_off, n_contigs, d_genome_off, n_genomes, k, c,
+                                      min_spacing, pseudotax, sem, out);
 }
 
-}  // namespace syl
-
-using namespace syl;
-
-extern "C" {
-
-int syl_sketch_genomes(syl_ctx *ctx, int mem, const uint8_t *bases, uint64_t n_bases,
-                       const uint64_t *contig_off, uint64_t n_contigs, const uint64_t *genome_off,
-                       uint64_t n_genomes, int k, uint64_t c, uint64_t min_spacing, int pseudotax,
-                       int individual, int sem, syl_genomes **out) {
-    if (!ctx || !out || (!bases && n_bases) || !contig_off || (!individual && !genome_off)) {
+// packed: the input is 2-bit words (device or host memory); else ASCII
+static int sketch_genomes_impl(syl_ctx *ctx, int mem, const uint8_t *bases, const uint32_t *packed, uint64_t n_bases,
+                               const uint64_t *contig_off, uint64_t n_contigs, const uint64_t *genome_off, uint64_t n_genomes,
+                               int k, uint64_t c, uint64_t min_spacing, int pseudotax, int individual, int sem,
+                               syl_genomes **out) {
+    if (!ctx || !out || (!bases && !packed && n_bases) || !contig_off || (!individual && !genome_off)) {
         set_error("NULL argument");
         return SYL_ERR_ARG;
     }
@@ -570,17 +568,26 @@ int syl_sketch_genomes(syl_ctx *ctx, int mem, const uint8_t *bases, uint64_t n_b
     SYL_CUDA(cudaSetDevice(ctx->device));
     syl::tl_ctx = ctx;
     cudaStream_t st = ctx->stream;
-    DevBuf<uint8_t> hb;
+    DevBuf<uint8_t> hb;   // host memory: staged copies, alive until the call's last sync
+    DevBuf<uint32_t> hp;
     DevBuf<uint64_t> hc, hg;
     const uint8_t *d_bases = bases;
+    const uint32_t *d_packed = packed;
     const uint64_t *d_coff = contig_off, *d_goff = genome_off;
     if (individual) n_genomes = n_contigs;
     if (mem == SYL_MEM_HOST) {
-        SYL_TRY(hb.alloc(n_bases + 64, st));
+        if (packed) {
+            const uint64_t nw = (n_bases + 15) / 16;
+            SYL_TRY(hp.alloc(nw + 16, st));
+            if (nw) SYL_CUDA(cudaMemcpyAsync(hp.p, packed, nw * 4, cudaMemcpyHostToDevice, st));
+            d_packed = hp.p;
+        } else {
+            SYL_TRY(hb.alloc(n_bases + 64, st));
+            if (n_bases) SYL_CUDA(cudaMemcpyAsync(hb.p, bases, n_bases, cudaMemcpyHostToDevice, st));
+            d_bases = hb.p;
+        }
         SYL_TRY(hc.alloc(n_contigs + 1, st));
-        if (n_bases) SYL_CUDA(cudaMemcpyAsync(hb.p, bases, n_bases, cudaMemcpyHostToDevice, st));
         SYL_CUDA(cudaMemcpyAsync(hc.p, contig_off, (n_contigs + 1) * 8, cudaMemcpyHostToDevice, st));
-        d_bases = hb.p;
         d_coff = hc.p;
         if (!individual) {
             SYL_TRY(hg.alloc(n_genomes + 1, st));
@@ -602,11 +609,33 @@ int syl_sketch_genomes(syl_ctx *ctx, int mem, const uint8_t *bases, uint64_t n_b
     g->device = ctx->device;
     g->k = k;
     g->c = c;
-    int rc = sketch_genomes_device(ctx, d_bases, n_bases, d_coff, n_contigs, d_goff, n_genomes, k, c, min_spacing,
+    int rc = sketch_genomes_device(ctx, d_bases, d_packed, n_bases, d_coff, n_contigs, d_goff, n_genomes, k, c, min_spacing,
                                    pseudotax, sem, g);
     if (rc != SYL_OK) { syl_genomes_free(g); return rc; }
     *out = g;
     return SYL_OK;
+}
+
+}  // namespace syl
+
+using namespace syl;
+
+extern "C" {
+
+int syl_sketch_genomes(syl_ctx *ctx, int mem, const uint8_t *bases, uint64_t n_bases,
+                       const uint64_t *contig_off, uint64_t n_contigs, const uint64_t *genome_off,
+                       uint64_t n_genomes, int k, uint64_t c, uint64_t min_spacing, int pseudotax,
+                       int individual, int sem, syl_genomes **out) {
+    return sketch_genomes_impl(ctx, mem, bases, nullptr, n_bases, contig_off, n_contigs, genome_off, n_genomes, k, c,
+                               min_spacing, pseudotax, individual, sem, out);
+}
+
+int syl_sketch_genomes_packed2(syl_ctx *ctx, int mem, const uint32_t *packed, uint64_t n_bases,
+                               const uint64_t *contig_off, uint64_t n_contigs, const uint64_t *genome_off,
+                               uint64_t n_genomes, int k, uint64_t c, uint64_t min_spacing, int pseudotax,
+                               int individual, int sem, syl_genomes **out) {
+    return sketch_genomes_impl(ctx, mem, nullptr, packed, n_bases, contig_off, n_contigs, genome_off, n_genomes, k, c,
+                               min_spacing, pseudotax, individual, sem, out);
 }
 
 int syl_genomes_upload(syl_ctx *ctx, int mem, const uint64_t *kmers, const uint64_t *kmer_off,

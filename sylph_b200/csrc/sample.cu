@@ -121,20 +121,25 @@ k_events_fix(EventRec *__restrict__ ev, const uint32_t *__restrict__ pend, const
 // Read pairs (src/sketch.rs:658-688 pair_kmer): the two keys come from the first 32 bases of BOTH mates; every event of
 // the pair carries them.  Events arrive with recflag = pair << 1 | EV_PENDING; the result is
 // recflag = pair << 2 | mate << 1 | NO_PAIR (a mate shorter than 33 bp, or --no-dedup).
+// ASCII input: bases1 / bases2; 2-bit input: packed1 / packed2 of n_words1 / n_words2 words.
+template <bool PACKED>
 __global__ void __launch_bounds__(EV_THREADS)
 k_events_fix_paired(EventRec *__restrict__ ev, const uint32_t *__restrict__ pend, const unsigned long long *__restrict__ p_begin,
                     const unsigned long long *__restrict__ p_end, uint64_t ev_cap, const uint8_t *__restrict__ bases1,
-                    const uint64_t *__restrict__ off1, const uint8_t *__restrict__ bases2, const uint64_t *__restrict__ off2,
-                    uint64_t mate, int no_dedup) {
+                    const uint32_t *__restrict__ packed1, uint64_t n_words1, const uint64_t *__restrict__ off1,
+                    const uint8_t *__restrict__ bases2, const uint32_t *__restrict__ packed2, uint64_t n_words2,
+                    const uint64_t *__restrict__ off2, uint64_t mate, int no_dedup) {
     __shared__ uint8_t lut[4][256];
-    for (int i = threadIdx.x; i < 256; i += EV_THREADS) {
-        const uint32_t code = byte_to_seq((uint32_t)i);
-        lut[0][i] = (uint8_t)(code << 6);
-        lut[1][i] = (uint8_t)(code << 4);
-        lut[2][i] = (uint8_t)(code << 2);
-        lut[3][i] = (uint8_t)code;
+    if (!PACKED) {
+        for (int i = threadIdx.x; i < 256; i += EV_THREADS) {
+            const uint32_t code = byte_to_seq((uint32_t)i);
+            lut[0][i] = (uint8_t)(code << 6);
+            lut[1][i] = (uint8_t)(code << 4);
+            lut[2][i] = (uint8_t)(code << 2);
+            lut[3][i] = (uint8_t)code;
+        }
+        __syncthreads();
     }
-    __syncthreads();
     const uint64_t i0 = *p_begin, i1 = *p_end;
     for (uint64_t i = i0 + (uint64_t)blockIdx.x * EV_THREADS + threadIdx.x; i < i1; i += (uint64_t)gridDim.x * EV_THREADS) {
         const uint32_t ei = pend[i];
@@ -146,11 +151,18 @@ k_events_fix_paired(EventRec *__restrict__ ev, const uint32_t *__restrict__ pend
         const bool has = !no_dedup && L1 >= 33 && L2 >= 33;  // 2 * 16 + 1 (:660)
         uint64_t p0 = 0, p1 = 0;
         if (has) {
-            uint32_t x[8];
-            load32_unaligned(bases1 + a1, x);
-            const uint32_t f = pack16(x, 0x6420, lut), g = pack16(x, 0x7531, lut);
-            load32_unaligned(bases2 + a2, x);
-            const uint32_t r = pack16(x, 0x6420, lut), t = pack16(x, 0x7531, lut);
+            uint32_t f, g, r, t;
+            if (!PACKED) {
+                uint32_t x[8];
+                load32_unaligned(bases1 + a1, x);
+                f = pack16(x, 0x6420, lut); g = pack16(x, 0x7531, lut);
+                load32_unaligned(bases2 + a2, x);
+                r = pack16(x, 0x6420, lut); t = pack16(x, 0x7531, lut);
+            } else {
+                const uint64_t x = packed64(packed1, n_words1, a1), y = packed64(packed2, n_words2, a2);
+                f = even_fields(x); g = even_fields(x << 2);
+                r = even_fields(y); t = even_fields(y << 2);
+            }
             p0 = ((uint64_t)f << 32) | r;  // ([kmer_f, kmer_r], [kmer_g, kmer_t]) (:685)
             p1 = ((uint64_t)g << 32) | t;
         }
@@ -1269,6 +1281,87 @@ static int sketch_reads_impl(syl_ctx *ctx, int mem, const uint8_t *bases, const 
     return SYL_ERR_CAPACITY;
 }
 
+// One mate file of a paired sample: ASCII bytes or 2-bit words, device resident after stage().
+struct MateInput {
+    const uint8_t *bases;
+    const uint32_t *packed;
+    uint64_t n_bases;
+    const uint64_t *off;
+    DevBuf<uint8_t> hb;  // host memory: staged copies, alive until the call's sync
+    DevBuf<uint32_t> hp;
+    DevBuf<uint64_t> ho;
+    uint64_t n_words() const { return (n_bases + 15) / 16; }
+    // one copy of the bases / words and one of the offsets
+    int stage(syl_ctx *ctx, bool is_packed, uint64_t n_pairs) {
+        cudaStream_t st = ctx->stream;
+        if (is_packed) {
+            SYL_TRY(hp.alloc(n_words() + 16, st));
+            if (n_bases) SYL_CUDA(cudaMemcpyAsync(hp.p, packed, n_words() * 4, cudaMemcpyHostToDevice, st));
+            packed = hp.p;
+        } else {
+            SYL_TRY(hb.alloc(n_bases + 64, st));
+            if (n_bases) SYL_CUDA(cudaMemcpyAsync(hb.p, bases, n_bases, cudaMemcpyHostToDevice, st));
+            bases = hb.p;
+        }
+        SYL_TRY(ho.alloc(n_pairs + 1, st));
+        SYL_CUDA(cudaMemcpyAsync(ho.p, off, (n_pairs + 1) * 8, cudaMemcpyHostToDevice, st));
+        off = ho.p;
+        return SYL_OK;
+    }
+};
+
+// packed: both mates are 2-bit words (m1.packed / m2.packed), else ASCII (m1.bases / m2.bases)
+static int sketch_read_pairs_impl(syl_ctx *ctx, int mem, bool packed, MateInput &m1, MateInput &m2, uint64_t n_pairs, int k,
+                                  uint64_t c, int no_dedup, int sem, syl_sample **out) {
+    if (!ctx || !out || (!m1.bases && !m1.packed && m1.n_bases) || (!m2.bases && !m2.packed && m2.n_bases) || !m1.off || !m2.off) {
+        set_error("NULL argument");
+        return SYL_ERR_ARG;
+    }
+    if (c == 0) { set_error("c must be >= 1"); return SYL_ERR_ARG; }
+    if (mem != SYL_MEM_HOST && mem != SYL_MEM_DEVICE) { set_error("bad mem"); return SYL_ERR_ARG; }
+    *out = nullptr;
+    SYL_CUDA(cudaSetDevice(ctx->device));
+    syl::tl_ctx = ctx;
+    cudaStream_t st = ctx->stream;
+    if (mem == SYL_MEM_HOST) {
+        SYL_TRY(m1.stage(ctx, packed, n_pairs));
+        SYL_TRY(m2.stage(ctx, packed, n_pairs));
+    }
+    uint64_t cap_override = 0;
+    for (int attempt = 0; attempt < 3; attempt++) {
+        SampleBuilder b{ctx, k, c, no_dedup, sem};
+        b.paired = true;
+        b.expect_bases = m1.n_bases + m2.n_bases;
+        b.expect_reads = 2 * n_pairs;
+        SYL_TRY(b.begin(cap_override));
+        unsigned long long *dc = b.d_count();
+        // mate 1, then mate 2: both use the PAIR index as read index; the pending list tells the mates apart
+        SYL_TRY(b.add(m1.bases, m1.packed, m1.n_bases, m1.off, 0, n_pairs, 0));
+        SYL_CUDA(cudaMemcpyAsync(dc + 17, dc + 1, 8, cudaMemcpyDeviceToDevice, st));  // pending entries of mate 1
+        SYL_TRY(b.add(m2.bases, m2.packed, m2.n_bases, m2.off, 0, n_pairs, 0));
+        SYL_CUDA(cudaMemsetAsync(dc + 18, 0, 8, st));
+        if (n_pairs) {
+            auto fix = packed ? k_events_fix_paired<true> : k_events_fix_paired<false>;
+            const uint64_t nw1 = packed ? m1.n_words() : 0, nw2 = packed ? m2.n_words() : 0;
+            fix<<<ctx->num_sms * 2, EV_THREADS, 0, st>>>(b.b_ev.p, b.b_pend.p, dc + 18, dc + 17, b.cap, m1.bases, m1.packed, nw1,
+                                                         m1.off, m2.bases, m2.packed, nw2, m2.off, 0, no_dedup);
+            fix<<<ctx->num_sms * 2, EV_THREADS, 0, st>>>(b.b_ev.p, b.b_pend.p, dc + 17, dc + 1, b.cap, m1.bases, m1.packed, nw1,
+                                                         m1.off, m2.bases, m2.packed, nw2, m2.off, 1, no_dedup);
+            ctx->launches += 2;
+            SYL_CUDA(cudaGetLastError());
+        }
+        b.n_reads = n_pairs;       // mean_read_length = mean length of mate 1 (src/sketch.rs:824-826)
+        b.n_bases = m1.n_bases;
+        uint64_t need = 0;
+        const int rc = b.finish(out, &need);
+        if (rc == SYL_ERR_CAPACITY) { cap_override = need + 16; continue; }
+        if (rc == SYL_OK) SYL_CUDA(cudaStreamSynchronize(st));  // the staged inputs go out of scope
+        return rc;
+    }
+    set_error("event capacity retry failed");
+    return SYL_ERR_CAPACITY;
+}
+
 }  // namespace syl
 
 using namespace syl;
@@ -1291,55 +1384,15 @@ int syl_sketch_reads_packed2(syl_ctx *ctx, int mem, const uint32_t *packed, uint
 int syl_sketch_read_pairs(syl_ctx *ctx, int mem, const uint8_t *bases1, uint64_t n_bases1, const uint64_t *rec_off1,
                           const uint8_t *bases2, uint64_t n_bases2, const uint64_t *rec_off2, uint64_t n_pairs,
                           int k, uint64_t c, int no_dedup, int sem, syl_sample **out) {
-    if (!ctx || !out || (!bases1 && n_bases1) || (!bases2 && n_bases2) || !rec_off1 || !rec_off2) { set_error("NULL argument"); return SYL_ERR_ARG; }
-    if (c == 0) { set_error("c must be >= 1"); return SYL_ERR_ARG; }
-    if (mem != SYL_MEM_HOST && mem != SYL_MEM_DEVICE) { set_error("bad mem"); return SYL_ERR_ARG; }
-    *out = nullptr;
-    SYL_CUDA(cudaSetDevice(ctx->device));
-    syl::tl_ctx = ctx;
-    cudaStream_t st = ctx->stream;
-    DevBuf<uint8_t> hb1, hb2;
-    DevBuf<uint64_t> ho1, ho2;
-    const uint8_t *d1 = bases1, *d2 = bases2;
-    const uint64_t *o1 = rec_off1, *o2 = rec_off2;
-    if (mem == SYL_MEM_HOST) {
-        SYL_TRY(hb1.alloc(n_bases1 + 64, st)); SYL_TRY(hb2.alloc(n_bases2 + 64, st));
-        SYL_TRY(ho1.alloc(n_pairs + 1, st)); SYL_TRY(ho2.alloc(n_pairs + 1, st));
-        if (n_bases1) SYL_CUDA(cudaMemcpyAsync(hb1.p, bases1, n_bases1, cudaMemcpyHostToDevice, st));
-        if (n_bases2) SYL_CUDA(cudaMemcpyAsync(hb2.p, bases2, n_bases2, cudaMemcpyHostToDevice, st));
-        SYL_CUDA(cudaMemcpyAsync(ho1.p, rec_off1, (n_pairs + 1) * 8, cudaMemcpyHostToDevice, st));
-        SYL_CUDA(cudaMemcpyAsync(ho2.p, rec_off2, (n_pairs + 1) * 8, cudaMemcpyHostToDevice, st));
-        d1 = hb1.p; d2 = hb2.p; o1 = ho1.p; o2 = ho2.p;
-    }
-    uint64_t cap_override = 0;
-    for (int attempt = 0; attempt < 3; attempt++) {
-        SampleBuilder b{ctx, k, c, no_dedup, sem};
-        b.paired = true;
-        b.expect_bases = n_bases1 + n_bases2;
-        b.expect_reads = 2 * n_pairs;
-        SYL_TRY(b.begin(cap_override));
-        unsigned long long *dc = b.d_count();
-        // mate 1, then mate 2: both use the PAIR index as read index; the pending list tells the mates apart
-        SYL_TRY(b.add(d1, nullptr, n_bases1, o1, 0, n_pairs, 0));
-        SYL_CUDA(cudaMemcpyAsync(dc + 17, dc + 1, 8, cudaMemcpyDeviceToDevice, st));  // pending entries of mate 1
-        SYL_TRY(b.add(d2, nullptr, n_bases2, o2, 0, n_pairs, 0));
-        SYL_CUDA(cudaMemsetAsync(dc + 18, 0, 8, st));
-        if (n_pairs) {
-            k_events_fix_paired<<<ctx->num_sms * 2, EV_THREADS, 0, st>>>(b.b_ev.p, b.b_pend.p, dc + 18, dc + 17, b.cap, d1, o1, d2, o2, 0, no_dedup);
-            k_events_fix_paired<<<ctx->num_sms * 2, EV_THREADS, 0, st>>>(b.b_ev.p, b.b_pend.p, dc + 17, dc + 1, b.cap, d1, o1, d2, o2, 1, no_dedup);
-            ctx->launches += 2;
-            SYL_CUDA(cudaGetLastError());
-        }
-        b.n_reads = n_pairs;       // mean_read_length = mean length of mate 1 (src/sketch.rs:824-826)
-        b.n_bases = n_bases1;
-        uint64_t need = 0;
-        const int rc = b.finish(out, &need);
-        if (rc == SYL_ERR_CAPACITY) { cap_override = need + 16; continue; }
-        if (rc == SYL_OK) SYL_CUDA(cudaStreamSynchronize(st));  // the staged inputs go out of scope
-        return rc;
-    }
-    set_error("event capacity retry failed");
-    return SYL_ERR_CAPACITY;
+    MateInput m1{bases1, nullptr, n_bases1, rec_off1}, m2{bases2, nullptr, n_bases2, rec_off2};
+    return sketch_read_pairs_impl(ctx, mem, false, m1, m2, n_pairs, k, c, no_dedup, sem, out);
+}
+
+int syl_sketch_read_pairs_packed2(syl_ctx *ctx, int mem, const uint32_t *packed1, uint64_t n_bases1, const uint64_t *rec_off1,
+                                  const uint32_t *packed2, uint64_t n_bases2, const uint64_t *rec_off2, uint64_t n_pairs,
+                                  int k, uint64_t c, int no_dedup, int sem, syl_sample **out) {
+    MateInput m1{nullptr, packed1, n_bases1, rec_off1}, m2{nullptr, packed2, n_bases2, rec_off2};
+    return sketch_read_pairs_impl(ctx, mem, true, m1, m2, n_pairs, k, c, no_dedup, sem, out);
 }
 
 int syl_pack_threads(void) { return default_pack_threads(); }

@@ -126,15 +126,15 @@ int seed_enqueue(syl_ctx *ctx, const SeedJob &job) {
 
 // Synchronous form: device-resident inputs, survivors to a device buffer. *n_out is the true
 // number of survivors even when it exceeds cap (then SYL_ERR_CAPACITY).
-// d_rec_off[i] - off_bias is the start of record i inside d_bases (off_bias lets a caller pass a
-// slice of a larger offset array unchanged).
-int seed_device(syl_ctx *ctx, const uint8_t *d_bases, uint64_t n_bases, const uint64_t *d_rec_off, uint64_t off_bias,
-                uint64_t n_rec, int k, uint64_t c, int sem, int with_pos, syl_survivor *d_out,
+// d_rec_off[i] - off_bias is the start of record i inside the batch (off_bias lets a caller pass a
+// slice of a larger offset array unchanged).  Exactly one of d_bases (ASCII) / d_packed (2-bit words) is set.
+int seed_device(syl_ctx *ctx, const uint8_t *d_bases, const uint32_t *d_packed, uint64_t n_bases, const uint64_t *d_rec_off,
+                uint64_t off_bias, uint64_t n_rec, int k, uint64_t c, int sem, int with_pos, syl_survivor *d_out,
                 uint64_t cap, uint64_t *n_out) {
     *n_out = 0;
     cudaStream_t st = ctx->stream;
     SeedJob job;
-    job.d_bases = d_bases; job.n_bases = n_bases; job.d_rec_off = d_rec_off; job.off_bias = off_bias; job.n_rec = n_rec;
+    job.d_bases = d_bases; job.d_packed = d_packed; job.n_bases = n_bases; job.d_rec_off = d_rec_off; job.off_bias = off_bias; job.n_rec = n_rec;
     job.k = k; job.c = c; job.sem = sem; job.with_pos = with_pos; job.d_out = d_out; job.cap = cap;
     job.d_count = reinterpret_cast<unsigned long long *>(ctx->d_counters);
     SYL_CUDA(cudaMemsetAsync(ctx->d_counters, 0, 2 * sizeof(uint64_t), st));
