@@ -3,12 +3,14 @@
 // Replaces sketch_genome (src/sketch.rs:550-622) and sketch_genome_individual (:481-548) for a
 // batch of genomes:
 //   (contig, pos, hash) tuples of all contigs        extract_markers_positions  :582 / :508
-//   vec.sort()                                        :593 -> radix sort by (contig, pos)
-//   k-mers seen >= 2x in the genome are dropped       :594-600,605 -> stable radix sort by hash:
-//        equal hashes of one genome end up adjacent (genomes own contiguous contig ranges)
-//   greedy min-spacing scan, per contig               :602-614 -> one thread per contig; the
-//        reference's `last_contig != contig` reset makes every contig's chain independent and
-//        its `last_pos == 0` sentinel can never collide with a real position (pos >= k-1)
+//   vec.sort()                                        :593 -> survivors in (contig, pos) order, from one of two
+//        front halves: k_seed's per-tile slots, already in position order (c >= 96), or seed_device and one
+//        radix sort by (contig, pos) (every c; the fallback of the slotted one)
+//   k-mers seen >= 2x in the genome are dropped       :594-600,605 -> one open-addressing table of survivor
+//        indices in which every genome owns a region (genomes own contiguous contig ranges)
+//   greedy min-spacing scan, per contig               :602-614 -> k_spacing; the reference's
+//        `last_contig != contig` reset makes every contig's chain independent and its `last_pos == 0`
+//        sentinel can never collide with a real position (pos >= k-1)
 //   kept -> genome_kmers, thinned -> pseudotax_tracked_nonused_kmers, both in position order
 #include <cub/cub.cuh>
 
@@ -42,43 +44,9 @@ __global__ void k_split(const syl_survivor *__restrict__ sv, uint64_t n, uint64_
     hash[i] = s.hash;
 }
 
-__global__ void k_iota32(uint32_t *idx, uint64_t n) {
-    uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (i < n) idx[i] = (uint32_t)i;
-}
-
 __global__ void k_iota64(uint64_t *v, uint64_t n) {
     uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (i < n) v[i] = i;
-}
-
-// contig -> genome (upper_bound over genome_off)
-__global__ void k_contig_genome(const uint64_t *__restrict__ genome_off, uint64_t n_genomes, uint64_t n_contigs,
-                                uint32_t *__restrict__ cg) {
-    uint64_t r = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (r >= n_contigs) return;
-    uint64_t lo = 0, hi = n_genomes + 1;
-    while (lo < hi) {
-        uint64_t mid = (lo + hi) >> 1;
-        if (genome_off[mid] > r) hi = mid; else lo = mid + 1;
-    }
-    cg[r] = (uint32_t)(lo - 1);
-}
-
-// hs/ix: survivors stably sorted by hash (ix = index into the position-sorted arrays).
-// A hash occurring >= 2x inside one genome marks all its occurrences (src/sketch.rs:594-600).
-__global__ void k_flag_dups(const uint64_t *__restrict__ hs, const uint32_t *__restrict__ ix, uint64_t n,
-                            const uint64_t *__restrict__ poskey, const uint32_t *__restrict__ cg,
-                            uint8_t *__restrict__ flag) {
-    uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= n) return;
-    const uint64_t h = hs[i];
-    const uint32_t me = ix[i];
-    const uint32_t g = cg[poskey[me] >> 32];
-    bool dup = false;
-    if (i > 0 && hs[i - 1] == h) dup |= cg[poskey[ix[i - 1]] >> 32] == g;
-    if (i + 1 < n && hs[i + 1] == h) dup |= cg[poskey[ix[i + 1]] >> 32] == g;
-    flag[me] = dup ? 0 : 3;  // 0 = duplicate (dropped); 3 = undecided, resolved by k_spacing
 }
 
 __device__ __forceinline__ uint64_t lower_bound_u64(const uint64_t *a, uint64_t n, uint64_t v) {
@@ -97,9 +65,9 @@ __device__ __forceinline__ uint64_t lower_bound_u64(const uint64_t *a, uint64_t 
 // clusters of closely spaced k-mers, each starting with such a head.  One thread per survivor:
 // heads walk their (tiny: ~1.15 elements at c=200) cluster; everything else returns.
 __global__ void k_spacing(const uint64_t *__restrict__ poskey, uint64_t n, uint64_t min_spacing,
-                          uint8_t *__restrict__ flag, const uint32_t *__restrict__ d_n = nullptr) {
+                          uint8_t *__restrict__ flag, const uint32_t *__restrict__ d_n) {
     const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (d_n && *d_n < n) n = *d_n;
+    if (*d_n < n) n = *d_n;
     if (i >= n || flag[i] == 0) return;
     const uint64_t key = poskey[i], contig = key >> 32, pos = key & 0xFFFFFFFFull;
     // previous non-duplicate survivor of the same contig
@@ -123,47 +91,6 @@ __global__ void k_spacing(const uint64_t *__restrict__ poskey, uint64_t n, uint6
         if (pk - last > min_spacing) { flag[k] = 1; last = pk; } else { flag[k] = 2; }
         prev = pk;
     }
-}
-
-struct FlagIs {
-    uint8_t want;
-    __host__ __device__ __forceinline__ FlagIs(uint8_t w) : want(w) {}
-    __host__ __device__ __forceinline__ bool operator()(const uint8_t &f) const { return f == want; }
-};
-
-// per-genome CSR offsets: number of flag==want survivors before the genome's first survivor
-__global__ void k_genome_offsets(const uint64_t *__restrict__ poskey, uint64_t n, const uint64_t *__restrict__ genome_off,
-                                 uint64_t n_genomes, const uint64_t *__restrict__ scan_kept,
-                                 const uint64_t *__restrict__ scan_tracked, uint64_t total_kept,
-                                 uint64_t total_tracked, const uint64_t *__restrict__ contig_off,
-                                 uint64_t *__restrict__ kmer_off, uint64_t *__restrict__ tracked_off,
-                                 uint64_t *__restrict__ gn_size) {
-    uint64_t g = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (g > n_genomes) return;
-    if (g == n_genomes) {
-        kmer_off[g] = total_kept;
-        tracked_off[g] = total_tracked;
-        return;
-    }
-    const uint64_t first = lower_bound_u64(poskey, n, genome_off[g] << 32);
-    kmer_off[g] = first < n ? scan_kept[first] : total_kept;
-    tracked_off[g] = first < n ? scan_tracked[first] : total_tracked;
-    gn_size[g] = contig_off[genome_off[g + 1]] - contig_off[genome_off[g]];  // src/sketch.rs:581
-}
-
-__global__ void k_scatter_flagged(const uint64_t *__restrict__ hash, const uint8_t *__restrict__ flag, uint64_t n,
-                                  const uint64_t *__restrict__ scan_kept, const uint64_t *__restrict__ scan_tracked,
-                                  uint64_t *__restrict__ kmers, uint64_t *__restrict__ tracked) {
-    uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= n) return;
-    const uint8_t f = flag[i];
-    if (f == 1) kmers[scan_kept[i]] = hash[i];
-    else if (f == 2 && tracked) tracked[scan_tracked[i]] = hash[i];
-}
-
-__global__ void k_flag_to_u64(const uint8_t *__restrict__ flag, uint64_t n, uint8_t want, uint64_t *__restrict__ out) {
-    uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (i < n) out[i] = flag[i] == want ? 1ull : 0ull;
 }
 
 __global__ void k_add_offset(const uint64_t *__restrict__ src, uint64_t n, uint64_t add, uint64_t *__restrict__ dst) {
@@ -198,143 +125,47 @@ static int genomes_alloc(syl_genomes *g, cudaStream_t st, uint64_t n_genomes, ui
     return SYL_OK;
 }
 
-// Generic post-pass: two library radix sorts (position, then hash).  Handles every input; used when the
-// slotted path below does not apply (tiny c, SYL_GENOME_POSTPASS=sort) or reports an overflow.
-// Exactly one of d_bases (ASCII) / d_packed (2-bit words) is set, here and in the two functions below.
-static int sketch_genomes_device_sort(syl_ctx *ctx, const uint8_t *d_bases, const uint32_t *d_packed, uint64_t n_bases,
-                                      const uint64_t *d_contig_off, uint64_t n_contigs, const uint64_t *d_genome_off,
-                                      uint64_t n_genomes, int k, uint64_t c, uint64_t min_spacing, int pseudotax, int sem,
-                                      syl_genomes *out) {
-    cudaStream_t st = ctx->stream;
-    // 1. survivors with positions
-    uint64_t scap = n_bases / c + n_bases / (4 * c) + 65536;
-    if (scap > n_bases) scap = n_bases + 16;
-    DevBuf<syl_survivor> sv;
-    uint64_t N = 0;
-    for (;;) {
-        SYL_TRY(sv.alloc(scap, st));
-        int rc = seed_device(ctx, d_bases, d_packed, n_bases, d_contig_off, 0, n_contigs, k, c, sem, /*with_pos=*/1, sv.p, scap, &N);
-        if (rc == SYL_ERR_CAPACITY) { scap = N + 16; continue; }
-        if (rc != SYL_OK) return rc;
-        break;
-    }
-    if (N >= 0xFFFFFFFFull) { set_error("more than 2^32-2 survivors in one genome batch; split the batch"); return SYL_ERR_ARG; }
-    DevBuf<uint64_t> key_a, key_b, hash_a, hash_b, scan_k, scan_t;
-    DevBuf<uint32_t> idx_a, idx_b, cg;
-    DevBuf<uint8_t> flag, tmp;
-    const uint64_t NA = std::max<uint64_t>(N, 1);
-    SYL_TRY(key_a.alloc(NA, st)); SYL_TRY(key_b.alloc(NA, st));
-    SYL_TRY(hash_a.alloc(NA, st)); SYL_TRY(hash_b.alloc(NA, st));
-    SYL_TRY(idx_a.alloc(NA, st)); SYL_TRY(idx_b.alloc(NA, st));
-    SYL_TRY(scan_k.alloc(NA, st)); SYL_TRY(scan_t.alloc(NA, st));
-    SYL_TRY(flag.alloc(NA, st));
-    SYL_TRY(cg.alloc(n_contigs, st));
-    k_contig_genome<<<nblk(n_contigs, 256), 256, 0, st>>>(d_genome_off, n_genomes, n_contigs, cg.p);
-    ctx->launches++;
-    uint64_t total_kept = 0, total_tracked = 0;
-    KernelTimer kt_post(ctx, SYL_KERNEL_GENOME_POST);
-    if (N) {
-        k_split<<<nblk(N, 256), 256, 0, st>>>(sv.p, N, key_a.p, hash_a.p);
-        // 2. position order: sort by (contig, pos)
-        const int pos_bits = 32 + bits_for(n_contigs);
-        const int hash_bits = bits_for(fmh_threshold(c));
-        size_t t1 = 0, t2 = 0, t3 = 0;
-        cub::DeviceRadixSort::SortPairs(nullptr, t1, key_a.p, key_b.p, hash_a.p, hash_b.p, N, 0, pos_bits, st);
-        cub::DeviceRadixSort::SortPairs(nullptr, t2, hash_b.p, hash_a.p, idx_a.p, idx_b.p, N, 0, hash_bits, st);
-        cub::DeviceScan::ExclusiveSum(nullptr, t3, scan_k.p, scan_k.p, N, st);
-        size_t tb = std::max(t1, std::max(t2, t3));
-        SYL_TRY(tmp.alloc(tb, st));
-        SYL_CUDA(cub::DeviceRadixSort::SortPairs(tmp.p, tb, key_a.p, key_b.p, hash_a.p, hash_b.p, N, 0, pos_bits, st));
-        // now: key_b = poskey sorted, hash_b = hashes in position order
-        // 3. duplicates inside a genome: stable sort of (hash, position index) by hash
-        k_iota32<<<nblk(N, 256), 256, 0, st>>>(idx_a.p, N);
-        tb = std::max(t1, std::max(t2, t3));
-        SYL_CUDA(cub::DeviceRadixSort::SortPairs(tmp.p, tb, hash_b.p, hash_a.p, idx_a.p, idx_b.p, N, 0, hash_bits, st));
-        k_flag_dups<<<nblk(N, 256), 256, 0, st>>>(hash_a.p, idx_b.p, N, key_b.p, cg.p, flag.p);
-        // 4. greedy spacing per contig
-        k_spacing<<<nblk(N, 256), 256, 0, st>>>(key_b.p, N, min_spacing, flag.p);
-        // 5. compaction
-        k_flag_to_u64<<<nblk(N, 256), 256, 0, st>>>(flag.p, N, 1, scan_k.p);
-        k_flag_to_u64<<<nblk(N, 256), 256, 0, st>>>(flag.p, N, 2, scan_t.p);
-        uint64_t *d_last = ctx->d_counters + 4;  // [4],[5]: last flags, [6],[7]: last scans
-        SYL_CUDA(cudaMemcpyAsync(d_last, scan_k.p + (N - 1), 8, cudaMemcpyDeviceToDevice, st));
-        SYL_CUDA(cudaMemcpyAsync(d_last + 1, scan_t.p + (N - 1), 8, cudaMemcpyDeviceToDevice, st));
-        tb = std::max(t1, std::max(t2, t3));
-        SYL_CUDA(cub::DeviceScan::ExclusiveSum(tmp.p, tb, scan_k.p, scan_k.p, N, st));
-        tb = std::max(t1, std::max(t2, t3));
-        SYL_CUDA(cub::DeviceScan::ExclusiveSum(tmp.p, tb, scan_t.p, scan_t.p, N, st));
-        SYL_CUDA(cudaMemcpyAsync(d_last + 2, scan_k.p + (N - 1), 8, cudaMemcpyDeviceToDevice, st));
-        SYL_CUDA(cudaMemcpyAsync(d_last + 3, scan_t.p + (N - 1), 8, cudaMemcpyDeviceToDevice, st));
-        SYL_CUDA(cudaMemcpyAsync(ctx->h_counters + 4, d_last, 32, cudaMemcpyDeviceToHost, st));
-        SYL_CUDA(cudaStreamSynchronize(st));
-        total_kept = ctx->h_counters[4] + ctx->h_counters[6];
-        total_tracked = ctx->h_counters[5] + ctx->h_counters[7];
-        ctx->launches += 7 + 4;
-    }
-    out->has_tracked = pseudotax ? 1 : 0;
-    if (!pseudotax) total_tracked = 0;
-    SYL_TRY(genomes_alloc(out, st, n_genomes, total_kept, total_tracked));
-    if (N) {
-        k_scatter_flagged<<<nblk(N, 256), 256, 0, st>>>(hash_b.p, flag.p, N, scan_k.p, scan_t.p, out->kmers,
-                                                         pseudotax ? out->tracked : nullptr);
-        ctx->launches++;
-    }
-    k_genome_offsets<<<nblk(n_genomes + 1, 128), 128, 0, st>>>(key_b.p, N, d_genome_off, n_genomes, scan_k.p, scan_t.p,
-                                                               total_kept, pseudotax ? total_tracked : 0, d_contig_off,
-                                                               out->kmer_off, out->tracked_off, out->gn_size);
-    ctx->launches++;
-    kt_post.stop();
-    SYL_CUDA(cudaGetLastError());
-    if (!pseudotax) SYL_CUDA(cudaMemsetAsync(out->tracked_off, 0, (n_genomes + 1) * 8, st));
-    SYL_CUDA(cudaStreamSynchronize(st));
-    return SYL_OK;
-}
-
 // ------------------------------------------------------------------------------------------------
-// Sort-free post-pass.
-//   * k_seed writes every tile's survivors into the tile's own slot (SlotOut), so the output is in
-//     tile = position order already; its flush orders the <= 512 survivors INSIDE a tile by
-//     (contig, position) in shared memory and compacts the tiles (scan of the per-tile counts).
-//   * duplicates (a hash seen twice in one genome, src/sketch.rs:594-600): a genome's survivors are now
-//     contiguous; they are grouped through one L2-resident open-addressing table in which every genome
-//     owns a region of twice its survivor count — no sort by hash, no per-CTA capacity to overflow.
-//   * k_spacing as before; kept / tracked survivors are compacted with block counts + one small scan.
-// One host synchronisation (the totals), like the read-sketch path.
+// Post-pass.  A front half puts the survivors in (contig, pos) order: the slotted one (k_seed's per-tile slots, no
+// sort) when c >= 96, the sorted one (radix sort) otherwise and whenever the slotted one overflows.  The back half
+// turns them into the CSR: duplicates through one table, k_spacing, kept / tracked survivors compacted with block
+// counts + one small scan.  N lives in device memory; the back half makes one host synchronisation (the totals).
 constexpr uint32_t GEN_SLOT = 512;        // survivors per tile slot (= the seeding kernel's staging capacity)
 
-// tile t: slot -> compact arrays at toff[t].  (Round 2 first ordered the slot here, by the rank of each survivor's
-// window start in a 32 768-bit map of the tile; that ranking now runs inside k_seed's flush, where the survivors are
-// still in shared memory, and this kernel is a copy.)
+// tile t: slot -> compact arrays at toff[t] (entries at or past cap are dropped: the back half then reports N > cap).
+// One warp per tile: k_seed's slotted flush already wrote the slot in position order, so this is a copy.
 __global__ void __launch_bounds__(256)
 k_tile_compact(const syl_survivor *__restrict__ slots, const uint32_t *__restrict__ tile_cnt, const uint32_t *__restrict__ toff,
-               uint64_t n_tiles, uint64_t *__restrict__ poskey, uint64_t *__restrict__ hash) {
-    // one warp per tile: the slot is already in position order (k_seed's slotted flush), so this is a copy
+               uint64_t n_tiles, uint32_t cap, uint64_t *__restrict__ poskey, uint64_t *__restrict__ hash) {
     const uint64_t t = (uint64_t)blockIdx.x * 8 + (threadIdx.x >> 5);
     if (t >= n_tiles) return;
     const uint32_t n = tile_cnt[t], out0 = toff[t];
     const syl_survivor *src = slots + t * GEN_SLOT;
-    for (uint32_t i = threadIdx.x & 31; i < n; i += 32) {
+    for (uint32_t i = threadIdx.x & 31; i < n && out0 + i < cap; i += 32) {
         const syl_survivor sv = src[i];
         poskey[out0 + i] = ((uint64_t)sv.rec << 32) | sv.pos;
         hash[out0 + i] = sv.hash;
     }
 }
 
-// gs[g] = index of genome g's first survivor (g = 0 .. n_genomes; gs[n_genomes] = N); N from device memory
-__global__ void k_genome_ranges(const uint64_t *__restrict__ poskey, const uint32_t *__restrict__ d_n, const uint64_t *__restrict__ genome_off,
-                                uint64_t n_genomes, uint32_t *__restrict__ gs) {
+// gs[g] = index of genome g's first survivor (g = 0 .. n_genomes); gs[n_genomes] = min(N, cap), the count every
+// later kernel of the back half works on
+__global__ void k_genome_ranges(const uint64_t *__restrict__ poskey, const uint32_t *__restrict__ d_n, uint32_t cap,
+                                const uint64_t *__restrict__ genome_off, uint64_t n_genomes, uint32_t *__restrict__ gs) {
     const uint64_t g = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (g > n_genomes) return;
-    const uint64_t N = *d_n;
-    gs[g] = g == n_genomes ? (uint32_t)N : (uint32_t)lower_bound_u64(poskey, N, genome_off[g] << 32);
+    const uint32_t N = min(*d_n, cap);
+    gs[g] = g == n_genomes ? N : (uint32_t)lower_bound_u64(poskey, N, genome_off[g] << 32);
 }
 
 // ---- duplicates (src/sketch.rs:594-600,605: a hash seen twice in one genome drops all its occurrences) ----
-// One open-addressing table for the whole batch in global memory (blocks touch only their genomes' regions): genome g owns the
-// slots [2 * gs[g], 2 * gs[g+1]) — load factor 1/2 whatever the genome's size or its share of repeats, so there is
-// no table-overflow case.  A key is the 64-bit hash (< 2^63 for every c >= 2); bit 63 of a stored key is the
-// "seen again" mark, set with an atomic OR by every later occurrence; the empty key is all ones.
-constexpr unsigned long long DUP_EMPTY = 0xFFFFFFFFFFFFFFFFull, DUP_MARK = 1ull << 63;
+// One open-addressing table of survivor indices for the whole batch in global memory: genome g owns the slots
+// [2 * gs[g], 2 * gs[g+1]) — load factor 1/2 whatever the genome's size or its share of repeats, so there is no
+// table-overflow case.  Slots are only ever filled, and all occurrences of a hash walk the same probe sequence, so
+// they all stop at the same slot: the first one that holds an occurrence of the hash.  The occurrence that fills
+// it stays undecided unless another one arrives; every later occurrence drops itself and the one in the slot.
+// No hash value or bit is reserved, so the rule holds for every c >= 1 (at c = 1 hashes use all 64 bits).
+constexpr uint32_t DUP_EMPTY = 0xFFFFFFFFu;  // no survivor index (N <= 2^32 - 2)
 
 // genome of survivor i: the last g with gs[g] <= i, searched between the genomes of the block's first and last
 // survivor (s_lo / s_hi, found once per block)
@@ -352,48 +183,30 @@ __device__ __forceinline__ uint32_t dup_genome_of(const uint32_t *__restrict__ g
     return lo;
 }
 
-__device__ __forceinline__ uint32_t dup_slot(unsigned long long h, uint32_t size) {
-    return (uint32_t)((((h >> 6) & 0xFFFFFFFFull) * size) >> 32);  // hashes are uniform below the threshold: so are these 32 bits
-}
+// 32 hash bits scaled to [0, size): hashes are uniform below the threshold, so are these bits.  64-bit, so that a
+// genome may own more than 2^32 slots.
+__device__ __forceinline__ uint64_t dup_slot(uint64_t h, uint64_t size) { return __umul64hi((h >> 6) << 32, size); }
 
+// flag[] = 3 (undecided) on entry; a hash occurring >= 2x in its genome leaves all its occurrences at 0 (dropped)
 __global__ void __launch_bounds__(256)
-k_dups_insert(const uint64_t *__restrict__ hash, const uint32_t *__restrict__ gs, uint64_t n_genomes, const uint32_t *__restrict__ d_n,
-              uint32_t cap, unsigned long long *__restrict__ table) {
+k_dups(const uint64_t *__restrict__ hash, const uint32_t *__restrict__ gs, uint64_t n_genomes, uint32_t *__restrict__ table,
+       uint8_t *__restrict__ flag) {
     __shared__ uint32_t s_lo, s_hi;
-    const uint32_t N = min(*d_n, cap), first = blockIdx.x * 256u;
+    const uint64_t N = gs[n_genomes], first = (uint64_t)blockIdx.x * 256;
     if (first >= N) return;
-    const uint32_t i = first + threadIdx.x;
-    const uint32_t g = dup_genome_of(gs, n_genomes, min(i, N - 1), first, min(first + 255u, N - 1), &s_lo, &s_hi);
+    const uint64_t i = first + threadIdx.x;
+    const uint32_t g = dup_genome_of(gs, n_genomes, (uint32_t)min(i, N - 1), (uint32_t)first, (uint32_t)min(first + 255, N - 1),
+                                     &s_lo, &s_hi);
     if (i >= N) return;
-    const uint32_t base = gs[g], size = 2u * (gs[g + 1] - base);
-    unsigned long long *T = table + 2ull * base;
-    const unsigned long long h = hash[i];
-    uint32_t sl = dup_slot(h, size);
-    for (;;) {
-        const unsigned long long prev = atomicCAS(&T[sl], DUP_EMPTY, h);
-        if (prev == DUP_EMPTY) break;
-        if ((prev & ~DUP_MARK) == h) { if (!(prev & DUP_MARK)) atomicOr(&T[sl], DUP_MARK); break; }
+    const uint64_t size = 2ull * (gs[g + 1] - gs[g]);
+    uint32_t *T = table + 2ull * gs[g];
+    const uint64_t h = hash[i];
+    for (uint64_t sl = dup_slot(h, size);;) {
+        const uint32_t j = atomicCAS(&T[sl], DUP_EMPTY, (uint32_t)i);
+        if (j == DUP_EMPTY) return;
+        if (hash[j] == h) { flag[i] = 0; flag[j] = 0; return; }
         if (++sl == size) sl = 0;
     }
-}
-
-// flag[i] = 0: the hash occurs >= 2x in its genome (dropped), 3: undecided (k_spacing decides kept / tracked)
-__global__ void __launch_bounds__(256)
-k_dups_flag(const uint64_t *__restrict__ hash, const uint32_t *__restrict__ gs, uint64_t n_genomes, const uint32_t *__restrict__ d_n,
-            uint32_t cap, const unsigned long long *__restrict__ table, uint8_t *__restrict__ flag) {
-    __shared__ uint32_t s_lo, s_hi;
-    const uint32_t N = min(*d_n, cap), first = blockIdx.x * 256u;
-    if (first >= N) return;
-    const uint32_t i = first + threadIdx.x;
-    const uint32_t g = dup_genome_of(gs, n_genomes, min(i, N - 1), first, min(first + 255u, N - 1), &s_lo, &s_hi);
-    if (i >= N) return;
-    const uint32_t base = gs[g], size = 2u * (gs[g + 1] - base);
-    const unsigned long long *T = table + 2ull * base;
-    const unsigned long long h = hash[i];
-    uint32_t sl = dup_slot(h, size);
-    unsigned long long k;
-    while (((k = T[sl]) & ~DUP_MARK) != h) { if (++sl == size) sl = 0; }  // every hash was inserted: the walk ends
-    flag[i] = (k & DUP_MARK) ? 0 : 3;
 }
 
 // per block of 1024 survivors: number of kept (flag 1) and tracked (flag 2) ones
@@ -457,54 +270,34 @@ __global__ void k_genome_offsets32(const uint32_t *__restrict__ gs, const uint32
     if (g < n_genomes) gn_size[g] = contig_off[genome_off[g + 1]] - contig_off[genome_off[g]];  // src/sketch.rs:581
 }
 
-// rc SYL_ERR_UNSUPPORTED: a slot / table overflowed — the caller takes the generic path
-static int sketch_genomes_device_slots(syl_ctx *ctx, const uint8_t *d_bases, const uint32_t *d_packed, uint64_t n_bases,
-                                       const uint64_t *d_contig_off, uint64_t n_contigs, const uint64_t *d_genome_off,
-                                       uint64_t n_genomes, int k, uint64_t c, uint64_t min_spacing, int pseudotax, int sem,
-                                       syl_genomes *out) {
+// poskey[i] = contig << 32 | pos and hash[i], i < N, in (contig, pos) order; N = *d_n (device memory), 1 <= cap < 2^32 - 1
+// bounds the arrays.  The element-wise grids are sized for cap (threads past N return).  Returns SYL_ERR_UNSUPPORTED with
+// the handle left empty when N > cap or *d_overflow (the slotted front half's slot overflow) is set: the caller redoes the
+// batch on the sorted front half.  kt, the post-pass timer the front half started, stops before the host synchronisation.
+static int genomes_back_half(syl_ctx *ctx, KernelTimer &kt, const uint64_t *poskey, const uint64_t *hash, const uint32_t *d_n,
+                             uint64_t cap, const uint32_t *d_overflow, const uint64_t *d_contig_off, const uint64_t *d_genome_off,
+                             uint64_t n_genomes, uint64_t min_spacing, int pseudotax, syl_genomes *out) {
     cudaStream_t st = ctx->stream;
-    const uint64_t n_tiles = seed_cta_tiles(n_bases);
-    if (n_tiles * GEN_SLOT >= 0xFFFFFFFFull) { set_error("genome batch too large; split the batch"); return SYL_ERR_ARG; }
-    const uint64_t cap = std::min<uint64_t>(n_tiles * GEN_SLOT, n_bases / c + n_bases / (4 * c) + 65536);  // compact survivors
-    DevBuf<syl_survivor> slots;
-    DevBuf<uint32_t> tile_cnt, toff, gs, bk, bt, bk_off, bt_off, scan_k, scan_t, t1, t2, flags32;
-    DevBuf<uint64_t> poskey, hash, tmp_k, tmp_t;
-    DevBuf<unsigned long long> dup_table;
+    DevBuf<uint32_t> gs, dup_table, bk, bt, bk_off, bt_off, scan_k, scan_t, t1, t2, t3, t4;
+    DevBuf<uint64_t> tmp_k, tmp_t;
     DevBuf<uint8_t> flag;
-    SYL_TRY(slots.alloc(n_tiles * GEN_SLOT, st));
-    SYL_TRY(tile_cnt.alloc(n_tiles, st)); SYL_TRY(toff.alloc(n_tiles + 1, st));
-    SYL_TRY(flags32.alloc(2, st));  // [0] slot overflow, [1] unused
-    SYL_CUDA(cudaMemsetAsync(flags32.p, 0, 8, st));
-    SYL_CUDA(cudaMemsetAsync(ctx->d_counters, 0, 2 * sizeof(uint64_t), st));
-    SeedJob job;
-    job.d_bases = d_bases; job.d_packed = d_packed; job.n_bases = n_bases; job.d_rec_off = d_contig_off; job.off_bias = 0; job.n_rec = n_contigs;
-    job.k = k; job.c = c; job.sem = sem; job.with_pos = 1; job.d_out = slots.p; job.cap = n_tiles * GEN_SLOT;
-    job.d_count = reinterpret_cast<unsigned long long *>(ctx->d_counters);
-    job.slot_cap = GEN_SLOT; job.d_tile_cnt = tile_cnt.p; job.d_slot_overflow = flags32.p;
-    SYL_TRY(seed_enqueue(ctx, job));
-    KernelTimer kt_post(ctx, SYL_KERNEL_GENOME_POST);
-    SYL_TRY(scan_u32(ctx, tile_cnt.p, n_tiles, toff.p, t1, t2));   // toff[n_tiles] = N (device)
-    const uint32_t *d_n = toff.p + n_tiles;
-    SYL_TRY(poskey.alloc(cap, st)); SYL_TRY(hash.alloc(cap, st)); SYL_TRY(flag.alloc(cap, st));
-    k_tile_compact<<<nblk(n_tiles, 8), 256, 0, st>>>(slots.p, tile_cnt.p, toff.p, n_tiles, poskey.p, hash.p);
     SYL_TRY(gs.alloc(n_genomes + 1, st));
-    k_genome_ranges<<<nblk(n_genomes + 1, 256), 256, 0, st>>>(poskey.p, d_n, d_genome_off, n_genomes, gs.p);
-    SYL_TRY(dup_table.alloc(2 * cap, st));
-    SYL_CUDA(cudaMemsetAsync(dup_table.p, 0xFF, 2 * cap * sizeof(unsigned long long), st));
-    k_dups_insert<<<nblk(cap, 256), 256, 0, st>>>(hash.p, gs.p, n_genomes, d_n, (uint32_t)cap, dup_table.p);
-    k_dups_flag<<<nblk(cap, 256), 256, 0, st>>>(hash.p, gs.p, n_genomes, d_n, (uint32_t)cap, dup_table.p, flag.p);
-    // N is only known on the device: size the element-wise grids for the capacity (threads past N return)
-    k_spacing<<<nblk(cap, 256), 256, 0, st>>>(poskey.p, cap, min_spacing, flag.p, d_n);
+    k_genome_ranges<<<nblk(n_genomes + 1, 256), 256, 0, st>>>(poskey, d_n, (uint32_t)cap, d_genome_off, n_genomes, gs.p);
+    const uint32_t *d_nc = gs.p + n_genomes;  // min(N, cap)
+    SYL_TRY(flag.alloc(cap, st)); SYL_TRY(dup_table.alloc(2 * cap, st));
+    SYL_CUDA(cudaMemsetAsync(flag.p, 3, cap, st));
+    SYL_CUDA(cudaMemsetAsync(dup_table.p, 0xFF, 2 * cap * sizeof(uint32_t), st));
+    k_dups<<<nblk(cap, 256), 256, 0, st>>>(hash, gs.p, n_genomes, dup_table.p, flag.p);
+    k_spacing<<<nblk(cap, 256), 256, 0, st>>>(poskey, cap, min_spacing, flag.p, d_nc);
     const uint64_t nb = (cap + 1023) / 1024;
     SYL_TRY(bk.alloc(nb, st)); SYL_TRY(bt.alloc(nb, st)); SYL_TRY(bk_off.alloc(nb + 1, st)); SYL_TRY(bt_off.alloc(nb + 1, st));
     SYL_TRY(scan_k.alloc(cap, st)); SYL_TRY(scan_t.alloc(cap, st)); SYL_TRY(tmp_k.alloc(cap, st)); SYL_TRY(tmp_t.alloc(cap, st));
-    k_flag_counts<<<(unsigned)nb, 256, 0, st>>>(flag.p, d_n, bk.p, bt.p);
+    k_flag_counts<<<(unsigned)nb, 256, 0, st>>>(flag.p, d_nc, bk.p, bt.p);
     SYL_TRY(scan_u32(ctx, bk.p, nb, bk_off.p, t1, t2));
-    DevBuf<uint32_t> t3, t4;
     SYL_TRY(scan_u32(ctx, bt.p, nb, bt_off.p, t3, t4));
-    k_scatter_flagged_blocks<<<(unsigned)nb, 1024, 0, st>>>(hash.p, flag.p, d_n, bk_off.p, bt_off.p, tmp_k.p, pseudotax ? tmp_t.p : nullptr,
+    k_scatter_flagged_blocks<<<(unsigned)nb, 1024, 0, st>>>(hash, flag.p, d_nc, bk_off.p, bt_off.p, tmp_k.p, pseudotax ? tmp_t.p : nullptr,
                                                             scan_k.p, scan_t.p);
-    ctx->launches += 8;
+    ctx->launches += 5;
     // per-genome offsets go straight into the handle; the k-mer arrays need the totals first
     out->has_tracked = pseudotax ? 1 : 0;
     out->stream = st;
@@ -513,20 +306,24 @@ static int sketch_genomes_device_slots(syl_ctx *ctx, const uint8_t *d_bases, con
     SYL_TRY(hblock_alloc(out->owner, (void **)&out->kmer_off, (n_genomes + 1) * 8));
     SYL_TRY(hblock_alloc(out->owner, (void **)&out->tracked_off, (n_genomes + 1) * 8));
     SYL_TRY(hblock_alloc(out->owner, (void **)&out->gn_size, std::max<uint64_t>(n_genomes, 1) * 8));
-    k_genome_offsets32<<<nblk(n_genomes + 1, 128), 128, 0, st>>>(gs.p, d_n, d_genome_off, n_genomes, scan_k.p, scan_t.p, bk_off.p + nb,
+    k_genome_offsets32<<<nblk(n_genomes + 1, 128), 128, 0, st>>>(gs.p, d_nc, d_genome_off, n_genomes, scan_k.p, scan_t.p, bk_off.p + nb,
                                                                  bt_off.p + nb, pseudotax, d_contig_off, out->kmer_off, out->tracked_off,
                                                                  out->gn_size);
     ctx->launches++;
-    kt_post.stop();
+    kt.stop();
     SYL_CUDA(cudaGetLastError());
-    uint32_t *h32 = reinterpret_cast<uint32_t *>(ctx->h_counters + 4);
-    SYL_CUDA(cudaMemcpyAsync(h32, flags32.p, 8, cudaMemcpyDeviceToHost, st));
-    SYL_CUDA(cudaMemcpyAsync(h32 + 2, bk_off.p + nb, 4, cudaMemcpyDeviceToHost, st));
-    SYL_CUDA(cudaMemcpyAsync(h32 + 3, bt_off.p + nb, 4, cudaMemcpyDeviceToHost, st));
-    SYL_CUDA(cudaMemcpyAsync(h32 + 4, d_n, 4, cudaMemcpyDeviceToHost, st));
-    SYL_CUDA(cudaStreamSynchronize(st));  // the one synchronisation of the call
-    if (h32[0] || h32[1] || h32[4] > cap) return SYL_ERR_UNSUPPORTED;
-    const uint64_t total_kept = h32[2], total_tracked = pseudotax ? h32[3] : 0;
+    uint32_t *h32 = reinterpret_cast<uint32_t *>(ctx->h_counters + 4);  // N, kept, tracked, slot overflow
+    SYL_CUDA(cudaMemcpyAsync(h32, d_n, 4, cudaMemcpyDeviceToHost, st));
+    SYL_CUDA(cudaMemcpyAsync(h32 + 1, bk_off.p + nb, 4, cudaMemcpyDeviceToHost, st));
+    SYL_CUDA(cudaMemcpyAsync(h32 + 2, bt_off.p + nb, 4, cudaMemcpyDeviceToHost, st));
+    if (d_overflow) SYL_CUDA(cudaMemcpyAsync(h32 + 3, d_overflow, 4, cudaMemcpyDeviceToHost, st));
+    SYL_CUDA(cudaStreamSynchronize(st));  // the one synchronisation of the back half
+    if (h32[0] > cap || (d_overflow && h32[3])) {
+        hblock_free(out->owner, out->kmer_off); hblock_free(out->owner, out->tracked_off); hblock_free(out->owner, out->gn_size);
+        out->kmer_off = out->tracked_off = out->gn_size = nullptr;
+        return SYL_ERR_UNSUPPORTED;
+    }
+    const uint64_t total_kept = h32[1], total_tracked = pseudotax ? h32[2] : 0;
     SYL_TRY(hblock_alloc(out->owner, (void **)&out->kmers, std::max<uint64_t>(total_kept, 1) * 8));
     SYL_TRY(hblock_alloc(out->owner, (void **)&out->tracked, std::max<uint64_t>(total_tracked, 1) * 8));
     out->total_kmers = total_kept;
@@ -536,22 +333,94 @@ static int sketch_genomes_device_slots(syl_ctx *ctx, const uint8_t *d_bases, con
     return SYL_OK;
 }
 
+// Slotted front half: k_seed writes every tile's survivors into the tile's own slot (SlotOut) in position order (its
+// flush ranks the <= 512 survivors of a tile by window start); a scan of the per-tile counts and k_tile_compact make
+// them one array.  No host synchronisation before the back half.  Exactly one of d_bases (ASCII) / d_packed (2-bit
+// words) is set, here and in the functions below.
+static int genomes_slotted(syl_ctx *ctx, const uint8_t *d_bases, const uint32_t *d_packed, uint64_t n_bases,
+                           const uint64_t *d_contig_off, uint64_t n_contigs, const uint64_t *d_genome_off, uint64_t n_genomes,
+                           int k, uint64_t c, uint64_t min_spacing, int pseudotax, int sem, syl_genomes *out) {
+    cudaStream_t st = ctx->stream;
+    const uint64_t n_tiles = seed_cta_tiles(n_bases);
+    if (n_tiles * GEN_SLOT >= 0xFFFFFFFFull) { set_error("genome batch too large; split the batch"); return SYL_ERR_ARG; }
+    const uint64_t cap = std::min<uint64_t>(n_tiles * GEN_SLOT, n_bases / c + n_bases / (4 * c) + 65536);  // compact survivors
+    DevBuf<syl_survivor> slots;
+    DevBuf<uint32_t> tile_cnt, toff, overflow, t1, t2;
+    DevBuf<uint64_t> poskey, hash;
+    SYL_TRY(slots.alloc(n_tiles * GEN_SLOT, st));
+    SYL_TRY(tile_cnt.alloc(n_tiles, st)); SYL_TRY(toff.alloc(n_tiles + 1, st));
+    SYL_TRY(overflow.alloc(1, st));
+    SYL_CUDA(cudaMemsetAsync(overflow.p, 0, 4, st));
+    SYL_CUDA(cudaMemsetAsync(ctx->d_counters, 0, 2 * sizeof(uint64_t), st));
+    SeedJob job;
+    job.d_bases = d_bases; job.d_packed = d_packed; job.n_bases = n_bases; job.d_rec_off = d_contig_off; job.off_bias = 0; job.n_rec = n_contigs;
+    job.k = k; job.c = c; job.sem = sem; job.with_pos = 1; job.d_out = slots.p; job.cap = n_tiles * GEN_SLOT;
+    job.d_count = reinterpret_cast<unsigned long long *>(ctx->d_counters);
+    job.slot_cap = GEN_SLOT; job.d_tile_cnt = tile_cnt.p; job.d_slot_overflow = overflow.p;
+    SYL_TRY(seed_enqueue(ctx, job));
+    KernelTimer kt_post(ctx, SYL_KERNEL_GENOME_POST);
+    SYL_TRY(scan_u32(ctx, tile_cnt.p, n_tiles, toff.p, t1, t2));   // toff[n_tiles] = N (device)
+    SYL_TRY(poskey.alloc(cap, st)); SYL_TRY(hash.alloc(cap, st));
+    k_tile_compact<<<nblk(n_tiles, 8), 256, 0, st>>>(slots.p, tile_cnt.p, toff.p, n_tiles, (uint32_t)cap, poskey.p, hash.p);
+    ctx->launches++;
+    return genomes_back_half(ctx, kt_post, poskey.p, hash.p, toff.p + n_tiles, cap, overflow.p, d_contig_off, d_genome_off,
+                             n_genomes, min_spacing, pseudotax, out);
+}
+
+// Sorted front half, for every input: survivors with positions from seed_device (one host synchronisation, which
+// also sizes the buffers), then one radix sort by (contig, pos) carrying the hash.
+static int genomes_sorted(syl_ctx *ctx, const uint8_t *d_bases, const uint32_t *d_packed, uint64_t n_bases,
+                          const uint64_t *d_contig_off, uint64_t n_contigs, const uint64_t *d_genome_off, uint64_t n_genomes,
+                          int k, uint64_t c, uint64_t min_spacing, int pseudotax, int sem, syl_genomes *out) {
+    cudaStream_t st = ctx->stream;
+    uint64_t scap = n_bases / c + n_bases / (4 * c) + 65536;
+    if (scap > n_bases) scap = n_bases + 16;
+    DevBuf<syl_survivor> sv;
+    uint64_t N = 0;
+    for (;;) {
+        SYL_TRY(sv.alloc(scap, st));
+        int rc = seed_device(ctx, d_bases, d_packed, n_bases, d_contig_off, 0, n_contigs, k, c, sem, /*with_pos=*/1, sv.p, scap, &N);
+        if (rc == SYL_ERR_CAPACITY) { scap = N + 16; continue; }
+        if (rc != SYL_OK) return rc;
+        break;
+    }
+    if (N >= 0xFFFFFFFFull) { set_error("more than 2^32-2 survivors in one genome batch; split the batch"); return SYL_ERR_ARG; }
+    KernelTimer kt_post(ctx, SYL_KERNEL_GENOME_POST);
+    const uint64_t NA = std::max<uint64_t>(N, 1);
+    DevBuf<uint64_t> key_b, hash_b;
+    SYL_TRY(key_b.alloc(NA, st)); SYL_TRY(hash_b.alloc(NA, st));
+    if (N) {
+        DevBuf<uint64_t> key_a, hash_a;
+        DevBuf<uint8_t> tmp;
+        SYL_TRY(key_a.alloc(N, st)); SYL_TRY(hash_a.alloc(N, st));
+        k_split<<<nblk(N, 256), 256, 0, st>>>(sv.p, N, key_a.p, hash_a.p);
+        const int pos_bits = 32 + bits_for(n_contigs);
+        size_t tb = 0;
+        cub::DeviceRadixSort::SortPairs(nullptr, tb, key_a.p, key_b.p, hash_a.p, hash_b.p, N, 0, pos_bits, st);
+        SYL_TRY(tmp.alloc(tb, st));
+        SYL_CUDA(cub::DeviceRadixSort::SortPairs(tmp.p, tb, key_a.p, key_b.p, hash_a.p, hash_b.p, N, 0, pos_bits, st));
+        ctx->launches += 2;
+    }
+    sv.release();
+    // seed_device left N (< 2^32 - 1) in the u64 d_counters[0]: its low word is the back half's count
+    return genomes_back_half(ctx, kt_post, key_b.p, hash_b.p, reinterpret_cast<const uint32_t *>(ctx->d_counters), NA, nullptr,
+                             d_contig_off, d_genome_off, n_genomes, min_spacing, pseudotax, out);
+}
+
 int sketch_genomes_device(syl_ctx *ctx, const uint8_t *d_bases, const uint32_t *d_packed, uint64_t n_bases,
                           const uint64_t *d_contig_off, uint64_t n_contigs, const uint64_t *d_genome_off, uint64_t n_genomes,
                           int k, uint64_t c, uint64_t min_spacing, int pseudotax, int sem, syl_genomes *out) {
-    const char *e = getenv("SYL_GENOME_POSTPASS");  // "sort" forces the generic path (tests); read per call
+    const char *e = getenv("SYL_GENOME_POSTPASS");  // "sort" forces the sorted front half (tests); read per call
     const bool force_sort = e && std::string(e) == "sort";
     // slots hold 512 survivors per 32K-base tile: c >= 96 keeps the expected number below 350
     if (!force_sort && c >= 96 && n_bases && n_contigs && n_genomes) {
-        const int rc = sketch_genomes_device_slots(ctx, d_bases, d_packed, n_bases, d_contig_off, n_contigs, d_genome_off,
-                                                   n_genomes, k, c, min_spacing, pseudotax, sem, out);
+        const int rc = genomes_slotted(ctx, d_bases, d_packed, n_bases, d_contig_off, n_contigs, d_genome_off, n_genomes, k, c,
+                                       min_spacing, pseudotax, sem, out);
         if (rc != SYL_ERR_UNSUPPORTED) return rc;
-        // a slot or table overflowed (low-complexity sequence): release what was allocated and take the generic path
-        hblock_free(out->owner, out->kmer_off); hblock_free(out->owner, out->tracked_off); hblock_free(out->owner, out->gn_size);
-        out->kmer_off = out->tracked_off = out->gn_size = nullptr;
+        // a slot or the compact arrays overflowed (low-complexity sequence): redo the batch on the sorted front half
     }
-    return sketch_genomes_device_sort(ctx, d_bases, d_packed, n_bases, d_contig_off, n_contigs, d_genome_off, n_genomes, k, c,
-                                      min_spacing, pseudotax, sem, out);
+    return genomes_sorted(ctx, d_bases, d_packed, n_bases, d_contig_off, n_contigs, d_genome_off, n_genomes, k, c, min_spacing,
+                          pseudotax, sem, out);
 }
 
 // packed: the input is 2-bit words (device or host memory); else ASCII

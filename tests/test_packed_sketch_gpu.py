@@ -258,7 +258,8 @@ def _contigs_at_tile_edges(rng, k):
 @pytest.mark.parametrize("postpass", ["slots", "sort"])
 @pytest.mark.parametrize("k,sem", [(31, 1), (21, 0)])
 def test_genomes_multicontig_at_tile_edges(ctx, monkeypatch, k, sem, postpass):
-    """c >= 96 takes the slotted post-pass unless SYL_GENOME_POSTPASS=sort; c < 96 always takes the sort path."""
+    """c >= 96 takes the slotted front half of the post-pass unless SYL_GENOME_POSTPASS=sort; c < 96 (down to c = 1,
+    where every hash below u64::MAX survives) always takes the sorted one."""
     monkeypatch.delenv("SYL_GENOME_POSTPASS", raising=False)
     if postpass == "sort":
         monkeypatch.setenv("SYL_GENOME_POSTPASS", "sort")
@@ -268,6 +269,9 @@ def test_genomes_multicontig_at_tile_edges(ctx, monkeypatch, k, sem, postpass):
     check_genomes_packed(ctx, buf, coff, goff, k=k, c=128, min_spacing=10, sem=sem, individual=True)
     check_genomes_packed(ctx, buf, coff, goff, k=k, c=11, sem=sem)
     check_genomes_packed(ctx, buf, coff, goff, k=k, c=3, min_spacing=5, sem=sem, pseudotax=False)
+    check_genomes_packed(ctx, buf, coff, goff, k=k, c=2, min_spacing=5, sem=sem)
+    d = check_genomes_packed(ctx, buf, coff, goff, k=k, c=1, sem=sem)
+    assert (np.concatenate([d["kmers"], d["tracked"]]) >= np.uint64(1 << 63)).any()   # c = 1: hashes use all 64 bits
 
 
 def test_genomes_every_byte_value(ctx):

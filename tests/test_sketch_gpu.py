@@ -47,6 +47,24 @@ def rand_seqs(rng, lengths, alphabet=b"ACGT"):
     return [bytes(rng.choice(list(alphabet), size=int(n)).astype(np.uint8)) for n in lengths]
 
 
+def check_repeat_and_shared(ctx, rng, k=31, c=200, sem=1):
+    """A segment x three times in genome 0 (twice in one contig): all its markers are dropped there.  A segment y
+    exactly once in each of genomes 1 and 2: all its markers are kept or tracked in both."""
+    from oracle import oracle as O
+    x, y, *f = rand_seqs(rng, [20000, 20000, 3000, 3000, 3000, 500, 500, 2000, 2000, 100, 4000, 1000])
+    contigs = [f[0] + x + f[1] + x + f[2], f[3] + x + f[4], f[5] + y + f[6], f[7], f[8] + y + f[9]]
+    buf, coff = flatten(contigs)
+    d = check_genomes(ctx, buf, coff, np.array([0, 2, 3, 5], dtype=np.uint64), k=k, c=c, sem=sem)
+
+    def sketch(g):
+        return (set(d["kmers"][int(d["kmer_off"][g]):int(d["kmer_off"][g + 1])].tolist())
+                | set(d["tracked"][int(d["tracked_off"][g]):int(d["tracked_off"][g + 1])].tolist()))
+    mx, my = (set(O.extract_markers(s, k=k, c=c, sem=sem).tolist()) for s in (x, y))
+    assert mx and my
+    assert not mx & sketch(0)
+    assert my <= sketch(1) and my <= sketch(2)
+
+
 def test_reads_dedup_k12(ctx):
     recs = read_fastx(os.path.join(DATA, "k12_R1.fq"))
     buf, off = flatten([s for _, s in recs])
@@ -154,7 +172,8 @@ def test_genomes_ecoli(ctx):
 @pytest.mark.parametrize("k,sem", [(31, 1), (21, 0)])
 def test_genomes_multicontig_with_repeats(ctx, k, sem):
     """Many genomes, ragged contigs (incl. < 2k and empty), repeated segments inside a genome
-    (must be dropped entirely) and shared segments across genomes (must be kept)."""
+    (must be dropped entirely) and shared segments across genomes (must be kept); c down to 1, where
+    every hash below u64::MAX survives."""
     rng = np.random.default_rng(77)
     shared = rand_seqs(rng, [5000])[0]
     contigs, goff = [], [0]
@@ -173,14 +192,18 @@ def test_genomes_multicontig_with_repeats(ctx, k, sem):
     buf, coff = flatten(contigs)
     check_genomes(ctx, buf, coff, np.array(goff, dtype=np.uint64), k=k, c=11, min_spacing=30, sem=sem)
     check_genomes(ctx, buf, coff, np.array(goff, dtype=np.uint64), k=k, c=3, min_spacing=5, sem=sem)
+    check_genomes(ctx, buf, coff, np.array(goff, dtype=np.uint64), k=k, c=2, min_spacing=5, sem=sem)
+    d = check_genomes(ctx, buf, coff, np.array(goff, dtype=np.uint64), k=k, c=1, min_spacing=30, sem=sem)
+    assert (np.concatenate([d["kmers"], d["tracked"]]) >= np.uint64(1 << 63)).any()   # c = 1: hashes use all 64 bits
+    check_repeat_and_shared(ctx, rng, k=k, c=1, sem=sem)
 
 
 @pytest.mark.parametrize("postpass", ["slots", "sort"])
 def test_genomes_c200_slotted_postpass(ctx, monkeypatch, postpass):
-    """c >= 96 takes the sort-free post-pass (per-tile slots, shared-memory duplicate tables, genome.cu); same
-    inputs through the generic radix-sort path.  Long contigs (many tiles), repeats inside a genome (dropped),
-    segments shared across genomes (kept), genomes with thousands of survivors (several hash partitions), empty
-    genomes, --individual-records, no tracked k-mers."""
+    """c >= 96 takes the slotted front half of the post-pass (per-tile slots, no sort, genome.cu); same inputs
+    through the sorted front half.  Long contigs (many tiles), repeats inside a genome (dropped), segments shared
+    across genomes (kept), genomes with thousands of survivors, empty genomes, --individual-records, no tracked
+    k-mers, batches without survivors or without contigs."""
     if postpass == "sort":
         monkeypatch.setenv("SYL_GENOME_POSTPASS", "sort")
     rng = np.random.default_rng(2024)
@@ -201,11 +224,21 @@ def test_genomes_c200_slotted_postpass(ctx, monkeypatch, postpass):
     buf, coff = flatten(contigs)
     goff = np.array(goff, dtype=np.uint64)
     d = check_genomes(ctx, buf, coff, goff, c=200)
-    assert int(np.diff(d["kmer_off"]).max()) > 6000       # more than one hash partition for the biggest genome
+    assert int(np.diff(d["kmer_off"]).max()) > 6000       # a genome with thousands of survivors
     check_genomes(ctx, buf, coff, goff, c=100, min_spacing=10)
     check_genomes(ctx, buf, coff, goff, c=200, pseudotax=False)
     check_genomes(ctx, buf, coff, goff, c=200, individual=True)
     check_genomes(ctx, buf, coff, goff, k=21, c=128, sem=0)
+    check_repeat_and_shared(ctx, rng, c=200)
+    # no survivors at all: every contig shorter than k, an empty contig and an empty genome
+    buf, coff = flatten([b"ACGT" * 7, b"", b"A" * 30, b"C" * 12])
+    d = check_genomes(ctx, buf, coff, np.array([0, 2, 2, 4], dtype=np.uint64), c=200)
+    assert d["kmers"].size == 0 and d["tracked"].size == 0 and not d["kmer_off"].any() and not d["tracked_off"].any()
+    assert d["gn_size"].tolist() == [28, 0, 42]
+    # no contigs at all
+    buf, coff = flatten([])
+    d = check_genomes(ctx, buf, coff, np.array([0, 0, 0], dtype=np.uint64), c=200)
+    assert d["kmers"].size == 0 and not d["kmer_off"].any() and d["gn_size"].tolist() == [0, 0]
 
 
 def test_genomes_low_complexity_overflows_the_tile_slots(ctx):
