@@ -30,6 +30,18 @@ for k, c in ((31, 200), (21, 50)):
     assert len(h) > 1000 and np.array_equal(h, eh) and np.array_equal(cnt, ec), (k, c, len(h), len(eh))
     assert s.num_dup_removed == nd, (s.num_dup_removed, nd)
     s.free()
+# scripted duplicate-removal histories (tests/dedup_scripts.py): every in-kernel replay, every fallback
+import torch
+from tests import dedup_scripts as D
+for name in D.SAMPLES:
+    b, o = D.single_sample(name, c=10).flat()
+    eh, ec, _, nd = O.sketch_reads(b, o, k=31, c=10)
+    src = (b, o) if SOURCE == "host" else (torch.from_numpy(b).cuda(), torch.from_numpy(o.view(np.int64)).cuda())
+    s = ctx.sketch_sequences(*src, k=31, c=10)
+    h, cnt = s.download()
+    assert np.array_equal(h, eh) and np.array_equal(cnt, ec), name
+    assert s.num_dup_removed == nd, (name, s.num_dup_removed, nd)
+    s.free()
 print("ok")
 """
 

@@ -103,8 +103,9 @@ def test_read_sketch_dedup_vs_pyref():
 
 
 def make_pairs(rng, n, genome, with_short=True):
-    """read pairs from one genome: exact duplicate pairs, pairs that share only mate 1's start, mates that overlap
-    (k-mers present in both mates), short mates (< 33 bp: no pair key)"""
+    """read pairs from one genome: exact duplicate pairs, pairs with the same mate 1 and a shifted mate 2 (no pair key
+    in common: each key mixes both mates), mates that overlap (k-mers present in both mates), short mates (< 33 bp: no
+    pair key)"""
     r1, r2 = [], []
     G = len(genome)
     for _ in range(n):

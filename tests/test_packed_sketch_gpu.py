@@ -81,8 +81,8 @@ def test_pairs_k12_fixture(ctx):
 
 @pytest.mark.parametrize("no_dedup", [False, True])
 def test_pairs_synthetic_with_duplicates(ctx, no_dedup):
-    """The duplicate-heavy set of the ASCII pair tests: duplicate pairs, pairs sharing one key, overlapping mates,
-    mates < 33 bp, one k-mer with hundreds of events."""
+    """The duplicate-heavy set of the ASCII pair tests: duplicate pairs, pairs with the same mate 1 only, overlapping
+    mates, mates < 33 bp, one k-mer with hundreds of events."""
     rng = np.random.default_rng(31)
     genome = rand_seq(rng, 30000, b"ACGT")
     r1, r2 = make_pairs(rng, 4000, genome)

@@ -40,8 +40,9 @@ def test_k12_pairs_fixture(ctx):
 @pytest.mark.parametrize("device", [False, True])
 @pytest.mark.parametrize("no_dedup", [False, True])
 def test_synthetic_pairs_with_duplicates(ctx, device, no_dedup):
-    """duplicate pairs, pairs sharing one key, overlapping mates (k-mer in both mates: counted once), mates < 33 bp
-    (no key), one k-mer with hundreds of events (dedup set far beyond 4: no MAX_DEDUP_COUNT for pairs)"""
+    """duplicate pairs, pairs with the same mate 1 only (no key in common), overlapping mates (k-mer in both mates:
+    counted once), mates < 33 bp (no key), one k-mer with hundreds of events (dedup set far beyond 4: no
+    MAX_DEDUP_COUNT for pairs)"""
     rng = np.random.default_rng(31)
     genome = rand_seq(rng, 30000, b"ACGT")
     r1, r2 = make_pairs(rng, 4000, genome)

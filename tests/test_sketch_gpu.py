@@ -81,8 +81,9 @@ def test_reads_o157_long(ctx):
 
 @pytest.mark.parametrize("no_dedup", [False, True])
 def test_reads_heavy_duplicates(ctx, no_dedup):
-    """Exercise the c<4 state machine: exact duplicate reads, shifted duplicates that share only
-    one pair key, reads > 400 bp (no pair), reads < 66 bp (no pair), homopolymers (p0 == p1)."""
+    """Exercise the c<4 state machine: exact duplicate reads, shortened copies (same start, no pair key in common),
+    reads > 400 bp (no pair), reads < 66 bp (no pair), homopolymers (p0 == p1).  Matches on one key only and across
+    the two key slots are in tests/test_dedup_scripts_gpu.py."""
     rng = np.random.default_rng(123)
     genome = rand_seqs(rng, [150000])[0]
     seqs = []
@@ -94,7 +95,7 @@ def test_reads_heavy_duplicates(ctx, no_dedup):
         if rng.random() < 0.3:
             seqs.append(s)                      # exact duplicate
         if rng.random() < 0.1:
-            seqs.append(genome[st:st + ln - 2])  # same start, different half => shares one key
+            seqs.append(genome[st:st + ln - 2])  # same start, middle window moved: both keys differ
     seqs += [b"A" * 150, b"A" * 150, b"A" * 150, b"ACGT" * 40, b"ACGT" * 40, b"", b"ACG"]
     order = rng.permutation(len(seqs))
     seqs = [seqs[i] for i in order]
