@@ -188,6 +188,8 @@ def poisson_cdf(lam, x):
     term = math.exp(-lam)
     tot = 0.0
     for i in range(x + 1):
+        if term == 0.0 and i > lam:  # every later term is 0 too (counts reach 2^32 - 1)
+            break
         tot += term
         term *= lam / (i + 1)
     return tot
@@ -273,8 +275,9 @@ def bootstrap_interval(full, k, min_count_correct):
 
 
 def get_stats(genome_kmers, sample, k=31, min_number_kmers=50.0, min_count_correct=3.0, min_ani=0.90, no_ci=False,
-              winner=None, genome_id=None):
-    """src/contain.rs:601-814 (pass 1 when winner is None) -> dict or None"""
+              winner=None, genome_id=None, mean_coverage=False, no_adj=False):
+    """src/contain.rs:601-814 (pass 1 when winner is None) -> dict or None.  mean_coverage: the final coverage of a
+    median >= 15 is the mean too (:722); no_adj: the final ANI is the naive one (:740)."""
     if len(genome_kmers) < min_number_kmers:
         return None
     covs, lost = [], 0
@@ -308,9 +311,9 @@ def get_stats(genome_kmers, sample, k=31, min_number_kmers=50.0, min_count_corre
     else:
         lam = ratio_lambda(full, min_count_correct)
         status = "LOW" if lam is None else "LAMBDA"
-    final_cov = lam if lam is not None else (geq1 if median < 15 else float(median))
+    final_cov = lam if lam is not None else (geq1 if median < 15 or mean_coverage else float(median))
     est = ani_from_lambda(lam, k, full)
-    final_ani = naive if (lam is None or est is None) else est
+    final_ani = naive if (lam is None or est is None or no_adj) else est
     if final_ani < min_ani:
         return None
     ci = None
@@ -321,14 +324,15 @@ def get_stats(genome_kmers, sample, k=31, min_number_kmers=50.0, min_count_corre
 
 
 def contain_sample(genomes, sample, k=31, pseudotax=False, min_number_kmers=50.0, min_count_correct=3.0,
-                   minimum_ani=None, redundant_ani=99.0, no_ci=False, unknown=None):
+                   minimum_ani=None, redundant_ani=99.0, no_ci=False, unknown=None, mean_coverage=False, no_adj=False):
     """Inner body of contain() for one sample (src/contain.rs:284-334), written from the reference
     source only.  genomes: list of dict(kmers=[..], tracked=[..], gn_size=int); sample: dict hash->count.
     Pass-1 results are taken in genome-index order (the reference's order is thread-timing dependent).
     unknown = (read_seq_id percent, mean_read_length, sample c): -u with --read-seq-id (:274-279, :377-408).
     -> list of dicts (get_stats fields + genome, rel_abund, seq_abund) in output order."""
     min_ani = minimum_ani / 100.0 if minimum_ani is not None else (0.95 if pseudotax else 0.90)  # :746-748
-    kw = dict(k=k, min_number_kmers=min_number_kmers, min_count_correct=min_count_correct, min_ani=min_ani, no_ci=no_ci)
+    kw = dict(k=k, min_number_kmers=min_number_kmers, min_count_correct=min_count_correct, min_ani=min_ani, no_ci=no_ci,
+              mean_coverage=mean_coverage, no_adj=no_adj)
     res = []
     for gi, g in enumerate(genomes):  # :286-292
         r = get_stats(g["kmers"], sample, **kw)

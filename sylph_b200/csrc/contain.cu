@@ -1183,6 +1183,9 @@ static int job_bootstrap(syl_profile_job *j, void *tab) {
     if (j->P.no_ci) return SYL_OK;
     ShardTable *t = reinterpret_cast<ShardTable *>(tab);
     SYL_CUDA(cudaMemsetAsync(j->reject.p, 0, (size_t)(j->R + 1) * 4, st));
+    // test hook (read per call): flag every row, so k_boot_seq replays all of them sequentially; the flags are
+    // reject[0..R) only, reject[R] is k_boot_iter_p's work counter and stays zero
+    if (getenv("SYL_BOOT_REPLAY") != nullptr) SYL_CUDA(cudaMemsetAsync(j->reject.p, 1, (size_t)j->R * 4, st));
     KernelTimer kt(ctx, SYL_KERNEL_BOOT);
     static int boot_ctas = 0;  // resident CTAs per SM (a partially filled second wave would double the tail)
     if (!boot_ctas && cudaOccupancyMaxActiveBlocksPerMultiprocessor(&boot_ctas, k_boot_iter_p, BOOT_THREADS, 0) != cudaSuccess) boot_ctas = 4;
