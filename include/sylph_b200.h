@@ -203,7 +203,8 @@ int syl_sketch_genomes_packed2(syl_ctx *ctx, int mem, const uint32_t *packed, ui
                                const uint64_t *contig_off, uint64_t n_contigs, const uint64_t *genome_off,
                                uint64_t n_genomes, int k, uint64_t c, uint64_t min_spacing, int pseudotax,
                                int individual, int sem, syl_genomes **out);
-/* Wrap existing sketches (e.g. a deserialised .syldb). tracked/tracked_off may be NULL. */
+/* Wrap existing sketches (e.g. a deserialised .syldb). tracked_off == NULL: no tracked k-mers (has_tracked = 0,
+ * profile refuses the db); tracked may be NULL when tracked_off[n_genomes] == 0. */
 int syl_genomes_upload(syl_ctx *ctx, int mem, const uint64_t *kmers, const uint64_t *kmer_off,
                        const uint64_t *tracked, const uint64_t *tracked_off, const uint64_t *gn_size,
                        uint64_t n_genomes, int k, uint64_t c, syl_genomes **out);
@@ -312,6 +313,9 @@ int syl_profile(syl_ctx *ctx, const syl_db *db, const syl_sample *const *samples
  *       syl_profile_shard_finish     the call's one host sync: derep, abundances, per-sample order; every
  *                                    rank returns the same rows (row.genome = global genome index)
  *
+ *     rows_per_rank == 0 takes the default, 256 + 96 * n_samples rounded up to a multiple of 256 when world > 1:
+ *     it does not depend on the shard, so every rank's table has the same size.  A rank whose shard holds no
+ *     genome runs every stage (zeroed table headers, no winner candidates) and takes part in every collective.
  *     SYL_ERR_CAPACITY from finish: redo with rows_per_rank >= *need_rows_per_rank (same verdict on every
  *     rank).  SYL_ERR_UNSUPPORTED: a k-mer count >= 256 was met (every rank sees it); use the gathered-
  *     survivor path (sylph_b200/dist.py profile_sharded_gather).  world == 1 is allowed (no collectives).

@@ -34,7 +34,8 @@ def main():
     dist.init_process_group("nccl", device_id=torch.device("cuda", local))
     ctx = sylph_b200.Context(local, stream=torch.cuda.current_stream().cuda_stream)
     ok = True
-    for G, glen, c, n_reads, n_samples in ((200, 120000, 20, 60000, 3), (96, 150000, 1000, 300000, 2)):
+    # G = 513 with one sample: 2 ranks hold 257 and 256 genomes, where a row table sized from the shard would differ
+    for G, glen, c, n_reads, n_samples in ((200, 120000, 20, 60000, 3), (96, 150000, 1000, 300000, 2), (513, 20000, 20, 30000, 1)):
         b0, b1 = D.shard_range(G, rank, world)
         bases, off = synth.db_chunk(b0, b1, glen, device="cuda")
         goff = torch.arange(b1 - b0 + 1, dtype=torch.int64, device="cuda")

@@ -1010,8 +1010,12 @@ static void job_release(syl_profile_job *j) {
     delete j;  // the scratch blocks go back to the owning ctx's cache (DevBuf::owner)
 }
 
-static uint64_t default_rows_per_rank(uint32_t S, uint64_t G) {
-    uint64_t R = std::min<uint64_t>((uint64_t)S * G, 256 + 96ull * S);
+// Row-table capacity when the caller gives none, a multiple of 256.  The ranks of a sharded profile gather their tables
+// with fixed-size collectives, so at world > 1 it depends on the sample count only (shards of 257 and 256 genomes
+// would otherwise get 512 and 256 rows); one GPU also caps it at the number of pairs.
+static uint64_t default_rows_per_rank(uint32_t S, uint64_t G, uint32_t world) {
+    uint64_t R = 256 + 96ull * S;
+    if (world == 1) R = std::min<uint64_t>((uint64_t)S * G, R);
     return (std::max<uint64_t>(R, 256) + 255) & ~255ull;
 }
 
@@ -1065,6 +1069,7 @@ static int enqueue_stats(syl_profile_job *j, const StatParams &P, bool pass2, vo
     const uint64_t NP = (uint64_t)j->S * j->G;
     ShardTable *t = reinterpret_cast<ShardTable *>(tab);
     uint32_t *lost = pass2 ? j->lost.p : nullptr;
+    if (NP == 0) return SYL_OK;  // an empty shard: no pairs, the table keeps its zeroed header
     KernelTimer kt(ctx, SYL_KERNEL_STATS);
     if (j->csr)
         k_stats<<<nblk(NP, STAT_WARPS), STAT_WARPS * 32, 0, ctx->stream>>>(j->cnt.p, j->off.p, j->covs.p, db->glen, lost, j->G, NP, db->genome_base,
@@ -1097,7 +1102,7 @@ static int job_begin(syl_ctx *ctx, const syl_db *db, const syl_sample *const *sa
     j->redundant_ani = pp.redundant_ani;
     JOB_TRY(check_unknown_args(p));
     if (p->estimate_unknown) { j->read_seq_id = p->read_seq_id; JOB_TRY(sample_metas(ctx, samples, n_samples, j->metas)); }
-    j->R = R ? ((R + 255) & ~255ull) : default_rows_per_rank(n_samples, db->n_genomes);
+    j->R = R ? ((R + 255) & ~255ull) : default_rows_per_rank(n_samples, db->n_genomes, world);
     j->tbytes = table_bytes(j->R);
     if (j->R * BOOT_ITERS >= 0xFFFF0000ull) { set_error("row capacity too large for the bootstrap work counter"); return fail(SYL_ERR_ARG); }
     const uint64_t NP = (uint64_t)j->S * j->G;

@@ -527,10 +527,13 @@ int syl_genomes_upload(syl_ctx *ctx, int mem, const uint64_t *kmers, const uint6
         nk = ctx->h_counters[8];
         nt = tracked_off ? ctx->h_counters[9] : 0;
     }
+    // tracked_off says whether the sketches carry tracked k-mers; tracked may be NULL when there are none (an empty
+    // torch tensor has no address)
+    if (nt && !tracked) { set_error("tracked_off counts tracked k-mers but tracked is NULL"); return SYL_ERR_ARG; }
     syl_genomes *g = new (std::nothrow) syl_genomes();
     if (!g) return SYL_ERR_OOM;
     g->device = ctx->device; g->k = k; g->c = c;
-    g->has_tracked = (tracked && tracked_off) ? 1 : 0;
+    g->has_tracked = tracked_off ? 1 : 0;
     int rc = genomes_alloc(g, st, n_genomes, nk, nt);
     if (rc != SYL_OK) { syl_genomes_free(g); return rc; }
     auto fill = [&]() -> int {  // any failure below frees the handle and its blocks
