@@ -175,9 +175,8 @@ class LineReader {
         bool got = false;
         for (;;) {
             if (pos_ == len_) {
-                const int n = bgzf_ ? bgzf_->read(buf_, sizeof buf_) : gzread(f_, buf_, sizeof buf_);
+                const int n = read_some();
                 if (n <= 0) {
-                    if (n < 0) err_ = true;  // damaged gzip stream / BGZF block: the file is invalid, not merely shorter
                     if (got && !line.empty() && line.back() == '\r') line.pop_back();
                     return got;
                 }
@@ -233,9 +232,21 @@ class LineReader {
         }
     }
   private:
+    // inflated bytes into buf_, 0 at the end of the file.  A damaged gzip stream / BGZF block makes the file invalid,
+    // not merely shorter; so does a gzip stream cut short, which zlib reports only through gzerror's Z_BUF_ERROR
+    int read_some() {
+        int n = bgzf_ ? bgzf_->read(buf_, sizeof buf_) : gzread(f_, buf_, sizeof buf_);
+        if (n == 0 && f_) {
+            int e = Z_OK;
+            gzerror(f_, &e);
+            if (e == Z_BUF_ERROR) n = -1;
+        }
+        if (n < 0) err_ = true;
+        return n;
+    }
     bool refill() {
-        const int n = bgzf_ ? bgzf_->read(buf_, sizeof buf_) : gzread(f_, buf_, sizeof buf_);
-        if (n <= 0) { if (n < 0) err_ = true; return false; }
+        const int n = read_some();
+        if (n <= 0) return false;
         len_ = (size_t)n;
         pos_ = 0;
         return true;

@@ -59,7 +59,17 @@ struct Args {
     std::string db_out = "database", sample_dir = "./", out_file, list_file;
     double min_ani = -1., min_number_kmers = 50., min_count_correct = 3., redundant_ani = 99.;
     int device = 0;
+    // test hooks (INTEGRATION.md), read once from the environment: small values make the split paths run on small inputs
+    uint64_t batch_bases = 1ull << 30;  // SYL_DRIVER_BATCH_BASES: a genome batch closes once it holds this many bases
+    uint64_t samples_per_call = 0;      // SYL_DRIVER_SAMPLES_PER_CALL: cap on samples per syl_query / syl_profile call (0 = none)
+    uint64_t rows0 = 0;                 // SYL_DRIVER_ROWS: initial row-buffer length (0 = sized from the call)
 };
+
+static uint64_t env_u64(const char *name, uint64_t dflt) {
+    const char *v = getenv(name);
+    if (!v || !*v) return dflt;
+    return std::max<uint64_t>(1, std::strtoull(v, nullptr, 10));
+}
 
 static Args parse(int argc, char **argv) {
     Args a;
@@ -106,10 +116,18 @@ static Args parse(int argc, char **argv) {
     if (!(a.k == 21 || a.k == 31)) die("Only k = 21, 31 are currently supported");  // src/cmdline.rs:57
     if (a.fpr < 0. || a.fpr >= 1.) die("Invalid value for --fpr. Exiting.");             // src/sketch.rs:158-161
     if (a.first_pairs.size() != a.second_pairs.size()) die("Different number of paired sequences. Exiting.");  // :163-166
+    // the reference's query / profile sketch pairs with the approximate cuckoo filter (src/contain.rs:201-210,
+    // DEFAULT_FPR), which is out of scope; an exact-set profile would silently differ from it
+    if (!a.first_pairs.empty() && (a.cmd == "query" || a.cmd == "profile"))
+        die("query/profile do not sketch read pairs (-1/-2) here: sylph sketches them with its approximate paired-end filter. "
+            "Run `sylph-b200 sketch -1 ... -2 ... --fpr 0` and pass the *.paired.sylsp files instead. Exiting.");
     if (a.estimate_unknown && !(a.read_seq_id > 0.))
         die("-u needs -I/--read-seq-id here: sylph's automatic read-identity estimate depends on hash-map iteration order (DESIGN.md)");
     if (!a.first_pairs.empty() && a.fpr != 0.)
         die("paired-end reads need --fpr 0 (the exact dedup set); the default approximate cuckoo filter is not bit-reproducible and out of scope");
+    a.batch_bases = env_u64("SYL_DRIVER_BATCH_BASES", a.batch_bases);
+    a.samples_per_call = env_u64("SYL_DRIVER_SAMPLES_PER_CALL", 0);
+    a.rows0 = env_u64("SYL_DRIVER_ROWS", 0);
     return a;
 }
 
@@ -185,7 +203,7 @@ static void sketch_genome_files(syl_ctx *ctx, const Args &a, const std::vector<s
         FlatRecords recs;
         std::vector<uint64_t> genome_off{0};
         std::vector<std::string> names, first_ids;
-        while (fi < files.size() && recs.bases.size() < (1ull << 30)) {
+        while (fi < files.size() && recs.bases.size() < a.batch_bases) {
             const std::string &f = files[fi];
             Parsed &p = *parsed[fi++];
             // a file that fails half way contributes nothing (records are merged only after a complete parse)
@@ -331,6 +349,11 @@ static int cmd_contain(syl_ctx *ctx, const Args &a, bool pseudotax) {
         for (const std::string &f : read_files) warn(f + " error: value of -c for contain is greater than the smallest value of -c for a genome sketch. Continuing without sketching.");
         read_files.clear();
     }
+    if (!read_files.empty() && a.k != gs[0].k) {  // src/contain.rs:578-584: raw reads are sketched with -k or not at all
+        for (const std::string &f : read_files)
+            warn(f + " -k " + std::to_string(a.k) + " is not equal to -k " + std::to_string(gs[0].k) + " found in sketches. Continuing without sketching.");
+        read_files.clear();
+    }
     parse_ahead(read_files, a.threads, false, [&](const std::string &f, Parsed &p) {
         if (!p.ok) { warn(f + " is not a valid fasta/fastq file; skipping."); return; }
         syl_sample *s = nullptr;
@@ -353,8 +376,9 @@ static int cmd_contain(syl_ctx *ctx, const Args &a, bool pseudotax) {
     if (!o) die("cannot open output file " + a.out_file);
     if (!pseudotax)  // src/contain.rs:461-480
         fprintf(o, "Sample_file\tGenome_file\tAdjusted_ANI\tEff_cov\tANI_5-95_percentile\tEff_lambda\tLambda_5-95_percentile\tMedian_cov\tMean_cov_geq1\tContainment_ind\tNaive_ANI\tContig_name\n");
-    else
-        fprintf(o, "Sample_file\tGenome_file\tTaxonomic_abundance\tSequence_abundance\tAdjusted_ANI\tEff_cov\tANI_5-95_percentile\tEff_lambda\tLambda_5-95_percentile\tMedian_cov\tMean_cov_geq1\tContainment_ind\tNaive_ANI\tkmers_reassigned\tContig_name\n");
+    else  // with -u the coverage column holds the true coverage (src/contain.rs:469-475)
+        fprintf(o, "Sample_file\tGenome_file\tTaxonomic_abundance\tSequence_abundance\tAdjusted_ANI\t%s\tANI_5-95_percentile\tEff_lambda\tLambda_5-95_percentile\tMedian_cov\tMean_cov_geq1\tContainment_ind\tNaive_ANI\tkmers_reassigned\tContig_name\n",
+                a.estimate_unknown ? "True_cov" : "Eff_cov");
     if (!samples.empty()) {
         syl_contain_params p;
         syl_contain_params_default(&p, (int)gs[0].k, pseudotax ? 1 : 0);
@@ -364,10 +388,11 @@ static int cmd_contain(syl_ctx *ctx, const Args &a, bool pseudotax) {
         p.estimate_unknown = a.estimate_unknown ? 1 : 0; p.read_seq_id = a.read_seq_id;
         // sample batches sized so that samples x genomes stays below the library's per-call limits (2^31 pairs,
         // 8 GB of per-pair histograms = 2^23 pairs); the reference walks the samples in chunks too (src/contain.rs:239-263)
-        const size_t per_call = std::max<size_t>(1, std::min<size_t>(samples.size(), (size_t)((1ull << 22) / std::max<size_t>(gs.size(), 1))));
+        size_t per_call = std::max<size_t>(1, std::min<size_t>(samples.size(), (size_t)((1ull << 22) / std::max<size_t>(gs.size(), 1))));
+        if (a.samples_per_call) per_call = std::min<size_t>(per_call, a.samples_per_call);
         for (size_t s0 = 0; s0 < samples.size(); s0 += per_call) {
             const size_t ns = std::min(per_call, samples.size() - s0);
-            std::vector<syl_ani_row> rows(std::max<size_t>(1024, std::min<size_t>(gs.size() * ns, 1u << 22)));
+            std::vector<syl_ani_row> rows(a.rows0 ? a.rows0 : std::max<size_t>(1024, std::min<size_t>(gs.size() * ns, 1u << 22)));
             uint64_t n = 0;
             for (;;) {
                 int rc = (pseudotax ? syl_profile : syl_query)(ctx, db, samples.data() + s0, (uint32_t)ns, &p, rows.data(), rows.size(), &n);
@@ -419,10 +444,12 @@ int main(int argc, char **argv) {
     syl_ctx *ctx = nullptr;
     check(syl_ctx_create(a.device, nullptr, &ctx), "syl_ctx_create");
     int rc;
-    if (a.cmd == "sketch") rc = cmd_sketch(ctx, a);
-    else if (a.cmd == "query") rc = cmd_contain(ctx, a, false);
-    else if (a.cmd == "profile") rc = cmd_contain(ctx, a, true);
-    else die("unknown command " + a.cmd + " (sketch | query | profile)");
+    try {  // e.g. a sketch path that cannot be written: exit 1 with the message instead of aborting
+        if (a.cmd == "sketch") rc = cmd_sketch(ctx, a);
+        else if (a.cmd == "query") rc = cmd_contain(ctx, a, false);
+        else if (a.cmd == "profile") rc = cmd_contain(ctx, a, true);
+        else die("unknown command " + a.cmd + " (sketch | query | profile)");
+    } catch (const std::exception &e) { die(e.what()); }
     syl_ctx_destroy(ctx);
     return rc;
 }
