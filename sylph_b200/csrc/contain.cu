@@ -33,6 +33,7 @@
 #include <vector>
 
 #include "common.cuh"
+#include "crmath.cuh"
 
 struct syl_db {
     int device = 0;
@@ -146,10 +147,11 @@ __device__ __forceinline__ RatioOut ratio_lambda_hist(const uint32_t *H, uint32_
     return r;
 }
 
-// src/contain.rs:817-847
+// src/contain.rs:817-847.  pow and exp correctly rounded (crmath.cuh): the ANI decides the -m gate and the winner
+// order, where CUDA's last bit and the reference's glibc last bit would print different rows.
 __device__ __forceinline__ bool ani_from_lambda_dev(double lambda, double k, uint64_t nz, uint64_t nfull, double *out) {
-    const double adj = (double)nz / (1. - exp(-lambda)) / (double)nfull;
-    const double ani = pow(adj, 1. / k);
+    const double adj = (double)nz / (1. - crm::cr_exp(-lambda)) / (double)nfull;
+    const double ani = crm::cr_pow(adj, 1. / k);
     if (ani < 0. || isnan(ani)) return false;
     *out = ani;
     return true;
@@ -165,7 +167,7 @@ __device__ __forceinline__ void stats_emit(uint32_t sample_idx, uint64_t g, uint
                                            const StatExtra X = StatExtra()) {
     const double k = (double)P.k;
     const uint64_t nfull = (uint64_t)(gl - n) + nz;
-    const double naive_ani = pow((double)n / (double)gl, 1. / k);
+    const double naive_ani = crm::cr_pow((double)n / (double)gl, 1. / k);
     const double geq1_mean = (double)sum / (double)n;  // :690 divides by covs.len()
     uint32_t status;
     double lam = 0.;

@@ -18,6 +18,7 @@ import threading
 import numpy as np
 import pytest
 
+from tests import ani_ties as T
 from tests import contain_scripts as S
 from tests.test_contain_gpu import compare, sort_query_rows
 from tests.util import DATA, flatten, read_fastx
@@ -562,3 +563,23 @@ def test_five_samples_of_unequal_size_one_call(ctx, syn, monkeypatch):
     for call, rows in got.items():
         assert set(rows["sample"].tolist()) >= {0, 2, 4}, call
         assert 1 not in set(rows["sample"].tolist()), call
+
+
+@pytest.mark.parametrize("pair", [T.WINNER_PAIRS[-1], T.TIE_PAIRS[0]], ids=["adjacent", "equal"])
+def test_near_tied_winner_across_two_ranks(ctx, monkeypatch, pair):
+    """Two genomes whose ANIs are adjacent doubles or equal (tests/ani_ties.py), sharing hit k-mers, one per rank: the
+    gathered k_rank_rows orders them like the oracle, in both genome orders."""
+    k, a, b = pair
+    assert k == 31
+    for specs in ([a, b], [b, a]):
+        case = T.Case(specs, shared=3)
+        samples = [SampleData(case.hash, case.count, 1)]
+        whole = Whole(ctx, case.db, 1, samples)
+        sh = Sharded([0, 1, 2], lambda cx, b0, b1: upload(cx, csr_slice(case.db, b0, b1), 1), samples)
+        try:
+            got, _ = run_sharded(monkeypatch, sh, {"minimum_ani": 0.0})
+            assert whole.check(got, {"minimum_ani": 0.0}) == 2
+            assert sorted(int(x) for x in got["profile"]["kmers_lost"]) == [0, 3]
+        finally:
+            sh.close()
+            whole.close()
