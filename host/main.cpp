@@ -1,7 +1,8 @@
-// sylph-b200 — host driver over libsylph_b200.so mirroring sylph's `sketch`, `query`, `profile`
+// sylph-b200 — host driver over libsylph_b200.so mirroring sylph's `sketch`, `query`, `profile`, `inspect`
 // (src/main.rs:25-30) for the in-scope paths: single-end reads, read pairs with the exact dedup set
-// (-1/-2 --fpr 0) and genomes, k in {21,31}.  Files are inflated and parsed by up to -t threads at a time
-// (the reference parallelises per file with rayon, src/sketch.rs:313,371,428) while the GPU works.
+// (-1/-2 --fpr 0) and genomes, k in {21,31}, with sample names (-S / --lS) and list inputs (-l --rl --gl --l1 --l2).
+// Files are inflated and parsed by up to -t threads at a time (the reference parallelises per file with rayon,
+// src/sketch.rs:313,371,428) while the GPU works.
 // File classification, defaults and TSV output follow the reference (src/cmdline.rs,
 // src/sketch.rs:95-127,276-479, src/contain.rs:18-94,115-351,461-480).  All compute goes through
 // the C ABI; there is no CPU path.
@@ -18,6 +19,7 @@
 
 #include "../include/sylph_b200.h"
 #include "fastx.hpp"
+#include "inspect.hpp"
 #include "sketch_io.hpp"
 
 using namespace host;
@@ -47,9 +49,17 @@ static std::string basename_of(const std::string &p) {
     return i == std::string::npos ? p : p.substr(i + 1);
 }
 
+// a single-end read file of `sketch` and the index of its sample name (-S / --lS), if any
+struct ReadInput { std::string file; size_t name; };
+
 struct Args {
     std::string cmd;
     std::vector<std::string> files, reads, genomes, first_pairs, second_pairs;
+    size_t n_positional = 0;  // files[0, n_positional) are positional, the rest are lines of -l
+    std::string read_list, genome_list, first_pair_list, second_pair_list, names_list;  // --rl --gl --l1 --l2 --lS
+    std::vector<std::string> sample_names;  // -S, or the lines of --lS
+    std::vector<ReadInput> sketch_reads;    // sketch: every single-end read file, in the order they are sketched
+    std::vector<std::string> sketch_genomes;
     bool estimate_unknown = false;
     double read_seq_id = -1.;  // -I / --read-seq-id (percent)
     int threads = 3;       // src/cmdline.rs:61,100
@@ -71,9 +81,48 @@ static uint64_t env_u64(const char *name, uint64_t dflt) {
     return std::max<uint64_t>(1, std::strtoull(v, nullptr, 10));
 }
 
+// the lines of a list file as BufRead::lines splits them ("\n", a trailing "\r" dropped)
+static void read_list(const std::string &path, std::vector<std::string> &out, bool skip_empty) {
+    LineReader lr(path);
+    if (!lr.ok()) die("cannot open list file " + path);
+    std::string line;
+    while (lr.next(line)) if (!skip_empty || !line.empty()) out.push_back(line);
+}
+
+// sketch's inputs in sylph's order (src/sketch.rs:164-250): reads and genomes from -l then positional files, then -r / -g,
+// then --rl / --gl; first mates -1 then --l1, second mates -2 then --l2.  Sample names go to the pairs, then to the
+// reads in that order (src/sketch.rs:260-293).  The reads are sketched in the driver's own order (-r, positional,
+// -l, --rl) and the genomes kept in it (-g, positional, -l, --gl), so runs without names write what they always did.
+static void resolve_sketch_inputs(Args &a) {
+    std::vector<std::string> pos_reads, list_reads;
+    a.sketch_genomes = a.genomes;
+    for (size_t i = 0; i < a.files.size(); i++) {
+        const std::string &f = a.files[i];
+        if (is_fasta(f)) a.sketch_genomes.push_back(f);
+        else if (is_fastq(f)) (i < a.n_positional ? pos_reads : list_reads).push_back(f);
+        else warn(f + " does not have a fasta/fastq/gzip type extension.");
+    }
+    std::vector<std::string> rl;
+    if (!a.genome_list.empty()) read_list(a.genome_list, a.sketch_genomes, false);
+    if (!a.read_list.empty()) read_list(a.read_list, rl, false);
+    const size_t o_list = a.first_pairs.size(), o_pos = o_list + list_reads.size(), o_r = o_pos + pos_reads.size(),
+                 o_rl = o_r + a.reads.size();
+    for (size_t i = 0; i < a.reads.size(); i++) a.sketch_reads.push_back({a.reads[i], o_r + i});
+    for (size_t i = 0; i < pos_reads.size(); i++) a.sketch_reads.push_back({pos_reads[i], o_pos + i});
+    for (size_t i = 0; i < list_reads.size(); i++) a.sketch_reads.push_back({list_reads[i], o_list + i});
+    for (size_t i = 0; i < rl.size(); i++) a.sketch_reads.push_back({rl[i], o_rl + i});
+    if (!a.names_list.empty()) {  // --lS wins over -S
+        a.sample_names.clear();
+        read_list(a.names_list, a.sample_names, false);
+    }
+    const bool named = !a.names_list.empty() || !a.sample_names.empty();
+    if (named && a.sample_names.size() != a.first_pairs.size() + a.sketch_reads.size())
+        die("Sample name length is not equal to the number of reads. Exiting");
+}
+
 static Args parse(int argc, char **argv) {
     Args a;
-    if (argc < 2) die("usage: sylph-b200 <sketch|query|profile> [options] files...");
+    if (argc < 2) die("usage: sylph-b200 <sketch|query|profile|inspect> [options] files...");
     a.cmd = argv[1];
     auto need = [&](int &i) -> std::string { if (i + 1 >= argc) die(std::string("missing value for ") + argv[i]); return argv[++i]; };
     for (int i = 2; i < argc; i++) {
@@ -104,18 +153,26 @@ static Args parse(int argc, char **argv) {
         else if (s == "--device") a.device = std::stoi(need(i));
         else if (s == "-u" || s == "--estimate-unknown") a.estimate_unknown = true;
         else if (s == "-I" || s == "--read-seq-id") a.read_seq_id = std::stod(need(i));
+        else if (a.cmd == "sketch" && (s == "-S" || s == "--sample-names")) {
+            while (i + 1 < argc && argv[i + 1][0] != '-') a.sample_names.push_back(argv[++i]);
+        }
+        else if (a.cmd == "sketch" && s == "--lS") a.names_list = need(i);
+        else if (a.cmd == "sketch" && s == "--rl") a.read_list = need(i);
+        else if (a.cmd == "sketch" && s == "--gl") a.genome_list = need(i);
+        else if (a.cmd == "sketch" && s == "--l1") a.first_pair_list = need(i);
+        else if (a.cmd == "sketch" && s == "--l2") a.second_pair_list = need(i);
         else if (!s.empty() && s[0] == '-') die("unknown option " + s);
         else a.files.push_back(s);
     }
-    if (!a.list_file.empty()) {
-        LineReader lr(a.list_file);
-        if (!lr.ok()) die("cannot open list file " + a.list_file);
-        std::string line;
-        while (lr.next(line)) if (!line.empty()) a.files.push_back(line);
-    }
+    a.n_positional = a.files.size();
+    if (!a.list_file.empty()) read_list(a.list_file, a.files, true);
     if (!(a.k == 21 || a.k == 31)) die("Only k = 21, 31 are currently supported");  // src/cmdline.rs:57
     if (a.fpr < 0. || a.fpr >= 1.) die("Invalid value for --fpr. Exiting.");             // src/sketch.rs:158-161
-    if (a.first_pairs.size() != a.second_pairs.size()) die("Different number of paired sequences. Exiting.");  // :163-166
+    if (a.first_pairs.size() != a.second_pairs.size()) die("Different number of paired sequences. Exiting.");  // :223-226
+    if (!a.first_pair_list.empty()) read_list(a.first_pair_list, a.first_pairs, false);
+    if (!a.second_pair_list.empty()) read_list(a.second_pair_list, a.second_pairs, false);
+    if (a.first_pairs.size() != a.second_pairs.size()) die("Different number of paired sequences. Exiting.");  // :246-249
+    if (a.cmd == "sketch") resolve_sketch_inputs(a);
     // the reference's query / profile sketch pairs with the approximate cuckoo filter (src/contain.rs:201-210,
     // DEFAULT_FPR), which is out of scope; an exact-set profile would silently differ from it
     if (!a.first_pairs.empty() && (a.cmd == "query" || a.cmd == "profile"))
@@ -244,30 +301,52 @@ static void sketch_genome_files(syl_ctx *ctx, const Args &a, const std::vector<s
     }
 }
 
-static int cmd_sketch(syl_ctx *ctx, const Args &a) {
-    std::vector<std::string> reads = a.reads, genomes = a.genomes;
-    for (const std::string &f : a.files) {
-        if (is_fasta(f)) genomes.push_back(f);
-        else if (is_fastq(f)) reads.push_back(f);
-        else warn(f + " does not have a fasta/fastq/gzip type extension.");
+// Path::file_name of a sample name (src/sketch.rs:346,401): its last component, with empty and "." components ignored
+static std::string name_file_component(const std::string &name) {
+    std::string last;
+    size_t i = 0;
+    while (i <= name.size()) {
+        size_t j = name.find('/', i);
+        if (j == std::string::npos) j = name.size();
+        const std::string c = name.substr(i, j - i);
+        if (!c.empty() && c != ".") last = c;
+        i = j + 1;
     }
+    if (last.empty() || last == "..") die("Sample name `" + name + "` does not end in a file name. Exiting");
+    return last;
+}
+
+static int cmd_sketch(syl_ctx *ctx, const Args &a) {
     const std::string dir = a.sample_dir.empty() || a.sample_dir.back() == '/' ? a.sample_dir : a.sample_dir + "/";
-    for (size_t i = 0; i < a.first_pairs.size(); i++) {  // src/sketch.rs:313-365
+    const bool named = !a.sample_names.empty();
+    // a named sketch carries its sample name and is written as <-d>/<file name of the sample name>[.paired].sylsp
+    auto write_sample = [&](SequencesSketch &s, const std::string &file, size_t name, const char *suffix) {
+        std::string stem = basename_of(file);
+        if (named) {
+            s.has_sample_name = true;
+            s.sample_name = a.sample_names[name];
+            stem = name_file_component(s.sample_name);
+        }
+        if (!dir.empty()) std::filesystem::create_directories(dir);
+        const std::string path = dir + stem + suffix;
+        write_sylsp(path, s);
+        info("Sketching " + path + " complete.");
+    };
+    for (size_t i = 0; i < a.first_pairs.size(); i++) {  // src/sketch.rs:310-364
         SequencesSketch s;
         if (!sketch_pair_files(ctx, a, a.first_pairs[i], a.second_pairs[i], s)) continue;
-        if (!dir.empty()) std::filesystem::create_directories(dir);
-        const std::string path = dir + basename_of(a.first_pairs[i]) + ".paired.sylsp";
-        write_sylsp(path, s);
-        info("Sketching " + path + " complete.");
+        write_sample(s, a.first_pairs[i], i, ".paired.sylsp");
     }
+    std::vector<std::string> reads;
+    for (const ReadInput &r : a.sketch_reads) reads.push_back(r.file);
+    size_t ri = 0;
     parse_ahead(reads, a.threads, false, [&](const std::string &f, Parsed &p) {
+        const size_t name = a.sketch_reads[ri++].name;
         SequencesSketch s;
         if (!sketch_reads_parsed(ctx, a, f, p, s)) return;
-        if (!dir.empty()) std::filesystem::create_directories(dir);
-        const std::string path = dir + basename_of(f) + ".sylsp";
-        write_sylsp(path, s);
-        info("Sketching " + path + " complete.");
+        write_sample(s, f, name, ".sylsp");
     });
+    const std::vector<std::string> &genomes = a.sketch_genomes;
     if (!genomes.empty()) {
         std::vector<GenomeSketch> gs;
         sketch_genome_files(ctx, a, genomes, !a.no_pseudotax, gs);
@@ -437,10 +516,44 @@ static int cmd_fastx_stats(const Args &a) {
     return 0;
 }
 
+// inspect (src/inspect.rs:117-182): databases first, then samples, each as one YAML list; no device is needed
+static int cmd_inspect(const Args &a) {
+    std::vector<std::string> db_files, sample_files;
+    for (const std::string &f : a.files) {
+        if (is_syldb(f)) db_files.push_back(f);
+        else if (is_sylsp(f)) sample_files.push_back(f);
+        else warn(f + " file is not a .sylsp or .syldb file. Skipping...");
+    }
+    FILE *o = a.out_file.empty() ? stdout : fopen(a.out_file.c_str(), "w");
+    if (!o) die("cannot open output file " + a.out_file);
+    auto put = [&](const std::string &text) {
+        if (!text.empty() && fwrite(text.data(), 1, text.size(), o) != text.size()) die("write failed: " + a.out_file);
+    };
+    try {
+        std::vector<DatabaseInspect> dbs(db_files.size());
+        for (size_t i = 0; i < db_files.size(); i++) {
+            if (inspect_db(db_files[i], dbs[i]))
+                info("Database file " + db_files[i] + " processed with " + std::to_string(dbs[i].genome_files.size()) + " genomes");
+            else
+                warn("The database sketch `" + db_files[i] + "` is empty. Skipping...");
+        }
+        put(databases_yaml(dbs));
+        std::vector<SampleInspect> samples;
+        for (const std::string &f : sample_files) {
+            samples.push_back(inspect_sample(f));
+            info("Sequence file " + f + " processed");
+        }
+        put(samples_yaml(samples));
+    } catch (const std::exception &e) { die(e.what()); }
+    if (o != stdout && fclose(o) != 0) die("write failed: " + a.out_file);
+    return 0;
+}
+
 int main(int argc, char **argv) {
     Args a = parse(argc, argv);
     host::inflate_threads() = std::max(1, a.threads);  // BGZF members of one file are inflated by this many threads
     if (a.cmd == "fastx-stats") return cmd_fastx_stats(a);
+    if (a.cmd == "inspect") return cmd_inspect(a);
     syl_ctx *ctx = nullptr;
     check(syl_ctx_create(a.device, nullptr, &ctx), "syl_ctx_create");
     int rc;
@@ -448,7 +561,7 @@ int main(int argc, char **argv) {
         if (a.cmd == "sketch") rc = cmd_sketch(ctx, a);
         else if (a.cmd == "query") rc = cmd_contain(ctx, a, false);
         else if (a.cmd == "profile") rc = cmd_contain(ctx, a, true);
-        else die("unknown command " + a.cmd + " (sketch | query | profile)");
+        else die("unknown command " + a.cmd + " (sketch | query | profile | inspect)");
     } catch (const std::exception &e) { die(e.what()); }
     syl_ctx_destroy(ctx);
     return rc;

@@ -67,6 +67,14 @@ class Reader {
         return n;
     }
     void raw(void *p, size_t n) { if (n && fread(p, 1, n, f_) != n) bad(); }
+    // step over n bytes without reading them (k-mer arrays of a GTDB-scale .syldb run to gigabytes); the last byte is
+    // read, so a file that ends inside the skipped range is invalid rather than silently short
+    void skip(uint64_t n) {
+        if (!n) return;
+        if (n > (uint64_t)INT64_MAX || fseeko(f_, (off_t)(n - 1), SEEK_CUR) != 0) bad();
+        uint8_t last;
+        raw(&last, 1);
+    }
     [[noreturn]] void bad() {
         throw std::runtime_error("The sketch `" + path_ + "` is not a valid sketch. Perhaps it is an older, incompatible version ");
     }
