@@ -58,21 +58,6 @@ void hblock_free(syl_ctx *ctx, void *p) {
 }
 void set_error(const std::string &msg) { g_last_error = msg; }
 
-// Stage caller memory on the device if needed. For SYL_MEM_DEVICE the pointer is used as is.
-template <typename T>
-struct Staged {
-    const T *p = nullptr;
-    DevBuf<T> buf;
-    int init(syl_ctx *ctx, int mem, const T *src, size_t n) {
-        if (mem == SYL_MEM_DEVICE) { p = src; return SYL_OK; }
-        if (mem != SYL_MEM_HOST) { set_error("bad mem"); return SYL_ERR_ARG; }
-        SYL_TRY(buf.alloc(n + 16 / sizeof(T) + 1, ctx->stream));
-        if (n) SYL_CUDA(cudaMemcpyAsync(buf.p, src, n * sizeof(T), cudaMemcpyHostToDevice, ctx->stream));
-        p = buf.p;
-        return SYL_OK;
-    }
-};
-
 }  // namespace syl
 
 using namespace syl;
@@ -144,13 +129,6 @@ void syl_ctx_destroy(syl_ctx *ctx) {
     for (auto &b : ctx->free_blocks) cudaFree(b.first);
     ctx->free_blocks.clear();
     if (syl::tl_ctx == ctx) syl::tl_ctx = nullptr;
-    for (int i = 0; i < 2; i++) {
-        if (ctx->stage_b[i]) cudaFree(ctx->stage_b[i]);
-        if (ctx->stage_o[i]) cudaFree(ctx->stage_o[i]);
-        if (ctx->ev_copied[i]) cudaEventDestroy(ctx->ev_copied[i]);
-        if (ctx->ev_used[i]) cudaEventDestroy(ctx->ev_used[i]);
-    }
-    if (ctx->copy_stream) cudaStreamDestroy(ctx->copy_stream);
     for (auto &t : ctx->timed_pending) { cudaEventDestroy(t.e0); cudaEventDestroy(t.e1); }
     for (auto e : ctx->event_pool) cudaEventDestroy(e);
     if (ctx->d_counters) cudaFree(ctx->d_counters);

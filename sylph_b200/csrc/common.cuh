@@ -63,13 +63,9 @@ struct syl_ctx {
     uint64_t kernel_launches[SYL_KERNEL_COUNT] = {};
     uint64_t seed_bases = 0;
     uint64_t ingest_h2d_bytes = 0, ingest_chunks_packed = 0, ingest_chunks_ascii = 0;  // last host-memory read sketch
-    void *ingest = nullptr;  // HostIngest (sample.cu): packer pool + pinned staging ring of the host-memory read path
-    // double-buffered H2D staging for host-memory ASCII inputs (SYL_HOST_INGEST=ascii; lazily allocated, reused across calls)
-    cudaStream_t copy_stream = nullptr;
-    cudaEvent_t ev_copied[2] = {nullptr, nullptr}, ev_used[2] = {nullptr, nullptr};
-    uint8_t *stage_b[2] = {nullptr, nullptr};
-    uint64_t *stage_o[2] = {nullptr, nullptr};
-    uint64_t stage_cap_b[2] = {0, 0}, stage_cap_o[2] = {0, 0};
+    // HostIngest (sample.cu) of the host-memory read path: packer pool, copy stream, pinned ring of packed chunks
+    // and two-slot device ring of ASCII chunks (lazily allocated, reused across calls)
+    void *ingest = nullptr;
     // grow-only cache of scratch blocks: all work of a ctx is ordered on ONE stream, so a block can
     // be handed to the next user as soon as the previous user's kernels are enqueued; steady-state
     // calls then make no allocator calls at all (the CUDA allocators take driver-wide locks and
@@ -236,6 +232,22 @@ struct DevBuf {
         }
         p = nullptr;
         n = 0;
+    }
+};
+
+// A whole caller input on the device: SYL_MEM_DEVICE pointers are used as they are, host memory is copied into a
+// stream-ordered buffer with 64 bytes of padding past the end (the seeding kernel's bulk loads read past the last base).
+template <typename T>
+struct Staged {
+    const T *p = nullptr;
+    DevBuf<T> buf;
+    int init(syl_ctx *ctx, int mem, const T *src, size_t n) {
+        if (mem == SYL_MEM_DEVICE) { p = src; return SYL_OK; }
+        if (mem != SYL_MEM_HOST) { set_error("bad mem"); return SYL_ERR_ARG; }
+        SYL_TRY(buf.alloc(n + 64 / sizeof(T), ctx->stream));
+        if (n) SYL_CUDA(cudaMemcpyAsync(buf.p, src, n * sizeof(T), cudaMemcpyHostToDevice, ctx->stream));
+        p = buf.p;
+        return SYL_OK;
     }
 };
 

@@ -437,48 +437,27 @@ static int sketch_genomes_impl(syl_ctx *ctx, int mem, const uint8_t *bases, cons
     SYL_CUDA(cudaSetDevice(ctx->device));
     syl::tl_ctx = ctx;
     cudaStream_t st = ctx->stream;
-    DevBuf<uint8_t> hb;   // host memory: staged copies, alive until the call's last sync
-    DevBuf<uint32_t> hp;
-    DevBuf<uint64_t> hc, hg;
-    const uint8_t *d_bases = bases;
-    const uint32_t *d_packed = packed;
-    const uint64_t *d_coff = contig_off, *d_goff = genome_off;
-    if (individual) n_genomes = n_contigs;
-    if (mem == SYL_MEM_HOST) {
-        if (packed) {
-            const uint64_t nw = (n_bases + 15) / 16;
-            SYL_TRY(hp.alloc(nw + 16, st));
-            if (nw) SYL_CUDA(cudaMemcpyAsync(hp.p, packed, nw * 4, cudaMemcpyHostToDevice, st));
-            d_packed = hp.p;
-        } else {
-            SYL_TRY(hb.alloc(n_bases + 64, st));
-            if (n_bases) SYL_CUDA(cudaMemcpyAsync(hb.p, bases, n_bases, cudaMemcpyHostToDevice, st));
-            d_bases = hb.p;
-        }
-        SYL_TRY(hc.alloc(n_contigs + 1, st));
-        SYL_CUDA(cudaMemcpyAsync(hc.p, contig_off, (n_contigs + 1) * 8, cudaMemcpyHostToDevice, st));
-        d_coff = hc.p;
-        if (!individual) {
-            SYL_TRY(hg.alloc(n_genomes + 1, st));
-            SYL_CUDA(cudaMemcpyAsync(hg.p, genome_off, (n_genomes + 1) * 8, cudaMemcpyHostToDevice, st));
-            d_goff = hg.p;
-        }
-    } else if (mem != SYL_MEM_DEVICE) {
-        set_error("bad mem");
-        return SYL_ERR_ARG;
-    }
+    Staged<uint8_t> sb;  // host memory: staged copies, alive until the call's last sync
+    Staged<uint32_t> sp;
+    Staged<uint64_t> sc, sg;
+    if (packed) SYL_TRY(sp.init(ctx, mem, packed, (n_bases + 15) / 16));
+    else SYL_TRY(sb.init(ctx, mem, bases, n_bases));
+    SYL_TRY(sc.init(ctx, mem, contig_off, n_contigs + 1));
     if (individual) {  // every record is its own genome (src/sketch.rs:481-548)
-        SYL_TRY(hg.alloc(n_contigs + 1, st));
-        k_iota64<<<nblk(n_contigs + 1, 256), 256, 0, st>>>(hg.p, n_contigs + 1);
+        n_genomes = n_contigs;
+        SYL_TRY(sg.buf.alloc(n_contigs + 1, st));
+        k_iota64<<<nblk(n_contigs + 1, 256), 256, 0, st>>>(sg.buf.p, n_contigs + 1);
         ctx->launches++;
-        d_goff = hg.p;
+        sg.p = sg.buf.p;
+    } else {
+        SYL_TRY(sg.init(ctx, mem, genome_off, n_genomes + 1));
     }
     syl_genomes *g = new (std::nothrow) syl_genomes();
     if (!g) return SYL_ERR_OOM;
     g->device = ctx->device;
     g->k = k;
     g->c = c;
-    int rc = sketch_genomes_device(ctx, d_bases, d_packed, n_bases, d_coff, n_contigs, d_goff, n_genomes, k, c, min_spacing,
+    int rc = sketch_genomes_device(ctx, sb.p, sp.p, n_bases, sc.p, n_contigs, sg.p, n_genomes, k, c, min_spacing,
                                    pseudotax, sem, g);
     if (rc != SYL_OK) { syl_genomes_free(g); return rc; }
     *out = g;

@@ -924,34 +924,77 @@ namespace syl {
 // ASCII bases in (pinned or pageable) host memory are cut into chunks on record boundaries; the ctx's
 // worker pool packs chunk i+1.. into a ring of pinned staging buffers (exact BYTE_TO_SEQ codes, 16
 // bases per word; record offsets rebased to u32) while chunk i crosses PCIe and earlier chunks are
-// seeded.  4.3 bytes of H2D traffic per 16 bases instead of 16.5 (SURVEY §8 f3).
+// seeded.  4.3 bytes of H2D traffic per 16 bases instead of 16.5 (SURVEY §8 f3).  Chunks may also cross
+// the link as ASCII, through a two-slot device ring: every chunk when packing is off (SYL_HOST_INGEST=ascii),
+// else chunks taken from the back of the sample while the packers lag behind.
 constexpr int ING_SLOTS = 4;
-constexpr uint64_t ING_CHUNK = 32ull << 20;   // bases per chunk (multiple of 16); SYL_INGEST_CHUNK overrides (tests)
-static uint64_t ingest_chunk() {
+constexpr uint64_t ING_CHUNK = 32ull << 20;        // bases per packed chunk (multiple of 16)
+constexpr uint64_t ING_ASCII_CHUNK = 128ull << 20; // bases per chunk when every chunk is shipped as ASCII
+constexpr uint64_t ING_MAXREC = 1ull << 19;        // records per packed chunk
+constexpr uint64_t ING_SLICE = 256ull << 10;       // bases per work item
+constexpr uint64_t ING_OSLICE = 64ull << 10;       // offsets per work item
+// SYL_INGEST_CHUNK overrides the chunk size of either mode (tests; read per call)
+static uint64_t ingest_chunk(uint64_t dflt) {
     if (const char *e = getenv("SYL_INGEST_CHUNK")) {
         const long long v = atoll(e);
         if (v >= 16) return (uint64_t)v & ~15ull;
     }
-    return ING_CHUNK;
+    return dflt;
 }
-constexpr uint64_t ING_MAXREC = 1ull << 19;   // records per chunk
-constexpr uint64_t ING_SLICE = 256ull << 10;  // bases per work item
-constexpr uint64_t ING_OSLICE = 64ull << 10;  // offsets per work item
+
+struct Chunk { uint64_t r0, r1, base, nb; };
+
+// records [r0, r1) per chunk: at most max_bases bases and max_recs records, at least one record
+static void plan_chunks(const uint64_t *rec_off, uint64_t n_reads, uint64_t max_bases, uint64_t max_recs,
+                        std::vector<Chunk> &chunks) {
+    uint64_t r0 = 0;
+    while (r0 < n_reads) {
+        const uint64_t base = rec_off[r0];
+        uint64_t lo = r0 + 1, hi = std::min(n_reads, r0 + max_recs);
+        while (lo < hi) {
+            const uint64_t mid = (lo + hi + 1) >> 1;
+            if (rec_off[mid] - base <= max_bases) lo = mid; else hi = mid - 1;
+        }
+        chunks.push_back({r0, lo, base, rec_off[lo] - base});
+        r0 = lo;
+    }
+}
 
 struct HostIngest {
     std::unique_ptr<PackPool> pool;
+    cudaStream_t copy_stream = nullptr;  // the H2D copies of both rings
+    // packed ring: words and chunk-relative u32 offsets, written by the pool
     uint32_t *h_words[ING_SLOTS] = {}, *h_off[ING_SLOTS] = {};  // pinned
     uint32_t *d_words[ING_SLOTS] = {}, *d_off32[ING_SLOTS] = {};
     uint64_t *d_off64[ING_SLOTS] = {};
     uint64_t cap_words = 0, cap_recs = 0;
     cudaEvent_t ev_copied[ING_SLOTS] = {}, ev_used[ING_SLOTS] = {};
-    // chunks that cross the link as ASCII while the packers are behind (pinned caller memory only)
+    // ASCII ring: bases and u64 offsets copied from caller memory as they are
     uint8_t *d_asc[2] = {};
     uint64_t *d_aoff[2] = {};
+    uint64_t cap_asc = 0, cap_aoff = 0;
     cudaEvent_t ev_a_copied[2] = {}, ev_a_used[2] = {};
-    cudaStream_t copy_stream = nullptr;
+    int a_slot = 0, a_last = -1;  // next ASCII slot; slot of the latest ASCII copy (-1: none yet)
 
-    void release_buffers() {
+    int init() {
+        if (copy_stream) return SYL_OK;
+        SYL_CUDA(cudaStreamCreateWithFlags(&copy_stream, cudaStreamNonBlocking));
+        for (int i = 0; i < ING_SLOTS; i++) {
+            SYL_CUDA(cudaEventCreateWithFlags(&ev_copied[i], cudaEventDisableTiming));
+            SYL_CUDA(cudaEventCreateWithFlags(&ev_used[i], cudaEventDisableTiming));
+        }
+        for (int i = 0; i < 2; i++) {
+            SYL_CUDA(cudaEventCreateWithFlags(&ev_a_copied[i], cudaEventDisableTiming));
+            SYL_CUDA(cudaEventCreateWithFlags(&ev_a_used[i], cudaEventDisableTiming));
+        }
+        return SYL_OK;
+    }
+    // the two streams that use the ring buffers: idle before a buffer is freed, and after a failed call
+    void drain(cudaStream_t st) {
+        cudaStreamSynchronize(st);
+        cudaStreamSynchronize(copy_stream);
+    }
+    void free_packed() {
         for (int i = 0; i < ING_SLOTS; i++) {
             if (h_words[i]) cudaFreeHost(h_words[i]);
             if (h_off[i]) cudaFreeHost(h_off[i]);
@@ -961,30 +1004,28 @@ struct HostIngest {
             h_words[i] = h_off[i] = d_words[i] = d_off32[i] = nullptr;
             d_off64[i] = nullptr;
         }
+        cap_words = cap_recs = 0;
+    }
+    void free_ascii() {
         for (int i = 0; i < 2; i++) {
             if (d_asc[i]) cudaFree(d_asc[i]);
             if (d_aoff[i]) cudaFree(d_aoff[i]);
             d_asc[i] = nullptr;
             d_aoff[i] = nullptr;
         }
-        cap_words = cap_recs = 0;
+        cap_asc = cap_aoff = 0;
     }
-    int ensure(uint64_t words, uint64_t recs) {
-        if (!copy_stream) {
-            SYL_CUDA(cudaStreamCreateWithFlags(&copy_stream, cudaStreamNonBlocking));
-            for (int i = 0; i < ING_SLOTS; i++) {
-                SYL_CUDA(cudaEventCreateWithFlags(&ev_copied[i], cudaEventDisableTiming));
-                SYL_CUDA(cudaEventCreateWithFlags(&ev_used[i], cudaEventDisableTiming));
-            }
-            for (int i = 0; i < 2; i++) {
-                SYL_CUDA(cudaEventCreateWithFlags(&ev_a_copied[i], cudaEventDisableTiming));
-                SYL_CUDA(cudaEventCreateWithFlags(&ev_a_used[i], cudaEventDisableTiming));
-            }
+    // room for every chunk of the plan, and for at least ING_CHUNK bases and 65536 records
+    int ensure_packed(cudaStream_t st, const std::vector<Chunk> &chunks) {
+        uint64_t words = ING_CHUNK / 16, recs = 65536;
+        for (const Chunk &c : chunks) {
+            words = std::max(words, (c.nb + 15) / 16);
+            recs = std::max(recs, c.r1 - c.r0 + 1);
         }
         if (words <= cap_words && recs <= cap_recs) return SYL_OK;
-        SYL_CUDA(cudaDeviceSynchronize());
+        drain(st);
         const uint64_t w = std::max(words, cap_words), r = std::max(recs, cap_recs);
-        release_buffers();
+        free_packed();
         for (int i = 0; i < ING_SLOTS; i++) {
             SYL_CUDA(cudaMallocHost((void **)&h_words[i], (w + 16) * 4));
             SYL_CUDA(cudaMallocHost((void **)&h_off[i], (r + 16) * 4));
@@ -992,17 +1033,55 @@ struct HostIngest {
             SYL_CUDA(cudaMalloc((void **)&d_off32[i], (r + 16) * 4));
             SYL_CUDA(cudaMalloc((void **)&d_off64[i], (r + 16) * 8));
         }
-        for (int i = 0; i < 2; i++) {
-            SYL_CUDA(cudaMalloc((void **)&d_asc[i], (w + 16) * 16));
-            SYL_CUDA(cudaMalloc((void **)&d_aoff[i], (r + 16) * 8));
-        }
         cap_words = w;
         cap_recs = r;
         return SYL_OK;
     }
+    // room for every chunk of the plan, and for at least min_bases bases and 65536 records
+    int ensure_ascii(cudaStream_t st, const std::vector<Chunk> &chunks, uint64_t min_bases) {
+        uint64_t nb = min_bases, recs = 65536;
+        for (const Chunk &c : chunks) {
+            nb = std::max(nb, c.nb);
+            recs = std::max(recs, c.r1 - c.r0 + 1);
+        }
+        if (nb <= cap_asc && recs <= cap_aoff) return SYL_OK;
+        drain(st);
+        nb = std::max(nb, cap_asc);
+        recs = std::max(recs, cap_aoff);
+        free_ascii();
+        for (int i = 0; i < 2; i++) {
+            SYL_CUDA(cudaMalloc((void **)&d_asc[i], nb + 256));  // the seeding kernel's bulk loads read past the last base
+            SYL_CUDA(cudaMalloc((void **)&d_aoff[i], (recs + 16) * 8));
+        }
+        cap_asc = nb;
+        cap_aoff = recs;
+        return SYL_OK;
+    }
+    // One chunk from caller memory through the ASCII ring and into the builder.  The copy of a slot waits until
+    // the previous chunk in it is seeded; the read indices travel with the chunk, so chunks may go in any order.
+    int ship_ascii(syl_ctx *ctx, SampleBuilder &b, const uint8_t *bases, const uint64_t *rec_off, const Chunk &c) {
+        const int slot = a_slot;
+        a_slot ^= 1;
+        const uint64_t nr = c.r1 - c.r0;
+        cudaStreamWaitEvent(copy_stream, ev_a_used[slot], 0);
+        if (cudaMemcpyAsync(d_asc[slot], bases + c.base, c.nb, cudaMemcpyHostToDevice, copy_stream) != cudaSuccess ||
+            cudaMemcpyAsync(d_aoff[slot], rec_off + c.r0, (nr + 1) * 8, cudaMemcpyHostToDevice, copy_stream) != cudaSuccess) {
+            set_error("H2D copy failed");
+            return SYL_ERR_CUDA;
+        }
+        ctx->ingest_h2d_bytes += c.nb + (nr + 1) * 8;
+        ctx->ingest_chunks_ascii++;
+        cudaEventRecord(ev_a_copied[slot], copy_stream);
+        cudaStreamWaitEvent(ctx->stream, ev_a_copied[slot], 0);
+        const int rc = b.add(d_asc[slot], nullptr, c.nb, d_aoff[slot], c.base, nr, c.r0);
+        cudaEventRecord(ev_a_used[slot], ctx->stream);
+        a_last = slot;
+        return rc;
+    }
     ~HostIngest() {
         pool.reset();
-        release_buffers();
+        free_packed();
+        free_ascii();
         for (int i = 0; i < ING_SLOTS; i++) {
             if (ev_copied[i]) cudaEventDestroy(ev_copied[i]);
             if (ev_used[i]) cudaEventDestroy(ev_used[i]);
@@ -1020,39 +1099,41 @@ void ingest_destroy(syl_ctx *ctx) {
     ctx->ingest = nullptr;
 }
 
-struct Chunk { uint64_t r0, r1, base, nb; };
-
-// records [r0, r1) per chunk: at most ING_CHUNK bases and ING_MAXREC records, at least one record
-static void plan_chunks(const uint64_t *rec_off, uint64_t n_reads, std::vector<Chunk> &chunks) {
-    const uint64_t CH = ingest_chunk();
-    uint64_t r0 = 0;
-    while (r0 < n_reads) {
-        const uint64_t base = rec_off[r0];
-        uint64_t lo = r0 + 1, hi = std::min(n_reads, r0 + ING_MAXREC);
-        while (lo < hi) {
-            const uint64_t mid = (lo + hi + 1) >> 1;
-            if (rec_off[mid] - base <= CH) lo = mid; else hi = mid - 1;
-        }
-        chunks.push_back({r0, lo, base, rec_off[lo] - base});
-        r0 = lo;
-    }
-}
-
-// host ASCII -> packed chunks -> builder
-static int feed_host_packed(syl_ctx *ctx, SampleBuilder &b, const uint8_t *bases, const uint64_t *rec_off, uint64_t n_reads) {
+// host ASCII -> chunks -> builder.  ascii_only: every chunk crosses the link as it is, front to back (1 byte of
+// H2D traffic per base, no host packing; pageable caller memory is fine).  Else the pool packs the chunks.
+static int feed_host(syl_ctx *ctx, SampleBuilder &b, const uint8_t *bases, const uint64_t *rec_off, uint64_t n_reads,
+                     bool ascii_only) {
     if (!ctx->ingest) ctx->ingest = new HostIngest();
     HostIngest &I = *static_cast<HostIngest *>(ctx->ingest);
-    if (!I.pool) I.pool.reset(new PackPool(default_pack_threads()));
-    std::vector<Chunk> chunks;
-    plan_chunks(rec_off, n_reads, chunks);
-    uint64_t max_words = 0, max_recs = 0;
-    for (const Chunk &c : chunks) {
-        if (c.nb >= 0xFFFFFFF0ull) { set_error("a single record of 4 GB or more"); return SYL_ERR_ARG; }
-        max_words = std::max(max_words, (c.nb + 15) / 16);
-        max_recs = std::max(max_recs, c.r1 - c.r0 + 1);
-    }
-    SYL_TRY(I.ensure(std::max<uint64_t>(max_words, ING_CHUNK / 16), std::max<uint64_t>(max_recs, 65536)));
+    SYL_TRY(I.init());
     cudaStream_t st = ctx->stream, cs = I.copy_stream;
+    std::vector<Chunk> chunks;
+    if (ascii_only) {
+        plan_chunks(rec_off, n_reads, ingest_chunk(ING_ASCII_CHUNK), n_reads, chunks);
+        SYL_TRY(I.ensure_ascii(st, chunks, ING_ASCII_CHUNK));
+        int rc = SYL_OK;
+        for (size_t ci = 0; ci < chunks.size() && rc == SYL_OK; ci++) rc = I.ship_ascii(ctx, b, bases, rec_off, chunks[ci]);
+        if (rc != SYL_OK) I.drain(st);
+        return rc;
+    }
+    plan_chunks(rec_off, n_reads, ingest_chunk(ING_CHUNK), ING_MAXREC, chunks);
+    for (const Chunk &c : chunks)  // the packed offsets are chunk-relative u32
+        if (c.nb >= 0xFFFFFFF0ull) { set_error("a single record of 4 GB or more"); return SYL_ERR_ARG; }
+    // Two resources work in parallel: the packers (host memory bandwidth / CPU quota) and the PCIe link.  Packed
+    // chunks are consumed from the front in order; whenever the front chunk is not packed yet and no ASCII copy
+    // is in flight, a chunk nobody has started is taken from the BACK and shipped as ASCII (4x the bytes, but the
+    // link would idle otherwise).  Needs pinned caller memory (a pageable copy would block this thread).
+    bool steal_ok = false;
+    {
+        cudaPointerAttributes pa;
+        if (cudaPointerGetAttributes(&pa, bases) == cudaSuccess) steal_ok = pa.type == cudaMemoryTypeHost;
+        else cudaGetLastError();
+        const char *e = getenv("SYL_HOST_INGEST");
+        if (e && std::string(e) == "packed-only") steal_ok = false;
+    }
+    SYL_TRY(I.ensure_packed(st, chunks));
+    if (steal_ok) SYL_TRY(I.ensure_ascii(st, chunks, ING_CHUNK));
+    if (!I.pool) I.pool.reset(new PackPool(default_pack_threads()));
     std::vector<PackItem> items;
     std::vector<uint32_t> chunk_items(chunks.size());
     for (size_t ci = 0; ci < chunks.size(); ci++) {
@@ -1067,23 +1148,9 @@ static int feed_host_packed(syl_ctx *ctx, SampleBuilder &b, const uint8_t *bases
         chunk_items[ci] = n_items;
     }
     I.pool->start(&items, &chunk_items, ING_SLOTS - 1);
-    // Two resources work in parallel: the packers (host memory bandwidth / CPU quota) and the PCIe link.  Packed
-    // chunks are consumed from the front in order; whenever the front chunk is not packed yet and no ASCII copy
-    // is in flight, a chunk nobody has started is taken from the BACK and shipped as ASCII (4x the bytes, but the
-    // link would idle otherwise).  Needs pinned caller memory (a pageable copy would block this thread).
-    bool steal_ok = false;
-    {
-        cudaPointerAttributes pa;
-        if (cudaPointerGetAttributes(&pa, bases) == cudaSuccess) steal_ok = pa.type == cudaMemoryTypeHost;
-        else cudaGetLastError();
-        const char *e = getenv("SYL_HOST_INGEST");
-        if (e && std::string(e) == "packed-only") steal_ok = false;
-    }
     const bool force_steal = getenv("SYL_INGEST_FORCE_STEAL") != nullptr;  // tests: alternate packed / ASCII chunks
     int rc = SYL_OK;
     int64_t f = 0, bk = (int64_t)chunks.size() - 1, last_packed = -1;
-    int a_slot = 0, a_last = -1;
-    uint64_t n_ascii = 0, n_packed = 0;
     bool steal_turn = true;  // force_steal only: alternate ASCII and packed chunks
     while (f <= bk && rc == SYL_OK) {
         const bool steal_first = force_steal && steal_ok && steal_turn;
@@ -1110,28 +1177,13 @@ static int feed_host_packed(syl_ctx *ctx, SampleBuilder &b, const uint8_t *bases
             }
             last_packed = f;
             f++;
-            n_packed++;
+            ctx->ingest_chunks_packed++;
             steal_turn = true;
             continue;
         }
-        const bool ascii_busy = !force_steal && a_last >= 0 && cudaEventQuery(I.ev_a_copied[a_last]) == cudaErrorNotReady;
+        const bool ascii_busy = !force_steal && I.a_last >= 0 && cudaEventQuery(I.ev_a_copied[I.a_last]) == cudaErrorNotReady;
         if (steal_ok && !ascii_busy && (!force_steal || steal_turn) && bk > f && I.pool->try_skip_chunk((uint32_t)bk)) {  // ---- ASCII chunk from the back
-            const Chunk &c = chunks[(size_t)bk];
-            const int slot = a_slot;
-            a_slot ^= 1;
-            const uint64_t nr = c.r1 - c.r0;
-            cudaStreamWaitEvent(cs, I.ev_a_used[slot], 0);
-            if (cudaMemcpyAsync(I.d_asc[slot], bases + c.base, c.nb, cudaMemcpyHostToDevice, cs) != cudaSuccess ||
-                cudaMemcpyAsync(I.d_aoff[slot], rec_off + c.r0, (nr + 1) * 8, cudaMemcpyHostToDevice, cs) != cudaSuccess) {
-                rc = SYL_ERR_CUDA; set_error("H2D copy failed"); break;
-            }
-            ctx->ingest_h2d_bytes += c.nb + (nr + 1) * 8;
-            cudaEventRecord(I.ev_a_copied[slot], cs);
-            cudaStreamWaitEvent(st, I.ev_a_copied[slot], 0);
-            rc = b.add(I.d_asc[slot], nullptr, c.nb, I.d_aoff[slot], c.base, nr, c.r0);
-            cudaEventRecord(I.ev_a_used[slot], st);
-            a_last = slot;
-            n_ascii++;
+            rc = I.ship_ascii(ctx, b, bases, rec_off, chunks[(size_t)bk]);
             bk--;
             steal_turn = false;
             continue;
@@ -1145,82 +1197,10 @@ static int feed_host_packed(syl_ctx *ctx, SampleBuilder &b, const uint8_t *bases
     }
     I.pool->open_gate((int64_t)1 << 60);  // all remaining items (skipped chunks included) drain
     I.pool->finish();
-    ctx->ingest_chunks_ascii += n_ascii;
-    ctx->ingest_chunks_packed += n_packed;
     static const bool dbg = getenv("SYL_DEBUG_TIMING") != nullptr;
     if (dbg) fprintf(stderr, "[host ingest] %zu chunks: %llu shipped as ASCII, %zu packed by %d threads\n", chunks.size(),
-                     (unsigned long long)n_ascii, chunks.size() - (size_t)n_ascii, I.pool->threads());
-    if (rc != SYL_OK) { cudaStreamSynchronize(cs); cudaStreamSynchronize(st); }
-    return rc;
-}
-
-// host ASCII -> ASCII chunks (SYL_HOST_INGEST=ascii): the round-1 path, 1 byte of H2D traffic per base
-static int feed_host_ascii(syl_ctx *ctx, SampleBuilder &b, const uint8_t *bases, const uint64_t *rec_off, uint64_t n_reads) {
-    const uint64_t CHUNK = 128ull << 20;
-    cudaStream_t st = ctx->stream;
-    if (!ctx->copy_stream) {
-        SYL_CUDA(cudaStreamCreateWithFlags(&ctx->copy_stream, cudaStreamNonBlocking));
-        for (int i = 0; i < 2; i++) {
-            SYL_CUDA(cudaEventCreateWithFlags(&ctx->ev_copied[i], cudaEventDisableTiming));
-            SYL_CUDA(cudaEventCreateWithFlags(&ctx->ev_used[i], cudaEventDisableTiming));
-        }
-    }
-    cudaStream_t cs = ctx->copy_stream;
-    int rc = SYL_OK;
-    uint64_t r0 = 0;
-    int slot = 0;
-    struct Pending { uint64_t nb, nr, bias; int slot; bool valid; } pend = {0, 0, 0, 0, false};
-    while (r0 < n_reads || pend.valid) {
-        Pending next = {0, 0, 0, slot, false};
-        if (r0 < n_reads) {
-            uint64_t lo = r0 + 1, hi = n_reads;
-            const uint64_t base = rec_off[r0];
-            while (lo < hi) {
-                uint64_t mid = (lo + hi + 1) >> 1;
-                if (rec_off[mid] - base <= CHUNK) lo = mid; else hi = mid - 1;
-            }
-            const uint64_t r1 = lo, nb = rec_off[r1] - base, nr = r1 - r0;
-            if (nb + 64 > ctx->stage_cap_b[slot]) {
-                cudaStreamSynchronize(st);
-                cudaStreamSynchronize(cs);
-                if (ctx->stage_b[slot]) cudaFree(ctx->stage_b[slot]);
-                ctx->stage_b[slot] = nullptr;
-                ctx->stage_cap_b[slot] = std::max<uint64_t>(nb + 64, CHUNK + 64);
-                if (cudaMalloc((void **)&ctx->stage_b[slot], ctx->stage_cap_b[slot]) != cudaSuccess) {
-                    ctx->stage_cap_b[slot] = 0; rc = SYL_ERR_OOM; set_error("staging alloc failed"); break;
-                }
-            }
-            if (nr + 1 > ctx->stage_cap_o[slot]) {
-                cudaStreamSynchronize(st);
-                cudaStreamSynchronize(cs);
-                if (ctx->stage_o[slot]) cudaFree(ctx->stage_o[slot]);
-                ctx->stage_o[slot] = nullptr;
-                ctx->stage_cap_o[slot] = (nr + 1) * 2;
-                if (cudaMalloc((void **)&ctx->stage_o[slot], ctx->stage_cap_o[slot] * 8) != cudaSuccess) {
-                    ctx->stage_cap_o[slot] = 0; rc = SYL_ERR_OOM; set_error("staging alloc failed"); break;
-                }
-            }
-            cudaStreamWaitEvent(cs, ctx->ev_used[slot], 0);  // previous user of this slot is done
-            if (cudaMemcpyAsync(ctx->stage_b[slot], bases + base, nb, cudaMemcpyHostToDevice, cs) != cudaSuccess ||
-                cudaMemcpyAsync(ctx->stage_o[slot], rec_off + r0, (nr + 1) * 8, cudaMemcpyHostToDevice, cs) != cudaSuccess) {
-                rc = SYL_ERR_CUDA; set_error("H2D copy failed"); break;
-            }
-            ctx->ingest_h2d_bytes += nb + (nr + 1) * 8;
-            ctx->ingest_chunks_ascii++;
-            cudaEventRecord(ctx->ev_copied[slot], cs);
-            next = {nb, nr, base, slot, true};
-            r0 = r1;
-            slot ^= 1;
-        }
-        if (pend.valid) {
-            cudaStreamWaitEvent(st, ctx->ev_copied[pend.slot], 0);
-            rc = b.add(ctx->stage_b[pend.slot], nullptr, pend.nb, ctx->stage_o[pend.slot], pend.bias, pend.nr, b.n_reads);
-            cudaEventRecord(ctx->ev_used[pend.slot], st);
-            if (rc != SYL_OK) break;
-        }
-        pend = next;
-    }
-    if (rc != SYL_OK) { cudaStreamSynchronize(cs); cudaStreamSynchronize(st); }
+                     (unsigned long long)ctx->ingest_chunks_ascii, chunks.size() - (size_t)ctx->ingest_chunks_ascii, I.pool->threads());
+    if (rc != SYL_OK) I.drain(st);
     return rc;
 }
 
@@ -1233,7 +1213,6 @@ static int sketch_reads_impl(syl_ctx *ctx, int mem, const uint8_t *bases, const 
     *out = nullptr;
     SYL_CUDA(cudaSetDevice(ctx->device));
     syl::tl_ctx = ctx;
-    cudaStream_t st = ctx->stream;
     // Host ASCII input: packed by the worker pool (fewer PCIe bytes) or shipped as it is.  Packing costs host memory
     // traffic (1.5 B per base: the packers read the ASCII, write the words, the copy engine reads them; ASCII costs 1 B
     // per base), so it pays while PCIe is the narrow resource — 1 to 4 processes per host — and loses once the ranks of
@@ -1254,20 +1233,18 @@ static int sketch_reads_impl(syl_ctx *ctx, int mem, const uint8_t *bases, const 
         SYL_TRY(b.begin(cap_override));
         const double t0 = now();
         int rc = SYL_OK;
-        DevBuf<uint32_t> hp;   // host packed input staged whole
-        DevBuf<uint64_t> ho;
+        Staged<uint32_t> sp;   // host packed input staged whole
+        Staged<uint64_t> so;
         if (mem == SYL_MEM_DEVICE) {
             rc = b.add(bases, packed, n_bases, rec_off, 0, n_reads, 0);
         } else if (packed) {
             const uint64_t nw = (n_bases + 15) / 16;
-            SYL_TRY(hp.alloc(nw + 16, st));
-            SYL_TRY(ho.alloc(n_reads + 1, st));
-            if (nw) SYL_CUDA(cudaMemcpyAsync(hp.p, packed, nw * 4, cudaMemcpyHostToDevice, st));
-            SYL_CUDA(cudaMemcpyAsync(ho.p, rec_off, (n_reads + 1) * 8, cudaMemcpyHostToDevice, st));
+            SYL_TRY(sp.init(ctx, mem, packed, nw));
+            SYL_TRY(so.init(ctx, mem, rec_off, n_reads + 1));
             ctx->ingest_h2d_bytes += nw * 4 + (n_reads + 1) * 8;
-            rc = b.add(nullptr, hp.p, n_bases, ho.p, 0, n_reads, 0);
+            rc = b.add(nullptr, sp.p, n_bases, so.p, 0, n_reads, 0);
         } else if (n_reads && n_bases) {
-            rc = host_ascii ? feed_host_ascii(ctx, b, bases, rec_off, n_reads) : feed_host_packed(ctx, b, bases, rec_off, n_reads);
+            rc = feed_host(ctx, b, bases, rec_off, n_reads, host_ascii);
         }
         if (rc != SYL_OK) return rc;
         const double t1 = now();
@@ -1281,33 +1258,13 @@ static int sketch_reads_impl(syl_ctx *ctx, int mem, const uint8_t *bases, const 
     return SYL_ERR_CAPACITY;
 }
 
-// One mate file of a paired sample: ASCII bytes or 2-bit words, device resident after stage().
+// One mate file of a paired sample: ASCII bytes or 2-bit words.
 struct MateInput {
     const uint8_t *bases;
     const uint32_t *packed;
     uint64_t n_bases;
     const uint64_t *off;
-    DevBuf<uint8_t> hb;  // host memory: staged copies, alive until the call's sync
-    DevBuf<uint32_t> hp;
-    DevBuf<uint64_t> ho;
     uint64_t n_words() const { return (n_bases + 15) / 16; }
-    // one copy of the bases / words and one of the offsets
-    int stage(syl_ctx *ctx, bool is_packed, uint64_t n_pairs) {
-        cudaStream_t st = ctx->stream;
-        if (is_packed) {
-            SYL_TRY(hp.alloc(n_words() + 16, st));
-            if (n_bases) SYL_CUDA(cudaMemcpyAsync(hp.p, packed, n_words() * 4, cudaMemcpyHostToDevice, st));
-            packed = hp.p;
-        } else {
-            SYL_TRY(hb.alloc(n_bases + 64, st));
-            if (n_bases) SYL_CUDA(cudaMemcpyAsync(hb.p, bases, n_bases, cudaMemcpyHostToDevice, st));
-            bases = hb.p;
-        }
-        SYL_TRY(ho.alloc(n_pairs + 1, st));
-        SYL_CUDA(cudaMemcpyAsync(ho.p, off, (n_pairs + 1) * 8, cudaMemcpyHostToDevice, st));
-        off = ho.p;
-        return SYL_OK;
-    }
 };
 
 // packed: both mates are 2-bit words (m1.packed / m2.packed), else ASCII (m1.bases / m2.bases)
@@ -1323,9 +1280,15 @@ static int sketch_read_pairs_impl(syl_ctx *ctx, int mem, bool packed, MateInput 
     SYL_CUDA(cudaSetDevice(ctx->device));
     syl::tl_ctx = ctx;
     cudaStream_t st = ctx->stream;
-    if (mem == SYL_MEM_HOST) {
-        SYL_TRY(m1.stage(ctx, packed, n_pairs));
-        SYL_TRY(m2.stage(ctx, packed, n_pairs));
+    Staged<uint8_t> sb[2];  // host memory: staged copies, alive until the call's sync
+    Staged<uint32_t> sp[2];
+    Staged<uint64_t> so[2];
+    MateInput *m[2] = {&m1, &m2};
+    for (int i = 0; i < 2; i++) {
+        if (packed) { SYL_TRY(sp[i].init(ctx, mem, m[i]->packed, m[i]->n_words())); m[i]->packed = sp[i].p; }
+        else { SYL_TRY(sb[i].init(ctx, mem, m[i]->bases, m[i]->n_bases)); m[i]->bases = sb[i].p; }
+        SYL_TRY(so[i].init(ctx, mem, m[i]->off, n_pairs + 1));
+        m[i]->off = so[i].p;
     }
     uint64_t cap_override = 0;
     for (int attempt = 0; attempt < 3; attempt++) {

@@ -1,4 +1,4 @@
-// Scheduler stress test of syl::PackPool without a GPU: mirrors the chunk loop of feed_host_packed (sample.cu) —
+// Scheduler stress test of syl::PackPool without a GPU: mirrors the packed chunk loop of feed_host (sample.cu) —
 // packed chunks in order from the front behind a gate of R staging slots, chunks taken over by the caller from the
 // back, forced alternation (SYL_INGEST_FORCE_STEAL).  Must terminate.
 #include "host_pack.hpp"

@@ -96,6 +96,54 @@ def test_host_ingest_chunk_ring(ctx, monkeypatch):
         assert np.array_equal(h, eh) and np.array_equal(c, ec) and s.num_dup_removed == nd, chunk
 
 
+def ascii_chunk_plan(off, chunk):
+    """Records [r0, r1) per chunk of ASCII-only host ingest: as many as fit in `chunk` bases, at least one."""
+    plan, r0 = [], 0
+    while r0 < len(off) - 1:
+        r1 = max(r0 + 1, int(np.searchsorted(off, off[r0] + np.uint64(chunk), side="right")) - 1)
+        plan.append((r0, r1))
+        r0 = r1
+    return plan
+
+
+@pytest.mark.parametrize("pinned", [True, False])
+def test_host_ingest_ascii_only_chunks(ctx, monkeypatch, pinned):
+    """SYL_HOST_INGEST=ascii: every chunk crosses the link as ASCII, front to back through the two-slot ring, from
+    pinned or pageable caller memory.  Chunks far smaller than the input (every slot recycled many times), records
+    longer than a chunk, empty records, N and lower-case bases, duplicated reads in distant chunks.  The call ships
+    exactly the planned chunks: their bases and their offsets (one more than the chunk's records)."""
+    import torch
+    from oracle import oracle as O
+    chunk = 8192
+    rng = np.random.default_rng(9)
+    lengths = list(rng.integers(0, 400, size=3000)) + [30000, 9000, 0, 0, 0, 150, 33]
+    one, one_off = random_records(rng, [lengths[i] for i in rng.permutation(len(lengths))], alphabet=b"ACGTNacgtn")
+    # the first third of the reads twice, in distant chunks: order-dependent dedup
+    off = np.concatenate([one_off, one_off[-1] + one_off[1:np.searchsorted(one_off, len(one) // 3)]]).astype(np.uint64)
+    buf = np.concatenate([one, one])[: int(off[-1])]
+    assert (np.diff(off) == 0).any() and np.diff(off).max() > chunk
+    eh, ec, _, nd = O.sketch_reads(buf, off, c=11)
+    assert nd > 100
+    plan = ascii_chunk_plan(off, chunk)
+    assert len(plan) > 40
+    h2d_exp = sum(int(off[r1] - off[r0]) + 8 * (r1 - r0 + 1) for r0, r1 in plan)
+    if pinned:
+        hb = torch.empty(len(buf), dtype=torch.uint8, pin_memory=True)
+        hb.numpy()[:] = buf
+        ho = torch.empty(len(off), dtype=torch.int64, pin_memory=True)
+        ho.numpy()[:] = off.astype(np.int64)
+        b, o = hb.numpy(), ho.numpy().view(np.uint64)
+    else:
+        b, o = buf, off
+    monkeypatch.setenv("SYL_HOST_INGEST", "ascii")
+    monkeypatch.setenv("SYL_INGEST_CHUNK", str(chunk))
+    s = ctx.sketch_sequences(b, o, c=11)
+    h, c = s.download()
+    assert np.array_equal(h, eh) and np.array_equal(c, ec) and s.num_dup_removed == nd
+    h2d, n_packed, n_ascii = ctx.ingest_stats()
+    assert n_packed == 0 and n_ascii == len(plan) and h2d == h2d_exp
+
+
 TILE = 32768   # window starts per CTA tile of the seeding kernel (seed_kernel.cuh SEED_TILE)
 HALO = 48      # bases staged past the tile
 
