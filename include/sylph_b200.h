@@ -155,13 +155,16 @@ int syl_sketch_reads_packed2(syl_ctx *ctx, int mem, const uint32_t *packed, uint
  * (k-mer, pair key) set with no count threshold (:829-838, :855-865): pair_kmer (:658-688) keys from the first 32
  * bases of both mates, mate 1's k-mers first, mate 2's k-mers that also occur in mate 1 skipped (:849-853).
  * Mate i of pair p = record p of buffer i; n_pairs = records zipped from the two files; n_bases_i = rec_off_i[n_pairs].  The reference's default
- * (approximate scalable cuckoo filter, fpr 1e-4) is not bit-reproducible and stays out of scope (SURVEY R11). */
+ * (approximate scalable cuckoo filter, fpr 1e-4) is not bit-reproducible and stays out of scope (SURVEY R11).
+ * SYL_MEM_HOST: the sample crosses the link as chunks of pairs (both mates of a chunk 2-bit packed by the worker
+ * threads into one pinned staging buffer, or shipped as ASCII: SYL_HOST_INGEST as for syl_sketch_reads) while earlier
+ * chunks are seeded, so the device holds the staging rings and the events, never the sample's bases. */
 int syl_sketch_read_pairs(syl_ctx *ctx, int mem, const uint8_t *bases1, uint64_t n_bases1, const uint64_t *rec_off1,
                           const uint8_t *bases2, uint64_t n_bases2, const uint64_t *rec_off2, uint64_t n_pairs,
                           int k, uint64_t c, int no_dedup, int sem, syl_sample **out);
 /* The same for mates that are already 2-bit packed (layout: see syl_sketch_reads_packed2; one word buffer per mate file,
  * ceil(n_bases_i/16) words, rec_off_i in bases).  Same result as syl_sketch_read_pairs on the ASCII it was packed from.
- * SYL_MEM_HOST copies each word buffer and each offset array to the device once (4x fewer bytes than ASCII);
+ * SYL_MEM_HOST copies each word buffer and each offset array to the device whole, once (4x fewer bytes than ASCII; not chunked);
  * SYL_MEM_DEVICE word buffers must be 16-byte aligned (else SYL_ERR_ARG). */
 int syl_sketch_read_pairs_packed2(syl_ctx *ctx, int mem, const uint32_t *packed1, uint64_t n_bases1, const uint64_t *rec_off1,
                                   const uint32_t *packed2, uint64_t n_bases2, const uint64_t *rec_off2, uint64_t n_pairs,
@@ -170,9 +173,14 @@ int syl_sketch_read_pairs_packed2(syl_ctx *ctx, int mem, const uint32_t *packed1
 int syl_pack2(const uint8_t *bases, uint64_t n_bases, uint32_t *words, int n_threads);
 /* Worker threads the host-memory path of syl_sketch_reads packs with (for bench.py's e2e record). */
 int syl_pack_threads(void);
-/* What the last syl_sketch_reads(SYL_MEM_HOST, ASCII) call of this ctx moved: host-to-device bytes (bases + record
- * offsets, as copied) and how many of its chunks crossed the link as 2-bit words / as ASCII. */
+/* What the last syl_sketch_reads / syl_sketch_read_pairs(SYL_MEM_HOST, ASCII) call of this ctx moved: host-to-device
+ * bytes (bases + record offsets, as copied) and how many of its chunks (of reads, or of pairs) crossed the link as
+ * 2-bit words / as ASCII.  Host 2-bit input (the _packed2 calls) is staged whole: its bytes, no chunks. */
 int syl_ctx_ingest_stats(const syl_ctx *ctx, uint64_t *h2d_bytes, uint64_t *chunks_packed, uint64_t *chunks_ascii);
+/* Bytes the host-memory staging rings of this ctx hold now: on the device (allocated outside the block cache, so
+ * syl_ctx_device_bytes does not count them) and in pinned host memory.  They grow to the largest chunk seen and
+ * live until the ctx is destroyed. */
+int syl_ctx_ingest_ring_bytes(const syl_ctx *ctx, uint64_t *device_bytes, uint64_t *pinned_bytes);
 /* Wrap an existing sketch (e.g. a deserialised .sylsp).  Pairs need not be sorted; hashes must
  * be distinct. */
 int syl_sample_upload(syl_ctx *ctx, int mem, const uint64_t *hash, const uint32_t *count,

@@ -95,10 +95,18 @@ class Context:
     KERNELS = {"seed": 0, "group_dedup": 1, "join": 2, "join2": 3, "stats": 4, "boot": 5, "genome_post": 6, "pack": 7}
 
     def ingest_stats(self):
-        """-> (h2d_bytes, chunks_packed, chunks_ascii) of the last host-memory sketch_sequences call."""
+        """-> (h2d_bytes, chunks_packed, chunks_ascii) of the last host-memory sketch_sequences or
+        sketch_pair_sequences call."""
         a, b, c = C.c_uint64(0), C.c_uint64(0), C.c_uint64(0)
         _lib.check(_lib.lib().syl_ctx_ingest_stats(self._h, C.byref(a), C.byref(b), C.byref(c)))
         return a.value, b.value, c.value
+
+    def ingest_ring_bytes(self):
+        """-> (device_bytes, pinned_bytes) of the host-memory staging rings (syl_ctx_ingest_ring_bytes); device_bytes()
+        does not count them."""
+        d, h = C.c_uint64(0), C.c_uint64(0)
+        _lib.check(_lib.lib().syl_ctx_ingest_ring_bytes(self._h, C.byref(d), C.byref(h)))
+        return d.value, h.value
 
     def device_bytes(self, reset_peak=False):
         """-> (held, peak): bytes of device memory the ctx holds, and the high-water mark of that plus the index

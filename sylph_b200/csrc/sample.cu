@@ -14,6 +14,8 @@
 // event counts).  Groups that do not fit take the generic path: two stable LSD radix sorts by
 // (hash, read index) and one thread per (contiguous) k-mer segment.  Within one read the order
 // of repeated k-mers is irrelevant (identical events; the second is a duplicate either way).
+// Read pairs (sketch_pair_sequences with --fpr 0, src/sketch.rs:771-895) take the same groups with their own
+// per-k-mer rule (k_group_dedup<true>), and the same generic path with k_dedup_paired.
 #include <cub/cub.cuh>
 
 #include <chrono>
@@ -122,13 +124,15 @@ k_events_fix(EventRec *__restrict__ ev, const uint32_t *__restrict__ pend, const
 // the pair carries them.  Events arrive with recflag = pair << 1 | EV_PENDING; the result is
 // recflag = pair << 2 | mate << 1 | NO_PAIR (a mate shorter than 33 bp, or --no-dedup).
 // ASCII input: bases1 / bases2; 2-bit input: packed1 / packed2 of n_words1 / n_words2 words.
+// The batch holds pairs [rec_base, ..): off1 / off2 start at pair rec_base, and off - bias is a start inside the batch.
 template <bool PACKED>
 __global__ void __launch_bounds__(EV_THREADS)
 k_events_fix_paired(EventRec *__restrict__ ev, const uint32_t *__restrict__ pend, const unsigned long long *__restrict__ p_begin,
                     const unsigned long long *__restrict__ p_end, uint64_t ev_cap, const uint8_t *__restrict__ bases1,
                     const uint32_t *__restrict__ packed1, uint64_t n_words1, const uint64_t *__restrict__ off1,
                     const uint8_t *__restrict__ bases2, const uint32_t *__restrict__ packed2, uint64_t n_words2,
-                    const uint64_t *__restrict__ off2, uint64_t mate, int no_dedup) {
+                    const uint64_t *__restrict__ off2, uint64_t bias1, uint64_t bias2, uint64_t rec_base, uint64_t mate,
+                    int no_dedup) {
     __shared__ uint8_t lut[4][256];
     if (!PACKED) {
         for (int i = threadIdx.x; i < 256; i += EV_THREADS) {
@@ -146,8 +150,8 @@ k_events_fix_paired(EventRec *__restrict__ ev, const uint32_t *__restrict__ pend
         if (ei >= ev_cap) continue;
         EventRec *e = ev + ei;
         const uint64_t pair = (e->recflag & ~EV_PENDING) >> 1;
-        const uint64_t a1 = off1[pair], a2 = off2[pair];
-        const uint64_t L1 = off1[pair + 1] - a1, L2 = off2[pair + 1] - a2;
+        const uint64_t a1 = off1[pair - rec_base] - bias1, a2 = off2[pair - rec_base] - bias2;
+        const uint64_t L1 = off1[pair - rec_base + 1] - bias1 - a1, L2 = off2[pair - rec_base + 1] - bias2 - a2;
         const bool has = !no_dedup && L1 >= 33 && L2 >= 33;  // 2 * 16 + 1 (:660)
         uint64_t p0 = 0, p1 = 0;
         if (has) {
@@ -329,6 +333,50 @@ struct GroupSmem {
     uint16_t longs[GRP_CAP / 2];      //  1 KB  slots of k-mers that need the warp-cooperative replay
 };
 
+// Read pairs: dup_removal_lsh_full_exact with threshold None (src/sketch.rs:829-865) for one k-mer whose len events
+// are S.member[a0 ..), recflag = pair << 2 | mate << 1 | NO_PAIR.  There is no MAX_DEDUP_COUNT, so every event is
+// tested, but nothing has to be replayed in order: the dedup set an event sees is the keys of the earlier paired
+// events that were not skipped, "earlier" is a compare of (recflag, event index), and c > 0 means that any event
+// that was not skipped comes earlier.  Two passes over the k-mer's events, each event against all others; the
+// caller's threads take events first, first + step, .. (one thread: 0, 1; a warp: lane, 32).
+constexpr uint64_t EV_SKIP = 1ull << 63;   // mate-2 event whose k-mer mate 1 of the same pair holds too (:849-853)
+constexpr uint32_t GRP_PAIR_THREAD = 8;    // events up to which one thread does the k-mer's len^2 compares; a warp beyond
+
+__device__ __forceinline__ void pair_mark_skipped(GroupSmem &S, uint32_t a0, uint32_t len, uint32_t first, uint32_t step) {
+    for (uint32_t e = first; e < len; e += step) {
+        const uint32_t m = S.member[a0 + e];
+        const uint64_t rf = S.rf[m];
+        if (!(rf & 2ull)) continue;
+        bool in_mate1 = false;
+        for (uint32_t q = 0; q < len; q++) in_mate1 |= S.rf[S.member[a0 + q]] == (rf ^ 2ull);  // NO_PAIR is the pair's
+        if (in_mate1) S.rf[m] = rf | EV_SKIP;
+    }
+}
+
+__device__ __forceinline__ void pair_count(const GroupSmem &S, uint32_t a0, uint32_t len, uint32_t first, uint32_t step,
+                                           uint32_t &c, uint32_t &dups) {
+    for (uint32_t e = first; e < len; e += step) {
+        const uint32_t m = S.member[a0 + e];
+        const uint64_t rf = S.rf[m];
+        if (rf & EV_SKIP) continue;
+        if (rf & NO_PAIR) { c++; continue; }  // a mate under 33 bp, or --no-dedup
+        const uint64_t ka = S.p0[m], kb = S.p1[m];
+        bool earlier = false, hit = false;
+        for (uint32_t q = 0; q < len; q++) {
+            const uint32_t mq = S.member[a0 + q];
+            const uint64_t rq = S.rf[mq];
+            if ((rq & EV_SKIP) || !(rq < rf || (rq == rf && mq < m))) continue;
+            earlier = true;
+            if (rq & NO_PAIR) continue;
+            const uint64_t qa = S.p0[mq], qb = S.p1[mq];
+            hit |= ka == qa || ka == qb || kb == qa || kb == qb;
+        }
+        // the second look-up sees the first key's insertion: ka == kb is a hit, a duplicate once c > 0 (:704-722)
+        if (hit || (ka == kb && earlier)) dups++; else c++;
+    }
+}
+
+template <bool PAIRED>
 __global__ void __launch_bounds__(GRP_THREADS)
 k_group_dedup(const EventRec *__restrict__ ev, const uint32_t *__restrict__ g_cnt, uint32_t slot, uint64_t Mb, uint32_t nbk,
               int no_dedup, uint64_t *__restrict__ st_hash, uint32_t *__restrict__ st_cnt,
@@ -414,6 +462,8 @@ k_group_dedup(const EventRec *__restrict__ ev, const uint32_t *__restrict__ g_cn
     //     has more than four events AND a duplicate among the first four needs more; it is queued
     //     for the warp-cooperative path below.
     //     The thread also counts its k-mer into its bucket (local index) for the output ordering.
+    //     PAIRED: pair_mark_skipped / pair_count instead, by this thread up to GRP_PAIR_THREAD events, by a warp
+    //     beyond; a group of pairs leaves the kernel only when it is past its slot.
     uint16_t *lb_cnt = S.ev_slot, *lb_off = S.ev_slot + GRP_BPG;  // ev_slot is dead: 2 x GRP_BPG u16
     if (tid < (int)GRP_BPG) lb_cnt[tid] = 0;
     __syncthreads();
@@ -426,7 +476,11 @@ k_group_dedup(const EventRec *__restrict__ ev, const uint32_t *__restrict__ g_cn
             atomicAdd(reinterpret_cast<unsigned int *>(lb_cnt) + (lb >> 1), (lb & 1) ? 0x10000u : 1u);
         }
         uint32_t c = 0;
-        if (no_dedup || len == 1) {
+        if (PAIRED) {
+            if (len > GRP_PAIR_THREAD) { S.longs[atomicAdd(&S.nlong, 1u)] = (uint16_t)sl; continue; }
+            if (len == 1) c = 1;
+            else { pair_mark_skipped(S, a0, len, 0, 1); pair_count(S, a0, len, 0, 1, c, my_dups); }
+        } else if (no_dedup || len == 1) {
             c = len;  // a first occurrence is never a duplicate (c == 0)
         } else {
             constexpr uint64_t INF = 0xFFFFFFFFFFFFFFFFull;
@@ -478,6 +532,16 @@ k_group_dedup(const EventRec *__restrict__ ev, const uint32_t *__restrict__ g_cn
     for (uint32_t li = wid; li < S.nlong; li += GRP_THREADS / 32) {
         const uint32_t sl = S.longs[li];
         const uint32_t a0 = S.soff[sl], len = S.soff[sl + 1] - a0;
+        if (PAIRED) {
+            uint32_t c = 0, dups = 0;
+            pair_mark_skipped(S, a0, len, lane, 32);
+            __syncwarp();
+            pair_count(S, a0, len, lane, 32, c, dups);
+            c = __reduce_add_sync(0xffffffffu, c);
+            dups = __reduce_add_sync(0xffffffffu, dups);
+            if (lane == 0) { S.scnt[sl] = (uint16_t)c; my_dups += dups; }
+            continue;
+        }
         uint32_t c = 0, done = 0, nset = 0;
         uint64_t last_key = 0, dset = 0;  // lane q keeps dedup-set entry q in `dset` (32 entries, then the group falls back)
         uint32_t last_m = 0;
@@ -622,6 +686,16 @@ static inline int bits_for(uint64_t maxval) {
     return b;
 }
 
+// One mate's (or a single-end sample's) share of a seeding batch, device resident: ASCII bytes or 2-bit words, and
+// the offsets of the batch's records (off[i] - off_bias is the start of record i inside the batch).
+struct Batch {
+    const uint8_t *bases;
+    const uint32_t *packed;
+    uint64_t nb;
+    const uint64_t *off;
+    uint64_t off_bias;
+};
+
 // Accumulates events over one or more seeding batches, then finishes into a syl_sample.
 // Nothing in begin() / add() synchronises with the host: the event array is sized up front from the
 // expected number of survivors, the seeding kernel appends at a running device counter, and every
@@ -634,11 +708,8 @@ struct SampleBuilder {
     uint64_t c;
     int no_dedup, sem;
     uint64_t n_reads = 0, n_bases = 0, cap = 0;
-    bool paired = false;     // read pairs (syl_sketch_read_pairs): events wait for k_events_fix_paired, generic post-pass only
-    bool generic_postpass() const {
-        static const bool env_sort = []() { const char *e = getenv("SYL_SAMPLE_POSTPASS"); return e && std::string(e) == "sort"; }();
-        return env_sort || paired;
-    }
+    bool paired = false;     // read pairs (syl_sketch_read_pairs): every event waits for k_events_fix_paired
+    bool sorted = false;     // SYL_SAMPLE_POSTPASS=sort (read in begin(), per call): no groups, the generic post-pass
     // Event array: ng group slots of `slot` events each, then the overflow list of cap events (everything
     // in the overflow list without groups).  A scratch block of the ctx cache.
     DevBuf<EventRec> b_ev;
@@ -649,7 +720,8 @@ struct SampleBuilder {
     uint32_t nbk = 0, ng = 0, slot = 0;
     uint64_t Mb = 0;
     DevBuf<uint32_t> g_cnt;  // events per group
-    // ctx->d_counters slots: [0] events in the overflow list, [1] pending events, [2] duplicates removed, [3] pending snapshot
+    // ctx->d_counters slots: [0] events in the overflow list, [1] pending events, [2] duplicates removed, [3] pending snapshot,
+    // [17], [18] add_pair's snapshots
     unsigned long long *d_count() const { return reinterpret_cast<unsigned long long *>(ctx->d_counters); }
     uint64_t ev_total() const { return (uint64_t)ng * slot + cap; }
 
@@ -657,7 +729,9 @@ struct SampleBuilder {
         cudaStream_t st = ctx->stream;
         const uint64_t win = expect_bases > expect_reads * (uint64_t)(k - 1) ? expect_bases - expect_reads * (uint64_t)(k - 1) : 0;
         const uint64_t n_exp = win / c;
-        if (!generic_postpass()) {
+        const char *pp = getenv("SYL_SAMPLE_POSTPASS");
+        sorted = pp && std::string(pp) == "sort";
+        if (!sorted) {
             static const uint32_t grp_cap = []() { const char *e = getenv("SYL_GROUP_CAP"); int v = e ? atoi(e) : GRP_CAP; return (uint32_t)std::min(std::max(v, 32), GRP_CAP); }();
             slot = grp_cap;
             const uint64_t g = n_exp / GRP_T + 1;
@@ -686,8 +760,10 @@ struct SampleBuilder {
     // one batch of reads, device resident (ASCII bytes or 2-bit words); read indices continue from the
     // previous batch.  The seeding kernel appends the batch's events (hash, read, pair keys) to the event array.
     // rec_base: index of the batch's first read in the sample (batches may arrive in any order)
-    int add(const uint8_t *d_bases, const uint32_t *d_packed, uint64_t nb, const uint64_t *d_off, uint64_t off_bias, uint64_t nr,
-            uint64_t rec_base) {
+    int add(const Batch &m, uint64_t nr, uint64_t rec_base) {
+        const uint8_t *d_bases = m.bases;
+        const uint32_t *d_packed = m.packed;
+        const uint64_t nb = m.nb, *d_off = m.off, off_bias = m.off_bias;
         cudaStream_t st = ctx->stream;
         if (nr == 0) return SYL_OK;
         unsigned long long *dc = d_count();
@@ -707,6 +783,32 @@ struct SampleBuilder {
         }
         n_reads += nr;
         n_bases += nb;
+        return SYL_OK;
+    }
+
+    int add_batch(const Batch *m, uint64_t nr, uint64_t rec_base) {  // m[0], and m[1] for pairs
+        return paired ? add_pair(m[0], m[1], nr, rec_base) : add(m[0], nr, rec_base);
+    }
+
+    // one batch of read pairs [rec_base, rec_base + nr): mate 1, then mate 2, both with the PAIR index as read index;
+    // the pending list tells the mates apart.  The keys need the first 32 bases of both mates, so the batch's events
+    // are completed here, while both are resident.
+    int add_pair(const Batch &m1, const Batch &m2, uint64_t nr, uint64_t rec_base) {
+        cudaStream_t st = ctx->stream;
+        if (nr == 0) return SYL_OK;
+        unsigned long long *dc = d_count();
+        SYL_CUDA(cudaMemcpyAsync(dc + 18, dc + 1, 8, cudaMemcpyDeviceToDevice, st));  // pending entries before the batch
+        SYL_TRY(add(m1, nr, rec_base));
+        SYL_CUDA(cudaMemcpyAsync(dc + 17, dc + 1, 8, cudaMemcpyDeviceToDevice, st));  // ... after mate 1
+        SYL_TRY(add(m2, nr, rec_base));
+        auto fix = m1.packed ? k_events_fix_paired<true> : k_events_fix_paired<false>;
+        const uint64_t nw1 = m1.packed ? (m1.nb + 15) / 16 : 0, nw2 = m2.packed ? (m2.nb + 15) / 16 : 0;
+        for (uint64_t mate = 0; mate < 2; mate++)
+            fix<<<ctx->num_sms * 2, EV_THREADS, 0, st>>>(b_ev.p, b_pend.p, mate ? dc + 17 : dc + 18, mate ? dc + 1 : dc + 17, ev_total(),
+                                                         m1.bases, m1.packed, nw1, m1.off, m2.bases, m2.packed, nw2, m2.off,
+                                                         m1.off_bias, m2.off_bias, rec_base, mate, no_dedup);
+        ctx->launches += 2;
+        SYL_CUDA(cudaGetLastError());
         return SYL_OK;
     }
 
@@ -801,11 +903,11 @@ struct SampleBuilder {
         s->mean_read_length = n_reads ? (double)n_bases / (double)n_reads : 0.;
         auto fail = [&](int rc) { syl_sample_free(s); return rc; };
 #define SB_CUDA(x) do { cudaError_t _e = (x); if (_e != cudaSuccess) { set_error(std::string(#x) + ": " + cudaGetErrorString(_e)); return fail(_e == cudaErrorMemoryAllocation ? SYL_ERR_OOM : SYL_ERR_CUDA); } } while (0)
-        if (n_reads == 0 || n_bases == 0) { *out = s; return SYL_OK; }
+        if (n_reads == 0 || expect_bases == 0) { *out = s; return SYL_OK; }  // pairs: n_bases is mate 1's, which may be empty
         unsigned long long *dc = d_count();
         EventRec *ev = b_ev.p;
         int rc;
-        if (generic_postpass()) {
+        if (sorted) {
             SB_CUDA(cudaMemcpyAsync(ctx->h_counters, dc, 8, cudaMemcpyDeviceToHost, st));
             SB_CUDA(cudaStreamSynchronize(st));
             const uint64_t N = ctx->h_counters[0];
@@ -842,11 +944,12 @@ struct SampleBuilder {
             (rc = foff.alloc((uint64_t)ng + 1, st)) || (rc = g_src.alloc(ng, st)))
             return fail(rc);
         unsigned long long *d_ndup = dc + 2;
-        SB_CUDA(cudaFuncSetAttribute(k_group_dedup, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(GroupSmem)));
+        auto group_dedup = paired ? k_group_dedup<true> : k_group_dedup<false>;
+        SB_CUDA(cudaFuncSetAttribute(group_dedup, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(GroupSmem)));
         {
             KernelTimer kt(ctx, SYL_KERNEL_GROUP_DEDUP);
-            k_group_dedup<<<ng, GRP_THREADS, sizeof(GroupSmem), st>>>(ev, g_cnt.p, slot, Mb, nbk, no_dedup,
-                                                                       st_hash.p, st_cnt.p, g_nuniq.p, g_n.p, g_fb.p, d_ndup);
+            group_dedup<<<ng, GRP_THREADS, sizeof(GroupSmem), st>>>(ev, g_cnt.p, slot, Mb, nbk, no_dedup,
+                                                                     st_hash.p, st_cnt.p, g_nuniq.p, g_n.p, g_fb.p, d_ndup);
         }
         k_scan_u32<<<1, 1024, 0, st>>>(g_nuniq.p, ng, uoff.p);
         k_fallback_sizes<<<nblk(ng, 256), 256, 0, st>>>(g_n.p, g_fb.p, ng, fsz.p);
@@ -942,20 +1045,35 @@ static uint64_t ingest_chunk(uint64_t dflt) {
     return dflt;
 }
 
-struct Chunk { uint64_t r0, r1, base, nb; };
+// One mate's ASCII input in host memory; a single-end sample has one, a sample of read pairs two with the same records.
+struct HostMate { const uint8_t *bases; const uint64_t *rec_off; };
 
-// records [r0, r1) per chunk: at most max_bases bases and max_recs records, at least one record
-static void plan_chunks(const uint64_t *rec_off, uint64_t n_reads, uint64_t max_bases, uint64_t max_recs,
+// Records (pairs) [r0, r1); per mate the first base and the number of bases.  A slot of either ring holds mate 1 at
+// its start and mate 2 behind it at mate2_at(nb[0]) bases: one ring, one copy of the words and one of the offsets per
+// chunk, whatever the number of mates.  Offsets: mate m's r1 - r0 + 1 entries start at entry m * (r1 - r0 + 1).
+struct Chunk {
+    uint64_t r0, r1, base[2], nb[2];
+    uint64_t n_off() const { return r1 - r0 + 1; }
+};
+// 256 bases: mate 2's words start 64-byte aligned and its ASCII 256-byte aligned (the seeding kernel's bulk copies need 16)
+static uint64_t mate2_at(uint64_t nb1) { return (nb1 + 255) & ~255ull; }
+static uint64_t footprint(const Chunk &c, int n_mates) { return n_mates == 2 ? mate2_at(c.nb[0]) + c.nb[1] : c.nb[0]; }
+
+// records [r0, r1) per chunk: at most max_bases bases (of all mates together) and max_recs records, at least one record
+static void plan_chunks(const HostMate *m, int n_mates, uint64_t n_reads, uint64_t max_bases, uint64_t max_recs,
                         std::vector<Chunk> &chunks) {
+    auto at = [&](uint64_t r) { return m[0].rec_off[r] + (n_mates == 2 ? m[1].rec_off[r] : 0); };
     uint64_t r0 = 0;
     while (r0 < n_reads) {
-        const uint64_t base = rec_off[r0];
+        const uint64_t base = at(r0);
         uint64_t lo = r0 + 1, hi = std::min(n_reads, r0 + max_recs);
         while (lo < hi) {
             const uint64_t mid = (lo + hi + 1) >> 1;
-            if (rec_off[mid] - base <= max_bases) lo = mid; else hi = mid - 1;
+            if (at(mid) - base <= max_bases) lo = mid; else hi = mid - 1;
         }
-        chunks.push_back({r0, lo, base, rec_off[lo] - base});
+        Chunk c{r0, lo, {0, 0}, {0, 0}};
+        for (int i = 0; i < n_mates; i++) { c.base[i] = m[i].rec_off[r0]; c.nb[i] = m[i].rec_off[lo] - c.base[i]; }
+        chunks.push_back(c);
         r0 = lo;
     }
 }
@@ -1016,11 +1134,11 @@ struct HostIngest {
         cap_asc = cap_aoff = 0;
     }
     // room for every chunk of the plan, and for at least ING_CHUNK bases and 65536 records
-    int ensure_packed(cudaStream_t st, const std::vector<Chunk> &chunks) {
+    int ensure_packed(cudaStream_t st, const std::vector<Chunk> &chunks, int n_mates) {
         uint64_t words = ING_CHUNK / 16, recs = 65536;
         for (const Chunk &c : chunks) {
-            words = std::max(words, (c.nb + 15) / 16);
-            recs = std::max(recs, c.r1 - c.r0 + 1);
+            words = std::max(words, (footprint(c, n_mates) + 15) / 16);
+            recs = std::max(recs, n_mates * c.n_off());
         }
         if (words <= cap_words && recs <= cap_recs) return SYL_OK;
         drain(st);
@@ -1038,11 +1156,11 @@ struct HostIngest {
         return SYL_OK;
     }
     // room for every chunk of the plan, and for at least min_bases bases and 65536 records
-    int ensure_ascii(cudaStream_t st, const std::vector<Chunk> &chunks, uint64_t min_bases) {
+    int ensure_ascii(cudaStream_t st, const std::vector<Chunk> &chunks, int n_mates, uint64_t min_bases) {
         uint64_t nb = min_bases, recs = 65536;
         for (const Chunk &c : chunks) {
-            nb = std::max(nb, c.nb);
-            recs = std::max(recs, c.r1 - c.r0 + 1);
+            nb = std::max(nb, footprint(c, n_mates));
+            recs = std::max(recs, n_mates * c.n_off());
         }
         if (nb <= cap_asc && recs <= cap_aoff) return SYL_OK;
         drain(st);
@@ -1059,21 +1177,25 @@ struct HostIngest {
     }
     // One chunk from caller memory through the ASCII ring and into the builder.  The copy of a slot waits until
     // the previous chunk in it is seeded; the read indices travel with the chunk, so chunks may go in any order.
-    int ship_ascii(syl_ctx *ctx, SampleBuilder &b, const uint8_t *bases, const uint64_t *rec_off, const Chunk &c) {
+    int ship_ascii(syl_ctx *ctx, SampleBuilder &b, const HostMate *m, int n_mates, const Chunk &c) {
         const int slot = a_slot;
         a_slot ^= 1;
-        const uint64_t nr = c.r1 - c.r0;
+        const uint64_t nr = c.r1 - c.r0, no = c.n_off();
         cudaStreamWaitEvent(copy_stream, ev_a_used[slot], 0);
-        if (cudaMemcpyAsync(d_asc[slot], bases + c.base, c.nb, cudaMemcpyHostToDevice, copy_stream) != cudaSuccess ||
-            cudaMemcpyAsync(d_aoff[slot], rec_off + c.r0, (nr + 1) * 8, cudaMemcpyHostToDevice, copy_stream) != cudaSuccess) {
-            set_error("H2D copy failed");
-            return SYL_ERR_CUDA;
+        Batch bt[2] = {};
+        for (int i = 0; i < n_mates; i++) {
+            bt[i] = {d_asc[slot] + (i ? mate2_at(c.nb[0]) : 0), nullptr, c.nb[i], d_aoff[slot] + i * no, c.base[i]};
+            if ((c.nb[i] && cudaMemcpyAsync((void *)bt[i].bases, m[i].bases + c.base[i], c.nb[i], cudaMemcpyHostToDevice, copy_stream) != cudaSuccess) ||
+                cudaMemcpyAsync((void *)bt[i].off, m[i].rec_off + c.r0, no * 8, cudaMemcpyHostToDevice, copy_stream) != cudaSuccess) {
+                set_error("H2D copy failed");
+                return SYL_ERR_CUDA;
+            }
+            ctx->ingest_h2d_bytes += c.nb[i] + no * 8;
         }
-        ctx->ingest_h2d_bytes += c.nb + (nr + 1) * 8;
         ctx->ingest_chunks_ascii++;
         cudaEventRecord(ev_a_copied[slot], copy_stream);
         cudaStreamWaitEvent(ctx->stream, ev_a_copied[slot], 0);
-        const int rc = b.add(d_asc[slot], nullptr, c.nb, d_aoff[slot], c.base, nr, c.r0);
+        const int rc = b.add_batch(bt, nr, c.r0);
         cudaEventRecord(ev_a_used[slot], ctx->stream);
         a_last = slot;
         return rc;
@@ -1099,40 +1221,42 @@ void ingest_destroy(syl_ctx *ctx) {
     ctx->ingest = nullptr;
 }
 
-// host ASCII -> chunks -> builder.  ascii_only: every chunk crosses the link as it is, front to back (1 byte of
+// host ASCII -> chunks -> builder, for a single-end sample (one mate) and for read pairs (two: a chunk is a range of
+// pairs, both mates in one slot).  ascii_only: every chunk crosses the link as it is, front to back (1 byte of
 // H2D traffic per base, no host packing; pageable caller memory is fine).  Else the pool packs the chunks.
-static int feed_host(syl_ctx *ctx, SampleBuilder &b, const uint8_t *bases, const uint64_t *rec_off, uint64_t n_reads,
-                     bool ascii_only) {
+static int feed_host(syl_ctx *ctx, SampleBuilder &b, const HostMate *m, int n_mates, uint64_t n_reads, bool ascii_only) {
     if (!ctx->ingest) ctx->ingest = new HostIngest();
     HostIngest &I = *static_cast<HostIngest *>(ctx->ingest);
     SYL_TRY(I.init());
     cudaStream_t st = ctx->stream, cs = I.copy_stream;
     std::vector<Chunk> chunks;
     if (ascii_only) {
-        plan_chunks(rec_off, n_reads, ingest_chunk(ING_ASCII_CHUNK), n_reads, chunks);
-        SYL_TRY(I.ensure_ascii(st, chunks, ING_ASCII_CHUNK));
+        plan_chunks(m, n_mates, n_reads, ingest_chunk(ING_ASCII_CHUNK), n_reads, chunks);
+        SYL_TRY(I.ensure_ascii(st, chunks, n_mates, ING_ASCII_CHUNK));
         int rc = SYL_OK;
-        for (size_t ci = 0; ci < chunks.size() && rc == SYL_OK; ci++) rc = I.ship_ascii(ctx, b, bases, rec_off, chunks[ci]);
+        for (size_t ci = 0; ci < chunks.size() && rc == SYL_OK; ci++) rc = I.ship_ascii(ctx, b, m, n_mates, chunks[ci]);
         if (rc != SYL_OK) I.drain(st);
         return rc;
     }
-    plan_chunks(rec_off, n_reads, ingest_chunk(ING_CHUNK), ING_MAXREC, chunks);
+    plan_chunks(m, n_mates, n_reads, ingest_chunk(ING_CHUNK), ING_MAXREC / n_mates, chunks);
     for (const Chunk &c : chunks)  // the packed offsets are chunk-relative u32
-        if (c.nb >= 0xFFFFFFF0ull) { set_error("a single record of 4 GB or more"); return SYL_ERR_ARG; }
+        if (c.nb[0] >= 0xFFFFFFF0ull || c.nb[1] >= 0xFFFFFFF0ull) { set_error("a single record of 4 GB or more"); return SYL_ERR_ARG; }
     // Two resources work in parallel: the packers (host memory bandwidth / CPU quota) and the PCIe link.  Packed
     // chunks are consumed from the front in order; whenever the front chunk is not packed yet and no ASCII copy
     // is in flight, a chunk nobody has started is taken from the BACK and shipped as ASCII (4x the bytes, but the
     // link would idle otherwise).  Needs pinned caller memory (a pageable copy would block this thread).
-    bool steal_ok = false;
-    {
+    bool steal_ok = true;
+    for (int i = 0; i < n_mates; i++) {
         cudaPointerAttributes pa;
-        if (cudaPointerGetAttributes(&pa, bases) == cudaSuccess) steal_ok = pa.type == cudaMemoryTypeHost;
-        else cudaGetLastError();
+        if (cudaPointerGetAttributes(&pa, m[i].bases) == cudaSuccess) steal_ok = steal_ok && pa.type == cudaMemoryTypeHost;
+        else { cudaGetLastError(); steal_ok = false; }
+    }
+    {
         const char *e = getenv("SYL_HOST_INGEST");
         if (e && std::string(e) == "packed-only") steal_ok = false;
     }
-    SYL_TRY(I.ensure_packed(st, chunks));
-    if (steal_ok) SYL_TRY(I.ensure_ascii(st, chunks, ING_CHUNK));
+    SYL_TRY(I.ensure_packed(st, chunks, n_mates));
+    if (steal_ok) SYL_TRY(I.ensure_ascii(st, chunks, n_mates, ING_CHUNK));
     if (!I.pool) I.pool.reset(new PackPool(default_pack_threads()));
     std::vector<PackItem> items;
     std::vector<uint32_t> chunk_items(chunks.size());
@@ -1140,11 +1264,14 @@ static int feed_host(syl_ctx *ctx, SampleBuilder &b, const uint8_t *bases, const
         const Chunk &c = chunks[ci];
         const int slot = (int)(ci % ING_SLOTS);
         uint32_t n_items = 0;
-        for (uint64_t o = 0; o < c.nb; o += ING_SLICE, n_items++)
-            items.push_back({bases + c.base + o, std::min(ING_SLICE, c.nb - o), I.h_words[slot] + o / 16, nullptr, 0, 0, nullptr, (uint32_t)ci});
-        const uint64_t no = c.r1 - c.r0 + 1;
-        for (uint64_t o = 0; o < no; o += ING_OSLICE, n_items++)
-            items.push_back({nullptr, 0, nullptr, rec_off + c.r0 + o, c.base, std::min(ING_OSLICE, no - o), I.h_off[slot] + o, (uint32_t)ci});
+        const uint64_t no = c.n_off();
+        for (int i = 0; i < n_mates; i++) {
+            uint32_t *words = I.h_words[slot] + (i ? mate2_at(c.nb[0]) / 16 : 0);
+            for (uint64_t o = 0; o < c.nb[i]; o += ING_SLICE, n_items++)
+                items.push_back({m[i].bases + c.base[i] + o, std::min(ING_SLICE, c.nb[i] - o), words + o / 16, nullptr, 0, 0, nullptr, (uint32_t)ci});
+            for (uint64_t o = 0; o < no; o += ING_OSLICE, n_items++)
+                items.push_back({nullptr, 0, nullptr, m[i].rec_off + c.r0 + o, c.base[i], std::min(ING_OSLICE, no - o), I.h_off[slot] + i * no + o, (uint32_t)ci});
+        }
         chunk_items[ci] = n_items;
     }
     I.pool->start(&items, &chunk_items, ING_SLOTS - 1);
@@ -1158,7 +1285,7 @@ static int feed_host(syl_ctx *ctx, SampleBuilder &b, const uint8_t *bases, const
             const size_t ci = (size_t)f;
             const Chunk &c = chunks[ci];
             const int slot = (int)(ci % ING_SLOTS);
-            const uint64_t nw = (c.nb + 15) / 16, no = c.r1 - c.r0 + 1;
+            const uint64_t nw = (footprint(c, n_mates) + 15) / 16, no = n_mates * c.n_off();  // both mates in one copy each
             cudaStreamWaitEvent(cs, I.ev_used[slot], 0);  // the seeding of the previous chunk in this slot is done
             if (cudaMemcpyAsync(I.d_words[slot], I.h_words[slot], nw * 4, cudaMemcpyHostToDevice, cs) != cudaSuccess ||
                 cudaMemcpyAsync(I.d_off32[slot], I.h_off[slot], no * 4, cudaMemcpyHostToDevice, cs) != cudaSuccess) {
@@ -1169,7 +1296,10 @@ static int feed_host(syl_ctx *ctx, SampleBuilder &b, const uint8_t *bases, const
             cudaStreamWaitEvent(st, I.ev_copied[slot], 0);
             k_off32_to_64<<<nblk(no, 256), 256, 0, st>>>(I.d_off32[slot], no, I.d_off64[slot]);
             ctx->launches++;
-            rc = b.add(nullptr, I.d_words[slot], c.nb, I.d_off64[slot], 0, c.r1 - c.r0, c.r0);
+            Batch bt[2] = {};
+            for (int i = 0; i < n_mates; i++)
+                bt[i] = {nullptr, I.d_words[slot] + (i ? mate2_at(c.nb[0]) / 16 : 0), c.nb[i], I.d_off64[slot] + i * c.n_off(), 0};
+            rc = b.add_batch(bt, c.r1 - c.r0, c.r0);
             cudaEventRecord(I.ev_used[slot], st);
             if (last_packed >= 0) {  // the pinned buffers of the previous packed chunk have crossed the link: refill them
                 cudaEventSynchronize(I.ev_copied[last_packed % ING_SLOTS]);
@@ -1183,7 +1313,7 @@ static int feed_host(syl_ctx *ctx, SampleBuilder &b, const uint8_t *bases, const
         }
         const bool ascii_busy = !force_steal && I.a_last >= 0 && cudaEventQuery(I.ev_a_copied[I.a_last]) == cudaErrorNotReady;
         if (steal_ok && !ascii_busy && (!force_steal || steal_turn) && bk > f && I.pool->try_skip_chunk((uint32_t)bk)) {  // ---- ASCII chunk from the back
-            rc = I.ship_ascii(ctx, b, bases, rec_off, chunks[(size_t)bk]);
+            rc = I.ship_ascii(ctx, b, m, n_mates, chunks[(size_t)bk]);
             bk--;
             steal_turn = false;
             continue;
@@ -1204,6 +1334,18 @@ static int feed_host(syl_ctx *ctx, SampleBuilder &b, const uint8_t *bases, const
     return rc;
 }
 
+// Host ASCII input: packed by the worker pool (fewer PCIe bytes) or shipped as it is.  Packing costs host memory
+// traffic (1.5 B per base: the packers read the ASCII, write the words, the copy engine reads them; ASCII costs 1 B
+// per base), so it pays while PCIe is the narrow resource — 1 to 4 processes per host — and loses once the ranks of
+// a host saturate its memory system instead (measured with 8 ranks on one host: 20.2 ms per 1 Gbp step shipping
+// ASCII, 32.7 ms packing; with 1 and 2 ranks packing wins, 10.2 vs 19.9 and 16.4 vs 19.9 ms).
+// SYL_HOST_INGEST = ascii | packed | packed-only overrides (read per call: the tests switch it at run time).
+static bool host_ingest_ascii() {
+    const char *hi_env = getenv("SYL_HOST_INGEST");
+    static const int local_ranks = []() { const char *e = getenv("LOCAL_WORLD_SIZE"); return e ? atoi(e) : 1; }();
+    return hi_env ? std::string(hi_env) == "ascii" : local_ranks > 4;
+}
+
 // packed: the input is 2-bit words (device or host memory); else ASCII
 static int sketch_reads_impl(syl_ctx *ctx, int mem, const uint8_t *bases, const uint32_t *packed, uint64_t n_bases,
                              const uint64_t *rec_off, uint64_t n_reads, int k, uint64_t c, int no_dedup, int sem, syl_sample **out) {
@@ -1213,15 +1355,7 @@ static int sketch_reads_impl(syl_ctx *ctx, int mem, const uint8_t *bases, const 
     *out = nullptr;
     SYL_CUDA(cudaSetDevice(ctx->device));
     syl::tl_ctx = ctx;
-    // Host ASCII input: packed by the worker pool (fewer PCIe bytes) or shipped as it is.  Packing costs host memory
-    // traffic (1.5 B per base: the packers read the ASCII, write the words, the copy engine reads them; ASCII costs 1 B
-    // per base), so it pays while PCIe is the narrow resource — 1 to 4 processes per host — and loses once the ranks of
-    // a host saturate its memory system instead (measured with 8 ranks on one host: 20.2 ms per 1 Gbp step shipping
-    // ASCII, 32.7 ms packing; with 1 and 2 ranks packing wins, 10.2 vs 19.9 and 16.4 vs 19.9 ms).
-    // SYL_HOST_INGEST = ascii | packed | packed-only overrides (read per call: the tests switch it at run time).
-    const char *hi_env = getenv("SYL_HOST_INGEST");
-    static const int local_ranks = []() { const char *e = getenv("LOCAL_WORLD_SIZE"); return e ? atoi(e) : 1; }();
-    const bool host_ascii = hi_env ? std::string(hi_env) == "ascii" : local_ranks > 4;
+    const bool host_ascii = host_ingest_ascii();
     static const bool dbg = getenv("SYL_DEBUG_TIMING") != nullptr;
     auto now = []() { return std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now().time_since_epoch()).count(); };
     uint64_t cap_override = 0;
@@ -1236,15 +1370,16 @@ static int sketch_reads_impl(syl_ctx *ctx, int mem, const uint8_t *bases, const 
         Staged<uint32_t> sp;   // host packed input staged whole
         Staged<uint64_t> so;
         if (mem == SYL_MEM_DEVICE) {
-            rc = b.add(bases, packed, n_bases, rec_off, 0, n_reads, 0);
+            rc = b.add({bases, packed, n_bases, rec_off, 0}, n_reads, 0);
         } else if (packed) {
             const uint64_t nw = (n_bases + 15) / 16;
             SYL_TRY(sp.init(ctx, mem, packed, nw));
             SYL_TRY(so.init(ctx, mem, rec_off, n_reads + 1));
             ctx->ingest_h2d_bytes += nw * 4 + (n_reads + 1) * 8;
-            rc = b.add(nullptr, sp.p, n_bases, so.p, 0, n_reads, 0);
+            rc = b.add({nullptr, sp.p, n_bases, so.p, 0}, n_reads, 0);
         } else if (n_reads && n_bases) {
-            rc = feed_host(ctx, b, bases, rec_off, n_reads, host_ascii);
+            const HostMate hm{bases, rec_off};
+            rc = feed_host(ctx, b, &hm, 1, n_reads, host_ascii);
         }
         if (rc != SYL_OK) return rc;
         const double t1 = now();
@@ -1267,7 +1402,8 @@ struct MateInput {
     uint64_t n_words() const { return (n_bases + 15) / 16; }
 };
 
-// packed: both mates are 2-bit words (m1.packed / m2.packed), else ASCII (m1.bases / m2.bases)
+// packed: both mates are 2-bit words (m1.packed / m2.packed), else ASCII (m1.bases / m2.bases).  Host ASCII goes
+// through feed_host as chunks of pairs; host 2-bit words (a quarter of the bytes) are staged whole.
 static int sketch_read_pairs_impl(syl_ctx *ctx, int mem, bool packed, MateInput &m1, MateInput &m2, uint64_t n_pairs, int k,
                                   uint64_t c, int no_dedup, int sem, syl_sample **out) {
     if (!ctx || !out || (!m1.bases && !m1.packed && m1.n_bases) || (!m2.bases && !m2.packed && m2.n_bases) || !m1.off || !m2.off) {
@@ -1280,45 +1416,36 @@ static int sketch_read_pairs_impl(syl_ctx *ctx, int mem, bool packed, MateInput 
     SYL_CUDA(cudaSetDevice(ctx->device));
     syl::tl_ctx = ctx;
     cudaStream_t st = ctx->stream;
-    Staged<uint8_t> sb[2];  // host memory: staged copies, alive until the call's sync
-    Staged<uint32_t> sp[2];
+    const bool fed = mem == SYL_MEM_HOST && !packed;
+    const HostMate hm[2] = {{m1.bases, m1.off}, {m2.bases, m2.off}};
+    Staged<uint32_t> sp[2];  // host 2-bit words: staged copies, alive until the call's sync
     Staged<uint64_t> so[2];
     MateInput *m[2] = {&m1, &m2};
-    for (int i = 0; i < 2; i++) {
+    for (int i = 0; i < 2 && !fed; i++) {
         if (packed) { SYL_TRY(sp[i].init(ctx, mem, m[i]->packed, m[i]->n_words())); m[i]->packed = sp[i].p; }
-        else { SYL_TRY(sb[i].init(ctx, mem, m[i]->bases, m[i]->n_bases)); m[i]->bases = sb[i].p; }
         SYL_TRY(so[i].init(ctx, mem, m[i]->off, n_pairs + 1));
         m[i]->off = so[i].p;
     }
+    const bool host_ascii = host_ingest_ascii();
     uint64_t cap_override = 0;
     for (int attempt = 0; attempt < 3; attempt++) {
         SampleBuilder b{ctx, k, c, no_dedup, sem};
         b.paired = true;
         b.expect_bases = m1.n_bases + m2.n_bases;
         b.expect_reads = 2 * n_pairs;
-        SYL_TRY(b.begin(cap_override));
-        unsigned long long *dc = b.d_count();
-        // mate 1, then mate 2: both use the PAIR index as read index; the pending list tells the mates apart
-        SYL_TRY(b.add(m1.bases, m1.packed, m1.n_bases, m1.off, 0, n_pairs, 0));
-        SYL_CUDA(cudaMemcpyAsync(dc + 17, dc + 1, 8, cudaMemcpyDeviceToDevice, st));  // pending entries of mate 1
-        SYL_TRY(b.add(m2.bases, m2.packed, m2.n_bases, m2.off, 0, n_pairs, 0));
-        SYL_CUDA(cudaMemsetAsync(dc + 18, 0, 8, st));
-        if (n_pairs) {
-            auto fix = packed ? k_events_fix_paired<true> : k_events_fix_paired<false>;
-            const uint64_t nw1 = packed ? m1.n_words() : 0, nw2 = packed ? m2.n_words() : 0;
-            fix<<<ctx->num_sms * 2, EV_THREADS, 0, st>>>(b.b_ev.p, b.b_pend.p, dc + 18, dc + 17, b.cap, m1.bases, m1.packed, nw1,
-                                                         m1.off, m2.bases, m2.packed, nw2, m2.off, 0, no_dedup);
-            fix<<<ctx->num_sms * 2, EV_THREADS, 0, st>>>(b.b_ev.p, b.b_pend.p, dc + 17, dc + 1, b.cap, m1.bases, m1.packed, nw1,
-                                                         m1.off, m2.bases, m2.packed, nw2, m2.off, 1, no_dedup);
-            ctx->launches += 2;
-            SYL_CUDA(cudaGetLastError());
+        if (mem == SYL_MEM_HOST) {
+            ctx->ingest_chunks_packed = ctx->ingest_chunks_ascii = 0;
+            ctx->ingest_h2d_bytes = fed ? 0 : (m1.n_words() + m2.n_words()) * 4 + 2 * (n_pairs + 1) * 8;
         }
+        SYL_TRY(b.begin(cap_override));
+        if (!fed) SYL_TRY(b.add_pair({m1.bases, m1.packed, m1.n_bases, m1.off, 0}, {m2.bases, m2.packed, m2.n_bases, m2.off, 0}, n_pairs, 0));
+        else if (n_pairs && b.expect_bases) SYL_TRY(feed_host(ctx, b, hm, 2, n_pairs, host_ascii));
         b.n_reads = n_pairs;       // mean_read_length = mean length of mate 1 (src/sketch.rs:824-826)
         b.n_bases = m1.n_bases;
         uint64_t need = 0;
         const int rc = b.finish(out, &need);
-        if (rc == SYL_ERR_CAPACITY) { cap_override = need + 16; continue; }
-        if (rc == SYL_OK) SYL_CUDA(cudaStreamSynchronize(st));  // the staged inputs go out of scope
+        if (rc == SYL_ERR_CAPACITY) { cap_override = need + 16; continue; }  // more events than estimated: redo (and re-feed) with the exact size
+        if (rc == SYL_OK && !fed) SYL_CUDA(cudaStreamSynchronize(st));  // the staged inputs go out of scope
         return rc;
     }
     set_error("event capacity retry failed");
@@ -1359,6 +1486,16 @@ int syl_sketch_read_pairs_packed2(syl_ctx *ctx, int mem, const uint32_t *packed1
 }
 
 int syl_pack_threads(void) { return default_pack_threads(); }
+
+int syl_ctx_ingest_ring_bytes(const syl_ctx *ctx, uint64_t *device_bytes, uint64_t *pinned_bytes) {
+    if (!ctx) { set_error("NULL argument"); return SYL_ERR_ARG; }
+    const HostIngest *I = static_cast<const HostIngest *>(ctx->ingest);
+    const uint64_t w = I && I->cap_words ? (I->cap_words + 16) * 4 : 0, r = I && I->cap_recs ? I->cap_recs + 16 : 0;
+    const uint64_t a = I && I->cap_asc ? I->cap_asc + 256 + (I->cap_aoff + 16) * 8 : 0;
+    if (device_bytes) *device_bytes = ING_SLOTS * (w + r * 12) + 2 * a;
+    if (pinned_bytes) *pinned_bytes = ING_SLOTS * (w + r * 4);
+    return SYL_OK;
+}
 
 int syl_ctx_ingest_stats(const syl_ctx *ctx, uint64_t *h2d_bytes, uint64_t *chunks_packed, uint64_t *chunks_ascii) {
     if (!ctx) { set_error("NULL argument"); return SYL_ERR_ARG; }
