@@ -75,13 +75,28 @@ __device__ __forceinline__ uint64_t packed64(const uint32_t *__restrict__ packed
     return ((uint64_t)__funnelshift_l(v1, v0, sh) << 32) | __funnelshift_l(v2, v1, sh);
 }
 
-// events pend[*p_begin .. *p_end) (indices into ev) belong to the batch (bases | packed, rec_off, off_bias)
-template <bool PACKED>
+// One mate's (or a single-end sample's) records: ASCII bytes or 2-bit words (nb bases either way), and the offsets of the
+// records (off[i] - off_bias is the start of record i among the bases).  In host memory off_bias is 0; on the device it
+// describes one seeding batch, whose off starts at the batch's first record.
+struct Mate {
+    const uint8_t *bases;
+    const uint32_t *packed;
+    uint64_t nb;
+    const uint64_t *off;
+    uint64_t off_bias;
+};
+
+// Events pend[*p_begin .. *p_end) (indices into ev) are the pending events of one batch of records [rec_base, ..), and
+// arrive with recflag = record << 1 | EV_PENDING.  The keys are built from 32 bases at the record's start and 32 more:
+//   single-end: from the middle of the read (pair_kmer_single); recflag = read << 1 | NO_PAIR as the seeding kernel set it.
+//   read pairs (src/sketch.rs:658-688 pair_kmer): from the start of mate 2, so every event of the pair carries the same
+//       keys; recflag = pair << 2 | mate << 1 | NO_PAIR (a mate shorter than 33 bp, or --no-dedup).  The batch's mate-2
+//       events start at pend[*p_mate2].
+template <bool PACKED, bool PAIRED>
 __global__ void __launch_bounds__(EV_THREADS)
 k_events_fix(EventRec *__restrict__ ev, const uint32_t *__restrict__ pend, const unsigned long long *__restrict__ p_begin,
-             const unsigned long long *__restrict__ p_end, uint64_t ev_cap, const uint8_t *__restrict__ bases,
-             const uint32_t *__restrict__ packed, uint64_t n_words, const uint64_t *__restrict__ rec_off, uint64_t off_bias,
-             uint64_t rec_base) {
+             const unsigned long long *__restrict__ p_mate2, const unsigned long long *__restrict__ p_end, uint64_t ev_cap,
+             const Mate m1, const Mate m2, uint64_t rec_base, int no_dedup) {
     __shared__ uint8_t lut[4][256];
     if (!PACKED) {
         for (int i = threadIdx.x; i < 256; i += EV_THREADS) {
@@ -93,84 +108,41 @@ k_events_fix(EventRec *__restrict__ ev, const uint32_t *__restrict__ pend, const
         }
         __syncthreads();
     }
-    const uint64_t i0 = *p_begin, i1 = *p_end;
+    const Mate &ms = PAIRED ? m2 : m1;  // where the second 32 bases come from
+    const uint64_t i0 = *p_begin, i1 = *p_end, i2 = PAIRED ? *p_mate2 : i1;
     for (uint64_t i = i0 + (uint64_t)blockIdx.x * EV_THREADS + threadIdx.x; i < i1; i += (uint64_t)gridDim.x * EV_THREADS) {
         const uint32_t ei = pend[i];
         if (ei >= ev_cap) continue;
         EventRec *e = ev + ei;
-        const uint64_t rf = e->recflag & ~EV_PENDING;
-        const uint64_t rec = (rf >> 1) - rec_base;
-        const uint64_t a = rec_off[rec] - off_bias;
-        const uint64_t L = rec_off[rec + 1] - off_bias - a;
-        uint32_t f, g, r, t;
-        if (!PACKED) {
-            uint32_t x[8];
-            load32_unaligned(bases + a, x);
-            f = pack16(x, 0x6420, lut); g = pack16(x, 0x7531, lut);
-            load32_unaligned(bases + a + L / 2, x);
-            r = pack16(x, 0x6420, lut); t = pack16(x, 0x7531, lut);
-        } else {
-            const uint64_t x = packed64(packed, n_words, a), y = packed64(packed, n_words, a + L / 2);
-            f = even_fields(x); g = even_fields(x << 2);
-            r = even_fields(y); t = even_fields(y << 2);
+        const uint64_t rf = e->recflag & ~EV_PENDING, rec = (rf >> 1) - rec_base;
+        // __ldg: Mate's pointers are not __restrict__, and the plain loads made the pair kernel 2.5 % slower (H100, 700 W)
+        auto start = [rec](const Mate &m, uint64_t r) { return __ldg(m.off + rec + r) - m.off_bias; };
+        const uint64_t a = start(m1, 0), L = start(m1, 1) - a;
+        uint64_t b = a + L / 2;
+        bool has = true;
+        if (PAIRED) {
+            b = start(ms, 0);
+            const uint64_t L2 = start(ms, 1) - b;
+            has = !no_dedup && L >= 33 && L2 >= 33;  // 2 * 16 + 1 (:660)
         }
-        e->recflag = rf;
-        e->p0 = ((uint64_t)f << 32) | r;  // doublepairs.0 = [kmer_f, kmer_r]
-        e->p1 = ((uint64_t)g << 32) | t;  // doublepairs.1 = [kmer_g, kmer_t]
-    }
-}
-
-// Read pairs (src/sketch.rs:658-688 pair_kmer): the two keys come from the first 32 bases of BOTH mates; every event of
-// the pair carries them.  Events arrive with recflag = pair << 1 | EV_PENDING; the result is
-// recflag = pair << 2 | mate << 1 | NO_PAIR (a mate shorter than 33 bp, or --no-dedup).
-// ASCII input: bases1 / bases2; 2-bit input: packed1 / packed2 of n_words1 / n_words2 words.
-// The batch holds pairs [rec_base, ..): off1 / off2 start at pair rec_base, and off - bias is a start inside the batch.
-template <bool PACKED>
-__global__ void __launch_bounds__(EV_THREADS)
-k_events_fix_paired(EventRec *__restrict__ ev, const uint32_t *__restrict__ pend, const unsigned long long *__restrict__ p_begin,
-                    const unsigned long long *__restrict__ p_end, uint64_t ev_cap, const uint8_t *__restrict__ bases1,
-                    const uint32_t *__restrict__ packed1, uint64_t n_words1, const uint64_t *__restrict__ off1,
-                    const uint8_t *__restrict__ bases2, const uint32_t *__restrict__ packed2, uint64_t n_words2,
-                    const uint64_t *__restrict__ off2, uint64_t bias1, uint64_t bias2, uint64_t rec_base, uint64_t mate,
-                    int no_dedup) {
-    __shared__ uint8_t lut[4][256];
-    if (!PACKED) {
-        for (int i = threadIdx.x; i < 256; i += EV_THREADS) {
-            const uint32_t code = byte_to_seq((uint32_t)i);
-            lut[0][i] = (uint8_t)(code << 6);
-            lut[1][i] = (uint8_t)(code << 4);
-            lut[2][i] = (uint8_t)(code << 2);
-            lut[3][i] = (uint8_t)code;
-        }
-        __syncthreads();
-    }
-    const uint64_t i0 = *p_begin, i1 = *p_end;
-    for (uint64_t i = i0 + (uint64_t)blockIdx.x * EV_THREADS + threadIdx.x; i < i1; i += (uint64_t)gridDim.x * EV_THREADS) {
-        const uint32_t ei = pend[i];
-        if (ei >= ev_cap) continue;
-        EventRec *e = ev + ei;
-        const uint64_t pair = (e->recflag & ~EV_PENDING) >> 1;
-        const uint64_t a1 = off1[pair - rec_base] - bias1, a2 = off2[pair - rec_base] - bias2;
-        const uint64_t L1 = off1[pair - rec_base + 1] - bias1 - a1, L2 = off2[pair - rec_base + 1] - bias2 - a2;
-        const bool has = !no_dedup && L1 >= 33 && L2 >= 33;  // 2 * 16 + 1 (:660)
         uint64_t p0 = 0, p1 = 0;
         if (has) {
             uint32_t f, g, r, t;
             if (!PACKED) {
                 uint32_t x[8];
-                load32_unaligned(bases1 + a1, x);
+                load32_unaligned(m1.bases + a, x);
                 f = pack16(x, 0x6420, lut); g = pack16(x, 0x7531, lut);
-                load32_unaligned(bases2 + a2, x);
+                load32_unaligned(ms.bases + b, x);
                 r = pack16(x, 0x6420, lut); t = pack16(x, 0x7531, lut);
             } else {
-                const uint64_t x = packed64(packed1, n_words1, a1), y = packed64(packed2, n_words2, a2);
+                const uint64_t x = packed64(m1.packed, (m1.nb + 15) / 16, a), y = packed64(ms.packed, (ms.nb + 15) / 16, b);
                 f = even_fields(x); g = even_fields(x << 2);
                 r = even_fields(y); t = even_fields(y << 2);
             }
-            p0 = ((uint64_t)f << 32) | r;  // ([kmer_f, kmer_r], [kmer_g, kmer_t]) (:685)
-            p1 = ((uint64_t)g << 32) | t;
+            p0 = ((uint64_t)f << 32) | r;  // doublepairs.0 = [kmer_f, kmer_r]
+            p1 = ((uint64_t)g << 32) | t;  // doublepairs.1 = [kmer_g, kmer_t]
         }
-        e->recflag = (pair << 2) | (mate << 1) | (has ? 0ull : NO_PAIR);
+        e->recflag = PAIRED ? ((rf >> 1) << 2) | ((uint64_t)(i >= i2) << 1) | (has ? 0ull : NO_PAIR) : rf;
         e->p0 = p0;
         e->p1 = p1;
     }
@@ -280,11 +252,6 @@ __global__ void k_dedup(const uint64_t *__restrict__ seg_off, const uint32_t *__
     }
     count[s] = c;
     if (dups) atomicAdd(n_dup, (unsigned long long)dups);
-}
-
-__global__ void k_copy_len(const uint32_t *__restrict__ len, uint32_t *__restrict__ count, uint64_t n) {
-    uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (i < n) count[i] = len[i];
 }
 
 
@@ -686,16 +653,6 @@ static inline int bits_for(uint64_t maxval) {
     return b;
 }
 
-// One mate's (or a single-end sample's) share of a seeding batch, device resident: ASCII bytes or 2-bit words, and
-// the offsets of the batch's records (off[i] - off_bias is the start of record i inside the batch).
-struct Batch {
-    const uint8_t *bases;
-    const uint32_t *packed;
-    uint64_t nb;
-    const uint64_t *off;
-    uint64_t off_bias;
-};
-
 // Accumulates events over one or more seeding batches, then finishes into a syl_sample.
 // Nothing in begin() / add() synchronises with the host: the event array is sized up front from the
 // expected number of survivors, the seeding kernel appends at a running device counter, and every
@@ -707,9 +664,10 @@ struct SampleBuilder {
     int k;
     uint64_t c;
     int no_dedup, sem;
-    uint64_t n_reads = 0, n_bases = 0, cap = 0;
-    bool paired = false;     // read pairs (syl_sketch_read_pairs): every event waits for k_events_fix_paired
-    bool sorted = false;     // SYL_SAMPLE_POSTPASS=sort (read in begin(), per call): no groups, the generic post-pass
+    bool paired;             // read pairs (syl_sketch_read_pairs): every event waits for k_events_fix<.., true>
+    uint64_t n_reads;        // records: reads, or pairs
+    double mean_read_length;
+    uint64_t cap = 0;
     // Event array: ng group slots of `slot` events each, then the overflow list of cap events (everything
     // in the overflow list without groups).  A scratch block of the ctx cache.
     DevBuf<EventRec> b_ev;
@@ -720,8 +678,8 @@ struct SampleBuilder {
     uint32_t nbk = 0, ng = 0, slot = 0;
     uint64_t Mb = 0;
     DevBuf<uint32_t> g_cnt;  // events per group
-    // ctx->d_counters slots: [0] events in the overflow list, [1] pending events, [2] duplicates removed, [3] pending snapshot,
-    // [17], [18] add_pair's snapshots
+    // ctx->d_counters slots: [0] events in the overflow list, [1] pending events, [2] duplicates removed; add() keeps
+    // [3] and [17] as snapshots of [1]
     unsigned long long *d_count() const { return reinterpret_cast<unsigned long long *>(ctx->d_counters); }
     uint64_t ev_total() const { return (uint64_t)ng * slot + cap; }
 
@@ -729,9 +687,8 @@ struct SampleBuilder {
         cudaStream_t st = ctx->stream;
         const uint64_t win = expect_bases > expect_reads * (uint64_t)(k - 1) ? expect_bases - expect_reads * (uint64_t)(k - 1) : 0;
         const uint64_t n_exp = win / c;
-        const char *pp = getenv("SYL_SAMPLE_POSTPASS");
-        sorted = pp && std::string(pp) == "sort";
-        if (!sorted) {
+        const char *pp = getenv("SYL_SAMPLE_POSTPASS");  // per call; "sort": no groups, every event takes the generic path
+        if (!(pp && std::string(pp) == "sort")) {
             static const uint32_t grp_cap = []() { const char *e = getenv("SYL_GROUP_CAP"); int v = e ? atoi(e) : GRP_CAP; return (uint32_t)std::min(std::max(v, 32), GRP_CAP); }();
             slot = grp_cap;
             const uint64_t g = n_exp / GRP_T + 1;
@@ -757,57 +714,32 @@ struct SampleBuilder {
         return SYL_OK;
     }
 
-    // one batch of reads, device resident (ASCII bytes or 2-bit words); read indices continue from the
-    // previous batch.  The seeding kernel appends the batch's events (hash, read, pair keys) to the event array.
-    // rec_base: index of the batch's first read in the sample (batches may arrive in any order)
-    int add(const Batch &m, uint64_t nr, uint64_t rec_base) {
-        const uint8_t *d_bases = m.bases;
-        const uint32_t *d_packed = m.packed;
-        const uint64_t nb = m.nb, *d_off = m.off, off_bias = m.off_bias;
+    // One batch of records [rec_base, rec_base + nr) (batches may arrive in any order), device resident: m[0] for
+    // reads, m[0] and m[1] for read pairs.  Each mate is seeded with the record index as read index; the seeding kernel
+    // appends the events (hash, record, pair keys) to the event array.  The pending events are then completed while
+    // the batch is resident: reads cut by a tile edge, whose keys come from global memory, and every event of a pair,
+    // whose keys need both mates.  d_counters[1] counts the pending events; [3] and [17] keep its value from before
+    // mate 1 and mate 2, so the batch's pending events are pend[[3] .. [1]) and mate 2's start at [17].
+    int add(const Mate *m, int n_mates, uint64_t nr, uint64_t rec_base) {
         cudaStream_t st = ctx->stream;
         if (nr == 0) return SYL_OK;
         unsigned long long *dc = d_count();
-        SYL_CUDA(cudaMemcpyAsync(dc + 3, dc + 1, 8, cudaMemcpyDeviceToDevice, st));  // pending entries before this batch
-        SeedJob job;
-        job.d_bases = d_bases; job.d_packed = d_packed; job.n_bases = nb; job.d_rec_off = d_off; job.off_bias = off_bias;
-        job.n_rec = nr; job.k = k; job.c = c; job.sem = sem; job.with_pos = 0; job.d_out = b_ev.p; job.cap = cap;
-        job.emit_events = 1; job.rec_base = rec_base; job.no_dedup = paired ? 2 : no_dedup; job.d_pend = b_pend.p;
-        job.d_group_cnt = g_cnt.p; job.Mb = Mb; job.nbk = nbk; job.ng = ng; job.slot = slot; job.d_count = dc;
-        SYL_TRY(seed_enqueue(ctx, job));
-        if (!no_dedup && !paired && nb) {  // reads cut by a tile edge: their pair keys come from global memory
-            const uint64_t n_words = (nb + 15) / 16;
-            if (d_packed) k_events_fix<true><<<ctx->num_sms * 2, EV_THREADS, 0, st>>>(b_ev.p, b_pend.p, dc + 3, dc + 1, ev_total(), nullptr, d_packed, n_words, d_off, off_bias, rec_base);
-            else k_events_fix<false><<<ctx->num_sms * 2, EV_THREADS, 0, st>>>(b_ev.p, b_pend.p, dc + 3, dc + 1, ev_total(), d_bases, nullptr, 0, d_off, off_bias, rec_base);
-            ctx->launches++;
-            SYL_CUDA(cudaGetLastError());
+        for (int i = 0; i < n_mates; i++) {
+            SYL_CUDA(cudaMemcpyAsync(dc + (i ? 17 : 3), dc + 1, 8, cudaMemcpyDeviceToDevice, st));
+            SeedJob job;
+            job.d_bases = m[i].bases; job.d_packed = m[i].packed; job.n_bases = m[i].nb; job.d_rec_off = m[i].off;
+            job.off_bias = m[i].off_bias; job.n_rec = nr; job.k = k; job.c = c; job.sem = sem; job.with_pos = 0;
+            job.d_out = b_ev.p; job.cap = cap; job.emit_events = 1; job.rec_base = rec_base;
+            job.no_dedup = paired ? 2 : no_dedup; job.d_pend = b_pend.p;
+            job.d_group_cnt = g_cnt.p; job.Mb = Mb; job.nbk = nbk; job.ng = ng; job.slot = slot; job.d_count = dc;
+            SYL_TRY(seed_enqueue(ctx, job));
         }
-        n_reads += nr;
-        n_bases += nb;
-        return SYL_OK;
-    }
-
-    int add_batch(const Batch *m, uint64_t nr, uint64_t rec_base) {  // m[0], and m[1] for pairs
-        return paired ? add_pair(m[0], m[1], nr, rec_base) : add(m[0], nr, rec_base);
-    }
-
-    // one batch of read pairs [rec_base, rec_base + nr): mate 1, then mate 2, both with the PAIR index as read index;
-    // the pending list tells the mates apart.  The keys need the first 32 bases of both mates, so the batch's events
-    // are completed here, while both are resident.
-    int add_pair(const Batch &m1, const Batch &m2, uint64_t nr, uint64_t rec_base) {
-        cudaStream_t st = ctx->stream;
-        if (nr == 0) return SYL_OK;
-        unsigned long long *dc = d_count();
-        SYL_CUDA(cudaMemcpyAsync(dc + 18, dc + 1, 8, cudaMemcpyDeviceToDevice, st));  // pending entries before the batch
-        SYL_TRY(add(m1, nr, rec_base));
-        SYL_CUDA(cudaMemcpyAsync(dc + 17, dc + 1, 8, cudaMemcpyDeviceToDevice, st));  // ... after mate 1
-        SYL_TRY(add(m2, nr, rec_base));
-        auto fix = m1.packed ? k_events_fix_paired<true> : k_events_fix_paired<false>;
-        const uint64_t nw1 = m1.packed ? (m1.nb + 15) / 16 : 0, nw2 = m2.packed ? (m2.nb + 15) / 16 : 0;
-        for (uint64_t mate = 0; mate < 2; mate++)
-            fix<<<ctx->num_sms * 2, EV_THREADS, 0, st>>>(b_ev.p, b_pend.p, mate ? dc + 17 : dc + 18, mate ? dc + 1 : dc + 17, ev_total(),
-                                                         m1.bases, m1.packed, nw1, m1.off, m2.bases, m2.packed, nw2, m2.off,
-                                                         m1.off_bias, m2.off_bias, rec_base, mate, no_dedup);
-        ctx->launches += 2;
+        if (!paired && (no_dedup || !m[0].nb)) return SYL_OK;  // no pending events
+        auto fix = paired ? (m[0].packed ? k_events_fix<true, true> : k_events_fix<false, true>)
+                          : (m[0].packed ? k_events_fix<true, false> : k_events_fix<false, false>);
+        fix<<<ctx->num_sms * 2, EV_THREADS, 0, st>>>(b_ev.p, b_pend.p, dc + 3, dc + 17, dc + 1, ev_total(), m[0],
+                                                     m[n_mates - 1], rec_base, no_dedup);
+        ctx->launches++;
         SYL_CUDA(cudaGetLastError());
         return SYL_OK;
     }
@@ -868,8 +800,7 @@ struct SampleBuilder {
         ctx->launches += 1;
         SYL_TRY(count.alloc(std::max<uint64_t>(U, 1), st));
         if (no_dedup && !paired) {
-            k_copy_len<<<nblk(U, 256), 256, 0, st>>>(seg_len.p, count.p, U);
-            ctx->launches++;
+            SYL_CUDA(cudaMemcpyAsync(count.p, seg_len.p, U * 4, cudaMemcpyDeviceToDevice, st));
         } else {
             tb = std::max(rle_bytes, scan_bytes);
             SYL_CUDA(cub::DeviceScan::ExclusiveSum(tmp2.p, tb, seg_len.p, seg_off.p, U, st));
@@ -900,86 +831,68 @@ struct SampleBuilder {
         s->stream = ctx->stream;
         s->k = k;
         s->c = c;
-        s->mean_read_length = n_reads ? (double)n_bases / (double)n_reads : 0.;
+        s->mean_read_length = mean_read_length;
         auto fail = [&](int rc) { syl_sample_free(s); return rc; };
 #define SB_CUDA(x) do { cudaError_t _e = (x); if (_e != cudaSuccess) { set_error(std::string(#x) + ": " + cudaGetErrorString(_e)); return fail(_e == cudaErrorMemoryAllocation ? SYL_ERR_OOM : SYL_ERR_CUDA); } } while (0)
-        if (n_reads == 0 || expect_bases == 0) { *out = s; return SYL_OK; }  // pairs: n_bases is mate 1's, which may be empty
+        if (n_reads == 0 || expect_bases == 0) { *out = s; return SYL_OK; }
         unsigned long long *dc = d_count();
         EventRec *ev = b_ev.p;
         int rc;
-        if (sorted) {
-            SB_CUDA(cudaMemcpyAsync(ctx->h_counters, dc, 8, cudaMemcpyDeviceToHost, st));
-            SB_CUDA(cudaStreamSynchronize(st));
-            const uint64_t N = ctx->h_counters[0];
-            if (N > cap) { *need_cap = N; syl_sample_free(s); return SYL_ERR_CAPACITY; }
-            if (N == 0) { *out = s; return SYL_OK; }
-            DevBuf<uint64_t> uq;
-            DevBuf<uint32_t> ct;
-            uint64_t U = 0, nd = 0;
-            DevBuf<uint64_t> e_h, e_rf, e_p0, e_p1;
-            if ((rc = e_h.alloc(N, st)) || (rc = e_rf.alloc(N, st)) || (rc = e_p0.alloc(N, st)) || (rc = e_p1.alloc(N, st))) return fail(rc);
-            k_unpack_events<<<nblk(N, 256), 256, 0, st>>>(ev, N, e_h.p, e_rf.p, e_p0.p, e_p1.p);
-            ctx->launches++;
-            if ((rc = dedup_sorted(e_h.p, e_rf.p, e_p0.p, e_p1.p, N, uq, ct, &U, &nd)) != SYL_OK) return fail(rc);
-            if ((rc = hblock_alloc(ctx, (void **)&s->hash, std::max<uint64_t>(U, 1) * 8))) return fail(rc);
-            if ((rc = hblock_alloc(ctx, (void **)&s->count, std::max<uint64_t>(U, 1) * 4))) return fail(rc);
-            SB_CUDA(cudaMemcpyAsync(s->hash, uq.p, U * 8, cudaMemcpyDeviceToDevice, st));
-            SB_CUDA(cudaMemcpyAsync(s->count, ct.p, U * 4, cudaMemcpyDeviceToDevice, st));
-            SB_CUDA(cudaStreamSynchronize(st));
-            s->n = U;
-            s->num_dup_removed = nd;
-            *out = s;
-            return SYL_OK;
-        }
         // ---- primary path: CTA-local grouping / dedup of the group slots (ng, slot, Mb, g_cnt: begin()).
         // The kernels read the group counts from device memory.
         const uint64_t n_slots = (uint64_t)ng * slot;
         DevBuf<uint32_t> st_cnt, g_nuniq, g_n, uoff, fsz, foff, g_src, tmp_c;
         DevBuf<uint64_t> st_hash, tmp_h;
         DevBuf<uint8_t> g_fb;
-        if ((rc = st_hash.alloc(n_slots, st)) || (rc = st_cnt.alloc(n_slots, st)) ||
-            (rc = tmp_h.alloc(n_slots, st)) || (rc = tmp_c.alloc(n_slots, st)) ||  // in-kernel uniques: <= the slotted events
-            (rc = g_nuniq.alloc(ng, st)) || (rc = g_n.alloc(ng, st)) ||
-            (rc = g_fb.alloc(ng, st)) || (rc = uoff.alloc((uint64_t)ng + 1, st)) || (rc = fsz.alloc(ng, st)) ||
-            (rc = foff.alloc((uint64_t)ng + 1, st)) || (rc = g_src.alloc(ng, st)))
-            return fail(rc);
-        unsigned long long *d_ndup = dc + 2;
-        auto group_dedup = paired ? k_group_dedup<true> : k_group_dedup<false>;
-        SB_CUDA(cudaFuncSetAttribute(group_dedup, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(GroupSmem)));
-        {
-            KernelTimer kt(ctx, SYL_KERNEL_GROUP_DEDUP);
-            group_dedup<<<ng, GRP_THREADS, sizeof(GroupSmem), st>>>(ev, g_cnt.p, slot, Mb, nbk, no_dedup,
-                                                                     st_hash.p, st_cnt.p, g_nuniq.p, g_n.p, g_fb.p, d_ndup);
+        if (ng) {
+            if ((rc = st_hash.alloc(n_slots, st)) || (rc = st_cnt.alloc(n_slots, st)) ||
+                (rc = tmp_h.alloc(n_slots, st)) || (rc = tmp_c.alloc(n_slots, st)) ||  // in-kernel uniques: <= the slotted events
+                (rc = g_nuniq.alloc(ng, st)) || (rc = g_n.alloc(ng, st)) ||
+                (rc = g_fb.alloc(ng, st)) || (rc = uoff.alloc((uint64_t)ng + 1, st)) || (rc = fsz.alloc(ng, st)) ||
+                (rc = foff.alloc((uint64_t)ng + 1, st)) || (rc = g_src.alloc(ng, st)))
+                return fail(rc);
+            auto group_dedup = paired ? k_group_dedup<true> : k_group_dedup<false>;
+            SB_CUDA(cudaFuncSetAttribute(group_dedup, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(GroupSmem)));
+            {
+                KernelTimer kt(ctx, SYL_KERNEL_GROUP_DEDUP);
+                group_dedup<<<ng, GRP_THREADS, sizeof(GroupSmem), st>>>(ev, g_cnt.p, slot, Mb, nbk, no_dedup,
+                                                                         st_hash.p, st_cnt.p, g_nuniq.p, g_n.p, g_fb.p, dc + 2);
+            }
+            k_scan_u32<<<1, 1024, 0, st>>>(g_nuniq.p, ng, uoff.p);
+            k_fallback_sizes<<<nblk(ng, 256), 256, 0, st>>>(g_n.p, g_fb.p, ng, fsz.p);
+            k_scan_u32<<<1, 1024, 0, st>>>(fsz.p, ng, foff.p);
+            k_compact_uniq<<<ng, 128, 0, st>>>(st_hash.p, st_cnt.p, slot, g_nuniq.p, uoff.p, g_fb.p, g_src.p, nullptr, nullptr,
+                                                tmp_h.p, tmp_c.p);
+            ctx->launches += 5;
+            SB_CUDA(cudaGetLastError());
+            SB_CUDA(cudaMemcpyAsync(ctx->h_counters + 4, uoff.p + ng, 4, cudaMemcpyDeviceToHost, st));
+            SB_CUDA(cudaMemcpyAsync(ctx->h_counters + 5, foff.p + ng, 4, cudaMemcpyDeviceToHost, st));
         }
-        k_scan_u32<<<1, 1024, 0, st>>>(g_nuniq.p, ng, uoff.p);
-        k_fallback_sizes<<<nblk(ng, 256), 256, 0, st>>>(g_n.p, g_fb.p, ng, fsz.p);
-        k_scan_u32<<<1, 1024, 0, st>>>(fsz.p, ng, foff.p);
-        k_compact_uniq<<<ng, 128, 0, st>>>(st_hash.p, st_cnt.p, slot, g_nuniq.p, uoff.p, g_fb.p, g_src.p, nullptr, nullptr,
-                                            tmp_h.p, tmp_c.p);
-        ctx->launches += 5;
-        SB_CUDA(cudaGetLastError());
         SB_CUDA(cudaMemcpyAsync(ctx->h_counters, dc, 24, cudaMemcpyDeviceToHost, st));  // events, pending, duplicates
-        SB_CUDA(cudaMemcpyAsync(ctx->h_counters + 4, uoff.p + ng, 4, cudaMemcpyDeviceToHost, st));
-        SB_CUDA(cudaMemcpyAsync(ctx->h_counters + 5, foff.p + ng, 4, cudaMemcpyDeviceToHost, st));
         SB_CUDA(cudaStreamSynchronize(st));  // the one synchronisation of a sketch
         const uint64_t N_ovf = ctx->h_counters[0];
         if (N_ovf > cap) { *need_cap = N_ovf; syl_sample_free(s); return SYL_ERR_CAPACITY; }
-        // the overflow list holds only events of groups past their slot, all of which are fallback groups
-        const uint64_t U1 = (uint32_t)ctx->h_counters[4], NF_slots = (uint32_t)ctx->h_counters[5], NF = NF_slots + N_ovf;
+        // the overflow list holds only events of groups past their slot, all of which are fallback groups (without
+        // groups: every event)
+        const uint64_t U1 = ng ? (uint32_t)ctx->h_counters[4] : 0, NF_slots = ng ? (uint32_t)ctx->h_counters[5] : 0;
+        const uint64_t NF = NF_slots + N_ovf;
         uint64_t ndup = ctx->h_counters[2];
         static const bool dbg = getenv("SYL_DEBUG_TIMING") != nullptr;
         if (dbg) fprintf(stderr, "[sample post-pass] groups %u of %u slots, overflow list %llu (cap %llu): in-kernel uniques %llu, events handed to the generic path %llu (%.2f %% of the slotted events)\n",
                          ng, slot, (unsigned long long)N_ovf, (unsigned long long)cap, (unsigned long long)U1, (unsigned long long)NF,
                          n_slots ? 100.0 * (double)NF_slots / (double)n_slots : 0.);
-        uint64_t U = U1;
-        if (NF) {  // fallback groups through the generic path (heavy-hitter k-mers, duplicate-heavy replays)
-            DevBuf<uint64_t> fh, f_rf, f_p0, f_p1, f_uq;
-            DevBuf<uint32_t> f_ct;
-            uint64_t U2 = 0, nd2 = 0;
+        // the generic path: fallback groups (heavy-hitter k-mers, duplicate-heavy replays) and the overflow list
+        DevBuf<uint64_t> fh, f_rf, f_p0, f_p1, f_uq;
+        DevBuf<uint32_t> f_ct;
+        uint64_t U2 = 0;
+        if (NF) {
+            uint64_t nd2 = 0;
             if ((rc = fh.alloc(NF, st)) || (rc = f_rf.alloc(NF, st)) || (rc = f_p0.alloc(NF, st)) || (rc = f_p1.alloc(NF, st)))
                 return fail(rc);
-            k_gather_fallback<<<ng, 256, 0, st>>>(ev, slot, g_n.p, g_fb.p, foff.p, fh.p, f_rf.p, f_p0.p, f_p1.p);
-            ctx->launches++;
+            if (ng) {
+                k_gather_fallback<<<ng, 256, 0, st>>>(ev, slot, g_n.p, g_fb.p, foff.p, fh.p, f_rf.p, f_p0.p, f_p1.p);
+                ctx->launches++;
+            }
             if (N_ovf) {
                 k_unpack_events<<<nblk(N_ovf, 256), 256, 0, st>>>(ev + n_slots, N_ovf, fh.p + NF_slots, f_rf.p + NF_slots,
                                                                   f_p0.p + NF_slots, f_p1.p + NF_slots);
@@ -987,30 +900,23 @@ struct SampleBuilder {
             }
             if ((rc = dedup_sorted(fh.p, f_rf.p, f_p0.p, f_p1.p, NF, f_uq, f_ct, &U2, &nd2)) != SYL_OK) return fail(rc);
             ndup += nd2;
-            U = U1 + U2;
-            if ((rc = hblock_alloc(ctx, (void **)&s->hash, std::max<uint64_t>(U, 1) * 8))) return fail(rc);
-            if ((rc = hblock_alloc(ctx, (void **)&s->count, std::max<uint64_t>(U, 1) * 4))) return fail(rc);
-            if (U2) {  // slot the generic path's pairs into their groups' positions, compact straight into the result
-                k_fallback_place<<<nblk(ng, 128), 128, 0, st>>>(g_fb.p, ng, nbk, Mb, f_uq.p, U2, g_nuniq.p, g_src.p);
-                k_scan_u32<<<1, 1024, 0, st>>>(g_nuniq.p, ng, uoff.p);
-                k_compact_uniq<<<ng, 128, 0, st>>>(st_hash.p, st_cnt.p, slot, g_nuniq.p, uoff.p, g_fb.p, g_src.p, f_uq.p, f_ct.p,
-                                                    s->hash, s->count);
-                ctx->launches += 3;
-                SB_CUDA(cudaGetLastError());
-            } else if (U) {
-                SB_CUDA(cudaMemcpyAsync(s->hash, tmp_h.p, U * 8, cudaMemcpyDeviceToDevice, st));
-                SB_CUDA(cudaMemcpyAsync(s->count, tmp_c.p, U * 4, cudaMemcpyDeviceToDevice, st));
-            }
-            SB_CUDA(cudaStreamSynchronize(st));  // f_uq / f_ct go out of scope
-        } else {
-            // exact-size result arrays; the copies are ordered on the ctx stream like every later use of the handle
-            if ((rc = hblock_alloc(ctx, (void **)&s->hash, std::max<uint64_t>(U, 1) * 8))) return fail(rc);
-            if ((rc = hblock_alloc(ctx, (void **)&s->count, std::max<uint64_t>(U, 1) * 4))) return fail(rc);
-            if (U) {
-                SB_CUDA(cudaMemcpyAsync(s->hash, tmp_h.p, U * 8, cudaMemcpyDeviceToDevice, st));
-                SB_CUDA(cudaMemcpyAsync(s->count, tmp_c.p, U * 4, cudaMemcpyDeviceToDevice, st));
-            }
         }
+        // exact-size result arrays; the copies are ordered on the ctx stream like every later use of the handle
+        const uint64_t U = U1 + U2;
+        if ((rc = hblock_alloc(ctx, (void **)&s->hash, std::max<uint64_t>(U, 1) * 8))) return fail(rc);
+        if ((rc = hblock_alloc(ctx, (void **)&s->count, std::max<uint64_t>(U, 1) * 4))) return fail(rc);
+        if (ng && U2) {  // slot the generic path's pairs into their groups' positions, compact straight into the result
+            k_fallback_place<<<nblk(ng, 128), 128, 0, st>>>(g_fb.p, ng, nbk, Mb, f_uq.p, U2, g_nuniq.p, g_src.p);
+            k_scan_u32<<<1, 1024, 0, st>>>(g_nuniq.p, ng, uoff.p);
+            k_compact_uniq<<<ng, 128, 0, st>>>(st_hash.p, st_cnt.p, slot, g_nuniq.p, uoff.p, g_fb.p, g_src.p, f_uq.p, f_ct.p,
+                                                s->hash, s->count);
+            ctx->launches += 3;
+            SB_CUDA(cudaGetLastError());
+        } else if (U) {  // the in-kernel uniques, or without groups the generic path's
+            SB_CUDA(cudaMemcpyAsync(s->hash, ng ? tmp_h.p : f_uq.p, U * 8, cudaMemcpyDeviceToDevice, st));
+            SB_CUDA(cudaMemcpyAsync(s->count, ng ? tmp_c.p : f_ct.p, U * 4, cudaMemcpyDeviceToDevice, st));
+        }
+        if (NF) SB_CUDA(cudaStreamSynchronize(st));  // f_uq / f_ct go out of scope
 #undef SB_CUDA
         s->n = U;
         s->num_dup_removed = ndup;
@@ -1045,9 +951,6 @@ static uint64_t ingest_chunk(uint64_t dflt) {
     return dflt;
 }
 
-// One mate's ASCII input in host memory; a single-end sample has one, a sample of read pairs two with the same records.
-struct HostMate { const uint8_t *bases; const uint64_t *rec_off; };
-
 // Records (pairs) [r0, r1); per mate the first base and the number of bases.  A slot of either ring holds mate 1 at
 // its start and mate 2 behind it at mate2_at(nb[0]) bases: one ring, one copy of the words and one of the offsets per
 // chunk, whatever the number of mates.  Offsets: mate m's r1 - r0 + 1 entries start at entry m * (r1 - r0 + 1).
@@ -1060,9 +963,9 @@ static uint64_t mate2_at(uint64_t nb1) { return (nb1 + 255) & ~255ull; }
 static uint64_t footprint(const Chunk &c, int n_mates) { return n_mates == 2 ? mate2_at(c.nb[0]) + c.nb[1] : c.nb[0]; }
 
 // records [r0, r1) per chunk: at most max_bases bases (of all mates together) and max_recs records, at least one record
-static void plan_chunks(const HostMate *m, int n_mates, uint64_t n_reads, uint64_t max_bases, uint64_t max_recs,
+static void plan_chunks(const Mate *m, int n_mates, uint64_t n_reads, uint64_t max_bases, uint64_t max_recs,
                         std::vector<Chunk> &chunks) {
-    auto at = [&](uint64_t r) { return m[0].rec_off[r] + (n_mates == 2 ? m[1].rec_off[r] : 0); };
+    auto at = [&](uint64_t r) { return m[0].off[r] + (n_mates == 2 ? m[1].off[r] : 0); };
     uint64_t r0 = 0;
     while (r0 < n_reads) {
         const uint64_t base = at(r0);
@@ -1072,7 +975,7 @@ static void plan_chunks(const HostMate *m, int n_mates, uint64_t n_reads, uint64
             if (at(mid) - base <= max_bases) lo = mid; else hi = mid - 1;
         }
         Chunk c{r0, lo, {0, 0}, {0, 0}};
-        for (int i = 0; i < n_mates; i++) { c.base[i] = m[i].rec_off[r0]; c.nb[i] = m[i].rec_off[lo] - c.base[i]; }
+        for (int i = 0; i < n_mates; i++) { c.base[i] = m[i].off[r0]; c.nb[i] = m[i].off[lo] - c.base[i]; }
         chunks.push_back(c);
         r0 = lo;
     }
@@ -1177,16 +1080,16 @@ struct HostIngest {
     }
     // One chunk from caller memory through the ASCII ring and into the builder.  The copy of a slot waits until
     // the previous chunk in it is seeded; the read indices travel with the chunk, so chunks may go in any order.
-    int ship_ascii(syl_ctx *ctx, SampleBuilder &b, const HostMate *m, int n_mates, const Chunk &c) {
+    int ship_ascii(syl_ctx *ctx, SampleBuilder &b, const Mate *m, int n_mates, const Chunk &c) {
         const int slot = a_slot;
         a_slot ^= 1;
         const uint64_t nr = c.r1 - c.r0, no = c.n_off();
         cudaStreamWaitEvent(copy_stream, ev_a_used[slot], 0);
-        Batch bt[2] = {};
+        Mate bt[2] = {};
         for (int i = 0; i < n_mates; i++) {
             bt[i] = {d_asc[slot] + (i ? mate2_at(c.nb[0]) : 0), nullptr, c.nb[i], d_aoff[slot] + i * no, c.base[i]};
             if ((c.nb[i] && cudaMemcpyAsync((void *)bt[i].bases, m[i].bases + c.base[i], c.nb[i], cudaMemcpyHostToDevice, copy_stream) != cudaSuccess) ||
-                cudaMemcpyAsync((void *)bt[i].off, m[i].rec_off + c.r0, no * 8, cudaMemcpyHostToDevice, copy_stream) != cudaSuccess) {
+                cudaMemcpyAsync((void *)bt[i].off, m[i].off + c.r0, no * 8, cudaMemcpyHostToDevice, copy_stream) != cudaSuccess) {
                 set_error("H2D copy failed");
                 return SYL_ERR_CUDA;
             }
@@ -1195,7 +1098,7 @@ struct HostIngest {
         ctx->ingest_chunks_ascii++;
         cudaEventRecord(ev_a_copied[slot], copy_stream);
         cudaStreamWaitEvent(ctx->stream, ev_a_copied[slot], 0);
-        const int rc = b.add_batch(bt, nr, c.r0);
+        const int rc = b.add(bt, n_mates, nr, c.r0);
         cudaEventRecord(ev_a_used[slot], ctx->stream);
         a_last = slot;
         return rc;
@@ -1224,7 +1127,7 @@ void ingest_destroy(syl_ctx *ctx) {
 // host ASCII -> chunks -> builder, for a single-end sample (one mate) and for read pairs (two: a chunk is a range of
 // pairs, both mates in one slot).  ascii_only: every chunk crosses the link as it is, front to back (1 byte of
 // H2D traffic per base, no host packing; pageable caller memory is fine).  Else the pool packs the chunks.
-static int feed_host(syl_ctx *ctx, SampleBuilder &b, const HostMate *m, int n_mates, uint64_t n_reads, bool ascii_only) {
+static int feed_host(syl_ctx *ctx, SampleBuilder &b, const Mate *m, int n_mates, uint64_t n_reads, bool ascii_only) {
     if (!ctx->ingest) ctx->ingest = new HostIngest();
     HostIngest &I = *static_cast<HostIngest *>(ctx->ingest);
     SYL_TRY(I.init());
@@ -1270,7 +1173,7 @@ static int feed_host(syl_ctx *ctx, SampleBuilder &b, const HostMate *m, int n_ma
             for (uint64_t o = 0; o < c.nb[i]; o += ING_SLICE, n_items++)
                 items.push_back({m[i].bases + c.base[i] + o, std::min(ING_SLICE, c.nb[i] - o), words + o / 16, nullptr, 0, 0, nullptr, (uint32_t)ci});
             for (uint64_t o = 0; o < no; o += ING_OSLICE, n_items++)
-                items.push_back({nullptr, 0, nullptr, m[i].rec_off + c.r0 + o, c.base[i], std::min(ING_OSLICE, no - o), I.h_off[slot] + i * no + o, (uint32_t)ci});
+                items.push_back({nullptr, 0, nullptr, m[i].off + c.r0 + o, c.base[i], std::min(ING_OSLICE, no - o), I.h_off[slot] + i * no + o, (uint32_t)ci});
         }
         chunk_items[ci] = n_items;
     }
@@ -1296,10 +1199,10 @@ static int feed_host(syl_ctx *ctx, SampleBuilder &b, const HostMate *m, int n_ma
             cudaStreamWaitEvent(st, I.ev_copied[slot], 0);
             k_off32_to_64<<<nblk(no, 256), 256, 0, st>>>(I.d_off32[slot], no, I.d_off64[slot]);
             ctx->launches++;
-            Batch bt[2] = {};
+            Mate bt[2] = {};
             for (int i = 0; i < n_mates; i++)
                 bt[i] = {nullptr, I.d_words[slot] + (i ? mate2_at(c.nb[0]) / 16 : 0), c.nb[i], I.d_off64[slot] + i * c.n_off(), 0};
-            rc = b.add_batch(bt, c.r1 - c.r0, c.r0);
+            rc = b.add(bt, n_mates, c.r1 - c.r0, c.r0);
             cudaEventRecord(I.ev_used[slot], st);
             if (last_packed >= 0) {  // the pinned buffers of the previous packed chunk have crossed the link: refill them
                 cudaEventSynchronize(I.ev_copied[last_packed % ING_SLOTS]);
@@ -1346,106 +1249,60 @@ static bool host_ingest_ascii() {
     return hi_env ? std::string(hi_env) == "ascii" : local_ranks > 4;
 }
 
-// packed: the input is 2-bit words (device or host memory); else ASCII
-static int sketch_reads_impl(syl_ctx *ctx, int mem, const uint8_t *bases, const uint32_t *packed, uint64_t n_bases,
-                             const uint64_t *rec_off, uint64_t n_reads, int k, uint64_t c, int no_dedup, int sem, syl_sample **out) {
-    if (!ctx || !out || (!bases && !packed && n_bases) || !rec_off) { set_error("NULL argument"); return SYL_ERR_ARG; }
+// A sample of n_reads records: reads (n_mates 1), or read pairs (n_mates 2: mate i of pair p is record p of m[i]).
+// packed: every mate is 2-bit words, else ASCII; mem: where all of it lives.  Device input is used in place, host
+// 2-bit words (a quarter of the bytes) are staged whole once per call, host ASCII goes through feed_host in chunks.
+// A sample with more events than estimated is redone (host ASCII: fed again) with the exact event capacity.
+static int sketch_reads_impl(syl_ctx *ctx, int mem, bool packed, const Mate *m, int n_mates, uint64_t n_reads, int k,
+                             uint64_t c, int no_dedup, int sem, syl_sample **out) {
+    bool null_arg = !ctx || !out;
+    for (int i = 0; i < n_mates; i++) null_arg = null_arg || (!m[i].bases && !m[i].packed && m[i].nb) || !m[i].off;
+    if (null_arg) { set_error("NULL argument"); return SYL_ERR_ARG; }
     if (c == 0) { set_error("c must be >= 1"); return SYL_ERR_ARG; }
     if (mem != SYL_MEM_HOST && mem != SYL_MEM_DEVICE) { set_error("bad mem"); return SYL_ERR_ARG; }
     *out = nullptr;
     SYL_CUDA(cudaSetDevice(ctx->device));
     syl::tl_ctx = ctx;
+    const bool fed = mem == SYL_MEM_HOST && !packed;
+    Mate dm[2] = {};  // the mates on the device, unless fed
+    Staged<uint32_t> sp[2];
+    Staged<uint64_t> so[2];
+    uint64_t expect_bases = 0, staged_bytes = 0;
+    for (int i = 0; i < n_mates; i++) {
+        expect_bases += m[i].nb;
+        if (fed) continue;
+        dm[i] = m[i];
+        if (packed) { SYL_TRY(sp[i].init(ctx, mem, m[i].packed, (m[i].nb + 15) / 16)); dm[i].packed = sp[i].p; }
+        SYL_TRY(so[i].init(ctx, mem, m[i].off, n_reads + 1));
+        dm[i].off = so[i].p;
+        if (mem == SYL_MEM_HOST) staged_bytes += (m[i].nb + 15) / 16 * 4 + (n_reads + 1) * 8;
+    }
+    // the mean length of mate 1 (for pairs src/sketch.rs:824-826)
+    const double mean_read_length = n_reads ? (double)m[0].nb / (double)n_reads : 0.;
     const bool host_ascii = host_ingest_ascii();
     static const bool dbg = getenv("SYL_DEBUG_TIMING") != nullptr;
     auto now = []() { return std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now().time_since_epoch()).count(); };
     uint64_t cap_override = 0;
     for (int attempt = 0; attempt < 3; attempt++) {
-        SampleBuilder b{ctx, k, c, no_dedup, sem};
-        b.expect_bases = n_bases;
-        b.expect_reads = n_reads;
-        if (mem == SYL_MEM_HOST) ctx->ingest_h2d_bytes = ctx->ingest_chunks_packed = ctx->ingest_chunks_ascii = 0;
+        SampleBuilder b{ctx, k, c, no_dedup, sem, n_mates == 2, n_reads, mean_read_length};
+        b.expect_bases = expect_bases;
+        b.expect_reads = n_mates * n_reads;
+        if (mem == SYL_MEM_HOST) {
+            ctx->ingest_h2d_bytes = staged_bytes;
+            ctx->ingest_chunks_packed = ctx->ingest_chunks_ascii = 0;
+        }
         SYL_TRY(b.begin(cap_override));
         const double t0 = now();
         int rc = SYL_OK;
-        Staged<uint32_t> sp;   // host packed input staged whole
-        Staged<uint64_t> so;
-        if (mem == SYL_MEM_DEVICE) {
-            rc = b.add({bases, packed, n_bases, rec_off, 0}, n_reads, 0);
-        } else if (packed) {
-            const uint64_t nw = (n_bases + 15) / 16;
-            SYL_TRY(sp.init(ctx, mem, packed, nw));
-            SYL_TRY(so.init(ctx, mem, rec_off, n_reads + 1));
-            ctx->ingest_h2d_bytes += nw * 4 + (n_reads + 1) * 8;
-            rc = b.add({nullptr, sp.p, n_bases, so.p, 0}, n_reads, 0);
-        } else if (n_reads && n_bases) {
-            const HostMate hm{bases, rec_off};
-            rc = feed_host(ctx, b, &hm, 1, n_reads, host_ascii);
-        }
+        if (!fed) rc = b.add(dm, n_mates, n_reads, 0);
+        else if (n_reads && expect_bases) rc = feed_host(ctx, b, m, n_mates, n_reads, host_ascii);
         if (rc != SYL_OK) return rc;
         const double t1 = now();
         uint64_t need = 0;
         rc = b.finish(out, &need);
-        if (dbg) fprintf(stderr, "[syl_sketch_reads host] feed %.2f ms, finish %.2f ms (attempt %d)\n", t1 - t0, now() - t1, attempt);
+        if (dbg) fprintf(stderr, "[%s] feed %.2f ms, finish %.2f ms (attempt %d)\n",
+                         n_mates == 2 ? "syl_sketch_read_pairs" : "syl_sketch_reads", t1 - t0, now() - t1, attempt);
         if (rc == SYL_ERR_CAPACITY) { cap_override = need + 16; continue; }  // more events than estimated: redo with the exact size
-        return rc;
-    }
-    set_error("event capacity retry failed");
-    return SYL_ERR_CAPACITY;
-}
-
-// One mate file of a paired sample: ASCII bytes or 2-bit words.
-struct MateInput {
-    const uint8_t *bases;
-    const uint32_t *packed;
-    uint64_t n_bases;
-    const uint64_t *off;
-    uint64_t n_words() const { return (n_bases + 15) / 16; }
-};
-
-// packed: both mates are 2-bit words (m1.packed / m2.packed), else ASCII (m1.bases / m2.bases).  Host ASCII goes
-// through feed_host as chunks of pairs; host 2-bit words (a quarter of the bytes) are staged whole.
-static int sketch_read_pairs_impl(syl_ctx *ctx, int mem, bool packed, MateInput &m1, MateInput &m2, uint64_t n_pairs, int k,
-                                  uint64_t c, int no_dedup, int sem, syl_sample **out) {
-    if (!ctx || !out || (!m1.bases && !m1.packed && m1.n_bases) || (!m2.bases && !m2.packed && m2.n_bases) || !m1.off || !m2.off) {
-        set_error("NULL argument");
-        return SYL_ERR_ARG;
-    }
-    if (c == 0) { set_error("c must be >= 1"); return SYL_ERR_ARG; }
-    if (mem != SYL_MEM_HOST && mem != SYL_MEM_DEVICE) { set_error("bad mem"); return SYL_ERR_ARG; }
-    *out = nullptr;
-    SYL_CUDA(cudaSetDevice(ctx->device));
-    syl::tl_ctx = ctx;
-    cudaStream_t st = ctx->stream;
-    const bool fed = mem == SYL_MEM_HOST && !packed;
-    const HostMate hm[2] = {{m1.bases, m1.off}, {m2.bases, m2.off}};
-    Staged<uint32_t> sp[2];  // host 2-bit words: staged copies, alive until the call's sync
-    Staged<uint64_t> so[2];
-    MateInput *m[2] = {&m1, &m2};
-    for (int i = 0; i < 2 && !fed; i++) {
-        if (packed) { SYL_TRY(sp[i].init(ctx, mem, m[i]->packed, m[i]->n_words())); m[i]->packed = sp[i].p; }
-        SYL_TRY(so[i].init(ctx, mem, m[i]->off, n_pairs + 1));
-        m[i]->off = so[i].p;
-    }
-    const bool host_ascii = host_ingest_ascii();
-    uint64_t cap_override = 0;
-    for (int attempt = 0; attempt < 3; attempt++) {
-        SampleBuilder b{ctx, k, c, no_dedup, sem};
-        b.paired = true;
-        b.expect_bases = m1.n_bases + m2.n_bases;
-        b.expect_reads = 2 * n_pairs;
-        if (mem == SYL_MEM_HOST) {
-            ctx->ingest_chunks_packed = ctx->ingest_chunks_ascii = 0;
-            ctx->ingest_h2d_bytes = fed ? 0 : (m1.n_words() + m2.n_words()) * 4 + 2 * (n_pairs + 1) * 8;
-        }
-        SYL_TRY(b.begin(cap_override));
-        if (!fed) SYL_TRY(b.add_pair({m1.bases, m1.packed, m1.n_bases, m1.off, 0}, {m2.bases, m2.packed, m2.n_bases, m2.off, 0}, n_pairs, 0));
-        else if (n_pairs && b.expect_bases) SYL_TRY(feed_host(ctx, b, hm, 2, n_pairs, host_ascii));
-        b.n_reads = n_pairs;       // mean_read_length = mean length of mate 1 (src/sketch.rs:824-826)
-        b.n_bases = m1.n_bases;
-        uint64_t need = 0;
-        const int rc = b.finish(out, &need);
-        if (rc == SYL_ERR_CAPACITY) { cap_override = need + 16; continue; }  // more events than estimated: redo (and re-feed) with the exact size
-        if (rc == SYL_OK && !fed) SYL_CUDA(cudaStreamSynchronize(st));  // the staged inputs go out of scope
         return rc;
     }
     set_error("event capacity retry failed");
@@ -1461,28 +1318,29 @@ extern "C" {
 int syl_sketch_reads(syl_ctx *ctx, int mem, const uint8_t *bases, uint64_t n_bases,
                      const uint64_t *rec_off, uint64_t n_reads, int k, uint64_t c, int no_dedup,
                      int sem, syl_sample **out) {
-    return sketch_reads_impl(ctx, mem, bases, nullptr, n_bases, rec_off, n_reads, k, c, no_dedup, sem, out);
+    const Mate m[1] = {{bases, nullptr, n_bases, rec_off, 0}};
+    return sketch_reads_impl(ctx, mem, false, m, 1, n_reads, k, c, no_dedup, sem, out);
 }
 
 int syl_sketch_reads_packed2(syl_ctx *ctx, int mem, const uint32_t *packed, uint64_t n_bases,
                              const uint64_t *rec_off, uint64_t n_reads, int k, uint64_t c, int no_dedup,
                              int sem, syl_sample **out) {
-    if (!packed && n_bases) { set_error("NULL argument"); return SYL_ERR_ARG; }
-    return sketch_reads_impl(ctx, mem, nullptr, packed, n_bases, rec_off, n_reads, k, c, no_dedup, sem, out);
+    const Mate m[1] = {{nullptr, packed, n_bases, rec_off, 0}};
+    return sketch_reads_impl(ctx, mem, true, m, 1, n_reads, k, c, no_dedup, sem, out);
 }
 
 int syl_sketch_read_pairs(syl_ctx *ctx, int mem, const uint8_t *bases1, uint64_t n_bases1, const uint64_t *rec_off1,
                           const uint8_t *bases2, uint64_t n_bases2, const uint64_t *rec_off2, uint64_t n_pairs,
                           int k, uint64_t c, int no_dedup, int sem, syl_sample **out) {
-    MateInput m1{bases1, nullptr, n_bases1, rec_off1}, m2{bases2, nullptr, n_bases2, rec_off2};
-    return sketch_read_pairs_impl(ctx, mem, false, m1, m2, n_pairs, k, c, no_dedup, sem, out);
+    const Mate m[2] = {{bases1, nullptr, n_bases1, rec_off1, 0}, {bases2, nullptr, n_bases2, rec_off2, 0}};
+    return sketch_reads_impl(ctx, mem, false, m, 2, n_pairs, k, c, no_dedup, sem, out);
 }
 
 int syl_sketch_read_pairs_packed2(syl_ctx *ctx, int mem, const uint32_t *packed1, uint64_t n_bases1, const uint64_t *rec_off1,
                                   const uint32_t *packed2, uint64_t n_bases2, const uint64_t *rec_off2, uint64_t n_pairs,
                                   int k, uint64_t c, int no_dedup, int sem, syl_sample **out) {
-    MateInput m1{nullptr, packed1, n_bases1, rec_off1}, m2{nullptr, packed2, n_bases2, rec_off2};
-    return sketch_read_pairs_impl(ctx, mem, true, m1, m2, n_pairs, k, c, no_dedup, sem, out);
+    const Mate m[2] = {{nullptr, packed1, n_bases1, rec_off1, 0}, {nullptr, packed2, n_bases2, rec_off2, 0}};
+    return sketch_reads_impl(ctx, mem, true, m, 2, n_pairs, k, c, no_dedup, sem, out);
 }
 
 int syl_pack_threads(void) { return default_pack_threads(); }

@@ -230,7 +230,7 @@ __device__ __forceinline__ void seed_resolve(const SeedSmem &S, SeedMeta &M, uin
         ev.hash = h;
         const int L = M.len[j];
         const bool has_pair = !no_dedup && L <= 400 && L >= 66;  // src/sketch.rs:923, :627
-        // no_dedup == 2: read pairs — the keys need both mates, every event is completed by k_events_fix_paired
+        // no_dedup == 2: read pairs — the keys need both mates, every event is completed by k_events_fix<.., true>
         ev.recflag = ((rec_base + rc + (uint64_t)j) << 1) | (no_dedup == 2 ? EV_PENDING : (has_pair ? 0ull : NO_PAIR));
         ev.p0 = 0;
         ev.p1 = 0;

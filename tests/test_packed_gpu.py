@@ -44,7 +44,7 @@ def test_seeding_packed_equals_oracle_all_byte_values(ctx, k, sem, device):
 @pytest.mark.parametrize("no_dedup", [False, True])
 def test_read_sketch_packed_equals_ascii_equals_oracle(ctx, device, no_dedup):
     """Pair keys come from the packed stream (in-tile) or from packed global memory (reads cut by a tile
-    edge: k_events_fix<packed>); duplicates make the dedup state machine depend on them."""
+    edge: k_events_fix<true, false>); duplicates make the dedup state machine depend on them."""
     from oracle import oracle as O
     from sylph_b200.api import pack2
     rng = np.random.default_rng(77)
