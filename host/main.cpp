@@ -73,6 +73,8 @@ struct Args {
     uint64_t batch_bases = 1ull << 30;  // SYL_DRIVER_BATCH_BASES: a genome batch closes once it holds this many bases
     uint64_t samples_per_call = 0;      // SYL_DRIVER_SAMPLES_PER_CALL: cap on samples per syl_query / syl_profile call (0 = none)
     uint64_t rows0 = 0;                 // SYL_DRIVER_ROWS: initial row-buffer length (0 = sized from the call)
+    uint64_t shard_entries = 0;         // SYL_DRIVER_SHARD_ENTRIES: query / profile through db shards of this many entries
+    uint64_t max_db_entries = 0;        // --max-db-entries: the same, as an option
 };
 
 static uint64_t env_u64(const char *name, uint64_t dflt) {
@@ -153,6 +155,7 @@ static Args parse(int argc, char **argv) {
         else if (s == "--device") a.device = std::stoi(need(i));
         else if (s == "-u" || s == "--estimate-unknown") a.estimate_unknown = true;
         else if (s == "-I" || s == "--read-seq-id") a.read_seq_id = std::stod(need(i));
+        else if (s == "--max-db-entries") a.max_db_entries = std::max<uint64_t>(1, std::stoull(need(i)));  // driver-only
         else if (a.cmd == "sketch" && (s == "-S" || s == "--sample-names")) {
             while (i + 1 < argc && argv[i + 1][0] != '-') a.sample_names.push_back(argv[++i]);
         }
@@ -185,6 +188,7 @@ static Args parse(int argc, char **argv) {
     a.batch_bases = env_u64("SYL_DRIVER_BATCH_BASES", a.batch_bases);
     a.samples_per_call = env_u64("SYL_DRIVER_SAMPLES_PER_CALL", 0);
     a.rows0 = env_u64("SYL_DRIVER_ROWS", 0);
+    a.shard_entries = env_u64("SYL_DRIVER_SHARD_ENTRIES", 0);
     return a;
 }
 
@@ -420,11 +424,29 @@ static int cmd_contain(syl_ctx *ctx, const Args &a, bool pseudotax) {
         std::vector<uint64_t>().swap(g.tracked);
     }
     const bool has_tr = gs[0].has_tracked;
+    // one index while the db fits one (fewer than 2^32-2 entries and 2^31-1 genomes) and no cap is set; otherwise db
+    // shards that every query / profile call sweeps once, reading the flat arrays from host memory
+    uint64_t shard_cap = a.max_db_entries;
+    if (a.shard_entries) shard_cap = shard_cap ? std::min(shard_cap, a.shard_entries) : a.shard_entries;
+    const bool sharded = shard_cap || nk + (has_tr ? nt : 0) >= 0xFFFFFFFEull || gs.size() >= 0x7FFFFFFFull;
     syl_db *db = nullptr;
-    check(syl_db_build_arrays(ctx, SYL_MEM_HOST, kmers.data(), koff.data(), has_tr ? tracked.data() : nullptr,
-                              has_tr ? toff.data() : nullptr, gsz.data(), gs.size(), (int)gs[0].k, db_c, 0, &db), "syl_db_build_arrays");
-    std::vector<uint64_t>().swap(kmers);
-    std::vector<uint64_t>().swap(tracked);
+    syl_db_shards *shards = nullptr;
+    if (!sharded) {
+        check(syl_db_build_arrays(ctx, SYL_MEM_HOST, kmers.data(), koff.data(), has_tr ? tracked.data() : nullptr,
+                                  has_tr ? toff.data() : nullptr, gsz.data(), gs.size(), (int)gs[0].k, db_c, 0, &db), "syl_db_build_arrays");
+        std::vector<uint64_t>().swap(kmers);
+        std::vector<uint64_t>().swap(tracked);
+    } else {
+        check(syl_db_shards_create(ctx, kmers.data(), koff.data(), has_tr ? tracked.data() : nullptr, has_tr ? toff.data() : nullptr,
+                                   gsz.data(), gs.size(), (int)gs[0].k, db_c, shard_cap, &shards), "syl_db_shards_create");
+        const uint64_t n_shards = syl_db_shards_count(shards);
+        for (uint64_t i = 0; i < n_shards; i++) {
+            uint64_t g0 = 0, ng = 0, ne = 0;
+            check(syl_db_shards_range(shards, i, &g0, &ng, &ne), "syl_db_shards_range");
+            info("Database shard " + std::to_string(i + 1) + "/" + std::to_string(n_shards) + ": genomes " + std::to_string(g0) + ".." +
+                 std::to_string(g0 + ng) + ", " + std::to_string(ne) + " index entries.");
+        }
+    }
     // samples
     std::vector<syl_sample *> samples;
     std::vector<std::string> names;
@@ -472,17 +494,21 @@ static int cmd_contain(syl_ctx *ctx, const Args &a, bool pseudotax) {
         p.minimum_ani = a.min_ani; p.redundant_ani = a.redundant_ani;
         p.estimate_unknown = a.estimate_unknown ? 1 : 0; p.read_seq_id = a.read_seq_id;
         // sample batches sized so that samples x genomes stays below the library's per-call limits (2^31 pairs,
-        // 8 GB of per-pair histograms = 2^23 pairs); the reference walks the samples in chunks too (src/contain.rs:239-263)
+        // 8 GB of per-pair histograms = 2^23 pairs); the reference walks the samples in chunks too (src/contain.rs:239-263).
+        // Shards take every sample in one call (the library batches them per shard), so each shard is built once.
         size_t per_call = std::max<size_t>(1, std::min<size_t>(samples.size(), (size_t)((1ull << 22) / std::max<size_t>(gs.size(), 1))));
         if (a.samples_per_call) per_call = std::min<size_t>(per_call, a.samples_per_call);
+        if (shards) per_call = samples.size();
         for (size_t s0 = 0; s0 < samples.size(); s0 += per_call) {
             const size_t ns = std::min(per_call, samples.size() - s0);
             std::vector<syl_ani_row> rows(a.rows0 ? a.rows0 : std::max<size_t>(1024, std::min<size_t>(gs.size() * ns, 1u << 22)));
             uint64_t n = 0;
             for (;;) {
-                int rc = (pseudotax ? syl_profile : syl_query)(ctx, db, samples.data() + s0, (uint32_t)ns, &p, rows.data(), rows.size(), &n);
-                if (rc == SYL_ERR_CAPACITY) { rows.resize(n); continue; }
-                check(rc, pseudotax ? "syl_profile" : "syl_query");
+                int rc = shards ? (pseudotax ? syl_profile_shards : syl_query_shards)(ctx, shards, samples.data() + s0, (uint32_t)ns, &p,
+                                                                                      rows.data(), rows.size(), &n)
+                                : (pseudotax ? syl_profile : syl_query)(ctx, db, samples.data() + s0, (uint32_t)ns, &p, rows.data(), rows.size(), &n);
+                if (rc == SYL_ERR_CAPACITY) { rows.resize(n); continue; }  // shards: the retry copies out the kept rows
+                check(rc, shards ? (pseudotax ? "syl_profile_shards" : "syl_query_shards") : (pseudotax ? "syl_profile" : "syl_query"));
                 break;
             }
             rows.resize(n);
@@ -502,6 +528,7 @@ static int cmd_contain(syl_ctx *ctx, const Args &a, bool pseudotax) {
     if (o != stdout) fclose(o);
     for (syl_sample *s : samples) syl_sample_free(s);
     syl_db_free(db);
+    syl_db_shards_free(shards);
     info("sylph finished.");
     return 0;
 }

@@ -21,7 +21,8 @@
  *     fail with SYL_ERR_CUDA.
  *   - hard limits (reported as SYL_ERR_ARG, never silently wrapped): fewer than 2^32-2 records per batch,
  *     fewer than 2^32-2 survivor events per sample, fewer than 2^32-2 index entries (genome_kmers + tracked)
- *     and 2^31 genomes per db shard, fewer than 2^31 (sample, genome) pairs per syl_query / syl_profile call.
+ *     and 2^31 genomes per db shard (a larger database from host memory: syl_db_shards, section 6), fewer than 2^31
+ *     (sample, genome) pairs per syl_query / syl_profile call.
  *     Above 2^23 pairs per call the 256-bin per-pair histograms would exceed 8 GB: syl_query / syl_profile
  *     then run in the CSR formulation (slower, one more host synchronisation), the sharded profile (5)
  *     reports SYL_ERR_UNSUPPORTED.
@@ -363,6 +364,48 @@ int syl_profile_shard_pass2(syl_profile_job *job);
 int syl_profile_shard_finish(syl_profile_job *job, syl_ani_row *rows, uint64_t cap, uint64_t *n_rows,
                              uint64_t *need_rows_per_rank);
 void syl_profile_job_free(syl_profile_job *job);
+
+/* ------------------------------------------------------------------------------------------
+ * (6) A database larger than one index, on ONE GPU, from host memory: e.g. GTDB at a small c, or several .syldb
+ *     profiled together (sylph keeps the whole database in host RAM, src/contain.rs:212-236).  The 2^32-2 entry
+ *     limit and the device memory then bound each shard, not the database.
+ *
+ * syl_db_shards_create borrows CSR arrays in HOST memory (arguments as in syl_db_build_arrays; the caller keeps them
+ * alive and unchanged until syl_db_shards_free) and cuts them into contiguous genome ranges of at most max_entries
+ * index entries (k-mers + tracked k-mers) each, greedily in genome order.  max_entries == 0: the largest shard the
+ * device's free memory allows at creation (16 bytes per entry after 4 GB and an eighth of it for the joins); never
+ * more than 2^32-3 entries or 2^31-2 genomes.  A genome larger than the cap is a shard of its own.  NULL arrays that
+ * the offsets say hold entries, offsets that do not start at 0 or decrease, device pointers, 2^32 genomes or more, and
+ * a genome of more than 2^32-3 entries are SYL_ERR_ARG, before anything is allocated.  Nothing is built yet.
+ * SYL_DB_SHARD_ENTRIES (test hook, read per create) caps max_entries further.
+ *
+ * syl_query_shards / syl_profile_shards return the rows, order and error codes of syl_query / syl_profile on one db
+ * of all genomes; row.genome is the global genome index.  Each call sweeps the shards once: it builds a shard's
+ * index (as syl_db_build_arrays, genome_base = the shard's first genome), runs pass 1 of all samples against it in
+ * batches of at most 2^22 (sample, genome) pairs, and frees it before building the next.  A call therefore costs one
+ * index build per shard, whatever the sample count: give it all samples at once.  Device memory peaks at one shard's
+ * build (see syl_db_build_arrays) plus the joins' scratch; the ctx's cached free blocks are released between shards.
+ *   query:   rows ordered by (sample, genome).
+ *   profile: pass 1 without CIs, then for each batch of samples an index of the union of their pass-1 survivors
+ *            (ascending global order, gathered into pinned host staging) and syl_profile on it.  A batch closes before
+ *            its union passes the shard cap; one sample's survivors may take up to max(cap, the free-memory default)
+ *            entries, beyond that SYL_ERR_UNSUPPORTED.
+ * SYL_ERR_CAPACITY: *n_rows holds the needed size, and the handle keeps the rows.  The NEXT call on the handle with the
+ * same samples (pointers), params and kind only copies them out (no index is built); any other call drops them.
+ * One ctx per handle; calls on one handle are serialised by the caller.
+ * ---------------------------------------------------------------------------------------- */
+typedef struct syl_db_shards syl_db_shards;
+int syl_db_shards_create(syl_ctx *ctx, const uint64_t *kmers, const uint64_t *kmer_off, const uint64_t *tracked,
+                         const uint64_t *tracked_off, const uint64_t *gn_size, uint64_t n_genomes, int k, uint64_t c,
+                         uint64_t max_entries, syl_db_shards **out);
+uint64_t syl_db_shards_count(const syl_db_shards *s);
+/* shard i: genomes [*first_genome, *first_genome + *n_genomes) holding *n_entries index entries (out pointers may be NULL) */
+int syl_db_shards_range(const syl_db_shards *s, uint64_t i, uint64_t *first_genome, uint64_t *n_genomes, uint64_t *n_entries);
+int syl_query_shards(syl_ctx *ctx, syl_db_shards *s, const syl_sample *const *samples, uint32_t n_samples,
+                     const syl_contain_params *p, syl_ani_row *rows, uint64_t cap, uint64_t *n_rows);
+int syl_profile_shards(syl_ctx *ctx, syl_db_shards *s, const syl_sample *const *samples, uint32_t n_samples,
+                       const syl_contain_params *p, syl_ani_row *rows, uint64_t cap, uint64_t *n_rows);
+void syl_db_shards_free(syl_db_shards *s);
 
 #ifdef __cplusplus
 }

@@ -100,6 +100,12 @@ SIGNATURES = {
     "syl_profile_shard_pass2": (_i, [_vp]),
     "syl_profile_shard_finish": (_i, [_vp, _vp, _u64, _pu64, _pu64]),
     "syl_profile_job_free": (None, [_vp]),
+    "syl_db_shards_create": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _u64, _i, _u64, _u64, _pp]),
+    "syl_db_shards_count": (_u64, [_vp]),
+    "syl_db_shards_range": (_i, [_vp, _u64, _pu64, _pu64, _pu64]),
+    "syl_query_shards": (_i, [_vp, _vp, _pp, _u32, C.POINTER(ContainParams), _vp, _u64, _pu64]),
+    "syl_profile_shards": (_i, [_vp, _vp, _pp, _u32, C.POINTER(ContainParams), _vp, _u64, _pu64]),
+    "syl_db_shards_free": (None, [_vp]),
 }
 
 

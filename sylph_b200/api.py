@@ -294,6 +294,16 @@ class Context:
                                                   C.byref(h)))
         return Db(self, h)
 
+    def db_shards(self, kmers, kmer_off, tracked=None, tracked_off=None, gn_size=None, k=31, c=200, max_entries=0):
+        """A database larger than one index, in host memory (syl_db_shards_create): cut into shards of at most
+        max_entries index entries (0 = what the device's free memory allows), each built once per query / profile
+        call.  The returned DbShards keeps the arrays referenced while it lives."""
+        keep = [_arg(a, np.uint64) for a in (kmers, kmer_off, tracked, tracked_off, gn_size)]
+        h = C.c_void_p()
+        _lib.check(_lib.lib().syl_db_shards_create(self._h, *[a[1] for a in keep], keep[1][2] - 1, k, c, int(max_entries),
+                                                   C.byref(h)))
+        return DbShards(self, h, [a[3] for a in keep])
+
     def _pairs(self, fn, db, samples, params, cap):
         L = _lib.lib()
         n = len(samples)
@@ -434,6 +444,46 @@ class Db:
         if self._h:
             _lib.lib().syl_db_free(self._h)
             self._h = None
+
+    def __del__(self):
+        try:
+            self.free()
+        except Exception:
+            pass
+
+
+class DbShards:
+    """A host-memory database swept shard by shard (syl_db_shards): the rows of Context.query / .profile on one db of
+    all genomes, with global genome indices."""
+
+    def __init__(self, ctx, handle, arrays):
+        self.ctx, self._h, self._arrays = ctx, handle, arrays
+
+    def __len__(self):
+        return int(_lib.lib().syl_db_shards_count(self._h))
+
+    def ranges(self):
+        """-> [(first_genome, n_genomes, n_entries)] per shard"""
+        out = []
+        for i in range(len(self)):
+            a, n, e = C.c_uint64(0), C.c_uint64(0), C.c_uint64(0)
+            _lib.check(_lib.lib().syl_db_shards_range(self._h, i, C.byref(a), C.byref(n), C.byref(e)))
+            out.append((a.value, n.value, e.value))
+        return out
+
+    def query(self, samples, params=None, cap=None):
+        params = params or contain_params(pseudotax=False)
+        return self.ctx._pairs(_lib.lib().syl_query_shards, self, samples, params, cap)
+
+    def profile(self, samples, params=None, cap=None):
+        params = params or contain_params(pseudotax=True)
+        return self.ctx._pairs(_lib.lib().syl_profile_shards, self, samples, params, cap)
+
+    def free(self):
+        if self._h:
+            _lib.lib().syl_db_shards_free(self._h)
+            self._h = None
+        self._arrays = None
 
     def __del__(self):
         try:

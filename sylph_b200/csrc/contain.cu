@@ -28,12 +28,16 @@
 #include <cub/cub.cuh>
 
 #include <algorithm>
+#include <chrono>
 #include <cmath>
+#include <cstdio>
+#include <cstring>
 #include <new>
 #include <vector>
 
 #include "common.cuh"
 #include "crmath.cuh"
+#include "shard_cut.hpp"
 
 struct syl_db {
     int device = 0;
@@ -1510,22 +1514,29 @@ static int contain_fast(syl_ctx *ctx, const syl_db *db, const syl_sample *const 
     return SYL_ERR_CAPACITY;
 }
 
-static int check_pair_args(syl_ctx *ctx, const syl_db *db, const syl_sample *const *samples, uint32_t n_samples,
-                           const syl_contain_params *p, syl_ani_row *rows, uint64_t cap, uint64_t *n_rows) {
-    if (!ctx || !db || !p || !n_rows || (n_samples && !samples) || (cap && !rows)) { set_error("NULL argument"); return SYL_ERR_ARG; }
+// the arguments of a query / profile call against a database of k-mer size k and sketch parameter c
+static int check_sample_args(syl_ctx *ctx, int k, uint64_t c, const syl_sample *const *samples, uint32_t n_samples,
+                             const syl_contain_params *p, syl_ani_row *rows, uint64_t cap, uint64_t *n_rows) {
+    if (!ctx || !p || !n_rows || (n_samples && !samples) || (cap && !rows)) { set_error("NULL argument"); return SYL_ERR_ARG; }
     for (uint32_t i = 0; i < n_samples; i++) {
         if (!samples[i]) { set_error("NULL sample"); return SYL_ERR_ARG; }
-        if (samples[i]->k != db->k) {  // src/contain.rs:608-615 (log::error + exit(1))
+        if (samples[i]->k != k) {  // src/contain.rs:608-615 (log::error + exit(1))
             set_error("k parameter for reads != k parameter for genome");
             return SYL_ERR_ARG;
         }
-        if (db->c < samples[i]->c) {   // src/contain.rs:616-623
+        if (c < samples[i]->c) {   // src/contain.rs:616-623
             set_error("c parameter for reads > c parameter for genome");
             return SYL_ERR_ARG;
         }
     }
-    if (p->k != db->k) { set_error("params.k != db k"); return SYL_ERR_ARG; }
+    if (p->k != k) { set_error("params.k != db k"); return SYL_ERR_ARG; }
     return SYL_OK;
+}
+
+static int check_pair_args(syl_ctx *ctx, const syl_db *db, const syl_sample *const *samples, uint32_t n_samples,
+                           const syl_contain_params *p, syl_ani_row *rows, uint64_t cap, uint64_t *n_rows) {
+    if (!db) { set_error("NULL argument"); return SYL_ERR_ARG; }
+    return check_sample_args(ctx, db->k, db->c, samples, n_samples, p, rows, cap, n_rows);
 }
 
 // ---- index build, host side -------------------------------------------------------------------
@@ -1816,6 +1827,268 @@ static int db_build(syl_ctx *ctx, const DbInput &in, const uint64_t *gn_size, in
 
 }  // namespace syl
 
+// A database in borrowed host arrays, cut into index shards (syl_db_shards_*).
+struct syl_db_shards {
+    syl_ctx *ctx = nullptr;
+    const uint64_t *kmers = nullptr, *kmer_off = nullptr, *tracked = nullptr, *tracked_off = nullptr, *gn_size = nullptr;
+    uint64_t G = 0;
+    int k = 31;
+    uint64_t c = 200;
+    uint64_t cap = 0;             // entries per shard, and per survivor index of several samples
+    uint64_t survivor_max = 0;    // entries of one sample's survivor index
+    std::vector<uint64_t> first;  // shard i = genomes [first[i], first[i + 1])
+    uint64_t calls = 0;
+    struct {                      // the rows of the last call, when they did not fit the caller's buffer
+        uint64_t call = 0;        // 0: nothing kept
+        bool profile = false;
+        syl_contain_params p{};
+        std::vector<const syl_sample *> samples;
+        std::vector<syl_ani_row> rows;
+    } kept;
+    uint64_t *pinned = nullptr;   // staging of the survivor k-mers (grow-only)
+    uint64_t pinned_n = 0;
+};
+
+namespace syl {
+
+constexpr uint64_t PAIRS_PER_CALL = 1ull << 22;  // (sample, genome) pairs per join: 4 GB of per-pair histograms
+
+// Entries per shard when the caller gives none: the device's free memory at 16 bytes per entry (the build's peak is
+// about 14), after an eighth of it and the histograms of PAIRS_PER_CALL pairs are set aside for the joins.
+static int default_shard_entries(uint64_t *out) {
+    size_t free_b = 0, total_b = 0;
+    SYL_CUDA(cudaMemGetInfo(&free_b, &total_b));
+    const uint64_t budget = free_b - free_b / 8, joins = PAIRS_PER_CALL * COV_BINS * 4;
+    const uint64_t e = budget > joins ? (budget - joins) / 16 : 0;
+    *out = std::min<uint64_t>(std::max<uint64_t>(e, 1ull << 20), SHARD_MAX_ENTRIES);
+    return SYL_OK;
+}
+
+static uint64_t shard_entries_env() {  // SYL_DB_SHARD_ENTRIES caps max_entries (tests; read per syl_db_shards_create)
+    if (const char *e = getenv("SYL_DB_SHARD_ENTRIES")) {
+        const long long v = atoll(e);
+        if (v >= 1) return (uint64_t)v;
+    }
+    return 0;
+}
+
+// Hand the ctx's cached free blocks back to the driver: each shard's index and join scratch are then allocated to that
+// shard's size, not next to the previous shard's.
+static double ms_since(std::chrono::steady_clock::time_point t) {
+    return std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t).count();
+}
+
+static int cache_trim(syl_ctx *ctx) {
+    SYL_CUDA(cudaStreamSynchronize(ctx->stream));
+    for (const auto &b : ctx->free_blocks) {
+        cudaFree(b.first);
+        ctx->cached_bytes -= b.second;
+    }
+    ctx->free_blocks.clear();
+    return SYL_OK;
+}
+
+// The index of genomes [a, b) straight from the borrowed host arrays; only the offsets are copied (rebased to 0).
+static int shard_build(const syl_db_shards *s, uint64_t a, uint64_t b, syl_db **out) {
+    const uint64_t G = b - a;
+    std::vector<uint64_t> ko(G + 1), to(s->tracked_off ? G + 1 : 0);
+    for (uint64_t i = 0; i <= G; i++) ko[i] = s->kmer_off[a + i] - s->kmer_off[a];
+    for (uint64_t i = 0; i < to.size(); i++) to[i] = s->tracked_off[a + i] - s->tracked_off[a];
+    const uint64_t nt = to.empty() ? 0 : to[G];
+    const DbInput in{SYL_MEM_HOST,
+                     {ko[G] ? s->kmers + s->kmer_off[a] : nullptr, nt ? s->tracked + s->tracked_off[a] : nullptr},
+                     {ko.data(), to.empty() ? nullptr : to.data()}, G, {ko[G], nt}};
+    return db_build(s->ctx, in, s->gn_size ? s->gn_size + a : nullptr, s->tracked_off ? 1 : 0, s->k, s->c, (uint32_t)a, out);
+}
+
+// Pass 1 (syl_query) of samples[0, S) against every shard in turn: each shard's index is built once, joined with all
+// samples in batches of at most PAIRS_PER_CALL pairs, and freed before the next one is built.  rows: by shard, then by
+// (sample, genome); row.genome is the global index.
+static int shards_sweep(syl_db_shards *s, const syl_sample *const *samples, uint32_t S, const syl_contain_params *p,
+                        std::vector<syl_ani_row> &rows) {
+    syl_ctx *ctx = s->ctx;
+    for (size_t i = 0; i + 1 < s->first.size(); i++) {
+        const uint64_t a = s->first[i], G = s->first[i + 1] - a;
+        SYL_TRY(cache_trim(ctx));
+        const auto t0 = std::chrono::steady_clock::now();
+        syl_db *db = nullptr;
+        SYL_TRY(shard_build(s, a, s->first[i + 1], &db));
+        const double build_ms = ms_since(t0);
+        const auto t1 = std::chrono::steady_clock::now();
+        const uint32_t per = (uint32_t)std::max<uint64_t>(1, std::min<uint64_t>(S, PAIRS_PER_CALL / std::max<uint64_t>(G, 1)));
+        int rc = SYL_OK;
+        for (uint32_t s0 = 0; s0 < S && rc == SYL_OK; s0 += per) {
+            std::vector<syl_ani_row> part;
+            rc = contain_fast(ctx, db, samples + s0, std::min(per, S - s0), p, false, part);
+            for (syl_ani_row &r : part) {
+                r.sample += s0;
+                rows.push_back(r);
+            }
+        }
+        static const bool dbg = getenv("SYL_DEBUG_TIMING") != nullptr;
+        if (dbg)
+            fprintf(stderr, "[db shard %zu/%zu] genomes %llu+%llu entries %llu: build %.1f ms, pass 1 %.1f ms\n", i + 1,
+                    s->first.size() - 1, (unsigned long long)a, (unsigned long long)G, (unsigned long long)db->N, build_ms, ms_since(t1));
+        syl_db_free(db);
+        SYL_TRY(rc);
+    }
+    return cache_trim(ctx);
+}
+
+// syl_profile of samples[s0, s1) on an index of the genomes `ids` (ascending global indices), gathered from the
+// borrowed arrays into pinned staging; rows appended with global sample and genome indices.
+static int survivor_profile(syl_db_shards *s, const std::vector<uint32_t> &ids, const syl_sample *const *samples,
+                            uint32_t s0, uint32_t s1, const syl_contain_params *p, std::vector<syl_ani_row> &out) {
+    const auto t0 = std::chrono::steady_clock::now();
+    const uint64_t n = ids.size();
+    std::vector<uint64_t> ko(n + 1, 0), to(n + 1, 0), gsz(n, 0);
+    for (uint64_t i = 0; i < n; i++) {
+        const uint32_t g = ids[i];
+        ko[i + 1] = ko[i] + s->kmer_off[g + 1] - s->kmer_off[g];
+        to[i + 1] = to[i] + s->tracked_off[g + 1] - s->tracked_off[g];
+        if (s->gn_size) gsz[i] = s->gn_size[g];
+    }
+    const uint64_t nk = ko[n], nt = to[n];
+    if (nk + nt > s->pinned_n) {
+        if (s->pinned) cudaFreeHost(s->pinned);
+        s->pinned = nullptr;
+        s->pinned_n = 0;
+        SYL_CUDA(cudaHostAlloc((void **)&s->pinned, (nk + nt) * 8, cudaHostAllocDefault));
+        s->pinned_n = nk + nt;
+    }
+    for (uint64_t i = 0; i < n; i++) {
+        const uint32_t g = ids[i];
+        std::copy(s->kmers + s->kmer_off[g], s->kmers + s->kmer_off[g + 1], s->pinned + ko[i]);
+        std::copy(s->tracked + s->tracked_off[g], s->tracked + s->tracked_off[g + 1], s->pinned + nk + to[i]);
+    }
+    syl_db *db = nullptr;
+    SYL_TRY(syl_db_build_arrays(s->ctx, SYL_MEM_HOST, s->pinned, ko.data(), s->pinned + nk, to.data(), gsz.data(), n, s->k,
+                                s->c, 0, &db));
+    const double build_ms = ms_since(t0);
+    const auto t1 = std::chrono::steady_clock::now();
+    std::vector<syl_ani_row> part;
+    const int rc = contain_fast(s->ctx, db, samples + s0, s1 - s0, p, true, part);
+    syl_db_free(db);
+    SYL_TRY(rc);
+    static const bool dbg = getenv("SYL_DEBUG_TIMING") != nullptr;
+    if (dbg)
+        fprintf(stderr, "[survivor index] samples %u..%u genomes %llu entries %llu: gather+build %.1f ms, profile %.1f ms\n", s0, s1,
+                (unsigned long long)n, (unsigned long long)(nk + nt), build_ms, ms_since(t1));
+    for (syl_ani_row &r : part) {
+        r.sample += s0;
+        r.genome = ids[r.genome];
+        out.push_back(r);
+    }
+    return SYL_OK;
+}
+
+// Profile over all shards, equal to syl_profile on one db of every genome: the winner table, pass 2, derep and the
+// abundances only ever see pass-1 survivors (src/contain.rs:284-334, 410-430).  So pass 1 runs per shard, without CIs
+// (never reported; the ANI gate comes before the bootstrap), and each batch of samples is profiled on an index of the
+// union of its survivors.  Ascending global order keeps the winner table's lowest-index tie rule.  A batch closes when
+// the union would pass the shard cap; one sample's survivors alone may take up to survivor_max entries.
+static int shards_profile(syl_db_shards *s, const syl_sample *const *samples, uint32_t S, const syl_contain_params *p,
+                          std::vector<syl_ani_row> &out) {
+    syl_contain_params p1 = *p;
+    p1.no_ci = 1;
+    p1.estimate_unknown = 0;
+    p1.read_seq_id = -1.;
+    if (p1.minimum_ani < 0.) p1.minimum_ani = 95.;  // profile's gate in a query-mode pass (make_params)
+    std::vector<std::vector<uint32_t>> surv(S);
+    {
+        std::vector<syl_ani_row> rows1;
+        SYL_TRY(shards_sweep(s, samples, S, &p1, rows1));
+        for (const syl_ani_row &r : rows1) surv[r.sample].push_back(r.genome);
+    }
+    std::vector<uint8_t> in(s->G, 0);
+    std::vector<uint32_t> ids;
+    uint64_t entries = 0;
+    uint32_t s0 = 0;
+    auto flush = [&](uint32_t s1) -> int {
+        if (!ids.empty()) {
+            std::sort(ids.begin(), ids.end());
+            SYL_TRY(survivor_profile(s, ids, samples, s0, s1, p, out));
+            SYL_TRY(cache_trim(s->ctx));
+        }
+        for (uint32_t g : ids) in[g] = 0;
+        ids.clear();
+        entries = 0;
+        s0 = s1;
+        return SYL_OK;
+    };
+    for (uint32_t i = 0; i < S; i++) {
+        uint64_t own = 0, add = 0, addg = 0;
+        for (uint32_t g : surv[i]) {
+            const uint64_t e = genome_entries(s->kmer_off, s->tracked_off, g);
+            own += e;
+            if (!in[g]) { add += e; addg++; }
+        }
+        if (own > s->survivor_max) {
+            set_error("the pass-1 survivors of sample " + std::to_string(i) + " hold " + std::to_string(own) +
+                      " index entries, more than one survivor index takes (" + std::to_string(s->survivor_max) + ")");
+            return SYL_ERR_UNSUPPORTED;
+        }
+        const uint64_t ng = ids.size() + addg;
+        if (i > s0 && (entries + add > s->cap || ng > SHARD_MAX_GENOMES || (uint64_t)(i - s0 + 1) * ng > PAIRS_PER_CALL)) {
+            SYL_TRY(flush(i));
+            add = own;
+        }
+        for (uint32_t g : surv[i])
+            if (!in[g]) { in[g] = 1; ids.push_back(g); }
+        entries += add;
+    }
+    return flush(S);
+}
+
+// syl_query_shards / syl_profile_shards
+static int shards_call(syl_ctx *ctx, syl_db_shards *s, const syl_sample *const *samples, uint32_t n_samples,
+                       const syl_contain_params *p, bool profile, syl_ani_row *rows, uint64_t cap, uint64_t *n_rows) {
+    if (!s) { set_error("NULL argument"); return SYL_ERR_ARG; }
+    SYL_TRY(check_sample_args(ctx, s->k, s->c, samples, n_samples, p, rows, cap, n_rows));
+    if (ctx != s->ctx) { set_error("db shards used with another ctx than the one that created them"); return SYL_ERR_ARG; }
+    SYL_TRY(check_unknown_args(p));
+    *n_rows = 0;
+    if (profile && !s->tracked_off) {  // src/contain.rs:231-234
+        set_error("Attempting profiling, but the database was sketched with the --disable-profiling option");
+        return SYL_ERR_ARG;
+    }
+    SYL_CUDA(cudaSetDevice(ctx->device));
+    syl::tl_ctx = ctx;
+    const uint64_t call = ++s->calls;
+    auto &kp = s->kept;
+    const bool retry = kp.call && kp.call + 1 == call && kp.profile == profile && !memcmp(&kp.p, p, sizeof *p) &&
+                       kp.samples == std::vector<const syl_sample *>(samples, samples + n_samples);
+    std::vector<syl_ani_row> out;
+    if (retry) out.swap(kp.rows);
+    kp.call = 0;
+    std::vector<syl_ani_row>().swap(kp.rows);
+    kp.samples.clear();
+    if (!retry && s->G && n_samples) {
+        if (profile) {
+            SYL_TRY(shards_profile(s, samples, n_samples, p, out));
+        } else {
+            SYL_TRY(shards_sweep(s, samples, n_samples, p, out));
+            std::sort(out.begin(), out.end(), [](const syl_ani_row &a, const syl_ani_row &b) {
+                return a.sample != b.sample ? a.sample < b.sample : a.genome < b.genome;
+            });
+        }
+    }
+    *n_rows = out.size();
+    if (out.size() > cap) {
+        kp.call = call;
+        kp.profile = profile;
+        kp.p = *p;
+        kp.samples.assign(samples, samples + n_samples);
+        kp.rows.swap(out);
+        set_error("row buffer too small");
+        return SYL_ERR_CAPACITY;
+    }
+    std::copy(out.begin(), out.end(), rows);
+    return SYL_OK;
+}
+
+}  // namespace syl
+
 using namespace syl;
 
 extern "C" {
@@ -2017,6 +2290,82 @@ int syl_profile(syl_ctx *ctx, const syl_db *db, const syl_sample *const *samples
     if (out.size() > cap) { set_error("row buffer too small"); return SYL_ERR_CAPACITY; }
     std::copy(out.begin(), out.end(), rows);
     return SYL_OK;
+}
+
+int syl_db_shards_create(syl_ctx *ctx, const uint64_t *kmers, const uint64_t *kmer_off, const uint64_t *tracked,
+                         const uint64_t *tracked_off, const uint64_t *gn_size, uint64_t n_genomes, int k, uint64_t c,
+                         uint64_t max_entries, syl_db_shards **out) {
+    if (!ctx || !kmer_off || !out) { set_error("NULL argument"); return SYL_ERR_ARG; }
+    *out = nullptr;
+    if (n_genomes > 0xFFFFFFFFull) { set_error("more than 2^32 genomes: row.genome is 32 bits"); return SYL_ERR_ARG; }
+    SYL_CUDA(cudaSetDevice(ctx->device));
+    for (const uint64_t *a : {kmers, kmer_off, tracked, tracked_off, gn_size}) {  // the sweep reads them on the host
+        cudaPointerAttributes at{};
+        if (!a) continue;
+        if (cudaPointerGetAttributes(&at, a) != cudaSuccess) {
+            cudaGetLastError();
+            continue;
+        }
+        if (at.type == cudaMemoryTypeDevice) { set_error("db shards borrow host arrays; a device pointer was given"); return SYL_ERR_ARG; }
+    }
+    bool bad = false;
+    for (const uint64_t *o : {kmer_off, tracked_off}) {
+        if (!o) continue;
+        bad |= o[0] != 0;
+        for (uint64_t i = 1; i <= n_genomes && !bad; i++) bad = o[i] < o[i - 1];
+    }
+    if (bad) { set_error("offsets must start at 0 and be monotone"); return SYL_ERR_ARG; }
+    if (kmer_off[n_genomes] && !kmers) { set_error("kmer_off counts k-mers but kmers is NULL"); return SYL_ERR_ARG; }
+    if (tracked_off && tracked_off[n_genomes] && !tracked) { set_error("tracked_off counts tracked k-mers but tracked is NULL"); return SYL_ERR_ARG; }
+    uint64_t dflt = 0;
+    SYL_TRY(default_shard_entries(&dflt));
+    uint64_t cap = max_entries ? std::min(max_entries, SHARD_MAX_ENTRIES) : dflt;
+    if (const uint64_t e = shard_entries_env()) cap = std::min(cap, e);
+    std::vector<uint64_t> first;
+    uint64_t big = 0;
+    if (!cut_shards(kmer_off, tracked_off, n_genomes, cap, first, &big)) {
+        set_error("genome " + std::to_string(big) + " alone holds more than 2^32-3 index entries");
+        return SYL_ERR_ARG;
+    }
+    syl_db_shards *s = new (std::nothrow) syl_db_shards();
+    if (!s) return SYL_ERR_OOM;
+    s->ctx = ctx;
+    s->kmers = kmers; s->kmer_off = kmer_off; s->tracked = tracked; s->tracked_off = tracked_off; s->gn_size = gn_size;
+    s->G = n_genomes;
+    s->k = k;
+    s->c = c;
+    s->cap = cap;
+    s->survivor_max = std::max(cap, dflt);
+    s->first.swap(first);
+    *out = s;
+    return SYL_OK;
+}
+
+uint64_t syl_db_shards_count(const syl_db_shards *s) { return s && !s->first.empty() ? s->first.size() - 1 : 0; }
+
+int syl_db_shards_range(const syl_db_shards *s, uint64_t i, uint64_t *first_genome, uint64_t *n_genomes, uint64_t *n_entries) {
+    if (!s || i >= syl_db_shards_count(s)) { set_error("NULL handle or shard index out of range"); return SYL_ERR_ARG; }
+    const uint64_t a = s->first[i], b = s->first[i + 1];
+    if (first_genome) *first_genome = a;
+    if (n_genomes) *n_genomes = b - a;
+    if (n_entries) *n_entries = s->kmer_off[b] - s->kmer_off[a] + (s->tracked_off ? s->tracked_off[b] - s->tracked_off[a] : 0);
+    return SYL_OK;
+}
+
+int syl_query_shards(syl_ctx *ctx, syl_db_shards *s, const syl_sample *const *samples, uint32_t n_samples,
+                     const syl_contain_params *p, syl_ani_row *rows, uint64_t cap, uint64_t *n_rows) {
+    return shards_call(ctx, s, samples, n_samples, p, false, rows, cap, n_rows);
+}
+
+int syl_profile_shards(syl_ctx *ctx, syl_db_shards *s, const syl_sample *const *samples, uint32_t n_samples,
+                       const syl_contain_params *p, syl_ani_row *rows, uint64_t cap, uint64_t *n_rows) {
+    return shards_call(ctx, s, samples, n_samples, p, true, rows, cap, n_rows);
+}
+
+void syl_db_shards_free(syl_db_shards *s) {
+    if (!s) return;
+    if (s->pinned) cudaFreeHost(s->pinned);
+    delete s;
 }
 
 }  // extern "C"
