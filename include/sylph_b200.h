@@ -85,7 +85,7 @@ int syl_ctx_seed_kernel_time(syl_ctx *ctx, double *total_ms, uint64_t *launches,
 enum {
     SYL_KERNEL_SEED = 0,        /* k_seed (all variants) */
     SYL_KERNEL_GROUP_DEDUP = 1, /* read-sketch post-pass: k_group_dedup */
-    SYL_KERNEL_JOIN = 2,        /* containment pass 1: k_join_hist (+ k_range_bounds, CSR formulation: k_join_csr) */
+    SYL_KERNEL_JOIN = 2,        /* containment pass 1: k_join_hist (+ k_range_bounds, CSR formulation: k_join2_order) */
     SYL_KERNEL_JOIN2 = 3,       /* containment pass 2: k_join2_order (+ k_local_best when sharded) */
     SYL_KERNEL_STATS = 4,       /* k_stats_hist / k_stats */
     SYL_KERNEL_BOOT = 5,        /* bootstrap: k_boot_iter_p (+ k_boot_seq, k_boot_final) */

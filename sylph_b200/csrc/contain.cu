@@ -490,10 +490,11 @@ __global__ void k_range_bounds(const SampleView *__restrict__ views, uint32_t S,
     rb[t] = (uint32_t)lo;
 }
 
-// Pass 1, histogram formulation: the genome ids of one k-mer's equal range [lo, e) -> count histograms of one sample.
-__device__ __forceinline__ void join_range(const uint32_t *__restrict__ gid, uint32_t lo, uint32_t e, uint32_t c,
-                                           uint8_t *__restrict__ touched, uint32_t *__restrict__ chist,
-                                           unsigned long long *__restrict__ ovf) {
+// f(g) for the genome index g of every entry of one k-mer's equal range [lo, e) of the db index.  Tracked entries
+// only take part in pass 2's winner decision, so they are skipped unless TRACKED.  The genome ids are loaded four at
+// a time: a long range walked one dependent load at a time holds its whole warp for range x DRAM latency.
+template <bool TRACKED = false, class F>
+__device__ __forceinline__ void walk_range(const uint32_t *__restrict__ gid, uint32_t lo, uint32_t e, F f) {
     for (uint32_t j = lo; j < e; j += 4) {
         uint32_t gq[4];
 #pragma unroll
@@ -501,18 +502,34 @@ __device__ __forceinline__ void join_range(const uint32_t *__restrict__ gid, uin
 #pragma unroll
         for (int q = 0; q < 4; q++) {
             if (j + q >= e) continue;
-            const uint32_t gv = gq[q];
-            if (gv & 1u) continue;  // tracked k-mers only take part in the winner decision
-            const uint32_t g = gv >> 1;
-            // no per-genome hit counter: the sample's k-mers concentrate on the few genomes that are
-            // present, and a million atomics on a handful of adjacent counters serialise in one L2
-            // slice (measured: 2/3 of this kernel's time).  The hit count is the histogram's total.
-            if (!touched[g]) touched[g] = 1;
-            if (c < COV_BINS) atomicAdd(&chist[(uint64_t)g * COV_BINS + c], 1u);
-            else atomicAdd(ovf, 1ull);
+            if (!TRACKED && (gq[q] & 1u)) continue;
+            f(gq[q] >> 1);
         }
     }
 }
+
+// What a walk produces: count histograms (JOIN_HIST), or the CSR formulation's count walk (cnt) or fill walk (covs).
+enum JoinOut { JOIN_HIST, JOIN_CSR_COUNT, JOIN_CSR_FILL };
+
+// Where the hits of a walk go, per (sample, genome) pair.  Histogram formulation: touched and the count histograms,
+// values >= COV_BINS only counted in ovf.  CSR formulation: the count walk adds up the hits per pair in cnt; after
+// the scan of cnt into off, the fill walk writes each hit's sample count to covs[off[pair] + cursor[pair]++].
+struct PairOut {
+    uint8_t *touched; uint32_t *chist; unsigned long long *ovf;
+    uint32_t *cnt; const uint64_t *off; uint32_t *cursor; uint32_t *covs;
+
+    template <JoinOut OUT>
+    __device__ __forceinline__ void hit(uint64_t pair, uint32_t c) const {
+        if (OUT == JOIN_CSR_COUNT) { atomicAdd(&cnt[pair], 1u); return; }
+        if (OUT == JOIN_CSR_FILL) { covs[off[pair] + atomicAdd(&cursor[pair], 1u)] = c; return; }
+        // no per-genome hit counter: the sample's k-mers concentrate on the few genomes that are
+        // present, and a million atomics on a handful of adjacent counters serialise in one L2
+        // slice (measured: 2/3 of the pass-1 join's time).  The hit count is the histogram's total.
+        if (!touched[pair]) touched[pair] = 1;
+        if (c < COV_BINS) atomicAdd(&chist[pair * COV_BINS + c], 1u);
+        else atomicAdd(ovf, 1ull);
+    }
+};
 
 // Pass-1 probe: every sample key looks up its equal range in the db index and records it in `hits` (for pass 2 and,
 // in the CSR formulation, for pass 1's count / fill walks).  PROBE_ONLY == false also accumulates the count histograms.
@@ -520,8 +537,7 @@ template <bool PROBE_ONLY>
 __global__ void k_join_hist(const SampleView *__restrict__ views, uint64_t G,
                             const uint64_t *__restrict__ keys, const uint32_t *__restrict__ gid, uint64_t N,
                             const uint32_t *__restrict__ bstart, uint64_t M, uint64_t NB, uint64_t maxkey,
-                            uint8_t *__restrict__ touched, uint32_t *__restrict__ chist,
-                            unsigned long long *__restrict__ ovf, uint2 *__restrict__ hits, uint64_t hits_stride, const KeyMap km) {
+                            const PairOut out, uint2 *__restrict__ hits, uint64_t hits_stride, const KeyMap km) {
   for_each_key(km, views, [&](const uint32_t smp, const uint64_t i) {
     const SampleView sv = views[smp];
     const uint64_t key = sv.hash[i];
@@ -561,7 +577,7 @@ __global__ void k_join_hist(const SampleView *__restrict__ views, uint64_t G,
     if (hits) hits[(uint64_t)smp * hits_stride + i] = make_uint2(lo, e - lo);  // equal range in the db
     if (!PROBE_ONLY) {
         const uint64_t row = (uint64_t)smp * G;
-        join_range(gid, lo, e, c, touched + row, chist + row * COV_BINS, ovf);
+        walk_range(gid, lo, e, [&](const uint32_t g) { out.hit<JOIN_HIST>(row + g, c); });
     }
   });
 }
@@ -915,11 +931,11 @@ static StatParams make_params(const syl_contain_params *p) {
 // Single GPU: the winner minimum is taken inside k_join2_order and nothing is gathered.  A coverage
 // count >= COV_BINS or more rows than the table holds is reported in the header; contain_fast then
 // redoes the call in the CSR formulation or with a larger table.
-// CSR formulation (single GPU only): k_join_hist<probe only> records the equal ranges, k_join_csr /
-// k_join2_order<.., CSR_*> walk them twice per pass (count hits per pair, CUB scan, scatter the hits'
-// sample counts) and k_stats replaces k_stats_hist; ranking, bootstrap and finish are shared.  Sizing
-// the value array after the pass-1 scan costs a second host synchronisation; pass 2 needs none, because
-// its hits are a subset of pass 1's (same ranges, winners only).
+// CSR formulation (single GPU only): k_join_hist<probe only> records the equal ranges and
+// k_join2_order<.., CSR_*> walks them twice per pass (count hits per pair, CUB scan, scatter the hits'
+// sample counts), with no winner in pass 1; k_stats replaces k_stats_hist; ranking, bootstrap and finish
+// are shared.  Sizing the value array after the pass-1 scan costs a second host synchronisation; pass 2
+// needs none, because its hits are a subset of pass 1's (same ranges, winners only).
 constexpr uint32_t ORD_NONE = 0x7F7F7F7Fu;  // memset-able; valid as int32 for the MIN all-reduce
 
 struct ShardTable { unsigned long long n_rows, n_boot, ovf, pad; };
@@ -969,98 +985,56 @@ k_rank_rows(const uint8_t *__restrict__ tabs, uint64_t tbytes, uint32_t world, u
     if (valid && mr == rank) order_tbl[(uint64_t)ms * G + (mg - genome_base)] = ord;
 }
 
-// per sample key: smallest order among the survivor genomes of its equal range in this shard (kept and
-// tracked k-mers both count, src/contain.rs:416-426)
+// smallest order (in the sample's row `ord` of the order table) among the genomes of the equal range [lo, e); kept
+// and tracked k-mers both count (src/contain.rs:416-426)
+__device__ __forceinline__ uint32_t range_winner(const uint32_t *__restrict__ gid, const uint32_t *__restrict__ ord, uint32_t lo,
+                                                 uint32_t e) {
+    uint32_t winner = ORD_NONE;
+    walk_range<true>(gid, lo, e, [&](const uint32_t g) { winner = min(winner, ord[g]); });
+    return winner;
+}
+
+// per sample key: the winner of its equal range in this shard
 __global__ void k_local_best(const SampleView *__restrict__ views, uint64_t G, const uint32_t *__restrict__ gid,
                              const uint2 *__restrict__ hits, uint64_t hits_stride, const uint32_t *__restrict__ order_tbl,
                              uint32_t *__restrict__ wbest, const KeyMap km) {
   for_each_key(km, views, [&](const uint32_t smp, const uint64_t i) {
     const uint2 h = hits[(uint64_t)smp * hits_stride + i];
-    uint32_t best = ORD_NONE;
-    const uint32_t *ord = order_tbl + (uint64_t)smp * G;
-    for (uint32_t j = h.x; j < h.x + h.y; j++) best = min(best, ord[gid[j] >> 1]);
-    wbest[(uint64_t)smp * hits_stride + i] = best;
+    wbest[(uint64_t)smp * hits_stride + i] = range_winner(gid, order_tbl + (uint64_t)smp * G, h.x, h.x + h.y);
   });
 }
 
-// CSR formulation of a pass: the count walk adds up the hits per pair in cnt; after the scan of cnt into off, the
-// fill walk writes each hit's sample count to covs[off[pair] + cursor[pair]++].
-struct CsrBufs { uint32_t *cnt; const uint64_t *off; uint32_t *cursor; uint32_t *covs; };
+// Which hits of a walk count.  WIN_NONE (pass 1): every kept hit.  Pass 2: only the winner's, and every other pass-1
+// survivor of the range loses the k-mer; the winner is the range's smallest order (WIN_FUSED, single GPU) or comes
+// from wbest, all-reduced over the shards (WIN_GIVEN).
+enum Winner { WIN_NONE, WIN_FUSED, WIN_GIVEN };
 
-template <bool FILL>
-__device__ __forceinline__ void csr_hit(const CsrBufs &b, uint64_t pair, uint32_t c) {
-    if (FILL) b.covs[b.off[pair] + atomicAdd(&b.cursor[pair], 1u)] = c;
-    else atomicAdd(&b.cnt[pair], 1u);
-}
-
-// pass 1 of the CSR formulation over the equal ranges recorded by k_join_hist<true>: every genome_kmers hit counts
-template <bool FILL>
-__global__ void k_join_csr(const SampleView *__restrict__ views, uint64_t G, const uint32_t *__restrict__ gid,
-                           const uint2 *__restrict__ hits, uint64_t hits_stride, const CsrBufs csr, const KeyMap km) {
-  for_each_key(km, views, [&](const uint32_t smp, const uint64_t i) {
-    const uint2 h = hits[(uint64_t)smp * hits_stride + i];
-    const uint64_t row = (uint64_t)smp * G;
-    const uint32_t c = views[smp].count[i];
-    for (uint32_t j = h.x; j < h.x + h.y; j++) {
-        const uint32_t gv = gid[j];
-        if (!(gv & 1u)) csr_hit<FILL>(csr, row + (gv >> 1), c);  // tracked k-mers only take part in pass 2's winner decision
-    }
-  });
-}
-
-// What a pass-2 walk produces: count histograms (touched / chist / ovf), or the CSR formulation's count walk
-// (cnt, and lost) or fill walk (covs).
-enum JoinOut { JOIN_HIST, JOIN_CSR_COUNT, JOIN_CSR_FILL };
-
-// pass 2 over the equal ranges recorded by pass 1.  FUSED: the winner (smallest order in the range) is
-// taken here (single GPU); else it comes from wbest (all-reduced over the shards).
-template <bool FUSED, JoinOut OUT = JOIN_HIST>
+// a walk over the equal ranges recorded by k_join_hist
+template <Winner W, JoinOut OUT>
 __global__ void k_join2_order(const SampleView *__restrict__ views, uint64_t G, const uint32_t *__restrict__ gid,
                               const uint2 *__restrict__ hits, uint64_t hits_stride, const uint32_t *__restrict__ order_tbl,
-                              const uint32_t *__restrict__ wbest, uint8_t *__restrict__ touched, uint32_t *__restrict__ lost,
-                              uint32_t *__restrict__ chist, unsigned long long *__restrict__ ovf, const CsrBufs csr, const KeyMap km) {
+                              const uint32_t *__restrict__ wbest, uint32_t *__restrict__ lost, const PairOut out, const KeyMap km) {
   for_each_key(km, views, [&](const uint32_t smp, const uint64_t i) {
     const uint2 h = hits[(uint64_t)smp * hits_stride + i];
     if (h.y == 0) return;
     const uint64_t row = (uint64_t)smp * G;
-    const uint32_t *ord = order_tbl + row;
+    const uint32_t *ord = W == WIN_NONE ? nullptr : order_tbl + row;
     const uint32_t lo = h.x, e = h.x + h.y, c = views[smp].count[i];
-    uint32_t winner;
-    if (FUSED) {
-        winner = ORD_NONE;
-        for (uint32_t j = lo; j < e; j += 4) {
-            uint32_t gq[4];
-#pragma unroll
-            for (int q = 0; q < 4; q++) gq[q] = j + q < e ? gid[j + q] : 0xFFFFFFFFu;
-#pragma unroll
-            for (int q = 0; q < 4; q++) if (j + q < e) winner = min(winner, ord[gq[q] >> 1]);
-        }
-    } else {
-        winner = wbest[(uint64_t)smp * hits_stride + i];
-    }
-    if (winner == ORD_NONE) return;  // no survivor holds this k-mer
-    for (uint32_t j = lo; j < e; j += 4) {
-        uint32_t gq[4];
-#pragma unroll
-        for (int q = 0; q < 4; q++) gq[q] = j + q < e ? gid[j + q] : 0xFFFFFFFFu;
-#pragma unroll
-        for (int q = 0; q < 4; q++) {
-            if (j + q >= e) continue;
-            const uint32_t gv = gq[q];
-            if (gv & 1u) continue;  // tracked k-mers only take part in the winner decision
-            const uint32_t g = gv >> 1;
+    uint32_t winner = ORD_NONE;
+    if (W == WIN_FUSED) winner = range_winner(gid, ord, lo, e);
+    if (W == WIN_GIVEN) winner = wbest[(uint64_t)smp * hits_stride + i];
+    if (W != WIN_NONE && winner == ORD_NONE) return;  // no survivor holds this k-mer
+    walk_range(gid, lo, e, [&](const uint32_t g) {
+        if (W != WIN_NONE) {
             const uint32_t o = ord[g];
-            if (o == ORD_NONE) continue;                       // not a pass-1 survivor
-            if (o != winner) {                                 // src/contain.rs:641-646
+            if (o == ORD_NONE) return;                 // not a pass-1 survivor
+            if (o != winner) {                         // src/contain.rs:641-646
                 if (OUT != JOIN_CSR_FILL) atomicAdd(&lost[row + g], 1u);
-                continue;
+                return;
             }
-            if (OUT != JOIN_HIST) { csr_hit<OUT == JOIN_CSR_FILL>(csr, row + g, c); continue; }
-            if (!touched[row + g]) touched[row + g] = 1;
-            if (c < COV_BINS) atomicAdd(&chist[(row + g) * COV_BINS + c], 1u);
-            else atomicAdd(ovf, 1ull);
         }
-    }
+        out.hit<OUT>(row + g, c);
+    });
   });
 }
 
@@ -1154,43 +1128,60 @@ static uint64_t default_rows_per_rank(uint32_t S, uint64_t G, uint32_t world) {
 
 static bool histograms_fit(uint64_t n_pairs) { return n_pairs * COV_BINS * 4 <= (8ull << 30); }
 
+// the per-pair outputs of pass 1 or 2 (the overflow counter is in that pass's row table)
+static PairOut pair_out(const syl_profile_job *j, bool pass2) {
+    ShardTable *t = reinterpret_cast<ShardTable *>(pass2 ? j->tab2.p : j->tab1.p);
+    return PairOut{j->touched.p, j->chist.p, &t->ovf, j->cnt.p, j->off.p, j->cursor.p, j->covs.p};
+}
+
+// zeroes the per-pair buffers that a pass adds into
+static int clear_pairs(syl_profile_job *j) {
+    cudaStream_t st = j->ctx->stream;
+    const uint64_t NP = (uint64_t)j->S * j->G;
+    if (j->csr) {
+        SYL_CUDA(cudaMemsetAsync(j->cnt.p, 0, (NP + 1) * 4, st));  // cnt[NP] = 0: off[NP] is the total
+        SYL_CUDA(cudaMemsetAsync(j->cursor.p, 0, NP * 4, st));
+    } else {
+        SYL_CUDA(cudaMemsetAsync(j->touched.p, 0, NP, st));
+        SYL_CUDA(cudaMemsetAsync(j->chist.p, 0, NP * COV_BINS * 4, st));
+    }
+    return SYL_OK;
+}
+
+// One walk over the equal ranges in j->hits into OUT.  Pass 1 walks only in the CSR formulation (the histogram one
+// accumulates inside the probe) and counts every kept hit.  Pass 2 counts the winner's hits, with the winner taken in
+// the walk on one GPU and from the all-reduced wbest across ranks (histogram formulation only).
+template <JoinOut OUT>
+static void join_walk(syl_profile_job *j, bool pass2) {
+    const syl_db *db = j->db;
+    if (!j->max_n || !db->N) return;
+    auto k = k_join2_order<WIN_FUSED, OUT>;
+    if constexpr (OUT == JOIN_HIST) {
+        if (j->world > 1) k = k_join2_order<WIN_GIVEN, OUT>;
+    } else {
+        if (!pass2) k = k_join2_order<WIN_NONE, OUT>;
+    }
+    KernelTimer kt(j->ctx, pass2 ? SYL_KERNEL_JOIN2 : SYL_KERNEL_JOIN);
+    k<<<j->jgrid, 128, 0, j->ctx->stream>>>(j->views.p, j->G, db->gid, j->hits.p, j->max_n, j->order.p, j->wbest.p, j->lost.p,
+                                            pair_out(j, pass2), j->km);
+    j->ctx->launches++;
+}
+
 // CSR formulation of one pass over the equal ranges in j->hits: count walk, scan, fill walk.  Pass 1 sizes covs,
 // which needs a host synchronisation; pass 2's hits are a subset of pass 1's, so that size bounds them as well.
 static int csr_walks(syl_profile_job *j, bool pass2) {
     syl_ctx *ctx = j->ctx;
     cudaStream_t st = ctx->stream;
-    const syl_db *db = j->db;
     const uint64_t NP = (uint64_t)j->S * j->G;
-    const bool walk = j->max_n && db->N;
-    SYL_CUDA(cudaMemsetAsync(j->cnt.p, 0, (NP + 1) * 4, st));  // cnt[NP] = 0: off[NP] is the total
-    SYL_CUDA(cudaMemsetAsync(j->cursor.p, 0, NP * 4, st));
-    CsrBufs b{j->cnt.p, j->off.p, j->cursor.p, j->covs.p};
-    if (walk) {
-        KernelTimer kt(ctx, pass2 ? SYL_KERNEL_JOIN2 : SYL_KERNEL_JOIN);
-        if (pass2)
-            k_join2_order<true, JOIN_CSR_COUNT><<<j->jgrid, 128, 0, st>>>(j->views.p, j->G, db->gid, j->hits.p, j->max_n, j->order.p, nullptr,
-                                                                          nullptr, j->lost.p, nullptr, nullptr, b, j->km);
-        else
-            k_join_csr<false><<<j->jgrid, 128, 0, st>>>(j->views.p, j->G, db->gid, j->hits.p, j->max_n, b, j->km);
-        ctx->launches++;
-    }
+    join_walk<JOIN_CSR_COUNT>(j, pass2);
     size_t tb = j->scan_bytes;
     SYL_CUDA(cub::DeviceScan::ExclusiveSum(j->scan_tmp.p, tb, j->cnt.p, j->off.p, (int)(NP + 1), st));
     if (!pass2) {
         SYL_CUDA(cudaMemcpyAsync(ctx->h_counters + 10, j->off.p + NP, 8, cudaMemcpyDeviceToHost, st));
         SYL_CUDA(cudaStreamSynchronize(st));
         SYL_TRY(j->covs.alloc(std::max<uint64_t>(ctx->h_counters[10], 1), st));
-        b.covs = j->covs.p;
     }
-    if (walk) {
-        KernelTimer kt(ctx, pass2 ? SYL_KERNEL_JOIN2 : SYL_KERNEL_JOIN);
-        if (pass2)
-            k_join2_order<true, JOIN_CSR_FILL><<<j->jgrid, 128, 0, st>>>(j->views.p, j->G, db->gid, j->hits.p, j->max_n, j->order.p, nullptr,
-                                                                         nullptr, j->lost.p, nullptr, nullptr, b, j->km);
-        else
-            k_join_csr<true><<<j->jgrid, 128, 0, st>>>(j->views.p, j->G, db->gid, j->hits.p, j->max_n, b, j->km);
-        ctx->launches++;
-    }
+    join_walk<JOIN_CSR_FILL>(j, pass2);
     SYL_CUDA(cudaGetLastError());
     return SYL_OK;
 }
@@ -1269,13 +1260,9 @@ static int job_begin(syl_ctx *ctx, const syl_db *db, const syl_sample *const *sa
     // a pageable source is staged by the driver before cudaMemcpyAsync returns: hv may go out of scope
     JOB_CUDA(cudaMemcpyAsync(j->views.p, hv.data(), n_samples * sizeof(SampleView), cudaMemcpyHostToDevice, st));
     if (profile && j->G) JOB_CUDA(cudaMemcpyAsync(j->gn_size.p, db->h_gn_size.data(), j->G * 8, cudaMemcpyHostToDevice, st));
-    if (!csr) {
-        JOB_CUDA(cudaMemsetAsync(j->touched.p, 0, NP, st));
-        JOB_CUDA(cudaMemsetAsync(j->chist.p, 0, NP * COV_BINS * 4, st));
-    }
+    JOB_TRY(clear_pairs(j));
     JOB_CUDA(cudaMemsetAsync(j->hits.p, 0, HN * sizeof(uint2), st));
     JOB_CUDA(cudaMemsetAsync(j->tab1.p, 0, sizeof(ShardTable), st));
-    ShardTable *t1 = reinterpret_cast<ShardTable *>(j->tab1.p);
     j->jgrid = dim3(nblk(std::max<uint64_t>(j->max_n, 1), 128), (unsigned)j->S);
     static const bool tile_env_off = getenv("SYL_JOIN_PLAIN") != nullptr;
     if (j->S > 1 && j->max_n && db->N && !tile_env_off) {
@@ -1291,15 +1278,11 @@ static int job_begin(syl_ctx *ctx, const syl_db *db, const syl_sample *const *sa
             j->jgrid = dim3((unsigned)(R * j->S), 1);
         }
     }
-    const dim3 jgrid = j->jgrid;
     if (j->max_n && db->N) {
         KernelTimer kt(ctx, SYL_KERNEL_JOIN);
-        if (csr)
-            k_join_hist<true><<<jgrid, 128, 0, st>>>(j->views.p, j->G, db->keys, db->gid, db->N, db->bstart, db->M, db->NB, db->maxkey,
-                                                     nullptr, nullptr, nullptr, j->hits.p, j->max_n, j->km);
-        else
-            k_join_hist<false><<<jgrid, 128, 0, st>>>(j->views.p, j->G, db->keys, db->gid, db->N, db->bstart, db->M, db->NB, db->maxkey,
-                                                      j->touched.p, j->chist.p, &t1->ovf, j->hits.p, j->max_n, j->km);
+        const auto probe = csr ? k_join_hist<true> : k_join_hist<false>;
+        probe<<<j->jgrid, 128, 0, st>>>(j->views.p, j->G, db->keys, db->gid, db->N, db->bstart, db->M, db->NB, db->maxkey,
+                                        pair_out(j, false), j->hits.p, j->max_n, j->km);
         ctx->launches++;
     }
     if (csr) JOB_TRY(csr_walks(j, false));
@@ -1360,29 +1343,12 @@ static int job_rank(syl_profile_job *j) {
 static int job_pass2(syl_profile_job *j) {
     syl_ctx *ctx = j->ctx;
     cudaStream_t st = ctx->stream;
-    const syl_db *db = j->db;
     const uint64_t NP = (uint64_t)j->S * j->G;
-    ShardTable *t2 = reinterpret_cast<ShardTable *>(j->tab2.p);
     SYL_CUDA(cudaMemsetAsync(j->lost.p, 0, NP * 4, st));
     SYL_CUDA(cudaMemsetAsync(j->tab2.p, 0, sizeof(ShardTable), st));
-    if (j->csr) {
-        SYL_TRY(csr_walks(j, true));
-    } else {
-        SYL_CUDA(cudaMemsetAsync(j->touched.p, 0, NP, st));
-        SYL_CUDA(cudaMemsetAsync(j->chist.p, 0, NP * COV_BINS * 4, st));
-        const dim3 jgrid = j->jgrid;
-        const CsrBufs no_csr{nullptr, nullptr, nullptr, nullptr};
-        if (j->max_n && db->N) {
-            KernelTimer kt(ctx, SYL_KERNEL_JOIN2);
-            if (j->world > 1)
-                k_join2_order<false><<<jgrid, 128, 0, st>>>(j->views.p, j->G, db->gid, j->hits.p, j->max_n, j->order.p, j->wbest.p, j->touched.p,
-                                                            j->lost.p, j->chist.p, &t2->ovf, no_csr, j->km);
-            else
-                k_join2_order<true><<<jgrid, 128, 0, st>>>(j->views.p, j->G, db->gid, j->hits.p, j->max_n, j->order.p, nullptr, j->touched.p,
-                                                           j->lost.p, j->chist.p, &t2->ovf, no_csr, j->km);
-            ctx->launches++;
-        }
-    }
+    SYL_TRY(clear_pairs(j));
+    if (j->csr) SYL_TRY(csr_walks(j, true));
+    else join_walk<JOIN_HIST>(j, true);
     StatExtra X;
     X.pair_stride = j->G;
     X.contain1_in = j->contain1.p;
