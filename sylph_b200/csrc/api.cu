@@ -104,8 +104,8 @@ int syl_ctx_create(int device, void *stream, syl_ctx **out) {
         uint64_t thresh = UINT64_MAX;
         cudaMemPoolSetAttribute(pool, cudaMemPoolAttrReleaseThreshold, &thresh);
     }
-    if (cudaMalloc((void **)&ctx->d_counters, 32 * sizeof(uint64_t)) != cudaSuccess ||
-        cudaMallocHost((void **)&ctx->h_counters, 32 * sizeof(uint64_t)) != cudaSuccess) {
+    if (cudaMalloc((void **)&ctx->d_counters, CNT_SLOTS * sizeof(uint64_t)) != cudaSuccess ||
+        cudaMallocHost((void **)&ctx->h_counters, CNT_SLOTS * sizeof(uint64_t)) != cudaSuccess) {
         set_error("ctx scratch allocation failed");
         syl_ctx_destroy(ctx);
         return SYL_ERR_OOM;
@@ -156,15 +156,14 @@ int syl_ctx_device_bytes(syl_ctx *ctx, uint64_t *held, uint64_t *peak, int reset
 
 int syl_ctx_enable_timing(syl_ctx *ctx, int on) {
     if (!ctx) { set_error("ctx is NULL"); return SYL_ERR_ARG; }
-    SYL_CUDA(cudaSetDevice(ctx->device));
-    syl::tl_ctx = ctx;
+    SYL_ENTER(ctx);
     ctx->timing = on != 0;
     return SYL_OK;
 }
 
 // resolve the recorded event pairs into the per-kernel totals (the stream must be idle)
 static int timers_resolve(syl_ctx *ctx) {
-    SYL_CUDA(cudaSetDevice(ctx->device));
+    SYL_ENTER(ctx);
     if (ctx->timed_pending.empty()) return SYL_OK;
     SYL_CUDA(cudaStreamSynchronize(ctx->stream));
     for (auto &t : ctx->timed_pending) {
@@ -203,8 +202,7 @@ static int seed_batch_impl(syl_ctx *ctx, int mem, const uint8_t *bases, const ui
         set_error("NULL argument");
         return SYL_ERR_ARG;
     }
-    SYL_CUDA(cudaSetDevice(ctx->device));
-    syl::tl_ctx = ctx;
+    SYL_ENTER(ctx);
     *n_out = 0;
     cudaStream_t st = ctx->stream;
     Staged<uint8_t> sb;
@@ -224,11 +222,11 @@ static int seed_batch_impl(syl_ctx *ctx, int mem, const uint8_t *bases, const ui
     job.d_rec_off = so.p; job.off_bias = 0; job.n_rec = n_rec; job.k = k; job.c = c; job.sem = sem; job.with_pos = with_pos;
     job.d_out = dst; job.cap = cap;
     job.d_count = reinterpret_cast<unsigned long long *>(ctx->d_counters);
-    SYL_CUDA(cudaMemsetAsync(ctx->d_counters, 0, 2 * sizeof(uint64_t), st));
+    SYL_CUDA(cudaMemsetAsync(ctx->d_counters, 0, 2 * sizeof(uint64_t), st));  // CNT_EVENTS, CNT_PENDING
     SYL_TRY(seed_enqueue(ctx, job));
-    SYL_CUDA(cudaMemcpyAsync(ctx->h_counters, ctx->d_counters, sizeof(uint64_t), cudaMemcpyDeviceToHost, st));
+    SYL_CUDA(cudaMemcpyAsync(ctx->h_counters + CNT_EVENTS, ctx->d_counters + CNT_EVENTS, 8, cudaMemcpyDeviceToHost, st));
     SYL_CUDA(cudaStreamSynchronize(st));
-    *n_out = ctx->h_counters[0];
+    *n_out = ctx->h_counters[CNT_EVENTS];
     if (*n_out > cap) { set_error("survivor buffer too small"); return SYL_ERR_CAPACITY; }
     if (mem != SYL_MEM_DEVICE && *n_out) {
         SYL_CUDA(cudaMemcpyAsync(out, d_out.p, *n_out * sizeof(syl_survivor), cudaMemcpyDeviceToHost, st));

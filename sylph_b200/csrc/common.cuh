@@ -7,6 +7,8 @@
 #include <stdint.h>
 #include <stdio.h>
 
+#include <memory>
+#include <new>
 #include <string>
 #include <unordered_map>
 #include <utility>
@@ -18,12 +20,6 @@ namespace syl {
 
 // ---- error plumbing -------------------------------------------------------------------------
 void set_error(const std::string &msg);
-
-struct Status {
-    int code;
-    Status(int c = SYL_OK) : code(c) {}
-    bool ok() const { return code == SYL_OK; }
-};
 
 #define SYL_CUDA(call)                                                                           \
     do {                                                                                         \
@@ -41,6 +37,13 @@ struct Status {
         if (_s != SYL_OK) return _s;                                                             \
     } while (0)
 
+// Entry of an API call on ctx: its device becomes current and DevBuf draws from its block cache.
+#define SYL_ENTER(ctx)                                                                           \
+    do {                                                                                         \
+        SYL_CUDA(cudaSetDevice(ctx->device));                                                    \
+        ::syl::tl_ctx = ctx;                                                                     \
+    } while (0)
+
 // ---- context --------------------------------------------------------------------------------
 }  // namespace syl
 
@@ -50,7 +53,7 @@ struct syl_ctx {
     bool own_stream = false;
     int num_sms = 132;
     uint64_t launches = 0;
-    // small persistent scratch: device counters + pinned host mirror
+    // small persistent scratch: device counters + pinned host mirror, slots named by syl::CounterSlot
     uint64_t *d_counters = nullptr;  // 32 x u64
     uint64_t *h_counters = nullptr;  // pinned
     // optional per-kernel timing (syl_ctx_enable_timing): every timed launch is bracketed by a pair of
@@ -142,6 +145,60 @@ struct syl_genomes {
 };
 
 namespace syl {
+
+// Slots of ctx->d_counters / h_counters, in slot order.  Two users of one slot never run within one call.
+constexpr int CNT_SLOTS = 32;
+enum CounterSlot : int {
+    CNT_EVENTS = 0,          // seeding: survivors, or events in the overflow list (SeedJob::d_count[0])
+    CNT_PENDING = 1,         // seeding: pending events (SeedJob::d_count[1]); the generic dedup's run count
+    CNT_DUPS = 2,            // read sketch: duplicates removed
+    CNT_PEND_MATE1 = 3,      // read sketch: CNT_PENDING before mate 1 of a batch
+    CNT_UNIQ_TOTAL = 4,      // read sketch: in-kernel uniques (u32)
+    CNT_BACK_HALF = 4,       // genome back half: N, kept, tracked, slot overflow as four u32 over slots 4 and 5
+    CNT_FALLBACK_TOTAL = 5,  // read sketch: events of the fallback groups (u32)
+    CNT_KMER_TOTAL = 8,      // last k-mer offset of device CSR input
+    CNT_TRACKED_TOTAL = 9,   // last tracked offset of device CSR input
+    CNT_BAD_OFFSETS = 10,    // index build: device offsets that do not start at 0 or decrease
+    CNT_COVS_TOTAL = 10,     // CSR formulation: coverage entries of pass 1
+    CNT_MAX_KEY = 14,        // index build: largest key
+    CNT_LARGE_BUCKETS = 15,  // index build: buckets of more than DB_MID entries
+    CNT_PEND_MATE2 = 17,     // read sketch: CNT_PENDING before mate 2 of a batch
+    CNT_SUM_COUNTS = 19,     // -u: sum of a sample's counts
+};
+static_assert(CNT_SUM_COUNTS < CNT_SLOTS, "the last slot is inside ctx->d_counters");
+static_assert(CNT_DUPS == CNT_EVENTS + 2 && CNT_PEND_MATE1 == CNT_EVENTS + 3 && CNT_LARGE_BUCKETS == CNT_MAX_KEY + 1,
+              "slots cleared or copied as one range");
+
+// Owner of a half-built handle: frees it with the handle's free function unless release()d.  A half-built index is
+// freed once the ctx stream has drained (contain.cu).
+struct HandleFree {
+    void operator()(syl_sample *s) const { syl_sample_free(s); }
+    void operator()(syl_genomes *g) const { syl_genomes_free(g); }
+    void operator()(syl_db *db) const;
+    void operator()(syl_profile_job *j) const { syl_profile_job_free(j); }
+};
+template <typename T>
+using Handle = std::unique_ptr<T, HandleFree>;
+
+// a new handle whose arrays will be blocks of ctx's cache, used on ctx's stream
+template <typename T>
+Handle<T> new_handle(syl_ctx *ctx) {
+    Handle<T> h(new (std::nothrow) T());
+    if (h) {
+        h->device = ctx->device;
+        h->owner = ctx;
+        h->stream = ctx->stream;
+    }
+    return h;
+}
+
+// CSR k-mer arrays that their offsets count nk / nt entries in: one may be NULL only when it is empty (an empty torch
+// tensor has no address)
+inline int check_kmer_arrays(const uint64_t *kmers, uint64_t nk, const uint64_t *tracked, uint64_t nt) {
+    if (nk && !kmers) { set_error("kmer_off counts k-mers but kmers is NULL"); return SYL_ERR_ARG; }
+    if (nt && !tracked) { set_error("tracked_off counts tracked k-mers but tracked is NULL"); return SYL_ERR_ARG; }
+    return SYL_OK;
+}
 
 // One survivor of a READ sketch as the dedup post-pass consumes it (32 bytes = one sector):
 // recflag = read index << 1 | NO_PAIR, plus EV_PENDING while the pair keys still have to be

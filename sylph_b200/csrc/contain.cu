@@ -1089,12 +1089,12 @@ static int sample_metas(syl_ctx *ctx, const syl_sample *const *samples, uint32_t
     for (uint32_t i = 0; i < n; i++) {
         syl_sample *s = const_cast<syl_sample *>(samples[i]);
         if (!s->sum_counts_valid) {
-            unsigned long long *d = reinterpret_cast<unsigned long long *>(ctx->d_counters + 19);
+            unsigned long long *d = reinterpret_cast<unsigned long long *>(ctx->d_counters + CNT_SUM_COUNTS);
             SYL_CUDA(cudaMemsetAsync(d, 0, 8, st));
             if (s->n) k_sum_counts<<<ctx->num_sms * 4, 256, 0, st>>>(s->count, s->n, d);
-            SYL_CUDA(cudaMemcpyAsync(ctx->h_counters + 19, d, 8, cudaMemcpyDeviceToHost, st));
+            SYL_CUDA(cudaMemcpyAsync(ctx->h_counters + CNT_SUM_COUNTS, d, 8, cudaMemcpyDeviceToHost, st));
             SYL_CUDA(cudaStreamSynchronize(st));
-            s->sum_counts = ctx->h_counters[19];
+            s->sum_counts = ctx->h_counters[CNT_SUM_COUNTS];
             s->sum_counts_valid = true;
         }
         out[i] = {s->mean_read_length, s->c, s->sum_counts};
@@ -1104,18 +1104,6 @@ static int sample_metas(syl_ctx *ctx, const syl_sample *const *samples, uint32_t
 
 // estimate_true_cov (src/contain.rs:377-389) for the rows of one call (query: all rows; profile: the kept rows)
 static inline double unknown_multiplier(const SampleMeta &m, int k) { return m.mean_read_length / (m.mean_read_length - (double)k + 1.); }
-
-static int check_unknown_args(const syl_contain_params *p) {
-    if (p->estimate_unknown && !(p->read_seq_id > 0.)) {
-        set_error("-u without --read-seq-id: the automatic read-identity estimate depends on hash-map iteration order (src/contain.rs:901-951)");
-        return SYL_ERR_UNSUPPORTED;
-    }
-    return SYL_OK;
-}
-
-static void job_release(syl_profile_job *j) {
-    delete j;  // the scratch blocks go back to the owning ctx's cache (DevBuf::owner)
-}
 
 // Row-table capacity when the caller gives none, a multiple of 256.  The ranks of a sharded profile gather their tables
 // with fixed-size collectives, so at world > 1 it depends on the sample count only (shards of 257 and 256 genomes
@@ -1177,9 +1165,9 @@ static int csr_walks(syl_profile_job *j, bool pass2) {
     size_t tb = j->scan_bytes;
     SYL_CUDA(cub::DeviceScan::ExclusiveSum(j->scan_tmp.p, tb, j->cnt.p, j->off.p, (int)(NP + 1), st));
     if (!pass2) {
-        SYL_CUDA(cudaMemcpyAsync(ctx->h_counters + 10, j->off.p + NP, 8, cudaMemcpyDeviceToHost, st));
+        SYL_CUDA(cudaMemcpyAsync(ctx->h_counters + CNT_COVS_TOTAL, j->off.p + NP, 8, cudaMemcpyDeviceToHost, st));
         SYL_CUDA(cudaStreamSynchronize(st));
-        SYL_TRY(j->covs.alloc(std::max<uint64_t>(ctx->h_counters[10], 1), st));
+        SYL_TRY(j->covs.alloc(std::max<uint64_t>(ctx->h_counters[CNT_COVS_TOTAL], 1), st));
     }
     join_walk<JOIN_CSR_FILL>(j, pass2);
     SYL_CUDA(cudaGetLastError());
@@ -1214,55 +1202,52 @@ static int job_begin(syl_ctx *ctx, const syl_db *db, const syl_sample *const *sa
                      const syl_contain_params *p, bool profile, bool csr, uint32_t world, uint32_t rank, uint64_t R,
                      syl_profile_job **out) {
     cudaStream_t st = ctx->stream;
-    syl_profile_job *j = new (std::nothrow) syl_profile_job();
-    if (!j) return SYL_ERR_OOM;
-    auto fail = [&](int rc) { job_release(j); return rc; };
-#define JOB_CUDA(x) do { cudaError_t _e = (x); if (_e != cudaSuccess) { set_error(std::string(#x) + ": " + cudaGetErrorString(_e)); return fail(_e == cudaErrorMemoryAllocation ? SYL_ERR_OOM : SYL_ERR_CUDA); } } while (0)
-#define JOB_TRY(x) do { int _r = (x); if (_r != SYL_OK) return fail(_r); } while (0)
+    Handle<syl_profile_job> h(new (std::nothrow) syl_profile_job());
+    if (!h) return SYL_ERR_OOM;
+    syl_profile_job *j = h.get();
     j->ctx = ctx; j->db = db; j->profile = profile; j->csr = csr; j->S = n_samples; j->G = db->n_genomes; j->world = world; j->rank = rank;
     syl_contain_params pp = *p;
     pp.pseudotax = profile ? 1 : 0;
     j->P = make_params(&pp);
     j->redundant_ani = pp.redundant_ani;
-    JOB_TRY(check_unknown_args(p));
-    if (p->estimate_unknown) { j->read_seq_id = p->read_seq_id; JOB_TRY(sample_metas(ctx, samples, n_samples, j->metas)); }
+    if (p->estimate_unknown) { j->read_seq_id = p->read_seq_id; SYL_TRY(sample_metas(ctx, samples, n_samples, j->metas)); }
     j->R = R ? ((R + 255) & ~255ull) : default_rows_per_rank(n_samples, db->n_genomes, world);
     j->tbytes = table_bytes(j->R);
-    if (j->R * BOOT_ITERS >= 0xFFFF0000ull) { set_error("row capacity too large for the bootstrap work counter"); return fail(SYL_ERR_ARG); }
+    if (j->R * BOOT_ITERS >= 0xFFFF0000ull) { set_error("row capacity too large for the bootstrap work counter"); return SYL_ERR_ARG; }
     const uint64_t NP = (uint64_t)j->S * j->G;
-    if (NP >= 0x7FFFFFFFull) { set_error("samples x genomes exceeds 2^31 pairs per call; split the sample batch"); return fail(SYL_ERR_ARG); }
-    if (!csr && !histograms_fit(NP)) { set_error("pair histograms exceed 8 GB; split the sample batch"); return fail(SYL_ERR_UNSUPPORTED); }
+    if (NP >= 0x7FFFFFFFull) { set_error("samples x genomes exceeds 2^31 pairs per call; split the sample batch"); return SYL_ERR_ARG; }
+    if (!csr && !histograms_fit(NP)) { set_error("pair histograms exceed 8 GB; split the sample batch"); return SYL_ERR_UNSUPPORTED; }
     std::vector<SampleView> hv(n_samples);
     for (uint32_t i = 0; i < n_samples; i++) {
         hv[i] = {samples[i]->hash, samples[i]->count, samples[i]->n};
         j->max_n = std::max<uint64_t>(j->max_n, samples[i]->n);
     }
     const uint64_t HN = std::max<uint64_t>((uint64_t)j->S * j->max_n, 1);
-    JOB_TRY(j->views.alloc(n_samples, st));
+    SYL_TRY(j->views.alloc(n_samples, st));
     if (csr) {
-        JOB_TRY(j->cnt.alloc(NP + 1, st)); JOB_TRY(j->cursor.alloc(NP, st)); JOB_TRY(j->off.alloc(NP + 1, st));
+        SYL_TRY(j->cnt.alloc(NP + 1, st)); SYL_TRY(j->cursor.alloc(NP, st)); SYL_TRY(j->off.alloc(NP + 1, st));
         cub::DeviceScan::ExclusiveSum(nullptr, j->scan_bytes, j->cnt.p, j->off.p, (int)(NP + 1), st);
-        JOB_TRY(j->scan_tmp.alloc(j->scan_bytes, st));
+        SYL_TRY(j->scan_tmp.alloc(j->scan_bytes, st));
     } else {
-        JOB_TRY(j->touched.alloc(NP, st)); JOB_TRY(j->chist.alloc(NP * COV_BINS, st));
+        SYL_TRY(j->touched.alloc(NP, st)); SYL_TRY(j->chist.alloc(NP * COV_BINS, st));
     }
-    JOB_TRY(j->hits.alloc(HN, st));
-    JOB_TRY(j->tab1.alloc(j->tbytes, st));
-    JOB_TRY(j->boot_rows.alloc(j->R, st)); JOB_TRY(j->hist.alloc(j->R * 17, st));
-    JOB_TRY(j->res_ani.alloc(j->R * BOOT_ITERS, st)); JOB_TRY(j->res_lambda.alloc(j->R * BOOT_ITERS, st));
-    JOB_TRY(j->res_ok.alloc(j->R * BOOT_ITERS, st)); JOB_TRY(j->reject.alloc(j->R + 1, st));  // [R] = the bootstrap's work counter
+    SYL_TRY(j->hits.alloc(HN, st));
+    SYL_TRY(j->tab1.alloc(j->tbytes, st));
+    SYL_TRY(j->boot_rows.alloc(j->R, st)); SYL_TRY(j->hist.alloc(j->R * 17, st));
+    SYL_TRY(j->res_ani.alloc(j->R * BOOT_ITERS, st)); SYL_TRY(j->res_lambda.alloc(j->R * BOOT_ITERS, st));
+    SYL_TRY(j->res_ok.alloc(j->R * BOOT_ITERS, st)); SYL_TRY(j->reject.alloc(j->R + 1, st));  // [R] = the bootstrap's work counter
     if (profile) {
-        JOB_TRY(j->lost.alloc(NP, st)); JOB_TRY(j->order.alloc(NP, st)); JOB_TRY(j->contain1.alloc(NP, st));
-        JOB_TRY(j->tab2.alloc(j->tbytes, st)); JOB_TRY(j->gn_size.alloc(std::max<uint64_t>(j->G, 1), st));
-        if (world > 1) { JOB_TRY(j->gat1.alloc(j->tbytes * world, st)); JOB_TRY(j->wbest.alloc(HN, st)); }
+        SYL_TRY(j->lost.alloc(NP, st)); SYL_TRY(j->order.alloc(NP, st)); SYL_TRY(j->contain1.alloc(NP, st));
+        SYL_TRY(j->tab2.alloc(j->tbytes, st)); SYL_TRY(j->gn_size.alloc(std::max<uint64_t>(j->G, 1), st));
+        if (world > 1) { SYL_TRY(j->gat1.alloc(j->tbytes * world, st)); SYL_TRY(j->wbest.alloc(HN, st)); }
     }
-    if (world > 1) JOB_TRY(j->gat2.alloc(j->tbytes * world, st));  // final tables of all ranks (profile: pass 2; query: pass 1)
+    if (world > 1) SYL_TRY(j->gat2.alloc(j->tbytes * world, st));  // final tables of all ranks (profile: pass 2; query: pass 1)
     // a pageable source is staged by the driver before cudaMemcpyAsync returns: hv may go out of scope
-    JOB_CUDA(cudaMemcpyAsync(j->views.p, hv.data(), n_samples * sizeof(SampleView), cudaMemcpyHostToDevice, st));
-    if (profile && j->G) JOB_CUDA(cudaMemcpyAsync(j->gn_size.p, db->h_gn_size.data(), j->G * 8, cudaMemcpyHostToDevice, st));
-    JOB_TRY(clear_pairs(j));
-    JOB_CUDA(cudaMemsetAsync(j->hits.p, 0, HN * sizeof(uint2), st));
-    JOB_CUDA(cudaMemsetAsync(j->tab1.p, 0, sizeof(ShardTable), st));
+    SYL_CUDA(cudaMemcpyAsync(j->views.p, hv.data(), n_samples * sizeof(SampleView), cudaMemcpyHostToDevice, st));
+    if (profile && j->G) SYL_CUDA(cudaMemcpyAsync(j->gn_size.p, db->h_gn_size.data(), j->G * 8, cudaMemcpyHostToDevice, st));
+    SYL_TRY(clear_pairs(j));
+    SYL_CUDA(cudaMemsetAsync(j->hits.p, 0, HN * sizeof(uint2), st));
+    SYL_CUDA(cudaMemsetAsync(j->tab1.p, 0, sizeof(ShardTable), st));
     j->jgrid = dim3(nblk(std::max<uint64_t>(j->max_n, 1), 128), (unsigned)j->S);
     static const bool tile_env_off = getenv("SYL_JOIN_PLAIN") != nullptr;
     if (j->S > 1 && j->max_n && db->N && !tile_env_off) {
@@ -1270,7 +1255,7 @@ static int job_begin(syl_ctx *ctx, const syl_db *db, const syl_sample *const *sa
         const uint64_t R = std::min<uint64_t>(std::max<uint64_t>(j->max_n / 100, 1), std::max<uint64_t>(db->NB, 1));
         const uint64_t bpr = (db->NB + R - 1) / R;
         if (R * j->S < 0x7FFFFFFFull) {
-            JOB_TRY(j->range_bounds.alloc((uint64_t)j->S * (R + 1), st));
+            SYL_TRY(j->range_bounds.alloc((uint64_t)j->S * (R + 1), st));
             KernelTimer kt(ctx, SYL_KERNEL_JOIN);
             k_range_bounds<<<nblk((uint64_t)j->S * (R + 1), 256), 256, 0, st>>>(j->views.p, j->S, (uint32_t)R, bpr, db->M, db->NB, j->range_bounds.p);
             ctx->launches++;
@@ -1285,15 +1270,15 @@ static int job_begin(syl_ctx *ctx, const syl_db *db, const syl_sample *const *sa
                                         pair_out(j, false), j->hits.p, j->max_n, j->km);
         ctx->launches++;
     }
-    if (csr) JOB_TRY(csr_walks(j, false));
+    if (csr) SYL_TRY(csr_walks(j, false));
     StatParams P1 = j->P;
     if (profile) P1.no_ci = 1;  // pass-1 confidence intervals are never reported (pass-2 rows replace them)
     StatExtra X;
     X.pair_stride = j->G;
     if (profile) X.contain1_out = j->contain1.p;
-    JOB_TRY(enqueue_stats(j, P1, false, j->tab1.p, X));
+    SYL_TRY(enqueue_stats(j, P1, false, j->tab1.p, X));
     j->stage = 1;
-    *out = j;
+    *out = h.release();
     return SYL_OK;
 }
 
@@ -1472,7 +1457,7 @@ static int contain_fast(syl_ctx *ctx, const syl_db *db, const syl_sample *const 
         }
         uint64_t need = 0;
         if (rc == SYL_OK) rc = job_finish(j, out, &need);
-        job_release(j);
+        syl_profile_job_free(j);
         if (rc == SYL_ERR_CAPACITY) { R = need + 256; out.clear(); continue; }
         if (rc == SYL_ERR_UNSUPPORTED && !csr) { csr = true; out.clear(); continue; }  // a count >= COV_BINS
         return rc;
@@ -1480,10 +1465,12 @@ static int contain_fast(syl_ctx *ctx, const syl_db *db, const syl_sample *const 
     return SYL_ERR_CAPACITY;
 }
 
-// the arguments of a query / profile call against a database of k-mer size k and sketch parameter c
-static int check_sample_args(syl_ctx *ctx, int k, uint64_t c, const syl_sample *const *samples, uint32_t n_samples,
-                             const syl_contain_params *p, syl_ani_row *rows, uint64_t cap, uint64_t *n_rows) {
+// The arguments of a query or profile call against a database of k-mer size k and sketch parameter c that has_tracked
+// k-mers or not; *n_rows is 0 once they are not NULL.
+static int check_contain_args(syl_ctx *ctx, int k, uint64_t c, bool has_tracked, bool profile, const syl_sample *const *samples,
+                              uint32_t n_samples, const syl_contain_params *p, syl_ani_row *rows, uint64_t cap, uint64_t *n_rows) {
     if (!ctx || !p || !n_rows || (n_samples && !samples) || (cap && !rows)) { set_error("NULL argument"); return SYL_ERR_ARG; }
+    *n_rows = 0;
     for (uint32_t i = 0; i < n_samples; i++) {
         if (!samples[i]) { set_error("NULL sample"); return SYL_ERR_ARG; }
         if (samples[i]->k != k) {  // src/contain.rs:608-615 (log::error + exit(1))
@@ -1496,13 +1483,23 @@ static int check_sample_args(syl_ctx *ctx, int k, uint64_t c, const syl_sample *
         }
     }
     if (p->k != k) { set_error("params.k != db k"); return SYL_ERR_ARG; }
+    if (p->estimate_unknown && !(p->read_seq_id > 0.)) {
+        set_error("-u without --read-seq-id: the automatic read-identity estimate depends on hash-map iteration order (src/contain.rs:901-951)");
+        return SYL_ERR_UNSUPPORTED;
+    }
+    if (profile && !has_tracked) {  // src/contain.rs:231-234
+        set_error("Attempting profiling, but the database was sketched with the --disable-profiling option");
+        return SYL_ERR_ARG;
+    }
     return SYL_OK;
 }
 
-static int check_pair_args(syl_ctx *ctx, const syl_db *db, const syl_sample *const *samples, uint32_t n_samples,
-                           const syl_contain_params *p, syl_ani_row *rows, uint64_t cap, uint64_t *n_rows) {
-    if (!db) { set_error("NULL argument"); return SYL_ERR_ARG; }
-    return check_sample_args(ctx, db->k, db->c, samples, n_samples, p, rows, cap, n_rows);
+// the rows of a call into the caller's buffer of cap rows; *n_rows is their number even when they do not fit
+static int copy_rows(const std::vector<syl_ani_row> &out, syl_ani_row *rows, uint64_t cap, uint64_t *n_rows) {
+    *n_rows = out.size();
+    if (out.size() > cap) { set_error("row buffer too small"); return SYL_ERR_CAPACITY; }
+    std::copy(out.begin(), out.end(), rows);
+    return SYL_OK;
 }
 
 // ---- index build, host side -------------------------------------------------------------------
@@ -1690,6 +1687,20 @@ static int db_sort_large(syl_ctx *ctx, syl_db *db, const std::vector<uint2> &lar
     return SYL_OK;
 }
 
+static const char *const BAD_OFFSETS = "offsets must start at 0 and be monotone";
+
+// CSR offsets of G genomes in host memory (tracked_off may be NULL): the chunk planner and the scatter's genome search
+// walk them, so they must start at 0 and never decrease
+static int check_host_offsets(const uint64_t *kmer_off, const uint64_t *tracked_off, uint64_t G) {
+    for (const uint64_t *o : {kmer_off, tracked_off}) {
+        if (!o) continue;
+        bool bad = o[0] != 0;
+        for (uint64_t i = 1; i <= G && !bad; i++) bad = o[i] < o[i - 1];
+        if (bad) { set_error(BAD_OFFSETS); return SYL_ERR_ARG; }
+    }
+    return SYL_OK;
+}
+
 static int check_db_size(uint64_t nk, uint64_t nt, uint64_t G) {
     if (nk >= 0xFFFFFFFFull || nt >= 0xFFFFFFFFull || nk + nt >= 0xFFFFFFFFull) {
         set_error("db shard holds more than 2^32-2 k-mers; shard the database");
@@ -1699,95 +1710,93 @@ static int check_db_size(uint64_t nk, uint64_t nt, uint64_t G) {
     return SYL_OK;
 }
 
+// a half-built index: its kernels may still be writing it
+void HandleFree::operator()(syl_db *db) const {
+    cudaStreamSynchronize(db->stream);
+    syl_db_free(db);
+}
+
 // The index of `in` (see "index build" above).  gn_size: G sizes in in.mem's memory, or NULL (zeros).
 static int db_build(syl_ctx *ctx, const DbInput &in, const uint64_t *gn_size, int has_tracked, int k, uint64_t c,
                     uint32_t genome_base, syl_db **out) {
     cudaStream_t st = ctx->stream;
     const uint64_t G = in.G, N = in.n[0] + in.n[1];
-    syl_db *db = new (std::nothrow) syl_db();
+    Handle<syl_db> db = new_handle<syl_db>(ctx);
     if (!db) return SYL_ERR_OOM;
-    db->device = ctx->device;
-    db->stream = st;
-    db->owner = ctx;
     db->n_genomes = G;
     db->genome_base = genome_base;
     db->N = N;
     db->has_tracked = has_tracked;
     db->k = k;
     db->c = c;
-    auto fail = [&](int rc) { cudaStreamSynchronize(st); syl_db_free(db); return rc; };
-#define DB_TRY(x) do { int _r = (x); if (_r != SYL_OK) return fail(_r); } while (0)
-#define DB_CUDA(x) do { cudaError_t _e = (x); if (_e != cudaSuccess) { set_error(std::string(#x) + ": " + cudaGetErrorString(_e)); return fail(SYL_ERR_CUDA); } } while (0)
-    DB_TRY(hblock_alloc(ctx, (void **)&db->keys, std::max<uint64_t>(N, 1) * 8));
-    DB_TRY(hblock_alloc(ctx, (void **)&db->gid, std::max<uint64_t>(N, 1) * 4));
-    DB_TRY(hblock_alloc(ctx, (void **)&db->glen, std::max<uint64_t>(G, 1) * 4));
+    SYL_TRY(hblock_alloc(ctx, (void **)&db->keys, std::max<uint64_t>(N, 1) * 8));
+    SYL_TRY(hblock_alloc(ctx, (void **)&db->gid, std::max<uint64_t>(N, 1) * 4));
+    SYL_TRY(hblock_alloc(ctx, (void **)&db->glen, std::max<uint64_t>(G, 1) * 4));
     db->h_gn_size.assign(G, 0);
     std::vector<uint32_t> h_glen;
     if (G) {
         if (in.mem == SYL_MEM_DEVICE) {
-            if (gn_size) DB_CUDA(cudaMemcpyAsync(db->h_gn_size.data(), gn_size, G * 8, cudaMemcpyDeviceToHost, st));
+            if (gn_size) SYL_CUDA(cudaMemcpyAsync(db->h_gn_size.data(), gn_size, G * 8, cudaMemcpyDeviceToHost, st));
             k_glen<<<nblk(G, 256), 256, 0, st>>>(in.off[0], G, db->glen);
             ctx->launches++;
         } else {
             if (gn_size) std::copy(gn_size, gn_size + G, db->h_gn_size.begin());
             h_glen.resize(G);
             for (uint64_t g = 0; g < G; g++) h_glen[g] = (uint32_t)(in.off[0][g + 1] - in.off[0][g]);
-            DB_CUDA(cudaMemcpyAsync(db->glen, h_glen.data(), G * 4, cudaMemcpyHostToDevice, st));
+            SYL_CUDA(cudaMemcpyAsync(db->glen, h_glen.data(), G * 4, cudaMemcpyHostToDevice, st));
         }
     }
     uint64_t NB = 1024;
     while (NB < N / 4) NB <<= 1;
     db->NB = NB;
-    DB_TRY(hblock_alloc(ctx, (void **)&db->bstart, (NB + 2) * 4));
-    DB_CUDA(cudaMemsetAsync(db->bstart, 0, (NB + 2) * 4, st));
+    SYL_TRY(hblock_alloc(ctx, (void **)&db->bstart, (NB + 2) * 4));
+    SYL_CUDA(cudaMemsetAsync(db->bstart, 0, (NB + 2) * 4, st));
     if (N) {
         DbFeed feed(ctx, in);
-        DB_TRY(feed.init());
-        unsigned long long *d_max = reinterpret_cast<unsigned long long *>(ctx->d_counters + 14);
-        DB_CUDA(cudaMemsetAsync(d_max, 0, 16, st));  // [14] max key, [15] large buckets
-        DB_TRY(feed.pass([&](const DbChunk &ch) { k_db_max<<<db_grid(ctx, ch), 256, 0, st>>>(ch, d_max); }));
-        DB_CUDA(cudaMemcpyAsync(ctx->h_counters + 14, d_max, 8, cudaMemcpyDeviceToHost, st));
-        DB_CUDA(cudaStreamSynchronize(st));
-        db->maxkey = ctx->h_counters[14];
+        SYL_TRY(feed.init());
+        unsigned long long *d_max = reinterpret_cast<unsigned long long *>(ctx->d_counters + CNT_MAX_KEY);
+        SYL_CUDA(cudaMemsetAsync(d_max, 0, 16, st));  // CNT_MAX_KEY, CNT_LARGE_BUCKETS
+        SYL_TRY(feed.pass([&](const DbChunk &ch) { k_db_max<<<db_grid(ctx, ch), 256, 0, st>>>(ch, d_max); }));
+        SYL_CUDA(cudaMemcpyAsync(ctx->h_counters + CNT_MAX_KEY, d_max, 8, cudaMemcpyDeviceToHost, st));
+        SYL_CUDA(cudaStreamSynchronize(st));
+        db->maxkey = ctx->h_counters[CNT_MAX_KEY];
         unsigned __int128 m = ((unsigned __int128)NB << 64) / ((unsigned __int128)db->maxkey + 1);
         db->M = m > (unsigned __int128)UINT64_MAX ? UINT64_MAX : (uint64_t)m;
         const uint64_t M = db->M;
-        DB_TRY(feed.pass([&](const DbChunk &ch) { k_db_hist<<<db_grid(ctx, ch), 256, 0, st>>>(ch, M, NB, db->bstart); }));
+        SYL_TRY(feed.pass([&](const DbChunk &ch) { k_db_hist<<<db_grid(ctx, ch), 256, 0, st>>>(ch, M, NB, db->bstart); }));
         {
             BuildBuf tmp(ctx);
             size_t tb = 0;
-            DB_CUDA(cub::DeviceScan::InclusiveSum(nullptr, tb, db->bstart, db->bstart, (int)(NB + 2), st));
-            DB_TRY(tmp.alloc(tb));
-            DB_CUDA(cub::DeviceScan::InclusiveSum(tmp.p, tb, db->bstart, db->bstart, (int)(NB + 2), st));
+            SYL_CUDA(cub::DeviceScan::InclusiveSum(nullptr, tb, db->bstart, db->bstart, (int)(NB + 2), st));
+            SYL_TRY(tmp.alloc(tb));
+            SYL_CUDA(cub::DeviceScan::InclusiveSum(tmp.p, tb, db->bstart, db->bstart, (int)(NB + 2), st));
             ctx->launches++;
         }
-        DB_TRY(feed.pass([&](const DbChunk &ch) {
+        SYL_TRY(feed.pass([&](const DbChunk &ch) {
             k_db_scatter<<<db_grid(ctx, ch), 256, 0, st>>>(ch, M, NB, db->bstart, db->keys, db->gid);
         }));
         // everything below reads the index only: the staging buffers go before the large-bucket temporaries come
         feed.stage[0].release();
         feed.stage[1].release();
         BuildBuf large(ctx);
-        DB_TRY(large.alloc((N / (DB_MID + 1) + 1) * sizeof(uint2)));
-        unsigned long long *d_nl = d_max + 1;
+        SYL_TRY(large.alloc((N / (DB_MID + 1) + 1) * sizeof(uint2)));
+        unsigned long long *d_nl = reinterpret_cast<unsigned long long *>(ctx->d_counters + CNT_LARGE_BUCKETS);
         k_db_sort_buckets<<<nblk(NB, DB_SORT_TILE), DB_SORT_TILE, 0, st>>>(db->bstart, NB, db->keys, db->gid,
                                                                             large.as<uint2>(), d_nl);
         ctx->launches++;
-        DB_CUDA(cudaGetLastError());
-        DB_CUDA(cudaMemcpyAsync(ctx->h_counters + 15, d_nl, 8, cudaMemcpyDeviceToHost, st));
-        DB_CUDA(cudaStreamSynchronize(st));
-        std::vector<uint2> h_large(ctx->h_counters[15]);
+        SYL_CUDA(cudaGetLastError());
+        SYL_CUDA(cudaMemcpyAsync(ctx->h_counters + CNT_LARGE_BUCKETS, d_nl, 8, cudaMemcpyDeviceToHost, st));
+        SYL_CUDA(cudaStreamSynchronize(st));
+        std::vector<uint2> h_large(ctx->h_counters[CNT_LARGE_BUCKETS]);
         if (!h_large.empty()) {
-            DB_CUDA(cudaMemcpyAsync(h_large.data(), large.p, h_large.size() * sizeof(uint2), cudaMemcpyDeviceToHost, st));
-            DB_CUDA(cudaStreamSynchronize(st));
+            SYL_CUDA(cudaMemcpyAsync(h_large.data(), large.p, h_large.size() * sizeof(uint2), cudaMemcpyDeviceToHost, st));
+            SYL_CUDA(cudaStreamSynchronize(st));
             large.release();
-            DB_TRY(db_sort_large(ctx, db, h_large));
+            SYL_TRY(db_sort_large(ctx, db.get(), h_large));
         }
     }
-    DB_CUDA(cudaStreamSynchronize(st));
-#undef DB_CUDA
-#undef DB_TRY
-    *out = db;
+    SYL_CUDA(cudaStreamSynchronize(st));
+    *out = db.release();
     return SYL_OK;
 }
 
@@ -2010,16 +2019,9 @@ static int shards_profile(syl_db_shards *s, const syl_sample *const *samples, ui
 static int shards_call(syl_ctx *ctx, syl_db_shards *s, const syl_sample *const *samples, uint32_t n_samples,
                        const syl_contain_params *p, bool profile, syl_ani_row *rows, uint64_t cap, uint64_t *n_rows) {
     if (!s) { set_error("NULL argument"); return SYL_ERR_ARG; }
-    SYL_TRY(check_sample_args(ctx, s->k, s->c, samples, n_samples, p, rows, cap, n_rows));
+    SYL_TRY(check_contain_args(ctx, s->k, s->c, s->tracked_off != nullptr, profile, samples, n_samples, p, rows, cap, n_rows));
     if (ctx != s->ctx) { set_error("db shards used with another ctx than the one that created them"); return SYL_ERR_ARG; }
-    SYL_TRY(check_unknown_args(p));
-    *n_rows = 0;
-    if (profile && !s->tracked_off) {  // src/contain.rs:231-234
-        set_error("Attempting profiling, but the database was sketched with the --disable-profiling option");
-        return SYL_ERR_ARG;
-    }
-    SYL_CUDA(cudaSetDevice(ctx->device));
-    syl::tl_ctx = ctx;
+    SYL_ENTER(ctx);
     const uint64_t call = ++s->calls;
     auto &kp = s->kept;
     const bool retry = kp.call && kp.call + 1 == call && kp.profile == profile && !memcmp(&kp.p, p, sizeof *p) &&
@@ -2039,18 +2041,15 @@ static int shards_call(syl_ctx *ctx, syl_db_shards *s, const syl_sample *const *
             });
         }
     }
-    *n_rows = out.size();
-    if (out.size() > cap) {
+    const int rc = copy_rows(out, rows, cap, n_rows);
+    if (rc == SYL_ERR_CAPACITY) {
         kp.call = call;
         kp.profile = profile;
         kp.p = *p;
         kp.samples.assign(samples, samples + n_samples);
         kp.rows.swap(out);
-        set_error("row buffer too small");
-        return SYL_ERR_CAPACITY;
     }
-    std::copy(out.begin(), out.end(), rows);
-    return SYL_OK;
+    return rc;
 }
 
 }  // namespace syl
@@ -2062,8 +2061,7 @@ extern "C" {
 int syl_db_build(syl_ctx *ctx, const syl_genomes *g, uint32_t genome_base, syl_db **out) {
     if (!ctx || !g || !out) { set_error("NULL argument"); return SYL_ERR_ARG; }
     *out = nullptr;
-    SYL_CUDA(cudaSetDevice(ctx->device));
-    syl::tl_ctx = ctx;
+    SYL_ENTER(ctx);
     const uint64_t nt = g->has_tracked ? g->total_tracked : 0;
     SYL_TRY(check_db_size(g->total_kmers, nt, g->n));
     const DbInput in{SYL_MEM_DEVICE, {g->kmers, g->tracked}, {g->kmer_off, g->tracked_off}, g->n, {g->total_kmers, nt}};
@@ -2076,8 +2074,7 @@ int syl_db_build_arrays(syl_ctx *ctx, int mem, const uint64_t *kmers, const uint
     if (!ctx || !kmer_off || !out) { set_error("NULL argument"); return SYL_ERR_ARG; }
     *out = nullptr;
     if (mem != SYL_MEM_HOST && mem != SYL_MEM_DEVICE) { set_error("bad mem"); return SYL_ERR_ARG; }
-    SYL_CUDA(cudaSetDevice(ctx->device));
-    syl::tl_ctx = ctx;
+    SYL_ENTER(ctx);
     cudaStream_t st = ctx->stream;
     if (n_genomes >= 0x7FFFFFFFull) return check_db_size(0, 0, n_genomes);
     uint64_t nk = 0, nt = 0;
@@ -2085,37 +2082,29 @@ int syl_db_build_arrays(syl_ctx *ctx, int mem, const uint64_t *kmers, const uint
         nk = kmer_off[n_genomes];
         nt = tracked_off ? tracked_off[n_genomes] : 0;
     } else {
-        SYL_CUDA(cudaMemcpyAsync(ctx->h_counters + 8, kmer_off + n_genomes, 8, cudaMemcpyDeviceToHost, st));
-        if (tracked_off) SYL_CUDA(cudaMemcpyAsync(ctx->h_counters + 9, tracked_off + n_genomes, 8, cudaMemcpyDeviceToHost, st));
+        SYL_CUDA(cudaMemcpyAsync(ctx->h_counters + CNT_KMER_TOTAL, kmer_off + n_genomes, 8, cudaMemcpyDeviceToHost, st));
+        if (tracked_off) SYL_CUDA(cudaMemcpyAsync(ctx->h_counters + CNT_TRACKED_TOTAL, tracked_off + n_genomes, 8, cudaMemcpyDeviceToHost, st));
         SYL_CUDA(cudaStreamSynchronize(st));
-        nk = ctx->h_counters[8];
-        nt = tracked_off ? ctx->h_counters[9] : 0;
+        nk = ctx->h_counters[CNT_KMER_TOTAL];
+        nt = tracked_off ? ctx->h_counters[CNT_TRACKED_TOTAL] : 0;
     }
     SYL_TRY(check_db_size(nk, nt, n_genomes));
-    if (nk && !kmers) { set_error("kmer_off counts k-mers but kmers is NULL"); return SYL_ERR_ARG; }
-    if (nt && !tracked) { set_error("tracked_off counts tracked k-mers but tracked is NULL"); return SYL_ERR_ARG; }
-    // the chunk planner and the scatter's genome search walk the offsets: they must start at 0 and never decrease
-    bool bad = false;
-    const uint64_t *offs[2] = {kmer_off, tracked_off};
+    SYL_TRY(check_kmer_arrays(kmers, nk, tracked, nt));
     if (mem == SYL_MEM_HOST) {
-        for (const uint64_t *o : offs) {
-            if (!o) continue;
-            bad |= o[0] != 0;
-            for (uint64_t i = 1; i <= n_genomes && !bad; i++) bad = o[i] < o[i - 1];
-        }
+        SYL_TRY(check_host_offsets(kmer_off, tracked_off, n_genomes));
     } else {
-        SYL_CUDA(cudaMemsetAsync(ctx->d_counters + 10, 0, 8, st));
-        for (const uint64_t *o : offs) {
+        unsigned long long *d_bad = reinterpret_cast<unsigned long long *>(ctx->d_counters + CNT_BAD_OFFSETS);
+        SYL_CUDA(cudaMemsetAsync(d_bad, 0, 8, st));
+        for (const uint64_t *o : {kmer_off, tracked_off}) {
             if (!o) continue;
-            k_check_offsets<<<nblk(n_genomes + 1, 256), 256, 0, st>>>(o, n_genomes + 1, reinterpret_cast<unsigned long long *>(ctx->d_counters + 10));
+            k_check_offsets<<<nblk(n_genomes + 1, 256), 256, 0, st>>>(o, n_genomes + 1, d_bad);
             ctx->launches++;
         }
         SYL_CUDA(cudaGetLastError());
-        SYL_CUDA(cudaMemcpyAsync(ctx->h_counters + 10, ctx->d_counters + 10, 8, cudaMemcpyDeviceToHost, st));
+        SYL_CUDA(cudaMemcpyAsync(ctx->h_counters + CNT_BAD_OFFSETS, d_bad, 8, cudaMemcpyDeviceToHost, st));
         SYL_CUDA(cudaStreamSynchronize(st));
-        bad = ctx->h_counters[10] != 0;
+        if (ctx->h_counters[CNT_BAD_OFFSETS]) { set_error(BAD_OFFSETS); return SYL_ERR_ARG; }
     }
-    if (bad) { set_error("offsets must start at 0 and be monotone"); return SYL_ERR_ARG; }
     const DbInput in{mem, {kmers, tracked}, {kmer_off, tracked_off}, n_genomes, {nk, nt}};
     return db_build(ctx, in, gn_size, tracked_off ? 1 : 0, k, c, genome_base, out);
 }
@@ -2125,7 +2114,7 @@ int syl_db_download(syl_ctx *ctx, const syl_db *db, uint64_t *keys, uint32_t *gi
     if (!ctx || !db) { set_error("NULL argument"); return SYL_ERR_ARG; }
     if (n_entries) *n_entries = db->N;
     if (n_buckets) *n_buckets = db->NB;
-    SYL_CUDA(cudaSetDevice(ctx->device));
+    SYL_ENTER(ctx);
     cudaStream_t st = ctx->stream;
     if (keys && db->N) SYL_CUDA(cudaMemcpyAsync(keys, db->keys, db->N * 8, cudaMemcpyDeviceToHost, st));
     if (gid && db->N) SYL_CUDA(cudaMemcpyAsync(gid, db->gid, db->N * 4, cudaMemcpyDeviceToHost, st));
@@ -2163,34 +2152,24 @@ void syl_contain_params_default(syl_contain_params *p, int k, int pseudotax) {
 
 int syl_query(syl_ctx *ctx, const syl_db *db, const syl_sample *const *samples, uint32_t n_samples,
               const syl_contain_params *p, syl_ani_row *rows, uint64_t cap, uint64_t *n_rows) {
-    SYL_TRY(check_pair_args(ctx, db, samples, n_samples, p, rows, cap, n_rows));
-    SYL_TRY(check_unknown_args(p));
-    *n_rows = 0;
-    SYL_CUDA(cudaSetDevice(ctx->device));
-    syl::tl_ctx = ctx;
+    if (!db) { set_error("NULL argument"); return SYL_ERR_ARG; }
+    SYL_TRY(check_contain_args(ctx, db->k, db->c, db->has_tracked, false, samples, n_samples, p, rows, cap, n_rows));
+    SYL_ENTER(ctx);
     if (db->n_genomes == 0 || n_samples == 0) return SYL_OK;
     std::vector<syl_ani_row> out;
     SYL_TRY(contain_fast(ctx, db, samples, n_samples, p, false, out));
-    *n_rows = out.size();
-    if (out.size() > cap) { set_error("row buffer too small"); return SYL_ERR_CAPACITY; }
-    std::copy(out.begin(), out.end(), rows);
-    return SYL_OK;
+    return copy_rows(out, rows, cap, n_rows);
 }
 
 int syl_profile_shard_begin(syl_ctx *ctx, const syl_db *db, const syl_sample *const *samples, uint32_t n_samples,
                             const syl_contain_params *p, uint32_t world, uint32_t rank, uint64_t rows_per_rank,
                             syl_profile_job **out) {
     uint64_t dummy = 0;
-    if (!out) { set_error("NULL argument"); return SYL_ERR_ARG; }
+    if (!out || !db) { set_error("NULL argument"); return SYL_ERR_ARG; }
     *out = nullptr;
-    SYL_TRY(check_pair_args(ctx, db, samples, n_samples, p, nullptr, 0, &dummy));
     if (world == 0 || rank >= world || n_samples == 0) { set_error("bad world / rank / sample count"); return SYL_ERR_ARG; }
-    if (!db->has_tracked) {  // src/contain.rs:231-234
-        set_error("Attempting profiling, but the database was sketched with the --disable-profiling option");
-        return SYL_ERR_ARG;
-    }
-    SYL_CUDA(cudaSetDevice(ctx->device));
-    syl::tl_ctx = ctx;
+    SYL_TRY(check_contain_args(ctx, db->k, db->c, db->has_tracked, true, samples, n_samples, p, nullptr, 0, &dummy));
+    SYL_ENTER(ctx);
     return job_begin(ctx, db, samples, n_samples, p, true, false, world, rank, rows_per_rank, out);
 }
 
@@ -2209,53 +2188,40 @@ int syl_profile_job_buffers(const syl_profile_job *j, void **d_table1, void **d_
 
 int syl_profile_shard_rank(syl_profile_job *j) {
     if (!j || j->stage != 1 || !j->profile) { set_error("profile job: wrong stage"); return SYL_ERR_ARG; }
-    SYL_CUDA(cudaSetDevice(j->ctx->device));
-    syl::tl_ctx = j->ctx;
+    SYL_ENTER(j->ctx);
     return job_rank(j);
 }
 
 int syl_profile_shard_pass2(syl_profile_job *j) {
     if (!j || j->stage != 2) { set_error("profile job: wrong stage"); return SYL_ERR_ARG; }
-    SYL_CUDA(cudaSetDevice(j->ctx->device));
-    syl::tl_ctx = j->ctx;
+    SYL_ENTER(j->ctx);
     return job_pass2(j);
 }
 
 int syl_profile_shard_finish(syl_profile_job *j, syl_ani_row *rows, uint64_t cap, uint64_t *n_rows, uint64_t *need_rows_per_rank) {
     if (!j || j->stage != 3 || !n_rows || (cap && !rows)) { set_error("profile job: wrong stage / NULL argument"); return SYL_ERR_ARG; }
-    SYL_CUDA(cudaSetDevice(j->ctx->device));
-    syl::tl_ctx = j->ctx;
+    SYL_ENTER(j->ctx);
     std::vector<syl_ani_row> out;
     uint64_t need = 0;
     const int rc = job_finish(j, out, &need);
     if (need_rows_per_rank) *need_rows_per_rank = need;
     if (rc != SYL_OK) return rc;
-    *n_rows = out.size();
-    if (out.size() > cap) { set_error("row buffer too small"); return SYL_ERR_CAPACITY; }
-    std::copy(out.begin(), out.end(), rows);
-    return SYL_OK;
+    return copy_rows(out, rows, cap, n_rows);
 }
 
-void syl_profile_job_free(syl_profile_job *j) { job_release(j); }
+void syl_profile_job_free(syl_profile_job *j) {
+    delete j;  // the scratch blocks go back to the owning ctx's cache (DevBuf::owner)
+}
 
 int syl_profile(syl_ctx *ctx, const syl_db *db, const syl_sample *const *samples, uint32_t n_samples,
                 const syl_contain_params *p, syl_ani_row *rows, uint64_t cap, uint64_t *n_rows) {
-    SYL_TRY(check_pair_args(ctx, db, samples, n_samples, p, rows, cap, n_rows));
-    SYL_TRY(check_unknown_args(p));
-    *n_rows = 0;
-    if (!db->has_tracked) {  // src/contain.rs:231-234
-        set_error("Attempting profiling, but the database was sketched with the --disable-profiling option");
-        return SYL_ERR_ARG;
-    }
-    SYL_CUDA(cudaSetDevice(ctx->device));
-    syl::tl_ctx = ctx;
+    if (!db) { set_error("NULL argument"); return SYL_ERR_ARG; }
+    SYL_TRY(check_contain_args(ctx, db->k, db->c, db->has_tracked, true, samples, n_samples, p, rows, cap, n_rows));
+    SYL_ENTER(ctx);
     if (db->n_genomes == 0 || n_samples == 0) return SYL_OK;
     std::vector<syl_ani_row> out;
     SYL_TRY(contain_fast(ctx, db, samples, n_samples, p, true, out));
-    *n_rows = out.size();
-    if (out.size() > cap) { set_error("row buffer too small"); return SYL_ERR_CAPACITY; }
-    std::copy(out.begin(), out.end(), rows);
-    return SYL_OK;
+    return copy_rows(out, rows, cap, n_rows);
 }
 
 int syl_db_shards_create(syl_ctx *ctx, const uint64_t *kmers, const uint64_t *kmer_off, const uint64_t *tracked,
@@ -2264,7 +2230,7 @@ int syl_db_shards_create(syl_ctx *ctx, const uint64_t *kmers, const uint64_t *km
     if (!ctx || !kmer_off || !out) { set_error("NULL argument"); return SYL_ERR_ARG; }
     *out = nullptr;
     if (n_genomes > 0xFFFFFFFFull) { set_error("more than 2^32 genomes: row.genome is 32 bits"); return SYL_ERR_ARG; }
-    SYL_CUDA(cudaSetDevice(ctx->device));
+    SYL_ENTER(ctx);
     for (const uint64_t *a : {kmers, kmer_off, tracked, tracked_off, gn_size}) {  // the sweep reads them on the host
         cudaPointerAttributes at{};
         if (!a) continue;
@@ -2274,15 +2240,8 @@ int syl_db_shards_create(syl_ctx *ctx, const uint64_t *kmers, const uint64_t *km
         }
         if (at.type == cudaMemoryTypeDevice) { set_error("db shards borrow host arrays; a device pointer was given"); return SYL_ERR_ARG; }
     }
-    bool bad = false;
-    for (const uint64_t *o : {kmer_off, tracked_off}) {
-        if (!o) continue;
-        bad |= o[0] != 0;
-        for (uint64_t i = 1; i <= n_genomes && !bad; i++) bad = o[i] < o[i - 1];
-    }
-    if (bad) { set_error("offsets must start at 0 and be monotone"); return SYL_ERR_ARG; }
-    if (kmer_off[n_genomes] && !kmers) { set_error("kmer_off counts k-mers but kmers is NULL"); return SYL_ERR_ARG; }
-    if (tracked_off && tracked_off[n_genomes] && !tracked) { set_error("tracked_off counts tracked k-mers but tracked is NULL"); return SYL_ERR_ARG; }
+    SYL_TRY(check_host_offsets(kmer_off, tracked_off, n_genomes));
+    SYL_TRY(check_kmer_arrays(kmers, kmer_off[n_genomes], tracked, tracked_off ? tracked_off[n_genomes] : 0));
     uint64_t dflt = 0;
     SYL_TRY(default_shard_entries(&dflt));
     uint64_t cap = max_entries ? std::min(max_entries, SHARD_MAX_ENTRIES) : dflt;

@@ -110,10 +110,8 @@ __global__ void k_copy_ranges(const uint64_t *__restrict__ src4, const uint64_t 
     for (uint64_t j = threadIdx.x; j < nt; j += blockDim.x) otracked[dt + j] = tracked[st + j];
 }
 
-// stream-ordered allocations on the creating ctx stream (no device-wide sync in steady-state loops)
-static int genomes_alloc(syl_genomes *g, cudaStream_t st, uint64_t n_genomes, uint64_t nk, uint64_t nt) {
-    g->stream = st;
-    g->owner = tl_ctx;
+// the arrays of a handle from new_handle: blocks of its owner's cache
+static int genomes_alloc(syl_genomes *g, uint64_t n_genomes, uint64_t nk, uint64_t nt) {
     SYL_TRY(hblock_alloc(g->owner, (void **)&g->kmers, std::max<uint64_t>(nk, 1) * 8));
     SYL_TRY(hblock_alloc(g->owner, (void **)&g->tracked, std::max<uint64_t>(nt, 1) * 8));
     SYL_TRY(hblock_alloc(g->owner, (void **)&g->kmer_off, (n_genomes + 1) * 8));
@@ -300,8 +298,6 @@ static int genomes_back_half(syl_ctx *ctx, KernelTimer &kt, const uint64_t *posk
     ctx->launches += 5;
     // per-genome offsets go straight into the handle; the k-mer arrays need the totals first
     out->has_tracked = pseudotax ? 1 : 0;
-    out->stream = st;
-    out->owner = tl_ctx;
     out->n = n_genomes;
     SYL_TRY(hblock_alloc(out->owner, (void **)&out->kmer_off, (n_genomes + 1) * 8));
     SYL_TRY(hblock_alloc(out->owner, (void **)&out->tracked_off, (n_genomes + 1) * 8));
@@ -312,7 +308,7 @@ static int genomes_back_half(syl_ctx *ctx, KernelTimer &kt, const uint64_t *posk
     ctx->launches++;
     kt.stop();
     SYL_CUDA(cudaGetLastError());
-    uint32_t *h32 = reinterpret_cast<uint32_t *>(ctx->h_counters + 4);  // N, kept, tracked, slot overflow
+    uint32_t *h32 = reinterpret_cast<uint32_t *>(ctx->h_counters + CNT_BACK_HALF);  // N, kept, tracked, slot overflow
     SYL_CUDA(cudaMemcpyAsync(h32, d_n, 4, cudaMemcpyDeviceToHost, st));
     SYL_CUDA(cudaMemcpyAsync(h32 + 1, bk_off.p + nb, 4, cudaMemcpyDeviceToHost, st));
     SYL_CUDA(cudaMemcpyAsync(h32 + 2, bt_off.p + nb, 4, cudaMemcpyDeviceToHost, st));
@@ -351,7 +347,7 @@ static int genomes_slotted(syl_ctx *ctx, const uint8_t *d_bases, const uint32_t 
     SYL_TRY(tile_cnt.alloc(n_tiles, st)); SYL_TRY(toff.alloc(n_tiles + 1, st));
     SYL_TRY(overflow.alloc(1, st));
     SYL_CUDA(cudaMemsetAsync(overflow.p, 0, 4, st));
-    SYL_CUDA(cudaMemsetAsync(ctx->d_counters, 0, 2 * sizeof(uint64_t), st));
+    SYL_CUDA(cudaMemsetAsync(ctx->d_counters, 0, 2 * sizeof(uint64_t), st));  // CNT_EVENTS, CNT_PENDING
     SeedJob job;
     job.d_bases = d_bases; job.d_packed = d_packed; job.n_bases = n_bases; job.d_rec_off = d_contig_off; job.off_bias = 0; job.n_rec = n_contigs;
     job.k = k; job.c = c; job.sem = sem; job.with_pos = 1; job.d_out = slots.p; job.cap = n_tiles * GEN_SLOT;
@@ -402,8 +398,8 @@ static int genomes_sorted(syl_ctx *ctx, const uint8_t *d_bases, const uint32_t *
         ctx->launches += 2;
     }
     sv.release();
-    // seed_device left N (< 2^32 - 1) in the u64 d_counters[0]: its low word is the back half's count
-    return genomes_back_half(ctx, kt_post, key_b.p, hash_b.p, reinterpret_cast<const uint32_t *>(ctx->d_counters), NA, nullptr,
+    // seed_device left N (< 2^32 - 1) in the u64 slot CNT_EVENTS: its low word is the back half's count
+    return genomes_back_half(ctx, kt_post, key_b.p, hash_b.p, reinterpret_cast<const uint32_t *>(ctx->d_counters + CNT_EVENTS), NA, nullptr,
                              d_contig_off, d_genome_off, n_genomes, min_spacing, pseudotax, out);
 }
 
@@ -434,8 +430,7 @@ static int sketch_genomes_impl(syl_ctx *ctx, int mem, const uint8_t *bases, cons
     }
     if (c == 0) { set_error("c must be >= 1"); return SYL_ERR_ARG; }
     *out = nullptr;
-    SYL_CUDA(cudaSetDevice(ctx->device));
-    syl::tl_ctx = ctx;
+    SYL_ENTER(ctx);
     cudaStream_t st = ctx->stream;
     Staged<uint8_t> sb;  // host memory: staged copies, alive until the call's last sync
     Staged<uint32_t> sp;
@@ -452,15 +447,13 @@ static int sketch_genomes_impl(syl_ctx *ctx, int mem, const uint8_t *bases, cons
     } else {
         SYL_TRY(sg.init(ctx, mem, genome_off, n_genomes + 1));
     }
-    syl_genomes *g = new (std::nothrow) syl_genomes();
+    Handle<syl_genomes> g = new_handle<syl_genomes>(ctx);
     if (!g) return SYL_ERR_OOM;
-    g->device = ctx->device;
     g->k = k;
     g->c = c;
-    int rc = sketch_genomes_device(ctx, sb.p, sp.p, n_bases, sc.p, n_contigs, sg.p, n_genomes, k, c, min_spacing,
-                                   pseudotax, sem, g);
-    if (rc != SYL_OK) { syl_genomes_free(g); return rc; }
-    *out = g;
+    SYL_TRY(sketch_genomes_device(ctx, sb.p, sp.p, n_bases, sc.p, n_contigs, sg.p, n_genomes, k, c, min_spacing, pseudotax,
+                                  sem, g.get()));
+    *out = g.release();
     return SYL_OK;
 }
 
@@ -491,8 +484,7 @@ int syl_genomes_upload(syl_ctx *ctx, int mem, const uint64_t *kmers, const uint6
                        uint64_t n_genomes, int k, uint64_t c, syl_genomes **out) {
     if (!ctx || !out || !kmer_off) { set_error("NULL argument"); return SYL_ERR_ARG; }
     *out = nullptr;
-    SYL_CUDA(cudaSetDevice(ctx->device));
-    syl::tl_ctx = ctx;
+    SYL_ENTER(ctx);
     cudaStream_t st = ctx->stream;
     cudaMemcpyKind kind = mem == SYL_MEM_DEVICE ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice;
     uint64_t nk = 0, nt = 0;
@@ -500,45 +492,37 @@ int syl_genomes_upload(syl_ctx *ctx, int mem, const uint64_t *kmers, const uint6
         nk = kmer_off[n_genomes];
         nt = tracked_off ? tracked_off[n_genomes] : 0;
     } else {
-        SYL_CUDA(cudaMemcpyAsync(ctx->h_counters + 8, kmer_off + n_genomes, 8, cudaMemcpyDeviceToHost, st));
-        if (tracked_off) SYL_CUDA(cudaMemcpyAsync(ctx->h_counters + 9, tracked_off + n_genomes, 8, cudaMemcpyDeviceToHost, st));
+        SYL_CUDA(cudaMemcpyAsync(ctx->h_counters + CNT_KMER_TOTAL, kmer_off + n_genomes, 8, cudaMemcpyDeviceToHost, st));
+        if (tracked_off) SYL_CUDA(cudaMemcpyAsync(ctx->h_counters + CNT_TRACKED_TOTAL, tracked_off + n_genomes, 8, cudaMemcpyDeviceToHost, st));
         SYL_CUDA(cudaStreamSynchronize(st));
-        nk = ctx->h_counters[8];
-        nt = tracked_off ? ctx->h_counters[9] : 0;
+        nk = ctx->h_counters[CNT_KMER_TOTAL];
+        nt = tracked_off ? ctx->h_counters[CNT_TRACKED_TOTAL] : 0;
     }
-    // tracked_off says whether the sketches carry tracked k-mers; tracked may be NULL when there are none (an empty
-    // torch tensor has no address)
-    if (nt && !tracked) { set_error("tracked_off counts tracked k-mers but tracked is NULL"); return SYL_ERR_ARG; }
-    syl_genomes *g = new (std::nothrow) syl_genomes();
+    SYL_TRY(check_kmer_arrays(nullptr, 0, tracked, nt));  // a NULL kmers fails in its copy
+    Handle<syl_genomes> g = new_handle<syl_genomes>(ctx);
     if (!g) return SYL_ERR_OOM;
-    g->device = ctx->device; g->k = k; g->c = c;
+    g->k = k; g->c = c;
     g->has_tracked = tracked_off ? 1 : 0;
-    int rc = genomes_alloc(g, st, n_genomes, nk, nt);
-    if (rc != SYL_OK) { syl_genomes_free(g); return rc; }
-    auto fill = [&]() -> int {  // any failure below frees the handle and its blocks
-        if (nk) SYL_CUDA(cudaMemcpyAsync(g->kmers, kmers, nk * 8, kind, st));
-        SYL_CUDA(cudaMemcpyAsync(g->kmer_off, kmer_off, (n_genomes + 1) * 8, kind, st));
-        if (g->has_tracked) {
-            if (nt) SYL_CUDA(cudaMemcpyAsync(g->tracked, tracked, nt * 8, kind, st));
-            SYL_CUDA(cudaMemcpyAsync(g->tracked_off, tracked_off, (n_genomes + 1) * 8, kind, st));
-        } else {
-            SYL_CUDA(cudaMemsetAsync(g->tracked_off, 0, (n_genomes + 1) * 8, st));
-        }
-        if (gn_size && n_genomes) SYL_CUDA(cudaMemcpyAsync(g->gn_size, gn_size, n_genomes * 8, kind, st));
-        else if (n_genomes) SYL_CUDA(cudaMemsetAsync(g->gn_size, 0, n_genomes * 8, st));
-        SYL_CUDA(cudaStreamSynchronize(st));
-        return SYL_OK;
-    };
-    if ((rc = fill()) != SYL_OK) { syl_genomes_free(g); return rc; }
-    *out = g;
+    SYL_TRY(genomes_alloc(g.get(), n_genomes, nk, nt));
+    if (nk) SYL_CUDA(cudaMemcpyAsync(g->kmers, kmers, nk * 8, kind, st));
+    SYL_CUDA(cudaMemcpyAsync(g->kmer_off, kmer_off, (n_genomes + 1) * 8, kind, st));
+    if (g->has_tracked) {
+        if (nt) SYL_CUDA(cudaMemcpyAsync(g->tracked, tracked, nt * 8, kind, st));
+        SYL_CUDA(cudaMemcpyAsync(g->tracked_off, tracked_off, (n_genomes + 1) * 8, kind, st));
+    } else {
+        SYL_CUDA(cudaMemsetAsync(g->tracked_off, 0, (n_genomes + 1) * 8, st));
+    }
+    if (gn_size && n_genomes) SYL_CUDA(cudaMemcpyAsync(g->gn_size, gn_size, n_genomes * 8, kind, st));
+    else if (n_genomes) SYL_CUDA(cudaMemsetAsync(g->gn_size, 0, n_genomes * 8, st));
+    SYL_CUDA(cudaStreamSynchronize(st));
+    *out = g.release();
     return SYL_OK;
 }
 
 int syl_genomes_concat(syl_ctx *ctx, const syl_genomes *const *parts, uint32_t n_parts, syl_genomes **out) {
     if (!ctx || !out || (n_parts && !parts)) { set_error("NULL argument"); return SYL_ERR_ARG; }
     *out = nullptr;
-    SYL_CUDA(cudaSetDevice(ctx->device));
-    syl::tl_ctx = ctx;
+    SYL_ENTER(ctx);
     cudaStream_t st = ctx->stream;
     uint64_t G = 0, nk = 0, nt = 0;
     for (uint32_t i = 0; i < n_parts; i++) {
@@ -549,14 +533,11 @@ int syl_genomes_concat(syl_ctx *ctx, const syl_genomes *const *parts, uint32_t n
         }
         G += parts[i]->n; nk += parts[i]->total_kmers; nt += parts[i]->total_tracked;
     }
-    syl_genomes *g = new (std::nothrow) syl_genomes();
+    Handle<syl_genomes> g = new_handle<syl_genomes>(ctx);
     if (!g) return SYL_ERR_OOM;
-    g->device = ctx->device;
     if (n_parts) { g->k = parts[0]->k; g->c = parts[0]->c; g->has_tracked = parts[0]->has_tracked; }
-    int rc = genomes_alloc(g, st, G, nk, nt);
-    if (rc != SYL_OK) { syl_genomes_free(g); return rc; }
+    SYL_TRY(genomes_alloc(g.get(), G, nk, nt));
     uint64_t g0 = 0, k0 = 0, t0 = 0;
-    auto fill = [&]() -> int {  // any failure below frees the handle and its blocks
     for (uint32_t i = 0; i < n_parts; i++) {
         const syl_genomes *p = parts[i];
         if (p->total_kmers) SYL_CUDA(cudaMemcpyAsync(g->kmers + k0, p->kmers, p->total_kmers * 8, cudaMemcpyDeviceToDevice, st));
@@ -573,18 +554,14 @@ int syl_genomes_concat(syl_ctx *ctx, const syl_genomes *const *parts, uint32_t n
     }
     SYL_CUDA(cudaGetLastError());
     SYL_CUDA(cudaStreamSynchronize(st));
-    return SYL_OK;
-    };
-    if ((rc = fill()) != SYL_OK) { syl_genomes_free(g); return rc; }
-    *out = g;
+    *out = g.release();
     return SYL_OK;
 }
 
 int syl_genomes_select(syl_ctx *ctx, const syl_genomes *g, const uint32_t *idx, uint32_t n, syl_genomes **out) {
     if (!ctx || !g || !out || (n && !idx)) { set_error("NULL argument"); return SYL_ERR_ARG; }
     *out = nullptr;
-    SYL_CUDA(cudaSetDevice(ctx->device));
-    syl::tl_ctx = ctx;
+    SYL_ENTER(ctx);
     cudaStream_t st = ctx->stream;
     std::vector<uint64_t> koff(g->n + 1), toff(g->n + 1), gs(std::max<uint64_t>(g->n, 1));
     SYL_CUDA(cudaMemcpyAsync(koff.data(), g->kmer_off, (g->n + 1) * 8, cudaMemcpyDeviceToHost, st));
@@ -600,29 +577,24 @@ int syl_genomes_select(syl_ctx *ctx, const syl_genomes *g, const uint32_t *idx, 
         ngs[i] = gs[a];
         src[4 * i] = koff[a]; src[4 * i + 1] = nko[i]; src[4 * i + 2] = toff[a]; src[4 * i + 3] = nto[i];
     }
-    syl_genomes *o = new (std::nothrow) syl_genomes();
+    Handle<syl_genomes> o = new_handle<syl_genomes>(ctx);
     if (!o) return SYL_ERR_OOM;
-    o->device = ctx->device; o->k = g->k; o->c = g->c; o->has_tracked = g->has_tracked;
-    int rc = genomes_alloc(o, st, n, nko[n], nto[n]);
-    if (rc != SYL_OK) { syl_genomes_free(o); return rc; }
+    o->k = g->k; o->c = g->c; o->has_tracked = g->has_tracked;
+    SYL_TRY(genomes_alloc(o.get(), n, nko[n], nto[n]));
     DevBuf<uint64_t> d_src;
-    if ((rc = d_src.alloc(4 * (uint64_t)std::max<uint32_t>(n, 1), st)) != SYL_OK) { syl_genomes_free(o); return rc; }
-    auto fill = [&]() -> int {  // any failure below frees the handle and its blocks
-        SYL_CUDA(cudaMemcpyAsync(o->kmer_off, nko.data(), (n + 1) * 8, cudaMemcpyHostToDevice, st));
-        SYL_CUDA(cudaMemcpyAsync(o->tracked_off, nto.data(), (n + 1) * 8, cudaMemcpyHostToDevice, st));
-        if (n) {
-            SYL_CUDA(cudaMemcpyAsync(o->gn_size, ngs.data(), (size_t)n * 8, cudaMemcpyHostToDevice, st));
-            SYL_CUDA(cudaMemcpyAsync(d_src.p, src.data(), (size_t)n * 32, cudaMemcpyHostToDevice, st));
-            k_copy_ranges<<<n, 256, 0, st>>>(d_src.p, g->kmers, g->tracked, o->kmers,
-                                             o->tracked, o->kmer_off, o->tracked_off);
-            ctx->launches++;
-            SYL_CUDA(cudaGetLastError());
-        }
-        SYL_CUDA(cudaStreamSynchronize(st));
-        return SYL_OK;
-    };
-    if ((rc = fill()) != SYL_OK) { syl_genomes_free(o); return rc; }
-    *out = o;
+    SYL_TRY(d_src.alloc(4 * (uint64_t)std::max<uint32_t>(n, 1), st));
+    SYL_CUDA(cudaMemcpyAsync(o->kmer_off, nko.data(), (n + 1) * 8, cudaMemcpyHostToDevice, st));
+    SYL_CUDA(cudaMemcpyAsync(o->tracked_off, nto.data(), (n + 1) * 8, cudaMemcpyHostToDevice, st));
+    if (n) {
+        SYL_CUDA(cudaMemcpyAsync(o->gn_size, ngs.data(), (size_t)n * 8, cudaMemcpyHostToDevice, st));
+        SYL_CUDA(cudaMemcpyAsync(d_src.p, src.data(), (size_t)n * 32, cudaMemcpyHostToDevice, st));
+        k_copy_ranges<<<n, 256, 0, st>>>(d_src.p, g->kmers, g->tracked, o->kmers,
+                                         o->tracked, o->kmer_off, o->tracked_off);
+        ctx->launches++;
+        SYL_CUDA(cudaGetLastError());
+    }
+    SYL_CUDA(cudaStreamSynchronize(st));
+    *out = o.release();
     return SYL_OK;
 }
 
@@ -636,8 +608,7 @@ uint64_t syl_genomes_c(const syl_genomes *g) { return g ? g->c : 0; }
 int syl_genomes_download(syl_ctx *ctx, const syl_genomes *g, uint64_t *kmers, uint64_t *kmer_off,
                          uint64_t *tracked, uint64_t *tracked_off, uint64_t *gn_size) {
     if (!ctx || !g) { set_error("NULL argument"); return SYL_ERR_ARG; }
-    SYL_CUDA(cudaSetDevice(ctx->device));
-    syl::tl_ctx = ctx;
+    SYL_ENTER(ctx);
     cudaStream_t st = ctx->stream;
     if (kmers && g->total_kmers) SYL_CUDA(cudaMemcpyAsync(kmers, g->kmers, g->total_kmers * 8, cudaMemcpyDeviceToHost, st));
     if (kmer_off) SYL_CUDA(cudaMemcpyAsync(kmer_off, g->kmer_off, (g->n + 1) * 8, cudaMemcpyDeviceToHost, st));

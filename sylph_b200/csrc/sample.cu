@@ -678,8 +678,8 @@ struct SampleBuilder {
     uint32_t nbk = 0, ng = 0, slot = 0;
     uint64_t Mb = 0;
     DevBuf<uint32_t> g_cnt;  // events per group
-    // ctx->d_counters slots: [0] events in the overflow list, [1] pending events, [2] duplicates removed; add() keeps
-    // [3] and [17] as snapshots of [1]
+    // ctx->d_counters: CNT_EVENTS (events in the overflow list), CNT_PENDING, CNT_DUPS; add() keeps CNT_PEND_MATE1 and
+    // CNT_PEND_MATE2 as snapshots of CNT_PENDING
     unsigned long long *d_count() const { return reinterpret_cast<unsigned long long *>(ctx->d_counters); }
     uint64_t ev_total() const { return (uint64_t)ng * slot + cap; }
 
@@ -710,7 +710,7 @@ struct SampleBuilder {
         if (ev_total() >= 0xFFFFFFFEull) { set_error("more than 2^32-2 survivor events in one sample"); return SYL_ERR_ARG; }
         SYL_TRY(b_ev.alloc(ev_total(), st));
         SYL_TRY(b_pend.alloc(ev_total(), st));
-        SYL_CUDA(cudaMemsetAsync(ctx->d_counters, 0, 4 * sizeof(uint64_t), st));
+        SYL_CUDA(cudaMemsetAsync(ctx->d_counters, 0, 4 * sizeof(uint64_t), st));  // CNT_EVENTS .. CNT_PEND_MATE1
         return SYL_OK;
     }
 
@@ -718,14 +718,15 @@ struct SampleBuilder {
     // reads, m[0] and m[1] for read pairs.  Each mate is seeded with the record index as read index; the seeding kernel
     // appends the events (hash, record, pair keys) to the event array.  The pending events are then completed while
     // the batch is resident: reads cut by a tile edge, whose keys come from global memory, and every event of a pair,
-    // whose keys need both mates.  d_counters[1] counts the pending events; [3] and [17] keep its value from before
-    // mate 1 and mate 2, so the batch's pending events are pend[[3] .. [1]) and mate 2's start at [17].
+    // whose keys need both mates.  CNT_PENDING counts the pending events; CNT_PEND_MATE1 / 2 keep its value from before
+    // mate 1 and mate 2, so the batch's pending events are pend[[CNT_PEND_MATE1] .. [CNT_PENDING]) and mate 2's start at
+    // [CNT_PEND_MATE2].
     int add(const Mate *m, int n_mates, uint64_t nr, uint64_t rec_base) {
         cudaStream_t st = ctx->stream;
         if (nr == 0) return SYL_OK;
         unsigned long long *dc = d_count();
         for (int i = 0; i < n_mates; i++) {
-            SYL_CUDA(cudaMemcpyAsync(dc + (i ? 17 : 3), dc + 1, 8, cudaMemcpyDeviceToDevice, st));
+            SYL_CUDA(cudaMemcpyAsync(dc + (i ? CNT_PEND_MATE2 : CNT_PEND_MATE1), dc + CNT_PENDING, 8, cudaMemcpyDeviceToDevice, st));
             SeedJob job;
             job.d_bases = m[i].bases; job.d_packed = m[i].packed; job.n_bases = m[i].nb; job.d_rec_off = m[i].off;
             job.off_bias = m[i].off_bias; job.n_rec = nr; job.k = k; job.c = c; job.sem = sem; job.with_pos = 0;
@@ -737,8 +738,8 @@ struct SampleBuilder {
         if (!paired && (no_dedup || !m[0].nb)) return SYL_OK;  // no pending events
         auto fix = paired ? (m[0].packed ? k_events_fix<true, true> : k_events_fix<false, true>)
                           : (m[0].packed ? k_events_fix<true, false> : k_events_fix<false, false>);
-        fix<<<ctx->num_sms * 2, EV_THREADS, 0, st>>>(b_ev.p, b_pend.p, dc + 3, dc + 17, dc + 1, ev_total(), m[0],
-                                                     m[n_mates - 1], rec_base, no_dedup);
+        fix<<<ctx->num_sms * 2, EV_THREADS, 0, st>>>(b_ev.p, b_pend.p, dc + CNT_PEND_MATE1, dc + CNT_PEND_MATE2, dc + CNT_PENDING,
+                                                     ev_total(), m[0], m[n_mates - 1], rec_base, no_dedup);
         ctx->launches++;
         SYL_CUDA(cudaGetLastError());
         return SYL_OK;
@@ -786,7 +787,7 @@ struct SampleBuilder {
         DevBuf<uint64_t> seg_off;
         DevBuf<uint32_t> seg_len;
         SYL_TRY(uniq.alloc(N, st)); SYL_TRY(seg_off.alloc(N + 1, st)); SYL_TRY(seg_len.alloc(N, st));
-        uint64_t *d_nruns = ctx->d_counters + 1;
+        uint64_t *d_nruns = ctx->d_counters + CNT_PENDING;
         size_t rle_bytes = 0, scan_bytes = 0;
         cub::DeviceRunLengthEncode::Encode(nullptr, rle_bytes, hs, uniq.p, seg_len.p, d_nruns, N, st);
         cub::DeviceScan::ExclusiveSum(nullptr, scan_bytes, seg_len.p, seg_off.p, N, st);
@@ -794,9 +795,9 @@ struct SampleBuilder {
         SYL_TRY(tmp2.alloc(std::max(rle_bytes, scan_bytes), st));
         size_t tb = std::max(rle_bytes, scan_bytes);
         SYL_CUDA(cub::DeviceRunLengthEncode::Encode(tmp2.p, tb, hs, uniq.p, seg_len.p, d_nruns, N, st));
-        SYL_CUDA(cudaMemcpyAsync(ctx->h_counters + 1, d_nruns, 8, cudaMemcpyDeviceToHost, st));
+        SYL_CUDA(cudaMemcpyAsync(ctx->h_counters + CNT_PENDING, d_nruns, 8, cudaMemcpyDeviceToHost, st));
         SYL_CUDA(cudaStreamSynchronize(st));
-        const uint64_t U = ctx->h_counters[1];
+        const uint64_t U = ctx->h_counters[CNT_PENDING];
         ctx->launches += 1;
         SYL_TRY(count.alloc(std::max<uint64_t>(U, 1), st));
         if (no_dedup && !paired) {
@@ -806,15 +807,15 @@ struct SampleBuilder {
             SYL_CUDA(cub::DeviceScan::ExclusiveSum(tmp2.p, tb, seg_len.p, seg_off.p, U, st));
             DevBuf<uint64_t> set;
             SYL_TRY(set.alloc(2 * N, st));
-            unsigned long long *d_ndup = reinterpret_cast<unsigned long long *>(ctx->d_counters + 2);
+            unsigned long long *d_ndup = reinterpret_cast<unsigned long long *>(ctx->d_counters + CNT_DUPS);
             SYL_CUDA(cudaMemsetAsync(d_ndup, 0, 8, st));
             if (paired) k_dedup_paired<<<nblk(U * 32, 128), 128, 0, st>>>(seg_off.p, seg_len.p, U, ord, ev_recflag, ev_p0, ev_p1, no_dedup, set.p, count.p, d_ndup);
             else k_dedup<<<nblk(U, 128), 128, 0, st>>>(seg_off.p, seg_len.p, U, ord, ev_recflag, ev_p0, ev_p1, set.p, count.p, d_ndup);
             ctx->launches += 2;
             SYL_CUDA(cudaGetLastError());
-            SYL_CUDA(cudaMemcpyAsync(ctx->h_counters + 2, d_ndup, 8, cudaMemcpyDeviceToHost, st));
+            SYL_CUDA(cudaMemcpyAsync(ctx->h_counters + CNT_DUPS, d_ndup, 8, cudaMemcpyDeviceToHost, st));
             SYL_CUDA(cudaStreamSynchronize(st));
-            *ndup_out = ctx->h_counters[2];
+            *ndup_out = ctx->h_counters[CNT_DUPS];
         }
         *U_out = U;
         return SYL_OK;
@@ -824,20 +825,14 @@ struct SampleBuilder {
     int finish(syl_sample **out, uint64_t *need_cap) {
         cudaStream_t st = ctx->stream;
         *need_cap = 0;
-        syl_sample *s = new (std::nothrow) syl_sample();
+        Handle<syl_sample> s = new_handle<syl_sample>(ctx);
         if (!s) return SYL_ERR_OOM;
-        s->device = ctx->device;
-        s->owner = ctx;
-        s->stream = ctx->stream;
         s->k = k;
         s->c = c;
         s->mean_read_length = mean_read_length;
-        auto fail = [&](int rc) { syl_sample_free(s); return rc; };
-#define SB_CUDA(x) do { cudaError_t _e = (x); if (_e != cudaSuccess) { set_error(std::string(#x) + ": " + cudaGetErrorString(_e)); return fail(_e == cudaErrorMemoryAllocation ? SYL_ERR_OOM : SYL_ERR_CUDA); } } while (0)
-        if (n_reads == 0 || expect_bases == 0) { *out = s; return SYL_OK; }
+        if (n_reads == 0 || expect_bases == 0) { *out = s.release(); return SYL_OK; }
         unsigned long long *dc = d_count();
         EventRec *ev = b_ev.p;
-        int rc;
         // ---- primary path: CTA-local grouping / dedup of the group slots (ng, slot, Mb, g_cnt: begin()).
         // The kernels read the group counts from device memory.
         const uint64_t n_slots = (uint64_t)ng * slot;
@@ -845,18 +840,17 @@ struct SampleBuilder {
         DevBuf<uint64_t> st_hash, tmp_h;
         DevBuf<uint8_t> g_fb;
         if (ng) {
-            if ((rc = st_hash.alloc(n_slots, st)) || (rc = st_cnt.alloc(n_slots, st)) ||
-                (rc = tmp_h.alloc(n_slots, st)) || (rc = tmp_c.alloc(n_slots, st)) ||  // in-kernel uniques: <= the slotted events
-                (rc = g_nuniq.alloc(ng, st)) || (rc = g_n.alloc(ng, st)) ||
-                (rc = g_fb.alloc(ng, st)) || (rc = uoff.alloc((uint64_t)ng + 1, st)) || (rc = fsz.alloc(ng, st)) ||
-                (rc = foff.alloc((uint64_t)ng + 1, st)) || (rc = g_src.alloc(ng, st)))
-                return fail(rc);
+            SYL_TRY(st_hash.alloc(n_slots, st)); SYL_TRY(st_cnt.alloc(n_slots, st));
+            SYL_TRY(tmp_h.alloc(n_slots, st)); SYL_TRY(tmp_c.alloc(n_slots, st));  // in-kernel uniques: <= the slotted events
+            SYL_TRY(g_nuniq.alloc(ng, st)); SYL_TRY(g_n.alloc(ng, st));
+            SYL_TRY(g_fb.alloc(ng, st)); SYL_TRY(uoff.alloc((uint64_t)ng + 1, st)); SYL_TRY(fsz.alloc(ng, st));
+            SYL_TRY(foff.alloc((uint64_t)ng + 1, st)); SYL_TRY(g_src.alloc(ng, st));
             auto group_dedup = paired ? k_group_dedup<true> : k_group_dedup<false>;
-            SB_CUDA(cudaFuncSetAttribute(group_dedup, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(GroupSmem)));
+            SYL_CUDA(cudaFuncSetAttribute(group_dedup, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(GroupSmem)));
             {
                 KernelTimer kt(ctx, SYL_KERNEL_GROUP_DEDUP);
                 group_dedup<<<ng, GRP_THREADS, sizeof(GroupSmem), st>>>(ev, g_cnt.p, slot, Mb, nbk, no_dedup,
-                                                                         st_hash.p, st_cnt.p, g_nuniq.p, g_n.p, g_fb.p, dc + 2);
+                                                                         st_hash.p, st_cnt.p, g_nuniq.p, g_n.p, g_fb.p, dc + CNT_DUPS);
             }
             k_scan_u32<<<1, 1024, 0, st>>>(g_nuniq.p, ng, uoff.p);
             k_fallback_sizes<<<nblk(ng, 256), 256, 0, st>>>(g_n.p, g_fb.p, ng, fsz.p);
@@ -864,19 +858,20 @@ struct SampleBuilder {
             k_compact_uniq<<<ng, 128, 0, st>>>(st_hash.p, st_cnt.p, slot, g_nuniq.p, uoff.p, g_fb.p, g_src.p, nullptr, nullptr,
                                                 tmp_h.p, tmp_c.p);
             ctx->launches += 5;
-            SB_CUDA(cudaGetLastError());
-            SB_CUDA(cudaMemcpyAsync(ctx->h_counters + 4, uoff.p + ng, 4, cudaMemcpyDeviceToHost, st));
-            SB_CUDA(cudaMemcpyAsync(ctx->h_counters + 5, foff.p + ng, 4, cudaMemcpyDeviceToHost, st));
+            SYL_CUDA(cudaGetLastError());
+            SYL_CUDA(cudaMemcpyAsync(ctx->h_counters + CNT_UNIQ_TOTAL, uoff.p + ng, 4, cudaMemcpyDeviceToHost, st));
+            SYL_CUDA(cudaMemcpyAsync(ctx->h_counters + CNT_FALLBACK_TOTAL, foff.p + ng, 4, cudaMemcpyDeviceToHost, st));
         }
-        SB_CUDA(cudaMemcpyAsync(ctx->h_counters, dc, 24, cudaMemcpyDeviceToHost, st));  // events, pending, duplicates
-        SB_CUDA(cudaStreamSynchronize(st));  // the one synchronisation of a sketch
-        const uint64_t N_ovf = ctx->h_counters[0];
-        if (N_ovf > cap) { *need_cap = N_ovf; syl_sample_free(s); return SYL_ERR_CAPACITY; }
+        SYL_CUDA(cudaMemcpyAsync(ctx->h_counters, dc, 24, cudaMemcpyDeviceToHost, st));  // CNT_EVENTS, CNT_PENDING, CNT_DUPS
+        SYL_CUDA(cudaStreamSynchronize(st));  // the one synchronisation of a sketch
+        const uint64_t N_ovf = ctx->h_counters[CNT_EVENTS];
+        if (N_ovf > cap) { *need_cap = N_ovf; return SYL_ERR_CAPACITY; }
         // the overflow list holds only events of groups past their slot, all of which are fallback groups (without
         // groups: every event)
-        const uint64_t U1 = ng ? (uint32_t)ctx->h_counters[4] : 0, NF_slots = ng ? (uint32_t)ctx->h_counters[5] : 0;
+        const uint64_t U1 = ng ? (uint32_t)ctx->h_counters[CNT_UNIQ_TOTAL] : 0;
+        const uint64_t NF_slots = ng ? (uint32_t)ctx->h_counters[CNT_FALLBACK_TOTAL] : 0;
         const uint64_t NF = NF_slots + N_ovf;
-        uint64_t ndup = ctx->h_counters[2];
+        uint64_t ndup = ctx->h_counters[CNT_DUPS];
         static const bool dbg = getenv("SYL_DEBUG_TIMING") != nullptr;
         if (dbg) fprintf(stderr, "[sample post-pass] groups %u of %u slots, overflow list %llu (cap %llu): in-kernel uniques %llu, events handed to the generic path %llu (%.2f %% of the slotted events)\n",
                          ng, slot, (unsigned long long)N_ovf, (unsigned long long)cap, (unsigned long long)U1, (unsigned long long)NF,
@@ -887,8 +882,7 @@ struct SampleBuilder {
         uint64_t U2 = 0;
         if (NF) {
             uint64_t nd2 = 0;
-            if ((rc = fh.alloc(NF, st)) || (rc = f_rf.alloc(NF, st)) || (rc = f_p0.alloc(NF, st)) || (rc = f_p1.alloc(NF, st)))
-                return fail(rc);
+            SYL_TRY(fh.alloc(NF, st)); SYL_TRY(f_rf.alloc(NF, st)); SYL_TRY(f_p0.alloc(NF, st)); SYL_TRY(f_p1.alloc(NF, st));
             if (ng) {
                 k_gather_fallback<<<ng, 256, 0, st>>>(ev, slot, g_n.p, g_fb.p, foff.p, fh.p, f_rf.p, f_p0.p, f_p1.p);
                 ctx->launches++;
@@ -898,29 +892,28 @@ struct SampleBuilder {
                                                                   f_p0.p + NF_slots, f_p1.p + NF_slots);
                 ctx->launches++;
             }
-            if ((rc = dedup_sorted(fh.p, f_rf.p, f_p0.p, f_p1.p, NF, f_uq, f_ct, &U2, &nd2)) != SYL_OK) return fail(rc);
+            SYL_TRY(dedup_sorted(fh.p, f_rf.p, f_p0.p, f_p1.p, NF, f_uq, f_ct, &U2, &nd2));
             ndup += nd2;
         }
         // exact-size result arrays; the copies are ordered on the ctx stream like every later use of the handle
         const uint64_t U = U1 + U2;
-        if ((rc = hblock_alloc(ctx, (void **)&s->hash, std::max<uint64_t>(U, 1) * 8))) return fail(rc);
-        if ((rc = hblock_alloc(ctx, (void **)&s->count, std::max<uint64_t>(U, 1) * 4))) return fail(rc);
+        SYL_TRY(hblock_alloc(ctx, (void **)&s->hash, std::max<uint64_t>(U, 1) * 8));
+        SYL_TRY(hblock_alloc(ctx, (void **)&s->count, std::max<uint64_t>(U, 1) * 4));
         if (ng && U2) {  // slot the generic path's pairs into their groups' positions, compact straight into the result
             k_fallback_place<<<nblk(ng, 128), 128, 0, st>>>(g_fb.p, ng, nbk, Mb, f_uq.p, U2, g_nuniq.p, g_src.p);
             k_scan_u32<<<1, 1024, 0, st>>>(g_nuniq.p, ng, uoff.p);
             k_compact_uniq<<<ng, 128, 0, st>>>(st_hash.p, st_cnt.p, slot, g_nuniq.p, uoff.p, g_fb.p, g_src.p, f_uq.p, f_ct.p,
                                                 s->hash, s->count);
             ctx->launches += 3;
-            SB_CUDA(cudaGetLastError());
+            SYL_CUDA(cudaGetLastError());
         } else if (U) {  // the in-kernel uniques, or without groups the generic path's
-            SB_CUDA(cudaMemcpyAsync(s->hash, ng ? tmp_h.p : f_uq.p, U * 8, cudaMemcpyDeviceToDevice, st));
-            SB_CUDA(cudaMemcpyAsync(s->count, ng ? tmp_c.p : f_ct.p, U * 4, cudaMemcpyDeviceToDevice, st));
+            SYL_CUDA(cudaMemcpyAsync(s->hash, ng ? tmp_h.p : f_uq.p, U * 8, cudaMemcpyDeviceToDevice, st));
+            SYL_CUDA(cudaMemcpyAsync(s->count, ng ? tmp_c.p : f_ct.p, U * 4, cudaMemcpyDeviceToDevice, st));
         }
-        if (NF) SB_CUDA(cudaStreamSynchronize(st));  // f_uq / f_ct go out of scope
-#undef SB_CUDA
+        if (NF) SYL_CUDA(cudaStreamSynchronize(st));  // f_uq / f_ct go out of scope
         s->n = U;
         s->num_dup_removed = ndup;
-        *out = s;
+        *out = s.release();
         return SYL_OK;
     }
 };
@@ -1261,8 +1254,7 @@ static int sketch_reads_impl(syl_ctx *ctx, int mem, bool packed, const Mate *m, 
     if (c == 0) { set_error("c must be >= 1"); return SYL_ERR_ARG; }
     if (mem != SYL_MEM_HOST && mem != SYL_MEM_DEVICE) { set_error("bad mem"); return SYL_ERR_ARG; }
     *out = nullptr;
-    SYL_CUDA(cudaSetDevice(ctx->device));
-    syl::tl_ctx = ctx;
+    SYL_ENTER(ctx);
     const bool fed = mem == SYL_MEM_HOST && !packed;
     Mate dm[2] = {};  // the mates on the device, unless fed
     Staged<uint32_t> sp[2];
@@ -1389,35 +1381,29 @@ int syl_sample_upload(syl_ctx *ctx, int mem, const uint64_t *hash, const uint32_
                       uint64_t n, int k, uint64_t c, syl_sample **out) {
     if (!ctx || !out || (n && (!hash || !count))) { set_error("NULL argument"); return SYL_ERR_ARG; }
     *out = nullptr;
-    SYL_CUDA(cudaSetDevice(ctx->device));
-    syl::tl_ctx = ctx;
+    SYL_ENTER(ctx);
     cudaStream_t st = ctx->stream;
-    syl_sample *s = new (std::nothrow) syl_sample();
+    Handle<syl_sample> s = new_handle<syl_sample>(ctx);
     if (!s) return SYL_ERR_OOM;
-    s->device = ctx->device; s->owner = ctx; s->stream = st; s->k = k; s->c = c; s->n = n;
-    auto fill = [&]() -> int {  // any failure below frees the handle and its blocks
-        SYL_TRY(hblock_alloc(ctx, (void **)&s->hash, std::max<uint64_t>(n, 1) * 8));
-        SYL_TRY(hblock_alloc(ctx, (void **)&s->count, std::max<uint64_t>(n, 1) * 4));
-        if (n) {
-            DevBuf<uint64_t> kin;
-            DevBuf<uint32_t> vin;
-            SYL_TRY(kin.alloc(n, st)); SYL_TRY(vin.alloc(n, st));
-            cudaMemcpyKind kind = mem == SYL_MEM_DEVICE ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice;
-            SYL_CUDA(cudaMemcpyAsync(kin.p, hash, n * 8, kind, st));
-            SYL_CUDA(cudaMemcpyAsync(vin.p, count, n * 4, kind, st));
-            size_t tb = 0;
-            cub::DeviceRadixSort::SortPairs(nullptr, tb, kin.p, s->hash, vin.p, s->count, n, 0, 64, st);
-            DevBuf<uint8_t> tmp;
-            SYL_TRY(tmp.alloc(tb, st));
-            SYL_CUDA(cub::DeviceRadixSort::SortPairs(tmp.p, tb, kin.p, s->hash, vin.p, s->count, n, 0, 64, st));
-            ctx->launches += 8;
-            SYL_CUDA(cudaStreamSynchronize(st));
-        }
-        return SYL_OK;
-    };
-    const int frc = fill();
-    if (frc != SYL_OK) { syl_sample_free(s); return frc; }
-    *out = s;
+    s->k = k; s->c = c; s->n = n;
+    SYL_TRY(hblock_alloc(ctx, (void **)&s->hash, std::max<uint64_t>(n, 1) * 8));
+    SYL_TRY(hblock_alloc(ctx, (void **)&s->count, std::max<uint64_t>(n, 1) * 4));
+    if (n) {
+        DevBuf<uint64_t> kin;
+        DevBuf<uint32_t> vin;
+        SYL_TRY(kin.alloc(n, st)); SYL_TRY(vin.alloc(n, st));
+        cudaMemcpyKind kind = mem == SYL_MEM_DEVICE ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice;
+        SYL_CUDA(cudaMemcpyAsync(kin.p, hash, n * 8, kind, st));
+        SYL_CUDA(cudaMemcpyAsync(vin.p, count, n * 4, kind, st));
+        size_t tb = 0;
+        cub::DeviceRadixSort::SortPairs(nullptr, tb, kin.p, s->hash, vin.p, s->count, n, 0, 64, st);
+        DevBuf<uint8_t> tmp;
+        SYL_TRY(tmp.alloc(tb, st));
+        SYL_CUDA(cub::DeviceRadixSort::SortPairs(tmp.p, tb, kin.p, s->hash, vin.p, s->count, n, 0, 64, st));
+        ctx->launches += 8;
+        SYL_CUDA(cudaStreamSynchronize(st));
+    }
+    *out = s.release();
     return SYL_OK;
 }
 
@@ -1428,8 +1414,7 @@ void syl_sample_set_mean_read_length(syl_sample *s, double v) { if (s) s->mean_r
 
 int syl_sample_download(syl_ctx *ctx, const syl_sample *s, uint64_t *hash, uint32_t *count) {
     if (!ctx || !s) { set_error("NULL argument"); return SYL_ERR_ARG; }
-    SYL_CUDA(cudaSetDevice(ctx->device));
-    syl::tl_ctx = ctx;
+    SYL_ENTER(ctx);
     if (s->n && hash) SYL_CUDA(cudaMemcpyAsync(hash, s->hash, s->n * 8, cudaMemcpyDeviceToHost, ctx->stream));
     if (s->n && count) SYL_CUDA(cudaMemcpyAsync(count, s->count, s->n * 4, cudaMemcpyDeviceToHost, ctx->stream));
     SYL_CUDA(cudaStreamSynchronize(ctx->stream));

@@ -137,11 +137,11 @@ int seed_device(syl_ctx *ctx, const uint8_t *d_bases, const uint32_t *d_packed, 
     job.d_bases = d_bases; job.d_packed = d_packed; job.n_bases = n_bases; job.d_rec_off = d_rec_off; job.off_bias = off_bias; job.n_rec = n_rec;
     job.k = k; job.c = c; job.sem = sem; job.with_pos = with_pos; job.d_out = d_out; job.cap = cap;
     job.d_count = reinterpret_cast<unsigned long long *>(ctx->d_counters);
-    SYL_CUDA(cudaMemsetAsync(ctx->d_counters, 0, 2 * sizeof(uint64_t), st));
+    SYL_CUDA(cudaMemsetAsync(ctx->d_counters, 0, 2 * sizeof(uint64_t), st));  // CNT_EVENTS, CNT_PENDING
     SYL_TRY(seed_enqueue(ctx, job));
-    SYL_CUDA(cudaMemcpyAsync(ctx->h_counters, ctx->d_counters, sizeof(uint64_t), cudaMemcpyDeviceToHost, st));
+    SYL_CUDA(cudaMemcpyAsync(ctx->h_counters + CNT_EVENTS, ctx->d_counters + CNT_EVENTS, 8, cudaMemcpyDeviceToHost, st));
     SYL_CUDA(cudaStreamSynchronize(st));
-    *n_out = ctx->h_counters[0];
+    *n_out = ctx->h_counters[CNT_EVENTS];
     if (*n_out > cap) {
         set_error("survivor buffer too small");
         return SYL_ERR_CAPACITY;
