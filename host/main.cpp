@@ -5,16 +5,22 @@
 // src/sketch.rs:313,371,428) while the GPU works.
 // File classification, defaults and TSV output follow the reference (src/cmdline.rs,
 // src/sketch.rs:95-127,276-479, src/contain.rs:18-94,115-351,461-480).  All compute goes through
-// the C ABI; there is no CPU path.
+// the C ABI; there is no CPU path.  --devices runs one context per listed device, each on its own worker thread.
 #include <algorithm>
+#include <atomic>
 #include <cmath>
+#include <condition_variable>
 #include <cstdio>
 #include <cstdlib>
+#include <exception>
 #include <filesystem>
 #include <future>
 #include <map>
 #include <memory>
+#include <mutex>
+#include <stdexcept>
 #include <string>
+#include <thread>
 #include <vector>
 
 #include "../include/sylph_b200.h"
@@ -26,9 +32,12 @@ using namespace host;
 
 static void info(const std::string &m) { fprintf(stderr, "INFO  [sylph-b200] %s\n", m.c_str()); }
 static void warn(const std::string &m) { fprintf(stderr, "WARN  [sylph-b200] %s\n", m.c_str()); }
+// die() exits at once and is only called on the main thread; code that may run on a worker thread throws instead
+// (fail, check), and main() prints the message and exits after every worker has stopped.
 [[noreturn]] static void die(const std::string &m) { fprintf(stderr, "ERROR [sylph-b200] %s\n", m.c_str()); exit(1); }
+[[noreturn]] static void fail(const std::string &m) { throw std::runtime_error(m); }
 static void check(int rc, const char *what) {
-    if (rc != SYL_OK) die(std::string(what) + ": " + syl_last_error());
+    if (rc != SYL_OK) fail(std::string(what) + ": " + syl_last_error());
 }
 static bool ends_with(const std::string &s, const std::string &suf) {
     return s.size() >= suf.size() && s.compare(s.size() - suf.size(), suf.size(), suf) == 0;
@@ -69,6 +78,8 @@ struct Args {
     std::string db_out = "database", sample_dir = "./", out_file, list_file;
     double min_ani = -1., min_number_kmers = 50., min_count_correct = 3., redundant_ani = 99.;
     int device = 0;
+    bool device_given = false;
+    std::vector<int> devices;  // --devices: one context per entry (a device may repeat); empty = {device}
     // test hooks (INTEGRATION.md), read once from the environment: small values make the split paths run on small inputs
     uint64_t batch_bases = 1ull << 30;  // SYL_DRIVER_BATCH_BASES: a genome batch closes once it holds this many bases
     uint64_t samples_per_call = 0;      // SYL_DRIVER_SAMPLES_PER_CALL: cap on samples per syl_query / syl_profile call (0 = none)
@@ -122,6 +133,23 @@ static void resolve_sketch_inputs(Args &a) {
         die("Sample name length is not equal to the number of reads. Exiting");
 }
 
+// --devices LIST: comma-separated CUDA device ordinals, each a plain decimal number
+static std::vector<int> parse_devices(const std::string &list) {
+    if (list.empty()) die("--devices: empty device list");
+    std::vector<int> out;
+    size_t i = 0;
+    while (i <= list.size()) {
+        size_t j = list.find(',', i);
+        if (j == std::string::npos) j = list.size();
+        const std::string t = list.substr(i, j - i);
+        if (t.empty() || t.size() > 6 || t.find_first_not_of("0123456789") != std::string::npos)
+            die("--devices " + list + ": `" + t + "` is not a device ordinal (a comma-separated list such as 0,1,2,3)");
+        out.push_back(std::stoi(t));
+        i = j + 1;
+    }
+    return out;
+}
+
 static Args parse(int argc, char **argv) {
     Args a;
     if (argc < 2) die("usage: sylph-b200 <sketch|query|profile|inspect> [options] files...");
@@ -152,7 +180,8 @@ static Args parse(int argc, char **argv) {
         else if (s == "--no-ci") a.no_ci = true;
         else if (s == "--no-adjust") a.no_adj = true;
         else if (s == "--mean-coverage") a.mean_cov = true;
-        else if (s == "--device") a.device = std::stoi(need(i));
+        else if (s == "--device") { a.device = std::stoi(need(i)); a.device_given = true; }
+        else if (s == "--devices") a.devices = parse_devices(need(i));  // driver-only
         else if (s == "-u" || s == "--estimate-unknown") a.estimate_unknown = true;
         else if (s == "-I" || s == "--read-seq-id") a.read_seq_id = std::stod(need(i));
         else if (s == "--max-db-entries") a.max_db_entries = std::max<uint64_t>(1, std::stoull(need(i)));  // driver-only
@@ -167,6 +196,8 @@ static Args parse(int argc, char **argv) {
         else if (!s.empty() && s[0] == '-') die("unknown option " + s);
         else a.files.push_back(s);
     }
+    if (a.device_given && !a.devices.empty()) die("--device and --devices exclude each other; list every device in --devices");
+    if (a.devices.empty()) a.devices.push_back(a.device);
     a.n_positional = a.files.size();
     if (!a.list_file.empty()) read_list(a.list_file, a.files, true);
     if (!(a.k == 21 || a.k == 31)) die("Only k = 21, 31 are currently supported");  // src/cmdline.rs:57
@@ -192,29 +223,120 @@ static Args parse(int argc, char **argv) {
     return a;
 }
 
+// ---- worker threads ------------------------------------------------------------------------------
+
+// Set once a worker has failed: the others take no new work item.
+static std::atomic<bool> g_abort{false};
+struct Aborted : std::exception {
+    const char *what() const noexcept override { return "aborted"; }
+};
+static void check_abort() {
+    if (g_abort) throw Aborted();
+}
+
+// -t: files being parsed, or parsed and not yet used, across every worker and queue of the process
+class ParseBudget {
+  public:
+    void reset(int n) { free_ = n; }
+    void acquire() {
+        std::unique_lock<std::mutex> lk(mu_);
+        cv_.wait(lk, [&]() { return free_ > 0 || g_abort; });
+        if (g_abort) throw Aborted();
+        free_--;
+    }
+    bool try_acquire() {
+        std::lock_guard<std::mutex> lk(mu_);
+        if (free_ <= 0) return false;
+        free_--;
+        return true;
+    }
+    void release() {
+        { std::lock_guard<std::mutex> lk(mu_); free_++; }
+        cv_.notify_one();
+    }
+    void wake() {
+        { std::lock_guard<std::mutex> lk(mu_); }
+        cv_.notify_all();
+    }
+  private:
+    std::mutex mu_;
+    std::condition_variable cv_;
+    int free_ = 1;
+};
+static ParseBudget g_parse;
+
+// Runs fn(w) for every worker w in [0, n), each on its own thread (on this one when n == 1), and joins them all.  The
+// first exception is rethrown here once every worker has stopped, so that exit() never runs beside a worker.
+template <typename F>
+static void run_workers(size_t n, F fn) {
+    if (n == 1) { fn(0); return; }
+    std::mutex mu;
+    std::exception_ptr first;
+    std::vector<std::thread> th;
+    for (size_t w = 0; w < n; w++)
+        th.emplace_back([&, w]() {
+            try {
+                fn(w);
+            } catch (...) {
+                {
+                    std::lock_guard<std::mutex> lk(mu);
+                    if (!first) first = std::current_exception();
+                }
+                g_abort = true;
+                g_parse.wake();
+            }
+        });
+    for (std::thread &t : th) t.join();
+    if (first) std::rethrow_exception(first);
+}
+
 // ---- sketching -----------------------------------------------------------------------------------
 
-// Inflate + parse `files` with up to `threads` of them in flight, handing them to `use` in order: the next files are
-// being read while the GPU sketches the current one.
+// Files inflated and parsed ahead of their use, handed out in order to whichever worker asks next: the next files are
+// being read while the GPUs sketch the current ones.  Each file in flight holds one unit of g_parse until it is used.
 struct Parsed { bool ok = false; FlatRecords recs; std::string first_id; };
-template <typename F>
-static void parse_ahead(const std::vector<std::string> &files, int threads, bool want_ids, F use) {
-    std::vector<std::future<std::unique_ptr<Parsed>>> inflight;
-    size_t next = 0;
-    auto launch = [&]() {
-        const std::string f = files[next++];
-        inflight.push_back(std::async(std::launch::async, [f, want_ids]() {
-            std::unique_ptr<Parsed> p(new Parsed());
-            p->ok = read_fastx(f, p->recs, want_ids, &p->first_id);
-            return p;
-        }));
-    };
-    for (size_t i = 0; i < files.size(); i++) {
-        while (next < files.size() && inflight.size() - i < (size_t)threads) launch();
-        std::unique_ptr<Parsed> p = inflight[i].get();
-        use(files[i], *p);
+struct ParsedFile {
+    size_t i = 0;
+    std::unique_ptr<Parsed> p;
+    ParsedFile() = default;
+    ParsedFile(const ParsedFile &) = delete;
+    ParsedFile &operator=(const ParsedFile &) = delete;
+    ~ParsedFile() { if (p) g_parse.release(); }
+};
+class ParseQueue {
+  public:
+    ParseQueue(const std::vector<std::string> &files, bool want_ids) : files_(files), want_ids_(want_ids), fut_(files.size()) {}
+    // false once every file has been taken
+    bool take(ParsedFile &out) {
+        std::unique_lock<std::mutex> lk(mu_);
+        if (taken_ == files_.size()) return false;
+        const size_t i = taken_++;
+        if (launched_ == i) {  // none of this queue's files is in flight: wait for a unit the other queues give back
+            g_parse.acquire();
+            launch();
+        }
+        while (launched_ < files_.size() && g_parse.try_acquire()) launch();
+        lk.unlock();
+        out.i = i;
+        out.p = fut_[i].get();
+        return true;
     }
-}
+  private:
+    void launch() {
+        const std::string f = files_[launched_];
+        const bool ids = want_ids_;
+        fut_[launched_++] = std::async(std::launch::async, [f, ids]() {
+            std::unique_ptr<Parsed> p(new Parsed());
+            p->ok = read_fastx(f, p->recs, ids, &p->first_id);
+            return p;
+        });
+    }
+    const std::vector<std::string> &files_;
+    const bool want_ids_;
+    std::mutex mu_;
+    std::vector<std::future<std::unique_ptr<Parsed>>> fut_;
+    size_t launched_ = 0, taken_ = 0;
+};
 
 static void store_sample(syl_ctx *ctx, syl_sample *s, const Args &a, const std::string &file, bool paired, SequencesSketch &out) {
     out.hashes.resize(syl_sample_size(s));
@@ -231,7 +353,7 @@ static bool sketch_pair_files(syl_ctx *ctx, const Args &a, const std::string &f1
     FlatRecords r1;
     const bool ok1 = read_fastx(f1, r1, false);
     std::unique_ptr<Parsed> p2 = fut.get();
-    if (!ok1 || !p2->ok) die("Paired end reading failed for '" + f1 + "' and '" + f2 + "'. Make sure the files are present or the sequences are valid.");
+    if (!ok1 || !p2->ok) fail("Paired end reading failed for '" + f1 + "' and '" + f2 + "'. Make sure the files are present or the sequences are valid.");
     const uint64_t n_pairs = std::min(r1.n(), p2->recs.n());
     syl_sample *s = nullptr;
     check(syl_sketch_read_pairs(ctx, SYL_MEM_HOST, r1.bases.data(), r1.offsets[n_pairs], r1.offsets.data(), p2->recs.bases.data(),
@@ -250,59 +372,90 @@ static bool sketch_reads_parsed(syl_ctx *ctx, const Args &a, const std::string &
     return true;
 }
 
-// sketches genome files in batches of <= ~1 Gbp through ONE syl_sketch_genomes call per batch
-static void sketch_genome_files(syl_ctx *ctx, const Args &a, const std::vector<std::string> &files, bool pseudotax,
-                                std::vector<GenomeSketch> &out) {
-    // parse ahead (-t files in flight); batches of <= ~1 Gbp go through one syl_sketch_genomes call
-    std::vector<std::unique_ptr<Parsed>> parsed(files.size());
-    {
-        size_t idx = 0;
-        parse_ahead(files, a.threads, a.individual, [&](const std::string &, Parsed &p) { parsed[idx++].reset(new Parsed(std::move(p))); });
-    }
-    size_t fi = 0;
-    while (fi < files.size()) {
+// Genome files in batches of <= batch_bases, one syl_sketch_genomes call per batch.  Batches are cut in file order
+// (whichever worker asks next cuts the next one) and their sketches are collected in batch order, so the result does not
+// depend on which context sketched which batch or when it finished.
+class GenomeBatches {
+  public:
+    GenomeBatches(const Args &a, const std::vector<std::string> &files, bool pseudotax)
+        : a_(a), files_(files), pseudotax_(pseudotax), queue_(files, a.individual) {}
+    // cut the next batch and sketch it on ctx; false once every file has been used
+    bool sketch_next(syl_ctx *ctx) {
+        check_abort();
         FlatRecords recs;
         std::vector<uint64_t> genome_off{0};
         std::vector<std::string> names, first_ids;
-        while (fi < files.size() && recs.bases.size() < a.batch_bases) {
-            const std::string &f = files[fi];
-            Parsed &p = *parsed[fi++];
-            // a file that fails half way contributes nothing (records are merged only after a complete parse)
-            if (!p.ok) { warn(f + " is not a valid fasta/fastq file; skipping."); continue; }
-            const FlatRecords &tmp = p.recs;
-            const uint64_t base = recs.bases.size();
-            recs.bases.insert(recs.bases.end(), tmp.bases.begin(), tmp.bases.end());
-            for (size_t i = 1; i < tmp.offsets.size(); i++) recs.offsets.push_back(base + tmp.offsets[i]);
-            if (!a.individual) {
-                genome_off.push_back(recs.n());
-                names.push_back(f);
-                first_ids.push_back(p.first_id);
-            } else {
-                for (size_t i = 0; i < tmp.n(); i++) { names.push_back(f); first_ids.push_back(tmp.ids[i]); }
+        size_t b = 0;
+        {
+            std::lock_guard<std::mutex> lk(cut_mu_);
+            if (done_) return false;
+            while (recs.bases.size() < a_.batch_bases) {
+                ParsedFile pf;
+                if (!queue_.take(pf)) { done_ = true; break; }
+                const std::string &f = files_[pf.i];
+                const Parsed &p = *pf.p;
+                // a file that fails half way contributes nothing (records are merged only after a complete parse)
+                if (!p.ok) { warn(f + " is not a valid fasta/fastq file; skipping."); continue; }
+                const FlatRecords &tmp = p.recs;
+                const uint64_t base = recs.bases.size();
+                recs.bases.insert(recs.bases.end(), tmp.bases.begin(), tmp.bases.end());
+                for (size_t i = 1; i < tmp.offsets.size(); i++) recs.offsets.push_back(base + tmp.offsets[i]);
+                if (!a_.individual) {
+                    genome_off.push_back(recs.n());
+                    names.push_back(f);
+                    first_ids.push_back(p.first_id);
+                } else {
+                    for (size_t i = 0; i < tmp.n(); i++) { names.push_back(f); first_ids.push_back(tmp.ids[i]); }
+                }
             }
-            parsed[fi - 1].reset();
+            b = batches_.size();
+            batches_.emplace_back();
         }
-        const uint64_t G = a.individual ? recs.n() : genome_off.size() - 1;
-        if (G == 0) continue;
+        const uint64_t G = a_.individual ? recs.n() : genome_off.size() - 1;
+        if (G == 0) return true;
         syl_genomes *g = nullptr;
         check(syl_sketch_genomes(ctx, SYL_MEM_HOST, recs.bases.data(), recs.bases.size(), recs.offsets.data(), recs.n(),
-                                 a.individual ? nullptr : genome_off.data(), G, (int)a.k, a.c, a.min_spacing, pseudotax ? 1 : 0,
-                                 a.individual ? 1 : 0, SYL_SEM_AVX2, &g), "syl_sketch_genomes");
+                                 a_.individual ? nullptr : genome_off.data(), G, (int)a_.k, a_.c, a_.min_spacing, pseudotax_ ? 1 : 0,
+                                 a_.individual ? 1 : 0, SYL_SEM_AVX2, &g), "syl_sketch_genomes");
         std::vector<uint64_t> kmers(syl_genomes_total_kmers(g)), koff(G + 1), tracked(syl_genomes_total_tracked(g)), toff(G + 1), gs(G);
         check(syl_genomes_download(ctx, g, kmers.data(), koff.data(), tracked.data(), toff.data(), gs.data()), "syl_genomes_download");
         syl_genomes_free(g);
+        std::vector<GenomeSketch> out(G);
         for (uint64_t i = 0; i < G; i++) {
-            GenomeSketch s;
+            GenomeSketch &s = out[i];
             s.genome_kmers.assign(kmers.begin() + koff[i], kmers.begin() + koff[i + 1]);
-            s.has_tracked = pseudotax;
-            if (pseudotax) s.tracked.assign(tracked.begin() + toff[i], tracked.begin() + toff[i + 1]);
+            s.has_tracked = pseudotax_;
+            if (pseudotax_) s.tracked.assign(tracked.begin() + toff[i], tracked.begin() + toff[i + 1]);
             s.file_name = names[i];
             s.first_contig_name = first_ids[i];
-            s.c = a.c; s.k = a.k; s.gn_size = gs[i]; s.min_spacing = a.min_spacing;
-            out.push_back(std::move(s));
+            s.c = a_.c; s.k = a_.k; s.gn_size = gs[i]; s.min_spacing = a_.min_spacing;
         }
-        info(std::to_string(out.size()) + " genomes processed.");
+        std::lock_guard<std::mutex> lk(cut_mu_);
+        n_done_ += G;
+        batches_[b] = std::move(out);
+        info(std::to_string(n_done_) + " genomes processed.");
+        return true;
     }
+    void collect(std::vector<GenomeSketch> &out) {
+        for (std::vector<GenomeSketch> &v : batches_)
+            for (GenomeSketch &g : v) out.push_back(std::move(g));
+    }
+  private:
+    const Args &a_;
+    const std::vector<std::string> &files_;
+    const bool pseudotax_;
+    ParseQueue queue_;
+    std::mutex cut_mu_;
+    bool done_ = false;
+    std::vector<std::vector<GenomeSketch>> batches_;
+    uint64_t n_done_ = 0;
+};
+
+static void sketch_genome_files(const std::vector<syl_ctx *> &ctxs, const Args &a, const std::vector<std::string> &files,
+                                bool pseudotax, std::vector<GenomeSketch> &out) {
+    GenomeBatches batches(a, files, pseudotax);
+    run_workers(ctxs.size(), [&](size_t w) { while (batches.sketch_next(ctxs[w])) {} });
+    batches.collect(out);
 }
 
 // Path::file_name of a sample name (src/sketch.rs:346,401): its last component, with empty and "." components ignored
@@ -316,13 +469,15 @@ static std::string name_file_component(const std::string &name) {
         if (!c.empty() && c != ".") last = c;
         i = j + 1;
     }
-    if (last.empty() || last == "..") die("Sample name `" + name + "` does not end in a file name. Exiting");
+    if (last.empty() || last == "..") fail("Sample name `" + name + "` does not end in a file name. Exiting");
     return last;
 }
 
-static int cmd_sketch(syl_ctx *ctx, const Args &a) {
+// Work items in this order: read pairs, single-end read files, genome batches; each idle context takes the next one.
+static int cmd_sketch(const std::vector<syl_ctx *> &ctxs, const Args &a) {
     const std::string dir = a.sample_dir.empty() || a.sample_dir.back() == '/' ? a.sample_dir : a.sample_dir + "/";
     const bool named = !a.sample_names.empty();
+    std::mutex dir_mu;
     // a named sketch carries its sample name and is written as <-d>/<file name of the sample name>[.paired].sylsp
     auto write_sample = [&](SequencesSketch &s, const std::string &file, size_t name, const char *suffix) {
         std::string stem = basename_of(file);
@@ -331,29 +486,40 @@ static int cmd_sketch(syl_ctx *ctx, const Args &a) {
             s.sample_name = a.sample_names[name];
             stem = name_file_component(s.sample_name);
         }
-        if (!dir.empty()) std::filesystem::create_directories(dir);
+        if (!dir.empty()) {
+            std::lock_guard<std::mutex> lk(dir_mu);
+            std::filesystem::create_directories(dir);
+        }
         const std::string path = dir + stem + suffix;
         write_sylsp(path, s);
         info("Sketching " + path + " complete.");
     };
-    for (size_t i = 0; i < a.first_pairs.size(); i++) {  // src/sketch.rs:310-364
-        SequencesSketch s;
-        if (!sketch_pair_files(ctx, a, a.first_pairs[i], a.second_pairs[i], s)) continue;
-        write_sample(s, a.first_pairs[i], i, ".paired.sylsp");
-    }
     std::vector<std::string> reads;
     for (const ReadInput &r : a.sketch_reads) reads.push_back(r.file);
-    size_t ri = 0;
-    parse_ahead(reads, a.threads, false, [&](const std::string &f, Parsed &p) {
-        const size_t name = a.sketch_reads[ri++].name;
-        SequencesSketch s;
-        if (!sketch_reads_parsed(ctx, a, f, p, s)) return;
-        write_sample(s, f, name, ".sylsp");
+    std::atomic<size_t> next_pair{0};
+    ParseQueue read_queue(reads, false);
+    GenomeBatches batches(a, a.sketch_genomes, !a.no_pseudotax);
+    run_workers(ctxs.size(), [&](size_t w) {
+        syl_ctx *ctx = ctxs[w];
+        for (size_t i; (i = next_pair++) < a.first_pairs.size();) {  // src/sketch.rs:310-364
+            check_abort();
+            SequencesSketch s;
+            if (!sketch_pair_files(ctx, a, a.first_pairs[i], a.second_pairs[i], s)) continue;
+            write_sample(s, a.first_pairs[i], i, ".paired.sylsp");
+        }
+        for (;;) {
+            check_abort();
+            ParsedFile pf;
+            if (!read_queue.take(pf)) break;
+            SequencesSketch s;
+            if (!sketch_reads_parsed(ctx, a, reads[pf.i], *pf.p, s)) continue;
+            write_sample(s, reads[pf.i], a.sketch_reads[pf.i].name, ".sylsp");
+        }
+        while (batches.sketch_next(ctx)) {}
     });
-    const std::vector<std::string> &genomes = a.sketch_genomes;
-    if (!genomes.empty()) {
+    if (!a.sketch_genomes.empty()) {
         std::vector<GenomeSketch> gs;
-        sketch_genome_files(ctx, a, genomes, !a.no_pseudotax, gs);
+        batches.collect(gs);
         if (gs.empty()) warn("No valid genomes to sketch; " + a.db_out + ".syldb is not output");
         else { write_syldb(a.db_out + ".syldb", gs); info("Wrote all genome sketches to " + a.db_out + ".syldb"); }
     }
@@ -382,7 +548,73 @@ static void print_row(FILE *o, const syl_ani_row &r, bool pseudotax, const std::
                 g.first_contig_name.c_str());
 }
 
-static int cmd_contain(syl_ctx *ctx, const Args &a, bool pseudotax) {
+// Contiguous blocks of samples, one per context, balanced by weight: sample i goes to the block its weight's midpoint
+// falls in, so every block holds at most total / n_blocks plus one sample's weight.  -> first sample of each block,
+// and the end (n_blocks + 1 entries).
+static std::vector<size_t> sample_blocks(const std::vector<uint64_t> &weight, size_t n_blocks) {
+    long double total = 0;
+    for (uint64_t w : weight) total += (long double)w;
+    std::vector<size_t> first(n_blocks + 1, weight.size());
+    long double before = 0;
+    size_t blk = 0;
+    first[0] = 0;
+    for (size_t i = 0; i < weight.size(); i++) {
+        // all weights 0: by count
+        const long double mid = total > 0 ? (before + (long double)weight[i] / 2) / total : ((long double)i + 0.5L) / weight.size();
+        const size_t b = std::min(n_blocks - 1, (size_t)(mid * n_blocks));
+        while (blk < b) first[++blk] = i;
+        before += (long double)weight[i];
+    }
+    return first;
+}
+
+// Sketch k-mers a sample is expected to bring, the weight of sample_blocks: a .sylsp's count from its header; raw reads
+// from the file size (a FASTQ byte is about half a base, gzip inflates about 4x, one k-mer per c bases)
+static uint64_t sample_weight(const std::string &f, bool sketched, uint64_t c) {
+    std::error_code ec;
+    const uint64_t bytes = std::filesystem::file_size(f, ec);
+    if (ec) return 0;
+    if (sketched) {
+        try { Reader r(f); return r.u64(); } catch (const std::exception &) { return 0; }  // read again (and reported) by its worker
+    }
+    const uint64_t bases = ends_with(f, ".gz") ? bytes * 2 : bytes / 2;
+    return bases / std::max<uint64_t>(c, 1);
+}
+
+// The rows of each sample printed in sample order, each sample as soon as it and every earlier one is done.
+class RowPrinter {
+  public:
+    RowPrinter(FILE *o, bool pseudotax, const std::vector<std::string> &names, const std::vector<GenomeSketch> &gs)
+        : o_(o), pseudotax_(pseudotax), names_(names), gs_(gs), rows_(names.size()), done_(names.size(), 0) {}
+    // sample i's rows (in the library's order), or none with `valid` false (a skipped file: no rows, no line)
+    void done(size_t i, std::vector<syl_ani_row> rows, bool valid) {
+        std::lock_guard<std::mutex> lk(mu_);
+        rows_[i] = std::move(rows);
+        done_[i] = valid ? 1 : 2;
+        for (; next_ < names_.size() && done_[next_]; next_++) {
+            std::vector<syl_ani_row> &r = rows_[next_];
+            if (!pseudotax_)  // src/contain.rs:332-334: stable sort by ANI descending
+                std::stable_sort(r.begin(), r.end(), [](const syl_ani_row &x, const syl_ani_row &y) { return x.final_est_ani > y.final_est_ani; });
+            for (const syl_ani_row &row : r) print_row(o_, row, pseudotax_, names_[next_], gs_[row.genome]);
+            if (done_[next_] == 1) info("Finished sample " + names_[next_] + ".");
+            std::vector<syl_ani_row>().swap(r);
+        }
+    }
+  private:
+    std::mutex mu_;
+    FILE *o_;
+    const bool pseudotax_;
+    const std::vector<std::string> &names_;
+    const std::vector<GenomeSketch> &gs_;
+    std::vector<std::vector<syl_ani_row>> rows_;
+    std::vector<uint8_t> done_;  // 0: pending, 1: rows, 2: skipped
+    size_t next_ = 0;
+};
+
+// One context's index: the whole db, or shards over the shared host arrays.
+struct ContextDb { syl_db *db = nullptr; syl_db_shards *shards = nullptr; };
+
+static int cmd_contain(const std::vector<syl_ctx *> &ctxs, const Args &a, bool pseudotax) {
     std::vector<std::string> db_files, genome_files, sample_files, read_files = a.reads;
     for (const std::string &f : a.files) {  // src/contain.rs:167-199
         if (is_syldb(f)) db_files.push_back(f);
@@ -400,7 +632,7 @@ static int cmd_contain(syl_ctx *ctx, const Args &a, bool pseudotax) {
         catch (const std::exception &e) { die(e.what()); }
     }
     if (!gs.empty() && gs[0].k != a.k && !genome_files.empty()) die("-k is not equal to -k found in sketches.");
-    if (!genome_files.empty()) sketch_genome_files(ctx, a, genome_files, pseudotax, gs);
+    if (!genome_files.empty()) sketch_genome_files(ctxs, a, genome_files, pseudotax, gs);
     if (gs.empty()) die("No genome sketches found; see sylph query/profile -h for help. Exiting");
     for (const GenomeSketch &g : gs) if (g.k != gs[0].k) die("Query sketches have inconsistent -k. Exiting.");
     if (pseudotax && !gs[0].has_tracked)
@@ -429,29 +661,49 @@ static int cmd_contain(syl_ctx *ctx, const Args &a, bool pseudotax) {
     uint64_t shard_cap = a.max_db_entries;
     if (a.shard_entries) shard_cap = shard_cap ? std::min(shard_cap, a.shard_entries) : a.shard_entries;
     const bool sharded = shard_cap || nk + (has_tr ? nt : 0) >= 0xFFFFFFFEull || gs.size() >= 0x7FFFFFFFull;
-    syl_db *db = nullptr;
-    syl_db_shards *shards = nullptr;
+    // every context builds its own index (or shards) from the same host arrays, which stay alive until all have
+    std::vector<ContextDb> dbs(ctxs.size());
+    run_workers(ctxs.size(), [&](size_t w) {
+        syl_ctx *ctx = ctxs[w];
+        if (!sharded) {
+            check(syl_db_build_arrays(ctx, SYL_MEM_HOST, kmers.data(), koff.data(), has_tr ? tracked.data() : nullptr,
+                                      has_tr ? toff.data() : nullptr, gsz.data(), gs.size(), (int)gs[0].k, db_c, 0, &dbs[w].db),
+                  "syl_db_build_arrays");
+            return;
+        }
+        auto create = [&](uint64_t cap) {
+            check(syl_db_shards_create(ctx, kmers.data(), koff.data(), has_tr ? tracked.data() : nullptr, has_tr ? toff.data() : nullptr,
+                                       gsz.data(), gs.size(), (int)gs[0].k, db_c, cap, &dbs[w].shards), "syl_db_shards_create");
+        };
+        create(shard_cap);
+        // without a cap the library cuts shards to this device's free memory; contexts sharing the device split it:
+        // each cuts again at its largest shard divided by the number of contexts on the device
+        const size_t share = (size_t)std::count(a.devices.begin(), a.devices.end(), a.devices[w]);
+        if (!shard_cap && share > 1) {
+            uint64_t largest = 1;
+            for (uint64_t i = 0; i < syl_db_shards_count(dbs[w].shards); i++) {
+                uint64_t g0 = 0, ng = 0, ne = 0;
+                check(syl_db_shards_range(dbs[w].shards, i, &g0, &ng, &ne), "syl_db_shards_range");
+                largest = std::max(largest, ne);
+            }
+            syl_db_shards_free(dbs[w].shards);
+            dbs[w].shards = nullptr;
+            create(std::max<uint64_t>(1, largest / share));
+        }
+    });
     if (!sharded) {
-        check(syl_db_build_arrays(ctx, SYL_MEM_HOST, kmers.data(), koff.data(), has_tr ? tracked.data() : nullptr,
-                                  has_tr ? toff.data() : nullptr, gsz.data(), gs.size(), (int)gs[0].k, db_c, 0, &db), "syl_db_build_arrays");
         std::vector<uint64_t>().swap(kmers);
         std::vector<uint64_t>().swap(tracked);
     } else {
-        check(syl_db_shards_create(ctx, kmers.data(), koff.data(), has_tr ? tracked.data() : nullptr, has_tr ? toff.data() : nullptr,
-                                   gsz.data(), gs.size(), (int)gs[0].k, db_c, shard_cap, &shards), "syl_db_shards_create");
-        const uint64_t n_shards = syl_db_shards_count(shards);
+        const uint64_t n_shards = syl_db_shards_count(dbs[0].shards);
         for (uint64_t i = 0; i < n_shards; i++) {
             uint64_t g0 = 0, ng = 0, ne = 0;
-            check(syl_db_shards_range(shards, i, &g0, &ng, &ne), "syl_db_shards_range");
+            check(syl_db_shards_range(dbs[0].shards, i, &g0, &ng, &ne), "syl_db_shards_range");
             info("Database shard " + std::to_string(i + 1) + "/" + std::to_string(n_shards) + ": genomes " + std::to_string(g0) + ".." +
                  std::to_string(g0 + ng) + ", " + std::to_string(ne) + " index entries.");
         }
     }
-    // samples
-    std::vector<syl_sample *> samples;
-    std::vector<std::string> names;
-    Args ra = a;
-    ra.k = gs[0].k;
+    // samples: raw reads, then sketches, cut into one contiguous block per context
     if (!read_files.empty() && a.c > gs[0].c) {
         for (const std::string &f : read_files) warn(f + " error: value of -c for contain is greater than the smallest value of -c for a genome sketch. Continuing without sketching.");
         read_files.clear();
@@ -461,24 +713,12 @@ static int cmd_contain(syl_ctx *ctx, const Args &a, bool pseudotax) {
             warn(f + " -k " + std::to_string(a.k) + " is not equal to -k " + std::to_string(gs[0].k) + " found in sketches. Continuing without sketching.");
         read_files.clear();
     }
-    parse_ahead(read_files, a.threads, false, [&](const std::string &f, Parsed &p) {
-        if (!p.ok) { warn(f + " is not a valid fasta/fastq file; skipping."); return; }
-        syl_sample *s = nullptr;
-        check(syl_sketch_reads(ctx, SYL_MEM_HOST, p.recs.bases.data(), p.recs.bases.size(), p.recs.offsets.data(), p.recs.n(), (int)ra.k, a.c, 0,
-                               SYL_SEM_AVX2, &s), "syl_sketch_reads");
-        samples.push_back(s);
-        names.push_back(f);
-    });
-    for (const std::string &f : sample_files) {
-        SequencesSketch sk;
-        try { sk = read_sylsp(f); } catch (const std::exception &e) { die(e.what()); }
-        if (sk.c > gs[0].c) { warn(f + " value of -c is greater than the smallest value of -c for a genome sketch. Exiting."); continue; }
-        syl_sample *s = nullptr;
-        check(syl_sample_upload(ctx, SYL_MEM_HOST, sk.hashes.data(), sk.counts.data(), sk.hashes.size(), (int)sk.k, sk.c, &s), "syl_sample_upload");
-        syl_sample_set_mean_read_length(s, sk.mean_read_length);
-        samples.push_back(s);
-        names.push_back(sk.has_sample_name ? sk.sample_name : sk.file_name);
-    }
+    const size_t n_reads = read_files.size(), n_samples = n_reads + sample_files.size();
+    std::vector<uint64_t> weight(n_samples);
+    if (ctxs.size() > 1)
+        for (size_t i = 0; i < n_samples; i++)
+            weight[i] = i < n_reads ? sample_weight(read_files[i], false, a.c) : sample_weight(sample_files[i - n_reads], true, a.c);
+    const std::vector<size_t> block = sample_blocks(weight, ctxs.size());
     FILE *o = a.out_file.empty() ? stdout : fopen(a.out_file.c_str(), "w");
     if (!o) die("cannot open output file " + a.out_file);
     if (!pseudotax)  // src/contain.rs:461-480
@@ -486,29 +726,71 @@ static int cmd_contain(syl_ctx *ctx, const Args &a, bool pseudotax) {
     else  // with -u the coverage column holds the true coverage (src/contain.rs:469-475)
         fprintf(o, "Sample_file\tGenome_file\tTaxonomic_abundance\tSequence_abundance\tAdjusted_ANI\t%s\tANI_5-95_percentile\tEff_lambda\tLambda_5-95_percentile\tMedian_cov\tMean_cov_geq1\tContainment_ind\tNaive_ANI\tkmers_reassigned\tContig_name\n",
                 a.estimate_unknown ? "True_cov" : "Eff_cov");
-    if (!samples.empty()) {
-        syl_contain_params p;
-        syl_contain_params_default(&p, (int)gs[0].k, pseudotax ? 1 : 0);
-        p.no_ci = a.no_ci; p.no_adj = a.no_adj; p.mean_coverage = a.mean_cov;
-        p.min_number_kmers = a.min_number_kmers; p.min_count_correct = a.min_count_correct;
-        p.minimum_ani = a.min_ani; p.redundant_ani = a.redundant_ani;
-        p.estimate_unknown = a.estimate_unknown ? 1 : 0; p.read_seq_id = a.read_seq_id;
+    syl_contain_params p;
+    syl_contain_params_default(&p, (int)gs[0].k, pseudotax ? 1 : 0);
+    p.no_ci = a.no_ci; p.no_adj = a.no_adj; p.mean_coverage = a.mean_cov;
+    p.min_number_kmers = a.min_number_kmers; p.min_count_correct = a.min_count_correct;
+    p.minimum_ani = a.min_ani; p.redundant_ani = a.redundant_ani;
+    p.estimate_unknown = a.estimate_unknown ? 1 : 0; p.read_seq_id = a.read_seq_id;
+    std::vector<std::string> names(n_samples);
+    RowPrinter printer(o, pseudotax, names, gs);
+    run_workers(ctxs.size(), [&](size_t w) {
+        syl_ctx *ctx = ctxs[w];
+        const size_t s_begin = block[w], s_end = block[w + 1];
+        std::vector<syl_sample *> samples;
+        std::vector<size_t> ids;  // global index of each sample of `samples`
+        // a raw read file is sketched on the context that queries it
+        std::vector<std::string> my_reads(read_files.begin() + std::min(s_begin, n_reads), read_files.begin() + std::min(s_end, n_reads));
+        ParseQueue queue(my_reads, false);
+        for (;;) {
+            check_abort();
+            ParsedFile pf;
+            if (!queue.take(pf)) break;
+            const size_t id = std::min(s_begin, n_reads) + pf.i;
+            const std::string &f = read_files[id];
+            names[id] = f;
+            if (!pf.p->ok) { warn(f + " is not a valid fasta/fastq file; skipping."); printer.done(id, {}, false); continue; }
+            const FlatRecords &r = pf.p->recs;
+            syl_sample *s = nullptr;
+            check(syl_sketch_reads(ctx, SYL_MEM_HOST, r.bases.data(), r.bases.size(), r.offsets.data(), r.n(), (int)gs[0].k, a.c, 0,
+                                   SYL_SEM_AVX2, &s), "syl_sketch_reads");
+            samples.push_back(s);
+            ids.push_back(id);
+        }
+        for (size_t id = std::max(s_begin, n_reads); id < s_end; id++) {
+            check_abort();
+            const std::string &f = sample_files[id - n_reads];
+            SequencesSketch sk = read_sylsp(f);
+            if (sk.c > gs[0].c) {
+                warn(f + " value of -c is greater than the smallest value of -c for a genome sketch. Exiting.");
+                printer.done(id, {}, false);
+                continue;
+            }
+            syl_sample *s = nullptr;
+            check(syl_sample_upload(ctx, SYL_MEM_HOST, sk.hashes.data(), sk.counts.data(), sk.hashes.size(), (int)sk.k, sk.c, &s), "syl_sample_upload");
+            syl_sample_set_mean_read_length(s, sk.mean_read_length);
+            samples.push_back(s);
+            ids.push_back(id);
+            names[id] = sk.has_sample_name ? sk.sample_name : sk.file_name;
+        }
         // sample batches sized so that samples x genomes stays below the library's per-call limits (2^31 pairs,
         // 8 GB of per-pair histograms = 2^23 pairs); the reference walks the samples in chunks too (src/contain.rs:239-263).
         // Shards take every sample in one call (the library batches them per shard), so each shard is built once.
+        const ContextDb &db = dbs[w];
         size_t per_call = std::max<size_t>(1, std::min<size_t>(samples.size(), (size_t)((1ull << 22) / std::max<size_t>(gs.size(), 1))));
         if (a.samples_per_call) per_call = std::min<size_t>(per_call, a.samples_per_call);
-        if (shards) per_call = samples.size();
+        if (db.shards) per_call = std::max<size_t>(1, samples.size());
         for (size_t s0 = 0; s0 < samples.size(); s0 += per_call) {
+            check_abort();
             const size_t ns = std::min(per_call, samples.size() - s0);
             std::vector<syl_ani_row> rows(a.rows0 ? a.rows0 : std::max<size_t>(1024, std::min<size_t>(gs.size() * ns, 1u << 22)));
             uint64_t n = 0;
             for (;;) {
-                int rc = shards ? (pseudotax ? syl_profile_shards : syl_query_shards)(ctx, shards, samples.data() + s0, (uint32_t)ns, &p,
-                                                                                      rows.data(), rows.size(), &n)
-                                : (pseudotax ? syl_profile : syl_query)(ctx, db, samples.data() + s0, (uint32_t)ns, &p, rows.data(), rows.size(), &n);
+                int rc = db.shards ? (pseudotax ? syl_profile_shards : syl_query_shards)(ctx, db.shards, samples.data() + s0, (uint32_t)ns, &p,
+                                                                                          rows.data(), rows.size(), &n)
+                                   : (pseudotax ? syl_profile : syl_query)(ctx, db.db, samples.data() + s0, (uint32_t)ns, &p, rows.data(), rows.size(), &n);
                 if (rc == SYL_ERR_CAPACITY) { rows.resize(n); continue; }  // shards: the retry copies out the kept rows
-                check(rc, shards ? (pseudotax ? "syl_profile_shards" : "syl_query_shards") : (pseudotax ? "syl_profile" : "syl_query"));
+                check(rc, db.shards ? (pseudotax ? "syl_profile_shards" : "syl_query_shards") : (pseudotax ? "syl_profile" : "syl_query"));
                 break;
             }
             rows.resize(n);
@@ -516,19 +798,17 @@ static int cmd_contain(syl_ctx *ctx, const Args &a, bool pseudotax) {
             for (uint32_t s = 0; s < ns; s++) {
                 size_t j = i;
                 while (j < rows.size() && rows[j].sample == s) j++;
-                if (!pseudotax)  // src/contain.rs:332-334: stable sort by ANI descending
-                    std::stable_sort(rows.begin() + i, rows.begin() + j,
-                                     [](const syl_ani_row &x, const syl_ani_row &y) { return x.final_est_ani > y.final_est_ani; });
-                for (size_t r = i; r < j; r++) print_row(o, rows[r], pseudotax, names[s0 + s], gs[rows[r].genome]);
-                info("Finished sample " + names[s0 + s] + ".");
+                printer.done(ids[s0 + s], std::vector<syl_ani_row>(rows.begin() + i, rows.begin() + j), true);
                 i = j;
             }
         }
-    }
+        for (syl_sample *s : samples) syl_sample_free(s);
+    });
     if (o != stdout) fclose(o);
-    for (syl_sample *s : samples) syl_sample_free(s);
-    syl_db_free(db);
-    syl_db_shards_free(shards);
+    for (ContextDb &db : dbs) {
+        syl_db_free(db.db);
+        syl_db_shards_free(db.shards);
+    }
     info("sylph finished.");
     return 0;
 }
@@ -544,6 +824,20 @@ static int cmd_fastx_stats(const Args &a) {
         for (size_t i = 0; i < recs.n(); i++) { h ^= recs.offsets[i + 1] - recs.offsets[i]; h *= 1099511628211ull; }
         for (const std::string &id : recs.ids) for (char c : id) { h ^= (uint8_t)c; h *= 1099511628211ull; }
         printf("%s\t%zu\t%zu\t%016llx\t%s\n", f.c_str(), recs.n(), recs.bases.size(), (unsigned long long)h, first.c_str());
+    }
+    return 0;
+}
+
+// sample-blocks: the split of samples of these weights over the --devices contexts, without a device
+// (first sample, samples and total weight of each block)
+static int cmd_sample_blocks(const Args &a) {
+    std::vector<uint64_t> w;
+    for (const std::string &f : a.files) w.push_back(std::stoull(f));
+    const std::vector<size_t> first = sample_blocks(w, a.devices.size());
+    for (size_t b = 0; b + 1 < first.size(); b++) {
+        uint64_t sum = 0;
+        for (size_t i = first[b]; i < first[b + 1]; i++) sum += w[i];
+        printf("%zu\t%zu\t%llu\n", first[b], first[b + 1] - first[b], (unsigned long long)sum);
     }
     return 0;
 }
@@ -586,15 +880,22 @@ int main(int argc, char **argv) {
     host::inflate_threads() = std::max(1, a.threads);  // BGZF members of one file are inflated by this many threads
     if (a.cmd == "fastx-stats") return cmd_fastx_stats(a);
     if (a.cmd == "inspect") return cmd_inspect(a);
-    syl_ctx *ctx = nullptr;
-    check(syl_ctx_create(a.device, nullptr, &ctx), "syl_ctx_create");
+    if (a.cmd == "sample-blocks") return cmd_sample_blocks(a);
+    g_parse.reset(a.threads);
+    // every context exists before the first sketch call: a context's packer pool is sized by the live contexts
+    std::vector<syl_ctx *> ctxs(a.devices.size(), nullptr);
+    for (size_t i = 0; i < ctxs.size(); i++) {
+        int rc = syl_ctx_create(a.devices[i], nullptr, &ctxs[i]);
+        if (rc != SYL_OK) die(std::string("syl_ctx_create") + (a.devices.size() > 1 ? " (device " + std::to_string(a.devices[i]) + ")" : "") +
+                              ": " + syl_last_error());
+    }
     int rc;
-    try {  // e.g. a sketch path that cannot be written: exit 1 with the message instead of aborting
-        if (a.cmd == "sketch") rc = cmd_sketch(ctx, a);
-        else if (a.cmd == "query") rc = cmd_contain(ctx, a, false);
-        else if (a.cmd == "profile") rc = cmd_contain(ctx, a, true);
+    try {  // e.g. a sketch path that cannot be written, or a library error on any context: exit 1 with the message
+        if (a.cmd == "sketch") rc = cmd_sketch(ctxs, a);
+        else if (a.cmd == "query") rc = cmd_contain(ctxs, a, false);
+        else if (a.cmd == "profile") rc = cmd_contain(ctxs, a, true);
         else die("unknown command " + a.cmd + " (sketch | query | profile | inspect)");
     } catch (const std::exception &e) { die(e.what()); }
-    syl_ctx_destroy(ctx);
+    for (syl_ctx *ctx : ctxs) syl_ctx_destroy(ctx);
     return rc;
 }

@@ -6,6 +6,7 @@
 #include <new>
 
 #include "common.cuh"
+#include "host_pack.hpp"
 
 namespace syl {
 
@@ -113,6 +114,7 @@ int syl_ctx_create(int device, void *stream, syl_ctx **out) {
     {
         std::lock_guard<std::mutex> lk(g_live_mu);
         g_live_ctx.push_back(ctx);
+        note_context(+1);
     }
     *out = ctx;
     return SYL_OK;
@@ -122,7 +124,9 @@ void syl_ctx_destroy(syl_ctx *ctx) {
     if (!ctx) return;
     {
         std::lock_guard<std::mutex> lk(g_live_mu);
-        g_live_ctx.erase(std::remove(g_live_ctx.begin(), g_live_ctx.end(), ctx), g_live_ctx.end());
+        const auto it = std::remove(g_live_ctx.begin(), g_live_ctx.end(), ctx);
+        if (it != g_live_ctx.end()) note_context(-1);  // not when a failed syl_ctx_create cleans up
+        g_live_ctx.erase(it, g_live_ctx.end());
     }
     cudaSetDevice(ctx->device);
     if (ctx->stream) cudaStreamSynchronize(ctx->stream);

@@ -1293,8 +1293,12 @@ static int job_bootstrap(syl_profile_job *j, void *tab) {
     // reject[0..R) only, reject[R] is k_boot_iter_p's work counter and stays zero
     if (getenv("SYL_BOOT_REPLAY") != nullptr) SYL_CUDA(cudaMemsetAsync(j->reject.p, 1, (size_t)j->R * 4, st));
     KernelTimer kt(ctx, SYL_KERNEL_BOOT);
-    static int boot_ctas = 0;  // resident CTAs per SM (a partially filled second wave would double the tail)
-    if (!boot_ctas && cudaOccupancyMaxActiveBlocksPerMultiprocessor(&boot_ctas, k_boot_iter_p, BOOT_THREADS, 0) != cudaSuccess) boot_ctas = 4;
+    // resident CTAs per SM (a partially filled second wave would double the tail); initialised once, because contexts
+    // on other threads of the process may get here at the same time
+    static const int boot_ctas = []() {
+        int n = 0;
+        return cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, k_boot_iter_p, BOOT_THREADS, 0) == cudaSuccess ? n : 4;
+    }();
     k_boot_iter_p<<<ctx->num_sms * std::max(boot_ctas, 1), BOOT_THREADS, 0, st>>>(j->hist.p, &t->n_boot, j->R, j->P, j->res_ani.p, j->res_lambda.p, j->res_ok.p, j->reject.p, j->reject.p + j->R);
     k_boot_seq<<<nblk(j->R, 32), 32, 0, st>>>(j->hist.p, (uint32_t)j->R, j->P, j->reject.p, j->res_ani.p, j->res_lambda.p, j->res_ok.p, &t->n_boot);
     k_boot_final<<<(unsigned)j->R, 128, 0, st>>>(j->boot_rows.p, (uint32_t)j->R, j->res_ani.p, j->res_lambda.p, j->res_ok.p, table_rows(tab), &t->n_boot);

@@ -8,6 +8,7 @@
 #include <stdlib.h>
 #include <string.h>
 
+#include <atomic>
 #include <chrono>
 
 #include <algorithm>
@@ -143,11 +144,12 @@ void pack2_range(const uint8_t *bases, uint64_t n_bases, uint32_t *words) {
     else pack2_scalar(bases, n_bases, words);
 }
 
-int default_pack_threads() {
-    if (const char *e = getenv("SYL_PACK_THREADS")) {
-        const int v = atoi(e);
-        if (v > 0) return std::min(v, 512);
-    }
+static std::atomic<int> g_live_contexts{0};
+void note_context(int delta) { g_live_contexts += delta; }
+int live_contexts() { return std::max(1, g_live_contexts.load()); }
+
+// the packer threads of one process (every context of it together)
+static int process_pack_threads() {
     unsigned hc = std::thread::hardware_concurrency();
     if (!hc) hc = 1;
     unsigned lw = 1;
@@ -176,6 +178,16 @@ int default_pack_threads() {
     }
     // the packer is memory-bound well before all cores of a big host are busy
     return (int)std::max(1u, std::min(hc > 2 ? hc / 2u : hc, 32u));
+}
+
+// The share of one context: the process's share divided by its live contexts.  The division comes after the cap of 32
+// because that cap stands for the host's memory system, which the contexts of one process share as well.
+int default_pack_threads() {
+    if (const char *e = getenv("SYL_PACK_THREADS")) {
+        const int v = atoi(e);
+        if (v > 0) return std::min(v, 512);
+    }
+    return std::max(1, process_pack_threads() / live_contexts());
 }
 
 PackPool::PackPool(int n_threads) {

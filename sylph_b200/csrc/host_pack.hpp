@@ -61,6 +61,13 @@ private:
     int64_t gate_ = -1;
 };
 
+// Live contexts of this process (syl_ctx_create / syl_ctx_destroy): contexts share the host's cores and memory
+// system, so the packer pool of a context and the ASCII-or-packed choice count them as well as LOCAL_WORLD_SIZE.
+void note_context(int delta);
+int live_contexts();  // at least 1
+
+// Packer threads of a new pool: SYL_PACK_THREADS, else this process's share of the host (cores, container quota,
+// LOCAL_WORLD_SIZE) divided by live_contexts().
 int default_pack_threads();
 
 }  // namespace syl

@@ -1235,11 +1235,13 @@ static int feed_host(syl_ctx *ctx, SampleBuilder &b, const Mate *m, int n_mates,
 // per base), so it pays while PCIe is the narrow resource — 1 to 4 processes per host — and loses once the ranks of
 // a host saturate its memory system instead (measured with 8 ranks on one host: 20.2 ms per 1 Gbp step shipping
 // ASCII, 32.7 ms packing; with 1 and 2 ranks packing wins, 10.2 vs 19.9 and 16.4 vs 19.9 ms).
-// SYL_HOST_INGEST = ascii | packed | packed-only overrides (read per call: the tests switch it at run time).
+// The producers of a host are its processes (LOCAL_WORLD_SIZE) times the live contexts of each (several devices driven
+// from one process).  SYL_HOST_INGEST = ascii | packed | packed-only overrides (read per call: the tests switch it at
+// run time).
 static bool host_ingest_ascii() {
     const char *hi_env = getenv("SYL_HOST_INGEST");
-    static const int local_ranks = []() { const char *e = getenv("LOCAL_WORLD_SIZE"); return e ? atoi(e) : 1; }();
-    return hi_env ? std::string(hi_env) == "ascii" : local_ranks > 4;
+    static const int local_ranks = []() { const char *e = getenv("LOCAL_WORLD_SIZE"); return e ? std::max(1, atoi(e)) : 1; }();
+    return hi_env ? std::string(hi_env) == "ascii" : local_ranks * live_contexts() > 4;
 }
 
 // A sample of n_reads records: reads (n_mates 1), or read pairs (n_mates 2: mate i of pair p is record p of m[i]).
