@@ -891,6 +891,15 @@ int main(int argc, char **argv) {
     }
     int rc;
     try {  // e.g. a sketch path that cannot be written, or a library error on any context: exit 1 with the message
+        // contexts that share a device split its free memory for their read sketches (a sample that does not fit its share
+        // is sketched in hash-range parts), as they split it for the database shards
+        for (size_t i = 0; i < ctxs.size(); i++) {
+            const size_t share = (size_t)std::count(a.devices.begin(), a.devices.end(), a.devices[i]);
+            if (share < 2) continue;
+            uint64_t free_b = 0;
+            check(syl_ctx_sample_memory(ctxs[i], nullptr, &free_b), "syl_ctx_sample_memory");
+            check(syl_ctx_set_sample_memory(ctxs[i], std::max<uint64_t>(1, free_b / share)), "syl_ctx_set_sample_memory");
+        }
         if (a.cmd == "sketch") rc = cmd_sketch(ctxs, a);
         else if (a.cmd == "query") rc = cmd_contain(ctxs, a, false);
         else if (a.cmd == "profile") rc = cmd_contain(ctxs, a, true);

@@ -20,7 +20,7 @@
  *   - there is NO CPU fallback: if no compute capability 9.0 device / kernel image is available, calls
  *     fail with SYL_ERR_CUDA.
  *   - hard limits (reported as SYL_ERR_ARG, never silently wrapped): fewer than 2^32-2 records per batch,
- *     fewer than 2^32-2 survivor events per sample, fewer than 2^32-2 index entries (genome_kmers + tracked)
+ *     fewer than 2^32-2 survivor events per hash-range part of a read sample (section 2), fewer than 2^32-2 index entries (genome_kmers + tracked)
  *     and 2^31 genomes per db shard (a larger database from host memory: syl_db_shards, section 6), fewer than 2^31
  *     (sample, genome) pairs per syl_query / syl_profile call.
  *     Above 2^23 pairs per call the 256-bin per-pair histograms would exceed 8 GB: syl_query / syl_profile
@@ -182,6 +182,24 @@ int syl_ctx_ingest_stats(const syl_ctx *ctx, uint64_t *h2d_bytes, uint64_t *chun
  * syl_ctx_device_bytes does not count them) and in pinned host memory.  They grow to the largest chunk seen and
  * live until the ctx is destroyed. */
 int syl_ctx_ingest_ring_bytes(const syl_ctx *ctx, uint64_t *device_bytes, uint64_t *pinned_bytes);
+/* Device memory of read and pair sketches (the four calls above).  The post-pass holds about 120 bytes per expected
+ * survivor event (bases / c), and host input adds its staging rings or, for 2-bit words, the staged words.  A sample
+ * whose one-pass estimate does not fit the budget is sketched in P parts (at most 64): contiguous hash ranges of
+ * [0, 2^64 / c), each in a pass of its own over the input (device input read in place, host 2-bit words staged once,
+ * host ASCII fed again for every part).  The parts' sketches wait in host memory and are assembled into the same
+ * sketch, num_dup_removed and mean_read_length as one pass gives.  A budget that even 64 parts exceed is SYL_ERR_OOM
+ * before anything is allocated; the message names the bytes needed.
+ * syl_ctx_set_sample_memory: max_bytes of device memory a sketch call may use (block-cache blocks plus staging rings);
+ *   0 (the default) = the device's free memory at call time plus what the ctx holds in cached free blocks and rings
+ *   (a sample whose one pass needs less than half of the free memory the ctx saw at its last look takes one pass
+ *   without looking again).
+ * syl_ctx_sample_memory: the budget set (0: default) and the device's free memory now (either pointer may be NULL),
+ *   e.g. to split one device between several contexts.
+ * syl_ctx_sample_parts: P of the last read or pair sketch of this ctx (1: one pass).
+ * SYL_SAMPLE_PARTS=N (test hook, read per call) forces N parts, at most one per post-pass bucket. */
+int syl_ctx_set_sample_memory(syl_ctx *ctx, uint64_t max_bytes);
+int syl_ctx_sample_memory(syl_ctx *ctx, uint64_t *max_bytes, uint64_t *free_bytes);
+int syl_ctx_sample_parts(const syl_ctx *ctx, uint32_t *parts);
 /* Wrap an existing sketch (e.g. a deserialised .sylsp).  Pairs need not be sorted; hashes must
  * be distinct. */
 int syl_sample_upload(syl_ctx *ctx, int mem, const uint64_t *hash, const uint32_t *count,

@@ -64,6 +64,9 @@ SIGNATURES = {
     "syl_pack_threads": (_i, []),
     "syl_ctx_ingest_stats": (_i, [_vp, _vp, _vp, _vp]),
     "syl_ctx_ingest_ring_bytes": (_i, [_vp, _pu64, _pu64]),
+    "syl_ctx_set_sample_memory": (_i, [_vp, _u64]),
+    "syl_ctx_sample_memory": (_i, [_vp, _pu64, _pu64]),
+    "syl_ctx_sample_parts": (_i, [_vp, C.POINTER(C.c_uint32)]),
     "syl_sample_upload": (_i, [_vp, _i, _vp, _vp, _u64, _i, _u64, _pp]),
     "syl_sample_size": (_u64, [_vp]),
     "syl_sample_mean_read_length": (_d, [_vp]),

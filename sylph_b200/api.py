@@ -108,6 +108,23 @@ class Context:
         _lib.check(_lib.lib().syl_ctx_ingest_ring_bytes(self._h, C.byref(d), C.byref(h)))
         return d.value, h.value
 
+    def set_sample_memory(self, max_bytes=0):
+        """Device bytes a read or pair sketch may use (syl_ctx_set_sample_memory); 0 = the free device memory at call
+        time.  A sample that does not fit is sketched in hash-range parts, with the same result."""
+        _lib.check(_lib.lib().syl_ctx_set_sample_memory(self._h, int(max_bytes)))
+
+    def sample_memory(self):
+        """-> (budget, free_bytes): the budget set (0: default) and the device's free memory now."""
+        b, f = C.c_uint64(0), C.c_uint64(0)
+        _lib.check(_lib.lib().syl_ctx_sample_memory(self._h, C.byref(b), C.byref(f)))
+        return b.value, f.value
+
+    def sample_parts(self):
+        """Hash-range parts the last read or pair sketch of this context was sketched in (1: one pass)."""
+        n = C.c_uint32(0)
+        _lib.check(_lib.lib().syl_ctx_sample_parts(self._h, C.byref(n)))
+        return n.value
+
     def device_bytes(self, reset_peak=False):
         """-> (held, peak): bytes of device memory the ctx holds, and the high-water mark of that plus the index
         build's temporaries since the last reset (syl_ctx_device_bytes)."""

@@ -60,6 +60,16 @@ void hblock_free(syl_ctx *ctx, void *p) {
 }
 void set_error(const std::string &msg) { g_last_error = msg; }
 
+int cache_trim(syl_ctx *ctx) {
+    SYL_CUDA(cudaStreamSynchronize(ctx->stream));
+    for (const auto &b : ctx->free_blocks) {
+        cudaFree(b.first);
+        ctx->cached_bytes -= b.second;
+    }
+    ctx->free_blocks.clear();
+    return SYL_OK;
+}
+
 }  // namespace syl
 
 using namespace syl;

@@ -15,6 +15,7 @@
 #include <vector>
 
 #include "../../include/sylph_b200.h"
+#include "sample_parts.hpp"
 
 namespace syl {
 
@@ -78,6 +79,11 @@ struct syl_ctx {
     size_t cached_bytes = 0;     // every block the cache has allocated: free, lent to a handle or to a live DevBuf
     size_t transient_bytes = 0;  // live temporaries allocated outside the cache (the index build's)
     size_t peak_bytes = 0;       // high-water mark of cached_bytes + transient_bytes (syl_ctx_device_bytes)
+    // read / pair sketches: device bytes a call may use (0: the free device memory at call time), and the number of
+    // hash-range parts the last one was sketched in (sample_parts.hpp)
+    uint64_t sample_budget = 0;
+    uint32_t sample_parts = 0;
+    uint64_t free_seen = 0;  // the device's free memory when a read sketch of this ctx last asked (cudaMemGetInfo)
 };
 
 namespace syl {
@@ -208,8 +214,6 @@ static_assert(sizeof(EventRec) == 32, "EventRec is one 32-byte sector");
 constexpr uint64_t NO_PAIR = 1ull;
 constexpr uint64_t EV_PENDING = 1ull << 63;
 
-constexpr uint32_t GRP_BPG = 32;  // hash buckets per read-sketch post-pass group (GroupOut in seed_kernel.cuh)
-
 // One batch for the seeding kernel (seed.cu: seed_enqueue).  Exactly one of d_bases (ASCII) / d_packed
 // (2-bit words: base 16w+j of the batch in bits [30-2j, 31-2j] of word w) is set.
 struct SeedJob {
@@ -229,7 +233,8 @@ struct SeedJob {
     uint32_t *d_pend = nullptr;           // indices of events whose pair keys are still missing
     uint32_t *d_group_cnt = nullptr;      // events: post-pass group counters (GroupOut in seed_kernel.cuh); nullptr = append
     uint64_t Mb = 0;
-    uint32_t nbk = 0, ng = 0, slot = 0;
+    uint32_t nbk = 0, ng = 0, slot = 0, g0 = 0;  // groups [g0, g0 + ng) of the map (Mb, nbk)
+    uint64_t lo = 0, hi = ~0ull;                  // events: the hashes [lo, hi) (one part of the sample)
     unsigned long long *d_count = nullptr;  // running device counters: [0] survivors / events, [1] pending events
     // slotted survivor output (genome sketching): see SlotOut in seed_kernel.cuh
     uint32_t slot_cap = 0;
@@ -239,6 +244,8 @@ uint64_t seed_cta_tiles(uint64_t n_bases);  // number of tiles of the seeding ke
 uint64_t seed_cta_tile_bases();             // window starts per tile of the seeding kernel
 int seed_enqueue(syl_ctx *ctx, const SeedJob &job);
 void ingest_destroy(syl_ctx *ctx);
+// hand the ctx's cached free blocks back to the driver (waits for the ctx stream)
+int cache_trim(syl_ctx *ctx);
 
 // stream-ordered temporary device buffer (cudaMallocAsync from the device's default pool)
 template <typename T>

@@ -1851,20 +1851,8 @@ static uint64_t shard_entries_env() {  // SYL_DB_SHARD_ENTRIES caps max_entries 
     return 0;
 }
 
-// Hand the ctx's cached free blocks back to the driver: each shard's index and join scratch are then allocated to that
-// shard's size, not next to the previous shard's.
 static double ms_since(std::chrono::steady_clock::time_point t) {
     return std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t).count();
-}
-
-static int cache_trim(syl_ctx *ctx) {
-    SYL_CUDA(cudaStreamSynchronize(ctx->stream));
-    for (const auto &b : ctx->free_blocks) {
-        cudaFree(b.first);
-        ctx->cached_bytes -= b.second;
-    }
-    ctx->free_blocks.clear();
-    return SYL_OK;
 }
 
 // The index of genomes [a, b) straight from the borrowed host arrays; only the offsets are copied (rebased to 0).
@@ -1888,6 +1876,7 @@ static int shards_sweep(syl_db_shards *s, const syl_sample *const *samples, uint
     syl_ctx *ctx = s->ctx;
     for (size_t i = 0; i + 1 < s->first.size(); i++) {
         const uint64_t a = s->first[i], G = s->first[i + 1] - a;
+        // each shard's index and join scratch are allocated to that shard's size, not next to the previous shard's
         SYL_TRY(cache_trim(ctx));
         const auto t0 = std::chrono::steady_clock::now();
         syl_db *db = nullptr;

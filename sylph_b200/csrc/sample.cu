@@ -268,8 +268,7 @@ __global__ void k_dedup(const uint64_t *__restrict__ seg_off, const uint32_t *__
 // or whose dedup set outgrows the per-thread buffer are handed to the generic radix-sort path below and
 // merged at the end.
 constexpr int GRP_THREADS = 256;
-constexpr int GRP_CAP = 1024;   // most events one CTA handles in shared memory (= slot per group)
-constexpr int GRP_T = 640;      // expected events per group: room in the slot for the spread of duplicate-heavy k-mers
+// GRP_CAP (slot per group) and GRP_T (expected events per group): sample_parts.hpp
 
 __device__ __forceinline__ uint32_t bucket_of(uint64_t h, uint64_t Mb, uint32_t nbk) {
     const uint32_t b = (uint32_t)__umul64hi(h, Mb);
@@ -346,7 +345,7 @@ __device__ __forceinline__ void pair_count(const GroupSmem &S, uint32_t a0, uint
 template <bool PAIRED>
 __global__ void __launch_bounds__(GRP_THREADS)
 k_group_dedup(const EventRec *__restrict__ ev, const uint32_t *__restrict__ g_cnt, uint32_t slot, uint64_t Mb, uint32_t nbk,
-              int no_dedup, uint64_t *__restrict__ st_hash, uint32_t *__restrict__ st_cnt,
+              uint32_t g0, int no_dedup, uint64_t *__restrict__ st_hash, uint32_t *__restrict__ st_cnt,
               uint32_t *__restrict__ g_nuniq, uint32_t *__restrict__ g_n,
               uint8_t *__restrict__ g_fallback, unsigned long long *__restrict__ n_dup) {
     extern __shared__ __align__(16) uint8_t grp_smem_raw[];
@@ -358,7 +357,7 @@ k_group_dedup(const EventRec *__restrict__ ev, const uint32_t *__restrict__ g_cn
         S.dups = 0;
         S.nlong = 0;
     }
-    const uint32_t e0 = g * slot, bf = g * GRP_BPG;
+    const uint32_t e0 = g * slot, bf = (g0 + g) * GRP_BPG;  // g0: first group of the sample's part (sample_parts.hpp)
     const uint32_t n_all = g_cnt[g], n = min(n_all, slot);  // events past the slot are in the overflow list
     if (tid == 0) { g_n[g] = n; g_nuniq[g] = 0; g_fallback[g] = n_all > slot; }
     if (n == 0 || n_all > slot) return;
@@ -603,7 +602,7 @@ __global__ void k_compact_uniq(const uint64_t *__restrict__ st_hash, const uint3
 // The generic path returns the fallback groups' unique pairs as ONE list sorted by hash.  Groups own
 // disjoint, increasing hash ranges (bucket = mulhi(hash, Mb) is monotone), so group g's slice is
 // [lower_bound(hash >= first hash of bucket bf), lower_bound(hash >= first hash of bucket be)).
-__global__ void k_fallback_place(const uint8_t *__restrict__ g_fallback, uint32_t ng, uint32_t nbk, uint64_t Mb,
+__global__ void k_fallback_place(const uint8_t *__restrict__ g_fallback, uint32_t ng, uint32_t g0, uint32_t nbk, uint64_t Mb,
                                  const uint64_t *__restrict__ f_hash, uint64_t fu, uint32_t *__restrict__ g_nuniq,
                                  uint32_t *__restrict__ g_src) {
     const uint32_t g = blockIdx.x * blockDim.x + threadIdx.x;
@@ -617,7 +616,7 @@ __global__ void k_fallback_place(const uint8_t *__restrict__ g_fallback, uint32_
         while (lo < hi) { uint64_t mid = (lo + hi) >> 1; if (f_hash[mid] < v) lo = mid + 1; else hi = mid; }
         return lo;
     };
-    const uint32_t bf = g * GRP_BPG, be = bf + GRP_BPG;
+    const uint32_t bf = (g0 + g) * GRP_BPG, be = bf + GRP_BPG;  // the part's group g is group g0 + g of the map
     const uint64_t a = bf == 0 ? 0 : lb(first_hash_of(bf));
     const uint64_t b = be >= nbk ? fu : lb(first_hash_of(be));
     g_src[g] = (uint32_t)a;
@@ -677,35 +676,34 @@ struct SampleBuilder {
     uint64_t expect_bases = 0, expect_reads = 0;
     uint32_t nbk = 0, ng = 0, slot = 0;
     uint64_t Mb = 0;
+    // the part of the sample this pass sketches (sample_parts.hpp): hashes [lo, hi), groups [g0, g0 + ng) of the map
+    uint64_t lo = 0, hi = 0;
+    uint32_t g0 = 0;
     DevBuf<uint32_t> g_cnt;  // events per group
     // ctx->d_counters: CNT_EVENTS (events in the overflow list), CNT_PENDING, CNT_DUPS; add() keeps CNT_PEND_MATE1 and
     // CNT_PEND_MATE2 as snapshots of CNT_PENDING
     unsigned long long *d_count() const { return reinterpret_cast<unsigned long long *>(ctx->d_counters); }
     uint64_t ev_total() const { return (uint64_t)ng * slot + cap; }
 
-    int begin(uint64_t cap_override) {
+    // map: the one-pass group map of the whole sample; part: the hashes this pass keeps (all of them: lo 0, hi thr).
+    // grouped: false for SYL_SAMPLE_POSTPASS=sort (no groups, every event takes the generic path).
+    int begin(const SampleMap &map, const SamplePart &part, bool grouped, uint64_t cap_override) {
         cudaStream_t st = ctx->stream;
-        const uint64_t win = expect_bases > expect_reads * (uint64_t)(k - 1) ? expect_bases - expect_reads * (uint64_t)(k - 1) : 0;
-        const uint64_t n_exp = win / c;
-        const char *pp = getenv("SYL_SAMPLE_POSTPASS");  // per call; "sort": no groups, every event takes the generic path
-        if (!(pp && std::string(pp) == "sort")) {
+        lo = part.lo;
+        hi = part.hi;
+        g0 = part.g0;
+        if (grouped) {
             static const uint32_t grp_cap = []() { const char *e = getenv("SYL_GROUP_CAP"); int v = e ? atoi(e) : GRP_CAP; return (uint32_t)std::min(std::max(v, 32), GRP_CAP); }();
             slot = grp_cap;
-            const uint64_t g = n_exp / GRP_T + 1;
-            if (g * GRP_BPG >= 0xFFFFFFFFull) { set_error("more than 2^32-2 survivor events in one sample"); return SYL_ERR_ARG; }
-            ng = (uint32_t)g;
-            nbk = ng * GRP_BPG;
-            const uint64_t thr = fmh_threshold(c);
-            unsigned __int128 mb = ((unsigned __int128)nbk << 64) / ((unsigned __int128)thr + 1);
-            Mb = mb > (unsigned __int128)UINT64_MAX ? UINT64_MAX : (uint64_t)mb;
+            ng = part.ng;
+            nbk = map.nbk;
+            Mb = map.Mb;
             SYL_TRY(g_cnt.alloc(ng, st));
             SYL_CUDA(cudaMemsetAsync(g_cnt.p, 0, (size_t)ng * 4, st));
         }
-        cap = expect_bases / c + expect_bases / (4 * c) + 65536;
-        if (cap > expect_bases) cap = expect_bases + 16;
         // with groups cap is the overflow list, almost always empty: 1/16 of the estimate; a sample that
         // needs more (duplicate-heavy, homopolymers) is redone with the exact length
-        if (ng) cap = cap / 16 + 65536;
+        cap = overflow_cap(part_bases(expect_bases, lo, hi, map.thr), c, grouped);
         if (cap_override) cap = cap_override;
         if (ev_total() >= 0xFFFFFFFEull) { set_error("more than 2^32-2 survivor events in one sample"); return SYL_ERR_ARG; }
         SYL_TRY(b_ev.alloc(ev_total(), st));
@@ -733,6 +731,7 @@ struct SampleBuilder {
             job.d_out = b_ev.p; job.cap = cap; job.emit_events = 1; job.rec_base = rec_base;
             job.no_dedup = paired ? 2 : no_dedup; job.d_pend = b_pend.p;
             job.d_group_cnt = g_cnt.p; job.Mb = Mb; job.nbk = nbk; job.ng = ng; job.slot = slot; job.d_count = dc;
+            job.g0 = g0; job.lo = lo; job.hi = hi;
             SYL_TRY(seed_enqueue(ctx, job));
         }
         if (!paired && (no_dedup || !m[0].nb)) return SYL_OK;  // no pending events
@@ -849,7 +848,7 @@ struct SampleBuilder {
             SYL_CUDA(cudaFuncSetAttribute(group_dedup, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(GroupSmem)));
             {
                 KernelTimer kt(ctx, SYL_KERNEL_GROUP_DEDUP);
-                group_dedup<<<ng, GRP_THREADS, sizeof(GroupSmem), st>>>(ev, g_cnt.p, slot, Mb, nbk, no_dedup,
+                group_dedup<<<ng, GRP_THREADS, sizeof(GroupSmem), st>>>(ev, g_cnt.p, slot, Mb, nbk, g0, no_dedup,
                                                                          st_hash.p, st_cnt.p, g_nuniq.p, g_n.p, g_fb.p, dc + CNT_DUPS);
             }
             k_scan_u32<<<1, 1024, 0, st>>>(g_nuniq.p, ng, uoff.p);
@@ -900,7 +899,7 @@ struct SampleBuilder {
         SYL_TRY(hblock_alloc(ctx, (void **)&s->hash, std::max<uint64_t>(U, 1) * 8));
         SYL_TRY(hblock_alloc(ctx, (void **)&s->count, std::max<uint64_t>(U, 1) * 4));
         if (ng && U2) {  // slot the generic path's pairs into their groups' positions, compact straight into the result
-            k_fallback_place<<<nblk(ng, 128), 128, 0, st>>>(g_fb.p, ng, nbk, Mb, f_uq.p, U2, g_nuniq.p, g_src.p);
+            k_fallback_place<<<nblk(ng, 128), 128, 0, st>>>(g_fb.p, ng, g0, nbk, Mb, f_uq.p, U2, g_nuniq.p, g_src.p);
             k_scan_u32<<<1, 1024, 0, st>>>(g_nuniq.p, ng, uoff.p);
             k_compact_uniq<<<ng, 128, 0, st>>>(st_hash.p, st_cnt.p, slot, g_nuniq.p, uoff.p, g_fb.p, g_src.p, f_uq.p, f_ct.p,
                                                 s->hash, s->count);
@@ -1244,10 +1243,85 @@ static bool host_ingest_ascii() {
     return hi_env ? std::string(hi_env) == "ascii" : local_ranks * live_contexts() > 4;
 }
 
+// Device bytes of the staging rings once feed_host has grown them for this sample (allocated outside the block cache,
+// kept until the ctx is destroyed; the ASCII ring of chunks taken from the back is counted whether or not it is used).
+// The sizes follow HostIngest::ensure_packed / ensure_ascii and syl_ctx_ingest_ring_bytes.
+static uint64_t ring_bytes_after(const syl_ctx *ctx, const Mate *m, int n_mates, uint64_t n_reads, bool ascii_only) {
+    const HostIngest *I = static_cast<const HostIngest *>(ctx->ingest);
+    uint64_t words = I ? I->cap_words : 0, recs = I ? I->cap_recs : 0, asc = I ? I->cap_asc : 0, aoff = I ? I->cap_aoff : 0;
+    std::vector<Chunk> chunks;
+    if (n_reads) {
+        if (ascii_only) plan_chunks(m, n_mates, n_reads, ingest_chunk(ING_ASCII_CHUNK), n_reads, chunks);
+        else plan_chunks(m, n_mates, n_reads, ingest_chunk(ING_CHUNK), ING_MAXREC / n_mates, chunks);
+    }
+    asc = std::max(asc, ascii_only ? ING_ASCII_CHUNK : ING_CHUNK);
+    aoff = std::max<uint64_t>(aoff, 65536);
+    if (!ascii_only) {
+        words = std::max(words, ING_CHUNK / 16);
+        recs = std::max<uint64_t>(recs, 65536);
+    }
+    for (const Chunk &c : chunks) {
+        asc = std::max(asc, footprint(c, n_mates));
+        aoff = std::max(aoff, n_mates * c.n_off());
+        if (ascii_only) continue;
+        words = std::max(words, (footprint(c, n_mates) + 15) / 16);
+        recs = std::max(recs, n_mates * c.n_off());
+    }
+    const uint64_t w = words ? (words + 16) * 4 : 0, r = recs ? recs + 16 : 0, a = asc + 256 + (aoff + 16) * 8;
+    return ING_SLOTS * (w + r * 12) + 2 * a;
+}
+
+// Bytes of the rings the ctx holds now (syl_ctx_ingest_ring_bytes)
+static uint64_t ring_bytes_now(const syl_ctx *ctx) {
+    uint64_t d = 0;
+    syl_ctx_ingest_ring_bytes(ctx, &d, nullptr);
+    return d;
+}
+
+// The hash-range parts of a sample (sample_parts.hpp) within the ctx's budget (syl_ctx_set_sample_memory; 0: the free
+// device memory now, plus the ctx's cached free blocks and rings, which the call reuses).  The fixed bytes are the
+// staging rings for host ASCII, or host 2-bit input staged whole.  SYL_SAMPLE_PARTS=N (read per call) forces N parts.
+// Nothing is allocated here: a budget the plan cannot meet fails before the call touches the device.
+static int plan_parts(syl_ctx *ctx, int mem, bool packed, bool ascii_only, const Mate *m, int n_mates, uint64_t n_reads,
+                      uint64_t bases, int k, uint64_t c, bool grouped, SamplePlan &plan) {
+    uint64_t fixed = 0;
+    for (int i = 0; i < n_mates; i++) fixed += (seed_cta_tiles(m[i].nb) + 1) * 4 + 256;  // the seeding kernel's tile table
+    if (mem == SYL_MEM_HOST && packed)
+        for (int i = 0; i < n_mates; i++) fixed += ((m[i].nb + 15) / 16 + 16) * 4 + (n_reads + 9) * 8;
+    else if (mem == SYL_MEM_HOST)
+        fixed += ring_bytes_after(ctx, m, n_mates, n_reads, ascii_only);
+    uint32_t forced = 0;
+    if (const char *e = getenv("SYL_SAMPLE_PARTS")) forced = (uint32_t)std::max(0, atoi(e));
+    uint64_t budget = ctx->sample_budget;
+    if (!budget) {
+        uint64_t held = ring_bytes_now(ctx);
+        for (const auto &b : ctx->free_blocks) held += b.second;
+        // cudaMemGetInfo costs about as much as a small sketch's post-pass: a sample whose one pass needs less than
+        // half of the free memory this ctx last saw takes one pass without asking again
+        if (!forced && plan_sample_parts(bases, n_reads, n_mates, k, c, grouped, UINT64_MAX, fixed, 0, plan) == PLAN_OK &&
+            plan.parts.size() == 1 && plan.need <= held + ctx->free_seen / 2)
+            return SYL_OK;
+        size_t free_b = 0, total_b = 0;
+        SYL_CUDA(cudaMemGetInfo(&free_b, &total_b));
+        ctx->free_seen = free_b;
+        budget = free_b + held;
+    }
+    switch (plan_sample_parts(bases, n_reads, n_mates, k, c, grouped, budget, fixed, forced, plan)) {
+        case PLAN_OK: return SYL_OK;
+        case PLAN_TOO_MANY_EVENTS: set_error("more than 2^32-2 survivor events in one sample part"); return SYL_ERR_ARG;
+        default:
+            set_error("sketching this sample needs " + std::to_string(plan.need) + " bytes of device memory in " +
+                      std::to_string(SAMPLE_MAX_PARTS) + " parts, the budget is " + std::to_string(budget) + " bytes");
+            return SYL_ERR_OOM;
+    }
+}
+
 // A sample of n_reads records: reads (n_mates 1), or read pairs (n_mates 2: mate i of pair p is record p of m[i]).
 // packed: every mate is 2-bit words, else ASCII; mem: where all of it lives.  Device input is used in place, host
 // 2-bit words (a quarter of the bytes) are staged whole once per call, host ASCII goes through feed_host in chunks.
-// A sample with more events than estimated is redone (host ASCII: fed again) with the exact event capacity.
+// A sample whose post-pass does not fit the ctx's budget is sketched in parts, one hash range per pass over the input
+// (host ASCII is fed again for every part); each part's sketch waits in host memory, and the parts, in range order,
+// are the sketch.  A part with more events than estimated is redone (host ASCII: fed again) with the exact event capacity.
 static int sketch_reads_impl(syl_ctx *ctx, int mem, bool packed, const Mate *m, int n_mates, uint64_t n_reads, int k,
                              uint64_t c, int no_dedup, int sem, syl_sample **out) {
     bool null_arg = !ctx || !out;
@@ -1258,12 +1332,21 @@ static int sketch_reads_impl(syl_ctx *ctx, int mem, bool packed, const Mate *m, 
     *out = nullptr;
     SYL_ENTER(ctx);
     const bool fed = mem == SYL_MEM_HOST && !packed;
+    const bool host_ascii = host_ingest_ascii();
+    const char *pp = getenv("SYL_SAMPLE_POSTPASS");  // per call; "sort": no groups, every event takes the generic path
+    const bool grouped = !(pp && std::string(pp) == "sort");
+    uint64_t expect_bases = 0;
+    for (int i = 0; i < n_mates; i++) expect_bases += m[i].nb;
+    SamplePlan plan;
+    SYL_TRY(plan_parts(ctx, mem, packed, host_ascii, m, n_mates, n_reads, expect_bases, k, c, grouped, plan));
+    const size_t P = plan.parts.size();
+    ctx->sample_parts = (uint32_t)P;
+    if (P > 1) SYL_TRY(cache_trim(ctx));  // every part's pass is allocated to its own size, not next to cached blocks
     Mate dm[2] = {};  // the mates on the device, unless fed
     Staged<uint32_t> sp[2];
     Staged<uint64_t> so[2];
-    uint64_t expect_bases = 0, staged_bytes = 0;
+    uint64_t staged_bytes = 0;
     for (int i = 0; i < n_mates; i++) {
-        expect_bases += m[i].nb;
         if (fed) continue;
         dm[i] = m[i];
         if (packed) { SYL_TRY(sp[i].init(ctx, mem, m[i].packed, (m[i].nb + 15) / 16)); dm[i].packed = sp[i].p; }
@@ -1273,34 +1356,74 @@ static int sketch_reads_impl(syl_ctx *ctx, int mem, bool packed, const Mate *m, 
     }
     // the mean length of mate 1 (for pairs src/sketch.rs:824-826)
     const double mean_read_length = n_reads ? (double)m[0].nb / (double)n_reads : 0.;
-    const bool host_ascii = host_ingest_ascii();
     static const bool dbg = getenv("SYL_DEBUG_TIMING") != nullptr;
     auto now = []() { return std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now().time_since_epoch()).count(); };
-    uint64_t cap_override = 0;
-    for (int attempt = 0; attempt < 3; attempt++) {
-        SampleBuilder b{ctx, k, c, no_dedup, sem, n_mates == 2, n_reads, mean_read_length};
-        b.expect_bases = expect_bases;
-        b.expect_reads = n_mates * n_reads;
-        if (mem == SYL_MEM_HOST) {
-            ctx->ingest_h2d_bytes = staged_bytes;
-            ctx->ingest_chunks_packed = ctx->ingest_chunks_ascii = 0;
+    uint64_t h2d = staged_bytes, n_packed = 0, n_ascii = 0;  // host ingest of the parts so far
+    std::vector<uint64_t> all_hash;  // the sketches of the parts so far (P > 1)
+    std::vector<uint32_t> all_cnt;
+    uint64_t ndup = 0;
+    for (size_t p = 0; p < P; p++) {
+        const SamplePart &part = plan.parts[p];
+        if (P > 1 && part.lo == part.hi) continue;  // a range no hash falls in
+        syl_sample *ps = nullptr;
+        uint64_t cap_override = 0;
+        int rc = SYL_ERR_CAPACITY;
+        for (int attempt = 0; attempt < 3 && rc == SYL_ERR_CAPACITY; attempt++) {
+            SampleBuilder b{ctx, k, c, no_dedup, sem, n_mates == 2, n_reads, mean_read_length};
+            b.expect_bases = expect_bases;
+            b.expect_reads = n_mates * n_reads;
+            if (mem == SYL_MEM_HOST) {
+                ctx->ingest_h2d_bytes = h2d;
+                ctx->ingest_chunks_packed = n_packed;
+                ctx->ingest_chunks_ascii = n_ascii;
+            }
+            SYL_TRY(b.begin(plan.map, part, grouped, cap_override));
+            const double t0 = now();
+            rc = SYL_OK;
+            if (!fed) rc = b.add(dm, n_mates, n_reads, 0);
+            else if (n_reads && expect_bases) rc = feed_host(ctx, b, m, n_mates, n_reads, host_ascii);
+            if (rc != SYL_OK) return rc;
+            const double t1 = now();
+            uint64_t need = 0;
+            rc = b.finish(&ps, &need);
+            if (dbg) fprintf(stderr, "[%s] feed %.2f ms, finish %.2f ms (attempt %d)%s\n",
+                             n_mates == 2 ? "syl_sketch_read_pairs" : "syl_sketch_reads", t1 - t0, now() - t1, attempt,
+                             P > 1 ? (", part " + std::to_string(p + 1) + "/" + std::to_string(P)).c_str() : "");
+            if (rc == SYL_ERR_CAPACITY) cap_override = need + 16;  // more events than estimated: redo with the exact size
         }
-        SYL_TRY(b.begin(cap_override));
-        const double t0 = now();
-        int rc = SYL_OK;
-        if (!fed) rc = b.add(dm, n_mates, n_reads, 0);
-        else if (n_reads && expect_bases) rc = feed_host(ctx, b, m, n_mates, n_reads, host_ascii);
-        if (rc != SYL_OK) return rc;
-        const double t1 = now();
-        uint64_t need = 0;
-        rc = b.finish(out, &need);
-        if (dbg) fprintf(stderr, "[%s] feed %.2f ms, finish %.2f ms (attempt %d)\n",
-                         n_mates == 2 ? "syl_sketch_read_pairs" : "syl_sketch_reads", t1 - t0, now() - t1, attempt);
-        if (rc == SYL_ERR_CAPACITY) { cap_override = need + 16; continue; }  // more events than estimated: redo with the exact size
-        return rc;
+        if (rc == SYL_ERR_CAPACITY) { set_error("event capacity retry failed"); return SYL_ERR_CAPACITY; }
+        SYL_TRY(rc);
+        if (P == 1) { *out = ps; return SYL_OK; }
+        Handle<syl_sample> hs(ps);
+        h2d = ctx->ingest_h2d_bytes;
+        n_packed = ctx->ingest_chunks_packed;
+        n_ascii = ctx->ingest_chunks_ascii;
+        const size_t u0 = all_hash.size();
+        all_hash.resize(u0 + hs->n);
+        all_cnt.resize(u0 + hs->n);
+        SYL_TRY(syl_sample_download(ctx, hs.get(), all_hash.data() + u0, all_cnt.data() + u0));
+        ndup += hs->num_dup_removed;
+        hs.reset();
+        SYL_TRY(cache_trim(ctx));
     }
-    set_error("event capacity retry failed");
-    return SYL_ERR_CAPACITY;
+    // the parts' sketches, in range order, into the exact-size handle
+    Handle<syl_sample> s = new_handle<syl_sample>(ctx);
+    if (!s) return SYL_ERR_OOM;
+    const uint64_t U = all_hash.size();
+    s->k = k;
+    s->c = c;
+    s->mean_read_length = mean_read_length;
+    s->num_dup_removed = ndup;
+    s->n = U;
+    SYL_TRY(hblock_alloc(ctx, (void **)&s->hash, std::max<uint64_t>(U, 1) * 8));
+    SYL_TRY(hblock_alloc(ctx, (void **)&s->count, std::max<uint64_t>(U, 1) * 4));
+    if (U) {
+        SYL_CUDA(cudaMemcpyAsync(s->hash, all_hash.data(), U * 8, cudaMemcpyHostToDevice, ctx->stream));
+        SYL_CUDA(cudaMemcpyAsync(s->count, all_cnt.data(), U * 4, cudaMemcpyHostToDevice, ctx->stream));
+        SYL_CUDA(cudaStreamSynchronize(ctx->stream));
+    }
+    *out = s.release();
+    return SYL_OK;
 }
 
 }  // namespace syl
@@ -1346,6 +1469,30 @@ int syl_ctx_ingest_ring_bytes(const syl_ctx *ctx, uint64_t *device_bytes, uint64
     const uint64_t a = I && I->cap_asc ? I->cap_asc + 256 + (I->cap_aoff + 16) * 8 : 0;
     if (device_bytes) *device_bytes = ING_SLOTS * (w + r * 12) + 2 * a;
     if (pinned_bytes) *pinned_bytes = ING_SLOTS * (w + r * 4);
+    return SYL_OK;
+}
+
+int syl_ctx_set_sample_memory(syl_ctx *ctx, uint64_t max_bytes) {
+    if (!ctx) { set_error("NULL argument"); return SYL_ERR_ARG; }
+    ctx->sample_budget = max_bytes;
+    return SYL_OK;
+}
+
+int syl_ctx_sample_memory(syl_ctx *ctx, uint64_t *max_bytes, uint64_t *free_bytes) {
+    if (!ctx) { set_error("NULL argument"); return SYL_ERR_ARG; }
+    if (max_bytes) *max_bytes = ctx->sample_budget;
+    if (free_bytes) {
+        SYL_ENTER(ctx);
+        size_t free_b = 0, total_b = 0;
+        SYL_CUDA(cudaMemGetInfo(&free_b, &total_b));
+        *free_bytes = free_b;
+    }
+    return SYL_OK;
+}
+
+int syl_ctx_sample_parts(const syl_ctx *ctx, uint32_t *parts) {
+    if (!ctx || !parts) { set_error("NULL argument"); return SYL_ERR_ARG; }
+    *parts = ctx->sample_parts;
     return SYL_OK;
 }
 

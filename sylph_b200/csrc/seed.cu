@@ -21,6 +21,7 @@
 //     3 ALU-pipe xor-shifts), one compare of the high word against the threshold
 //   * survivors (1/c of windows) are staged in shared memory and flushed with one global
 //     atomic per CTA
+#include <algorithm>
 #include <cstdlib>
 
 #include "seed_kernel.cuh"
@@ -105,9 +106,10 @@ int seed_enqueue(syl_ctx *ctx, const SeedJob &job) {
         k_tile_first_rec<<<(unsigned)nb, bs, 0, st>>>(job.d_rec_off, job.off_bias, job.n_rec, n_tiles, SEED_TILE, tile_rec.p);
         ctx->launches++;
     }
-    const uint64_t thr = fmh_threshold(job.c);
+    // events of one part of a sample (sample_parts.hpp): hashes below the part's upper bound hi <= fmh_threshold
+    const uint64_t thr = job.emit_events ? std::min(job.hi, fmh_threshold(job.c)) : fmh_threshold(job.c);
     const ImadConst ic = {{0u, 0u, 0u}, 1u, 0u};
-    const GroupOut go{job.emit_events ? job.d_group_cnt : nullptr, job.Mb, job.nbk, job.ng, job.slot};
+    const GroupOut go{job.emit_events ? job.d_group_cnt : nullptr, job.Mb, job.nbk, job.ng, job.slot, job.g0, job.lo};
     const SlotOut slot{job.emit_events ? 0u : job.slot_cap, job.d_tile_cnt, job.d_slot_overflow};
     const size_t smem = sizeof(SeedSmem);
     const seed_kern_t kern = job.emit_events ? (job.k == 31 ? seed_kernels_k31_ev(W, packed) : seed_kernels_k21_ev(W, packed))

@@ -66,15 +66,19 @@ __device__ __forceinline__ uint16_t *seed_stage_pos(SeedMeta &M) {
 // counter *g_count; its group then takes the post-pass's generic path.  cnt == nullptr: no groups, every
 // event is appended at *g_count (read pairs, SYL_SAMPLE_POSTPASS=sort).  Appends past cap are counted
 // but dropped; the caller compares the final count with cap and redoes the sample.
+// A sample sketched in parts (sample_parts.hpp) emits only the hashes [lo, hi) of one part per pass (the launcher
+// passes hi as the kernel's threshold, so the hot loop's high-word test already skips the hashes above the part); the
+// part owns groups [g0, g0 + ng) of the one-pass map (Mb, nbk) and its slots are numbered from g0.
 struct GroupOut {
     uint32_t *cnt;  // events per group (can exceed slot)
     uint64_t Mb;
-    uint32_t nbk, ng, slot;
+    uint32_t nbk, ng, slot, g0;
+    uint64_t lo;
     // position of the event in out, or ~0ull when it is dropped
     __device__ __forceinline__ uint64_t place(uint64_t h, unsigned long long *g_count, uint64_t cap) const {
         if (cnt) {
             uint32_t g = (uint32_t)__umul64hi(h, Mb);
-            g = (g < nbk ? g : nbk - 1) / GRP_BPG;
+            g = (g < nbk ? g : nbk - 1) / GRP_BPG - g0;
             const uint32_t i = atomicAdd(&cnt[g], 1u);
             if (i < slot) return (uint64_t)g * slot + i;
         }
@@ -212,6 +216,7 @@ __device__ __forceinline__ void seed_resolve(const SeedSmem &S, SeedMeta &M, uin
     const uint64_t rr = ((uint64_t)(__funnelshift_r(c1, c2, csh) & HI_MASK) << 32) | __funnelshift_r(c0, c1, csh);
     const uint64_t h = mm_hash64(f < rr ? f : rr);  // src/seeding.rs:131-137
     if (h >= thr) return;                           // src/seeding.rs:139
+    if (EMIT == 1 && h < go.lo) return;             // an earlier part's hash (thr is this part's upper bound)
     const unsigned int idx = atomicAdd(&M.stage_count, 1u);
     if (EMIT == 0) {
         syl_survivor sv;
