@@ -98,8 +98,9 @@ int syl_ctx_kernel_time(syl_ctx *ctx, int which, double *total_ms, uint64_t *lau
  * sample / genomes / db handles and of profile jobs, plus cached free blocks; between calls nothing else is
  * allocated through it).  peak: high-water mark of held plus the live temporaries of syl_db_build /
  * syl_db_build_arrays since the ctx was created or the peak last reset (reset_peak != 0 resets it after reading).
- * The host-memory read path's staging rings (syl_sketch_reads with SYL_MEM_HOST) are allocated directly and are
- * not counted. */
+ * The staging rings of the host-memory read and genome paths (syl_sketch_reads, syl_sketch_read_pairs and the genome
+ * calls with SYL_MEM_HOST; syl_ctx_ingest_ring_bytes) are allocated directly and are not counted; the buffer of a
+ * host genome larger than a chunk is a cached block and is. */
 int syl_ctx_device_bytes(syl_ctx *ctx, uint64_t *held, uint64_t *peak, int reset_peak);
 
 /* ------------------------------------------------------------------------------------------
@@ -174,13 +175,16 @@ int syl_sketch_read_pairs_packed2(syl_ctx *ctx, int mem, const uint32_t *packed1
 int syl_pack2(const uint8_t *bases, uint64_t n_bases, uint32_t *words, int n_threads);
 /* Worker threads the host-memory path of syl_sketch_reads packs with (for bench.py's e2e record). */
 int syl_pack_threads(void);
-/* What the last syl_sketch_reads / syl_sketch_read_pairs(SYL_MEM_HOST, ASCII) call of this ctx moved: host-to-device
- * bytes (bases + record offsets, as copied) and how many of its chunks (of reads, or of pairs) crossed the link as
- * 2-bit words / as ASCII.  Host 2-bit input (the _packed2 calls) is staged whole: its bytes, no chunks. */
+/* What the last syl_sketch_reads / syl_sketch_read_pairs(SYL_MEM_HOST, ASCII) call or syl_sketch_genomes /
+ * syl_sketch_genomes_packed2(SYL_MEM_HOST) call of this ctx moved: host-to-device bytes (bases or words + record
+ * offsets, as copied; for genomes also every chunk's genome offsets) and how many of its chunks (of reads, of pairs,
+ * of genomes) crossed the link as 2-bit words / as ASCII.  Host 2-bit reads and pairs are staged whole: their bytes,
+ * no chunks.  A genome larger than a chunk counts as one chunk of the form it crossed in. */
 int syl_ctx_ingest_stats(const syl_ctx *ctx, uint64_t *h2d_bytes, uint64_t *chunks_packed, uint64_t *chunks_ascii);
 /* Bytes the host-memory staging rings of this ctx hold now: on the device (allocated outside the block cache, so
- * syl_ctx_device_bytes does not count them) and in pinned host memory.  They grow to the largest chunk seen and
- * live until the ctx is destroyed. */
+ * syl_ctx_device_bytes does not count them) and in pinned host memory.  Read and genome calls share them.  They grow
+ * to the largest chunk seen (a genome larger than a chunk is staged in cached blocks instead, and does not grow them)
+ * and live until the ctx is destroyed. */
 int syl_ctx_ingest_ring_bytes(const syl_ctx *ctx, uint64_t *device_bytes, uint64_t *pinned_bytes);
 /* Device memory of read and pair sketches (the four calls above).  The post-pass holds about 120 bytes per expected
  * survivor event (bases / c), and host input adds its staging rings or, for 2-bit words, the staged words.  A sample
@@ -222,6 +226,14 @@ void syl_sample_free(syl_sample *s);
  *     a flat buffer.  genome_off[g]..genome_off[g+1] indexes contigs (records) of genome g.
  *     Result: CSR genome_kmers (position order) + CSR pseudotax_tracked_nonused_kmers +
  *     gn_size per genome (src/types.rs:163-173), resident on the device.
+ *     SYL_MEM_HOST: the batch crosses the link in chunks of whole genomes (whole contigs with individual != 0) of at most
+ *     the read path's chunk size and 2^19 contigs, through the staging rings of syl_sketch_reads (ASCII packed to 2 bits
+ *     by the worker threads or shipped as it is, SYL_HOST_INGEST as there; 2-bit words copied as they are), while
+ *     earlier chunks are sketched.  A genome larger than a chunk is copied on its own into one buffer as large as the
+ *     genome.  Each chunk is sketched with its genomes' survivors alone (the post-pass needs nothing else), and the
+ *     chunks' results are joined in order into one handle, the same as from device memory.  The device holds the output
+ *     (about 8 bytes per kept or tracked k-mer) twice at most, one chunk's working set (about 1.5 bytes per base of the
+ *     chunk) and the rings, never the batch's bases; the 2^32-2 survivor limit applies per chunk.
  * ---------------------------------------------------------------------------------------- */
 typedef struct syl_genomes syl_genomes;
 
@@ -231,7 +243,8 @@ int syl_sketch_genomes(syl_ctx *ctx, int mem, const uint8_t *bases, uint64_t n_b
                        int individual, int sem, syl_genomes **out);
 /* The same for contigs that are already 2-bit packed (layout: see syl_sketch_reads_packed2; ceil(n_bases/16) words,
  * contig_off in bases): e.g. a 2-bit genome store.  Same result as syl_sketch_genomes on the ASCII it was packed
- * from (gn_size comes from contig_off).  SYL_MEM_HOST copies the words once (4x fewer bytes than ASCII);
+ * from (gn_size comes from contig_off).  SYL_MEM_HOST copies each chunk's words (4x fewer bytes than ASCII) from the
+ * word of its first base, with no packing, into a ring slot; pageable words are copied chunk by chunk too.
  * SYL_MEM_DEVICE words must be 16-byte aligned (else SYL_ERR_ARG). */
 int syl_sketch_genomes_packed2(syl_ctx *ctx, int mem, const uint32_t *packed, uint64_t n_bases,
                                const uint64_t *contig_off, uint64_t n_contigs, const uint64_t *genome_off,

@@ -95,8 +95,8 @@ class Context:
     KERNELS = {"seed": 0, "group_dedup": 1, "join": 2, "join2": 3, "stats": 4, "boot": 5, "genome_post": 6, "pack": 7}
 
     def ingest_stats(self):
-        """-> (h2d_bytes, chunks_packed, chunks_ascii) of the last host-memory sketch_sequences or
-        sketch_pair_sequences call."""
+        """-> (h2d_bytes, chunks_packed, chunks_ascii) of the last host-memory sketch_sequences,
+        sketch_pair_sequences or sketch_genomes call."""
         a, b, c = C.c_uint64(0), C.c_uint64(0), C.c_uint64(0)
         _lib.check(_lib.lib().syl_ctx_ingest_stats(self._h, C.byref(a), C.byref(b), C.byref(c)))
         return a.value, b.value, c.value
@@ -241,7 +241,10 @@ class Context:
     def sketch_genomes(self, bases, contig_off, genome_off=None, k=31, c=200, min_spacing=30, pseudotax=True,
                        individual=False, sem=SEM_AVX2, packed_bases=None):
         """Batched sketch_genome / sketch_genome_individual (src/sketch.rs:550-622, 481-548).
-        packed_bases: `bases` holds 2-bit words (see pack2) for this many bases (syl_sketch_genomes_packed2)."""
+        packed_bases: `bases` holds 2-bit words (see pack2) for this many bases (syl_sketch_genomes_packed2).
+        Host inputs (numpy, CPU tensors; pinned memory lets the link run while the host packs) cross to the device in
+        chunks of whole genomes, so device memory holds the output and one chunk, not the batch; a genome larger than a
+        chunk is copied on its own.  The result is the same as from device memory."""
         _CTX_STREAM[0] = self._stream
         L = _lib.lib()
         mem_o, po, no, ko = _arg(contig_off, np.uint64)

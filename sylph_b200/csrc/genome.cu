@@ -18,6 +18,8 @@
 #include <vector>
 
 #include "common.cuh"
+#include "genome_chunks.hpp"
+#include "ingest.hpp"
 #include "scan.cuh"
 
 namespace syl {
@@ -334,7 +336,7 @@ static int genomes_back_half(syl_ctx *ctx, KernelTimer &kt, const uint64_t *posk
 // them one array.  No host synchronisation before the back half.  Exactly one of d_bases (ASCII) / d_packed (2-bit
 // words) is set, here and in the functions below.
 static int genomes_slotted(syl_ctx *ctx, const uint8_t *d_bases, const uint32_t *d_packed, uint64_t n_bases,
-                           const uint64_t *d_contig_off, uint64_t n_contigs, const uint64_t *d_genome_off, uint64_t n_genomes,
+                           const uint64_t *d_contig_off, uint64_t off_bias, uint64_t n_contigs, const uint64_t *d_genome_off, uint64_t n_genomes,
                            int k, uint64_t c, uint64_t min_spacing, int pseudotax, int sem, syl_genomes *out) {
     cudaStream_t st = ctx->stream;
     const uint64_t n_tiles = seed_cta_tiles(n_bases);
@@ -349,7 +351,7 @@ static int genomes_slotted(syl_ctx *ctx, const uint8_t *d_bases, const uint32_t 
     SYL_CUDA(cudaMemsetAsync(overflow.p, 0, 4, st));
     SYL_CUDA(cudaMemsetAsync(ctx->d_counters, 0, 2 * sizeof(uint64_t), st));  // CNT_EVENTS, CNT_PENDING
     SeedJob job;
-    job.d_bases = d_bases; job.d_packed = d_packed; job.n_bases = n_bases; job.d_rec_off = d_contig_off; job.off_bias = 0; job.n_rec = n_contigs;
+    job.d_bases = d_bases; job.d_packed = d_packed; job.n_bases = n_bases; job.d_rec_off = d_contig_off; job.off_bias = off_bias; job.n_rec = n_contigs;
     job.k = k; job.c = c; job.sem = sem; job.with_pos = 1; job.d_out = slots.p; job.cap = n_tiles * GEN_SLOT;
     job.d_count = reinterpret_cast<unsigned long long *>(ctx->d_counters);
     job.slot_cap = GEN_SLOT; job.d_tile_cnt = tile_cnt.p; job.d_slot_overflow = overflow.p;
@@ -366,7 +368,7 @@ static int genomes_slotted(syl_ctx *ctx, const uint8_t *d_bases, const uint32_t 
 // Sorted front half, for every input: survivors with positions from seed_device (one host synchronisation, which
 // also sizes the buffers), then one radix sort by (contig, pos) carrying the hash.
 static int genomes_sorted(syl_ctx *ctx, const uint8_t *d_bases, const uint32_t *d_packed, uint64_t n_bases,
-                          const uint64_t *d_contig_off, uint64_t n_contigs, const uint64_t *d_genome_off, uint64_t n_genomes,
+                          const uint64_t *d_contig_off, uint64_t off_bias, uint64_t n_contigs, const uint64_t *d_genome_off, uint64_t n_genomes,
                           int k, uint64_t c, uint64_t min_spacing, int pseudotax, int sem, syl_genomes *out) {
     cudaStream_t st = ctx->stream;
     uint64_t scap = n_bases / c + n_bases / (4 * c) + 65536;
@@ -375,7 +377,7 @@ static int genomes_sorted(syl_ctx *ctx, const uint8_t *d_bases, const uint32_t *
     uint64_t N = 0;
     for (;;) {
         SYL_TRY(sv.alloc(scap, st));
-        int rc = seed_device(ctx, d_bases, d_packed, n_bases, d_contig_off, 0, n_contigs, k, c, sem, /*with_pos=*/1, sv.p, scap, &N);
+        int rc = seed_device(ctx, d_bases, d_packed, n_bases, d_contig_off, off_bias, n_contigs, k, c, sem, /*with_pos=*/1, sv.p, scap, &N);
         if (rc == SYL_ERR_CAPACITY) { scap = N + 16; continue; }
         if (rc != SYL_OK) return rc;
         break;
@@ -403,20 +405,93 @@ static int genomes_sorted(syl_ctx *ctx, const uint8_t *d_bases, const uint32_t *
                              d_contig_off, d_genome_off, n_genomes, min_spacing, pseudotax, out);
 }
 
-int sketch_genomes_device(syl_ctx *ctx, const uint8_t *d_bases, const uint32_t *d_packed, uint64_t n_bases,
-                          const uint64_t *d_contig_off, uint64_t n_contigs, const uint64_t *d_genome_off, uint64_t n_genomes,
-                          int k, uint64_t c, uint64_t min_spacing, int pseudotax, int sem, syl_genomes *out) {
+// d_contig_off[i] - off_bias is the first base of contig i among the bases (seed_device)
+static int sketch_genomes_device(syl_ctx *ctx, const uint8_t *d_bases, const uint32_t *d_packed, uint64_t n_bases,
+                                 const uint64_t *d_contig_off, uint64_t off_bias, uint64_t n_contigs, const uint64_t *d_genome_off,
+                                 uint64_t n_genomes, int k, uint64_t c, uint64_t min_spacing, int pseudotax, int sem, syl_genomes *out) {
     const char *e = getenv("SYL_GENOME_POSTPASS");  // "sort" forces the sorted front half (tests); read per call
     const bool force_sort = e && std::string(e) == "sort";
     // slots hold 512 survivors per 32K-base tile: c >= 96 keeps the expected number below 350
     if (!force_sort && c >= 96 && n_bases && n_contigs && n_genomes) {
-        const int rc = genomes_slotted(ctx, d_bases, d_packed, n_bases, d_contig_off, n_contigs, d_genome_off, n_genomes, k, c,
+        const int rc = genomes_slotted(ctx, d_bases, d_packed, n_bases, d_contig_off, off_bias, n_contigs, d_genome_off, n_genomes, k, c,
                                        min_spacing, pseudotax, sem, out);
         if (rc != SYL_ERR_UNSUPPORTED) return rc;
         // a slot or the compact arrays overflowed (low-complexity sequence): redo the batch on the sorted front half
     }
-    return genomes_sorted(ctx, d_bases, d_packed, n_bases, d_contig_off, n_contigs, d_genome_off, n_genomes, k, c, min_spacing,
+    return genomes_sorted(ctx, d_bases, d_packed, n_bases, d_contig_off, off_bias, n_contigs, d_genome_off, n_genomes, k, c, min_spacing,
                           pseudotax, sem, out);
+}
+
+// genomes of parts[0 .. n_parts) one after the other into g (a new handle, k / c / has_tracked set): offsets rebased by
+// k_add_offset.  Ends with a synchronisation.
+static int genomes_concat_into(syl_ctx *ctx, const syl_genomes *const *parts, size_t n_parts, syl_genomes *g) {
+    cudaStream_t st = ctx->stream;
+    uint64_t G = 0, nk = 0, nt = 0;
+    for (size_t i = 0; i < n_parts; i++) { G += parts[i]->n; nk += parts[i]->total_kmers; nt += parts[i]->total_tracked; }
+    SYL_TRY(genomes_alloc(g, G, nk, nt));
+    uint64_t g0 = 0, k0 = 0, t0 = 0;
+    for (size_t i = 0; i < n_parts; i++) {
+        const syl_genomes *p = parts[i];
+        if (p->total_kmers) SYL_CUDA(cudaMemcpyAsync(g->kmers + k0, p->kmers, p->total_kmers * 8, cudaMemcpyDeviceToDevice, st));
+        if (p->total_tracked) SYL_CUDA(cudaMemcpyAsync(g->tracked + t0, p->tracked, p->total_tracked * 8, cudaMemcpyDeviceToDevice, st));
+        if (p->n) SYL_CUDA(cudaMemcpyAsync(g->gn_size + g0, p->gn_size, p->n * 8, cudaMemcpyDeviceToDevice, st));
+        k_add_offset<<<nblk(p->n + 1, 256), 256, 0, st>>>(p->kmer_off, p->n + 1, k0, g->kmer_off + g0);
+        k_add_offset<<<nblk(p->n + 1, 256), 256, 0, st>>>(p->tracked_off, p->n + 1, t0, g->tracked_off + g0);
+        ctx->launches += 2;
+        g0 += p->n; k0 += p->total_kmers; t0 += p->total_tracked;
+    }
+    if (n_parts == 0) {
+        SYL_CUDA(cudaMemsetAsync(g->kmer_off, 0, 8, st));
+        SYL_CUDA(cudaMemsetAsync(g->tracked_off, 0, 8, st));
+    }
+    SYL_CUDA(cudaGetLastError());
+    SYL_CUDA(cudaStreamSynchronize(st));
+    return SYL_OK;
+}
+
+// Host memory: the batch goes through the host feeder (ingest.hpp) in chunks of whole genomes (genome_chunks.hpp), and
+// every chunk is sketched on its own, with chunk-relative contig and genome offsets.  A genome's survivors all lie in
+// its chunk, so each chunk's CSR is exactly its genomes' rows of the whole batch's.  The chunks' sketches wait on the
+// device (chunks taken from the back of the plan arrive first) and are put together in plan order at the end: the
+// call holds the output twice at most, plus one chunk's working set and the feeder's rings, whatever the input's size.
+// genome_off == NULL: every contig is a genome.
+static int sketch_genomes_host(syl_ctx *ctx, const uint8_t *bases, const uint32_t *packed, uint64_t n_bases,
+                               const uint64_t *contig_off, uint64_t n_contigs, const uint64_t *genome_off, uint64_t n_genomes,
+                               int k, uint64_t c, uint64_t min_spacing, int pseudotax, int sem, syl_genomes *out) {
+    cudaStream_t st = ctx->stream;
+    const bool ascii_only = !packed && host_ingest_ascii();
+    std::vector<GenomeChunk> plan;
+    plan_genome_chunks(contig_off, genome_off, n_genomes, ingest_chunk(ascii_only ? ING_ASCII_CHUNK : ING_CHUNK), ING_MAXREC, plan);
+    // every chunk's genome offsets relative to its first contig, behind one another: one copy for the call
+    std::vector<uint64_t> h_goff, at(plan.size());
+    std::vector<Chunk> chunks(plan.size());
+    for (size_t i = 0; i < plan.size(); i++) {
+        const GenomeChunk &p = plan[i];
+        at[i] = h_goff.size();
+        for (uint64_t g = p.g0; g <= p.g1; g++) h_goff.push_back((genome_off ? genome_off[g] : g) - p.c0);
+        chunks[i] = Chunk{p.c0, p.c1, {contig_off[p.c0], 0}, {contig_off[p.c1] - contig_off[p.c0], 0}};
+        chunks[i].own = p.own;
+    }
+    DevBuf<uint64_t> d_goff;
+    SYL_TRY(d_goff.alloc(h_goff.size(), st));
+    if (!h_goff.empty()) SYL_CUDA(cudaMemcpyAsync(d_goff.p, h_goff.data(), h_goff.size() * 8, cudaMemcpyHostToDevice, st));
+    ctx->ingest_h2d_bytes = h_goff.size() * 8;
+    ctx->ingest_chunks_packed = ctx->ingest_chunks_ascii = 0;
+    std::vector<Handle<syl_genomes>> parts(plan.size());
+    const Mate m = {bases, packed, n_bases, contig_off, 0};
+    if (!chunks.empty()) SYL_TRY(feed_host(ctx, &m, 1, chunks, ascii_only, [&](const Mate *dm, size_t ci) {
+        const GenomeChunk &p = plan[ci];
+        Handle<syl_genomes> h = new_handle<syl_genomes>(ctx);
+        if (!h) return (int)SYL_ERR_OOM;
+        SYL_TRY(sketch_genomes_device(ctx, dm->bases, dm->packed, dm->nb, dm->off, dm->off_bias, p.c1 - p.c0, d_goff.p + at[ci],
+                                      p.g1 - p.g0, k, c, min_spacing, pseudotax, sem, h.get()));
+        parts[ci] = std::move(h);
+        return (int)SYL_OK;
+    }));
+    std::vector<const syl_genomes *> pp(parts.size());
+    for (size_t i = 0; i < parts.size(); i++) pp[i] = parts[i].get();
+    out->has_tracked = pseudotax ? 1 : 0;
+    return genomes_concat_into(ctx, pp.data(), pp.size(), out);
 }
 
 // packed: the input is 2-bit words (device or host memory); else ASCII
@@ -429,30 +504,29 @@ static int sketch_genomes_impl(syl_ctx *ctx, int mem, const uint8_t *bases, cons
         return SYL_ERR_ARG;
     }
     if (c == 0) { set_error("c must be >= 1"); return SYL_ERR_ARG; }
+    if (mem != SYL_MEM_HOST && mem != SYL_MEM_DEVICE) { set_error("bad mem"); return SYL_ERR_ARG; }
     *out = nullptr;
     SYL_ENTER(ctx);
     cudaStream_t st = ctx->stream;
-    Staged<uint8_t> sb;  // host memory: staged copies, alive until the call's last sync
-    Staged<uint32_t> sp;
-    Staged<uint64_t> sc, sg;
-    if (packed) SYL_TRY(sp.init(ctx, mem, packed, (n_bases + 15) / 16));
-    else SYL_TRY(sb.init(ctx, mem, bases, n_bases));
-    SYL_TRY(sc.init(ctx, mem, contig_off, n_contigs + 1));
-    if (individual) {  // every record is its own genome (src/sketch.rs:481-548)
-        n_genomes = n_contigs;
-        SYL_TRY(sg.buf.alloc(n_contigs + 1, st));
-        k_iota64<<<nblk(n_contigs + 1, 256), 256, 0, st>>>(sg.buf.p, n_contigs + 1);
-        ctx->launches++;
-        sg.p = sg.buf.p;
-    } else {
-        SYL_TRY(sg.init(ctx, mem, genome_off, n_genomes + 1));
-    }
+    if (individual) n_genomes = n_contigs;  // every record is its own genome (src/sketch.rs:481-548)
     Handle<syl_genomes> g = new_handle<syl_genomes>(ctx);
     if (!g) return SYL_ERR_OOM;
     g->k = k;
     g->c = c;
-    SYL_TRY(sketch_genomes_device(ctx, sb.p, sp.p, n_bases, sc.p, n_contigs, sg.p, n_genomes, k, c, min_spacing, pseudotax,
-                                  sem, g.get()));
+    if (mem == SYL_MEM_HOST) {
+        SYL_TRY(sketch_genomes_host(ctx, bases, packed, n_bases, contig_off, n_contigs, individual ? nullptr : genome_off, n_genomes,
+                                    k, c, min_spacing, pseudotax, sem, g.get()));
+    } else {
+        DevBuf<uint64_t> iota;
+        if (individual) {
+            SYL_TRY(iota.alloc(n_contigs + 1, st));
+            k_iota64<<<nblk(n_contigs + 1, 256), 256, 0, st>>>(iota.p, n_contigs + 1);
+            ctx->launches++;
+            genome_off = iota.p;
+        }
+        SYL_TRY(sketch_genomes_device(ctx, bases, packed, n_bases, contig_off, 0, n_contigs, genome_off, n_genomes, k, c, min_spacing,
+                                      pseudotax, sem, g.get()));
+    }
     *out = g.release();
     return SYL_OK;
 }
@@ -523,37 +597,17 @@ int syl_genomes_concat(syl_ctx *ctx, const syl_genomes *const *parts, uint32_t n
     if (!ctx || !out || (n_parts && !parts)) { set_error("NULL argument"); return SYL_ERR_ARG; }
     *out = nullptr;
     SYL_ENTER(ctx);
-    cudaStream_t st = ctx->stream;
-    uint64_t G = 0, nk = 0, nt = 0;
     for (uint32_t i = 0; i < n_parts; i++) {
         if (!parts[i]) { set_error("NULL part"); return SYL_ERR_ARG; }
         if (parts[i]->k != parts[0]->k || parts[i]->c != parts[0]->c || parts[i]->has_tracked != parts[0]->has_tracked) {
             set_error("parts disagree on k / c / has_tracked");
             return SYL_ERR_ARG;
         }
-        G += parts[i]->n; nk += parts[i]->total_kmers; nt += parts[i]->total_tracked;
     }
     Handle<syl_genomes> g = new_handle<syl_genomes>(ctx);
     if (!g) return SYL_ERR_OOM;
     if (n_parts) { g->k = parts[0]->k; g->c = parts[0]->c; g->has_tracked = parts[0]->has_tracked; }
-    SYL_TRY(genomes_alloc(g.get(), G, nk, nt));
-    uint64_t g0 = 0, k0 = 0, t0 = 0;
-    for (uint32_t i = 0; i < n_parts; i++) {
-        const syl_genomes *p = parts[i];
-        if (p->total_kmers) SYL_CUDA(cudaMemcpyAsync(g->kmers + k0, p->kmers, p->total_kmers * 8, cudaMemcpyDeviceToDevice, st));
-        if (p->total_tracked) SYL_CUDA(cudaMemcpyAsync(g->tracked + t0, p->tracked, p->total_tracked * 8, cudaMemcpyDeviceToDevice, st));
-        if (p->n) SYL_CUDA(cudaMemcpyAsync(g->gn_size + g0, p->gn_size, p->n * 8, cudaMemcpyDeviceToDevice, st));
-        k_add_offset<<<nblk(p->n + 1, 256), 256, 0, st>>>(p->kmer_off, p->n + 1, k0, g->kmer_off + g0);
-        k_add_offset<<<nblk(p->n + 1, 256), 256, 0, st>>>(p->tracked_off, p->n + 1, t0, g->tracked_off + g0);
-        ctx->launches += 2;
-        g0 += p->n; k0 += p->total_kmers; t0 += p->total_tracked;
-    }
-    if (n_parts == 0) {
-        SYL_CUDA(cudaMemsetAsync(g->kmer_off, 0, 8, st));
-        SYL_CUDA(cudaMemsetAsync(g->tracked_off, 0, 8, st));
-    }
-    SYL_CUDA(cudaGetLastError());
-    SYL_CUDA(cudaStreamSynchronize(st));
+    SYL_TRY(genomes_concat_into(ctx, parts, n_parts, g.get()));
     *out = g.release();
     return SYL_OK;
 }
