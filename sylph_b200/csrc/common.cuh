@@ -159,9 +159,9 @@ enum CounterSlot : int {
     CNT_PENDING = 1,         // seeding: pending events (SeedJob::d_count[1]); the generic dedup's run count
     CNT_DUPS = 2,            // read sketch: duplicates removed
     CNT_PEND_MATE1 = 3,      // read sketch: CNT_PENDING before mate 1 of a batch
-    CNT_UNIQ_TOTAL = 4,      // read sketch: in-kernel uniques (u32)
+    CNT_UNIQ_TOTAL = 4,      // read sketch: in-kernel uniques (u64, summed by k_group_dedup)
     CNT_BACK_HALF = 4,       // genome back half: N, kept, tracked, slot overflow as four u32 over slots 4 and 5
-    CNT_FALLBACK_TOTAL = 5,  // read sketch: events of the fallback groups (u32)
+    CNT_FALLBACK_TOTAL = 5,  // read sketch: slotted events of the fallback groups (u64, summed by k_group_dedup)
     CNT_KMER_TOTAL = 8,      // last k-mer offset of device CSR input
     CNT_TRACKED_TOTAL = 9,   // last tracked offset of device CSR input
     CNT_BAD_OFFSETS = 10,    // index build: device offsets that do not start at 0 or decrease

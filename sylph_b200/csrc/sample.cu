@@ -245,13 +245,14 @@ __global__ void k_dedup(const uint64_t *__restrict__ seg_off, const uint32_t *__
 //   the seeding kernel's flush (GroupOut, seed_kernel.cuh) : writes every event into the slot of its
 //       group g = bucket / GRP_BPG, bucket = min(mulhi(hash, Mb), nbk - 1) (monotone in the hash, uniform
 //       because hashes are uniform below thr); the groups are fixed in begin() at ~GRP_T expected events
-//   k_group_dedup : one CTA per group (<= slot events) groups the events by k-mer in shared memory
-//       and replays dup_removal_lsh_full_exact per k-mer
-//   k_compact_uniq : staged (hash,count) pairs -> dense arrays; buckets are monotone in the hash
-//       and every group is sorted, so the result is globally sorted without a merge.
+//   k_group_dedup : one CTA per group (<= slot events) groups the events by k-mer in shared memory,
+//       replays dup_removal_lsh_full_exact per k-mer and writes the group's sorted (hash, count) pairs into
+//       its slot of the staging arrays
+//   k_compact_uniq : staged pairs -> the exact-size result; buckets are monotone in the hash and every
+//       group is sorted, so the result is globally sorted without a merge.
 // Groups that do not fit (heavy-hitter k-mers: more events than the slot, the rest in the overflow list)
-// or whose dedup set outgrows the per-thread buffer are handed to the generic radix-sort path below and
-// merged at the end.
+// or whose dedup set outgrows the per-thread buffer are handed to the generic radix-sort path below, and
+// k_compact_uniq takes their uniques from there.
 constexpr int GRP_THREADS = 256;
 // GRP_CAP (slot per group) and GRP_T (expected events per group): sample_parts.hpp
 
@@ -266,16 +267,23 @@ __device__ __forceinline__ uint32_t bucket_of(uint64_t h, uint64_t Mb, uint32_t 
 // dup_removal_lsh_full_exact on each k-mer's first events in read order, (3) orders the resulting
 // unique (hash, count) pairs: the group's buckets are already monotone in the hash, so a pair's
 // position is its bucket's offset plus its rank among the ~10 pairs of the same bucket.
-constexpr int GRP_SLOTS = 2048;  // table slots (load factor <= 0.5)
+// Table slots: a group holds at most GRP_CAP events and usually far fewer distinct k-mers (≈220 of ≈640 events on
+// bench.py's sample, ≈640 on reads without repeats), so 1024 slots keep the probes short while the smaller table
+// lets more CTAs share an SM; with at most GRP_CAP distinct hashes a free or equal slot always exists.
+constexpr int GRP_SLOTS = 1024;
 constexpr int GRP_SELECT_STEPS = 64;  // selection steps before a duplicate-heavy k-mer goes to the generic path
 
+// Single-end groups keep the pair keys in global memory: only the k-mers with two or more events read them (the
+// sectors are still in L2), and the 16 KB less (28 KB in all) lets 7 CTAs share an SM.  Read pairs compare every key
+// of a k-mer with every other one, so their groups stage the keys.
+template <bool PAIRED>
 struct GroupSmem {
-    unsigned long long ht[GRP_SLOTS];  // 16 KB  hash per slot
-    uint64_t rf[GRP_CAP];              //  8 KB  recflag per event        | after the replay: unique hashes
-    uint64_t p0[GRP_CAP];              //  8 KB  first pair key per event | after the replay: unique counts (u32)
-    uint64_t p1[GRP_CAP];              //  8 KB  second pair key per event
-    uint16_t scnt[GRP_SLOTS];          //  4 KB  events per slot, then fill cursor, then the k-mer's count
-    uint16_t soff[GRP_SLOTS + 2];      //  4 KB  exclusive scan of scnt
+    unsigned long long ht[GRP_SLOTS];  //  8 KB  hash per slot
+    uint64_t rf[GRP_CAP];              //  8 KB  recflag per event
+    uint64_t p0[PAIRED ? GRP_CAP : 1]; //  8 KB  first pair key per event (PAIRED)
+    uint64_t p1[PAIRED ? GRP_CAP : 1]; //  8 KB  second pair key per event (PAIRED)
+    uint16_t scnt[GRP_SLOTS];          //  2 KB  events per slot, then fill cursor, then the k-mer's count
+    uint16_t soff[GRP_SLOTS + 2];      //  2 KB  exclusive scan of scnt
     uint16_t ev_slot[GRP_CAP];         //  2 KB  slot per event | after the member fill: 2 x GRP_BPG bucket counters / offsets
     uint16_t member[GRP_CAP];          //  2 KB  event indices grouped by slot
     uint16_t occ[GRP_CAP];             //  2 KB  occupied slots, compacted
@@ -293,7 +301,7 @@ struct GroupSmem {
 constexpr uint64_t EV_SKIP = 1ull << 63;   // mate-2 event whose k-mer mate 1 of the same pair holds too (:849-853)
 constexpr uint32_t GRP_PAIR_THREAD = 8;    // events up to which one thread does the k-mer's len^2 compares; a warp beyond
 
-__device__ __forceinline__ void pair_mark_skipped(GroupSmem &S, uint32_t a0, uint32_t len, uint32_t first, uint32_t step) {
+__device__ __forceinline__ void pair_mark_skipped(GroupSmem<true> &S, uint32_t a0, uint32_t len, uint32_t first, uint32_t step) {
     for (uint32_t e = first; e < len; e += step) {
         const uint32_t m = S.member[a0 + e];
         const uint64_t rf = S.rf[m];
@@ -304,7 +312,7 @@ __device__ __forceinline__ void pair_mark_skipped(GroupSmem &S, uint32_t a0, uin
     }
 }
 
-__device__ __forceinline__ void pair_count(const GroupSmem &S, uint32_t a0, uint32_t len, uint32_t first, uint32_t step,
+__device__ __forceinline__ void pair_count(const GroupSmem<true> &S, uint32_t a0, uint32_t len, uint32_t first, uint32_t step,
                                            uint32_t &c, uint32_t &dups) {
     for (uint32_t e = first; e < len; e += step) {
         const uint32_t m = S.member[a0 + e];
@@ -327,14 +335,15 @@ __device__ __forceinline__ void pair_count(const GroupSmem &S, uint32_t a0, uint
     }
 }
 
+// Single-end: 28 KB of shared memory and at most 32 registers, so 7 CTAs share an SM; pairs: 44 KB and 48, 5 CTAs.
 template <bool PAIRED>
-__global__ void __launch_bounds__(GRP_THREADS)
+__global__ void __launch_bounds__(GRP_THREADS, PAIRED ? 5 : 7)
 k_group_dedup(const EventRec *__restrict__ ev, const uint32_t *__restrict__ g_cnt, uint32_t slot, uint64_t Mb, uint32_t nbk,
               uint32_t g0, int no_dedup, uint64_t *__restrict__ st_hash, uint32_t *__restrict__ st_cnt,
               uint32_t *__restrict__ g_nuniq, uint32_t *__restrict__ g_n,
-              uint8_t *__restrict__ g_fallback, unsigned long long *__restrict__ n_dup) {
+              uint8_t *__restrict__ g_fallback, unsigned long long *__restrict__ counters) {
     extern __shared__ __align__(16) uint8_t grp_smem_raw[];
-    GroupSmem &S = *reinterpret_cast<GroupSmem *>(grp_smem_raw);
+    GroupSmem<PAIRED> &S = *reinterpret_cast<GroupSmem<PAIRED> *>(grp_smem_raw);
     const int tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
     const uint32_t g = blockIdx.x;
     if (tid == 0) {
@@ -344,18 +353,53 @@ k_group_dedup(const EventRec *__restrict__ ev, const uint32_t *__restrict__ g_cn
     }
     const uint32_t e0 = g * slot, bf = (g0 + g) * GRP_BPG;  // g0: first group of the sample's part (sample_parts.hpp)
     const uint32_t n_all = g_cnt[g], n = min(n_all, slot);  // events past the slot are in the overflow list
-    if (tid == 0) { g_n[g] = n; g_nuniq[g] = 0; g_fallback[g] = n_all > slot; }
-    if (n == 0 || n_all > slot) return;
+    // pair keys of event m of the group (single-end: from global memory, last use)
+    auto keys = [&](uint32_t m, uint64_t &ka, uint64_t &kb) {
+        if constexpr (PAIRED) { ka = S.p0[m]; kb = S.p1[m]; return; }
+        const uint4 k = __ldcs(reinterpret_cast<const uint4 *>(ev + e0 + m) + 1);
+        ka = ((uint64_t)k.y << 32) | k.x;
+        kb = ((uint64_t)k.w << 32) | k.z;
+    };
+    // a group that falls back hands its slotted events to the generic path; their number is summed for the host
+    auto leave = [&](bool fallback) {
+        g_nuniq[g] = 0;
+        g_fallback[g] = fallback;
+        if (fallback) atomicAdd(counters + CNT_FALLBACK_TOTAL, (unsigned long long)n);
+    };
+    if (tid == 0) g_n[g] = n;
+    if (n == 0 || n_all > slot) { if (tid == 0) leave(n != 0); return; }
+    // (1) stage the events, group equal hashes: slot per event, events per slot.  Every load of the thread's events is
+    //     in flight before the table is cleared, so the CTA waits for memory once, not once per event.
+    constexpr int EPT = GRP_CAP / GRP_THREADS;  // events per thread (n <= slot <= GRP_CAP)
+    static_assert(GRP_CAP % GRP_THREADS == 0, "whole events per thread");
+    uint4 ea[EPT], eb[PAIRED ? EPT : 1];
+#pragma unroll
+    for (int j = 0; j < EPT; j++) {
+        const uint32_t i = tid + j * GRP_THREADS;
+        if (i < n) {
+            const uint4 *src = reinterpret_cast<const uint4 *>(ev + e0 + i);
+            if constexpr (PAIRED) {
+                ea[j] = __ldcs(src);  // read once
+                eb[j] = __ldcs(src + 1);
+            } else {
+                ea[j] = __ldg(src);  // the keys of the same sector may be read in (2)
+            }
+        }
+    }
     for (int i = tid; i < GRP_SLOTS; i += GRP_THREADS) { S.ht[i] = 0xFFFFFFFFFFFFFFFFull; S.scnt[i] = 0; }
     __syncthreads();
-    // (1) stage the events, group equal hashes: slot per event, events per slot
-    for (uint32_t i = tid; i < n; i += GRP_THREADS) {
-        const uint4 *src = reinterpret_cast<const uint4 *>(ev + e0 + i);
-        const uint4 a = __ldcs(src), b = __ldcs(src + 1);  // read once
+#pragma unroll
+    for (int j = 0; j < EPT; j++) {
+        const uint32_t i = tid + j * GRP_THREADS;
+        if (i >= n) break;
+        const uint4 a = ea[j];
         const unsigned long long h = ((unsigned long long)a.y << 32) | a.x;
         S.rf[i] = ((uint64_t)a.w << 32) | a.z;
-        S.p0[i] = ((uint64_t)b.y << 32) | b.x;
-        S.p1[i] = ((uint64_t)b.w << 32) | b.z;
+        if constexpr (PAIRED) {
+            const uint4 b = eb[j];
+            S.p0[i] = ((uint64_t)b.y << 32) | b.x;
+            S.p1[i] = ((uint64_t)b.w << 32) | b.z;
+        }
         uint32_t sl = (uint32_t)(h ^ (h >> 23)) & (GRP_SLOTS - 1);
         for (;;) {
             const unsigned long long prev = atomicCAS(&S.ht[sl], 0xFFFFFFFFFFFFFFFFull, h);
@@ -427,7 +471,7 @@ k_group_dedup(const EventRec *__restrict__ ev, const uint32_t *__restrict__ g_cn
             atomicAdd(reinterpret_cast<unsigned int *>(lb_cnt) + (lb >> 1), (lb & 1) ? 0x10000u : 1u);
         }
         uint32_t c = 0;
-        if (PAIRED) {
+        if constexpr (PAIRED) {
             if (len > GRP_PAIR_THREAD) { S.longs[atomicAdd(&S.nlong, 1u)] = (uint16_t)sl; continue; }
             if (len == 1) c = 1;
             else { pair_mark_skipped(S, a0, len, 0, 1); pair_count(S, a0, len, 0, 1, c, my_dups); }
@@ -457,7 +501,8 @@ k_group_dedup(const EventRec *__restrict__ ev, const uint32_t *__restrict__ g_cn
                 if (ks[j] == INF) continue;  // len < 4
                 const uint32_t m = (uint32_t)ks[j] & 1023u;
                 if ((ks[j] >> 10) & NO_PAIR) { c++; continue; }
-                const uint64_t ka = S.p0[m], kb = S.p1[m];
+                uint64_t ka, kb;
+                keys(m, ka, kb);
                 bool found = (kb == ka);
 #pragma unroll
                 for (int i = 0; i < j; i++)
@@ -483,7 +528,7 @@ k_group_dedup(const EventRec *__restrict__ ev, const uint32_t *__restrict__ g_cn
     for (uint32_t li = wid; li < S.nlong; li += GRP_THREADS / 32) {
         const uint32_t sl = S.longs[li];
         const uint32_t a0 = S.soff[sl], len = S.soff[sl + 1] - a0;
-        if (PAIRED) {
+        if constexpr (PAIRED) {
             uint32_t c = 0, dups = 0;
             pair_mark_skipped(S, a0, len, lane, 32);
             __syncwarp();
@@ -517,7 +562,8 @@ k_group_dedup(const EventRec *__restrict__ ev, const uint32_t *__restrict__ g_cn
             }
             first = false; last_key = best; last_m = bm; done++;
             if (best & NO_PAIR) { c++; continue; }
-            const uint64_t ka = S.p0[bm], kb = S.p1[bm];
+            uint64_t ka, kb;
+            keys(bm, ka, kb);
             const bool in_a = __any_sync(0xffffffffu, lane < (int)nset && dset == ka);
             bool ret = in_a && c > 0;
             if (!in_a) { if (lane == (int)nset) dset = ka; nset++; }
@@ -531,8 +577,8 @@ k_group_dedup(const EventRec *__restrict__ ev, const uint32_t *__restrict__ g_cn
     }
     if (my_dups) atomicAdd(&S.dups, my_dups);
     __syncthreads();
-    if (S.overflow) { if (tid == 0) g_fallback[g] = 1; return; }
-    // (3) output order: lb_cnt holds the k-mers per bucket (counted in (2)).
+    if (S.overflow) { if (tid == 0) leave(true); return; }
+    // (3) output order: lb_cnt holds the k-mers per bucket (counted in (2)); the group's sorted uniques go to its slot.
     {
         uint16_t *list = S.member;  // event grouping is dead: k-mer slots ordered by bucket
         static_assert(GRP_BPG == 32, "one lane per bucket");
@@ -564,10 +610,16 @@ k_group_dedup(const EventRec *__restrict__ ev, const uint32_t *__restrict__ g_cn
             st_cnt[e0 + q0 + r] = S.scnt[sl];
         }
     }
-    if (tid == 0) { g_nuniq[g] = nu; if (S.dups) atomicAdd(n_dup, (unsigned long long)S.dups); }
+    if (tid == 0) {
+        g_nuniq[g] = nu;
+        g_fallback[g] = 0;
+        atomicAdd(counters + CNT_UNIQ_TOTAL, (unsigned long long)nu);
+        if (S.dups) atomicAdd(counters + CNT_DUPS, (unsigned long long)S.dups);
+    }
 }
 
-// staged pairs of group g live at [g * slot, g * slot + nuniq); dense destination starts at uoff[g]
+// The result from the staged pairs of group g, at [g * slot, g * slot + nuniq), or for a fallback group from the generic
+// path's uniques (k_fallback_place: g_src); the destination of group g starts at uoff[g]
 __global__ void k_compact_uniq(const uint64_t *__restrict__ st_hash, const uint32_t *__restrict__ st_cnt,
                                uint32_t slot, const uint32_t *__restrict__ g_nuniq,
                                const uint32_t *__restrict__ uoff, const uint8_t *__restrict__ g_fallback,
@@ -693,7 +745,7 @@ struct SampleBuilder {
         if (ev_total() >= 0xFFFFFFFEull) { set_error("more than 2^32-2 survivor events in one sample"); return SYL_ERR_ARG; }
         SYL_TRY(b_ev.alloc(ev_total(), st));
         SYL_TRY(b_pend.alloc(ev_total(), st));
-        SYL_CUDA(cudaMemsetAsync(ctx->d_counters, 0, 4 * sizeof(uint64_t), st));  // CNT_EVENTS .. CNT_PEND_MATE1
+        SYL_CUDA(cudaMemsetAsync(ctx->d_counters, 0, 6 * sizeof(uint64_t), st));  // CNT_EVENTS .. CNT_FALLBACK_TOTAL
         return SYL_OK;
     }
 
@@ -818,42 +870,40 @@ struct SampleBuilder {
         unsigned long long *dc = d_count();
         EventRec *ev = b_ev.p;
         // ---- primary path: CTA-local grouping / dedup of the group slots (ng, slot, Mb, g_cnt: begin()).
-        // The kernels read the group counts from device memory.
+        // The kernels read the group counts from device memory.  k_group_dedup writes each group's sorted uniques into
+        // the group's slot of the staging arrays and sums the uniques (and the slotted events of the fallback groups)
+        // into the device counters, so one scan of the per-group counts before the sync and one compaction into the
+        // exact-size result after it complete the sketch.
         const uint64_t n_slots = (uint64_t)ng * slot;
-        DevBuf<uint32_t> st_cnt, g_nuniq, g_n, uoff, fsz, foff, g_src, tmp_c;
-        DevBuf<uint64_t> st_hash, tmp_h;
+        DevBuf<uint32_t> st_cnt, g_nuniq, g_n, uoff, fsz, foff, g_src;
+        DevBuf<uint64_t> st_hash;
         DevBuf<uint8_t> g_fb;
         if (ng) {
-            SYL_TRY(st_hash.alloc(n_slots, st)); SYL_TRY(st_cnt.alloc(n_slots, st));
-            SYL_TRY(tmp_h.alloc(n_slots, st)); SYL_TRY(tmp_c.alloc(n_slots, st));  // in-kernel uniques: <= the slotted events
-            SYL_TRY(g_nuniq.alloc(ng, st)); SYL_TRY(g_n.alloc(ng, st));
-            SYL_TRY(g_fb.alloc(ng, st)); SYL_TRY(uoff.alloc((uint64_t)ng + 1, st)); SYL_TRY(fsz.alloc(ng, st));
-            SYL_TRY(foff.alloc((uint64_t)ng + 1, st)); SYL_TRY(g_src.alloc(ng, st));
+            SYL_TRY(st_hash.alloc(n_slots, st)); SYL_TRY(st_cnt.alloc(n_slots, st));  // in-kernel uniques <= slotted events
+            SYL_TRY(g_nuniq.alloc(ng, st)); SYL_TRY(g_n.alloc(ng, st)); SYL_TRY(g_fb.alloc(ng, st));
+            SYL_TRY(uoff.alloc((uint64_t)ng + 1, st)); SYL_TRY(g_src.alloc(ng, st));
             auto group_dedup = paired ? k_group_dedup<true> : k_group_dedup<false>;
-            SYL_CUDA(cudaFuncSetAttribute(group_dedup, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(GroupSmem)));
+            const int smem = paired ? (int)sizeof(GroupSmem<true>) : (int)sizeof(GroupSmem<false>);
+            SYL_CUDA(cudaFuncSetAttribute(group_dedup, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
             {
                 KernelTimer kt(ctx, SYL_KERNEL_GROUP_DEDUP);
-                group_dedup<<<ng, GRP_THREADS, sizeof(GroupSmem), st>>>(ev, g_cnt.p, slot, Mb, nbk, g0, no_dedup,
-                                                                         st_hash.p, st_cnt.p, g_nuniq.p, g_n.p, g_fb.p, dc + CNT_DUPS);
+                group_dedup<<<ng, GRP_THREADS, smem, st>>>(ev, g_cnt.p, slot, Mb, nbk, g0, no_dedup, st_hash.p, st_cnt.p,
+                                                            g_nuniq.p, g_n.p, g_fb.p, dc);
             }
             k_scan_u32<<<1, 1024, 0, st>>>(g_nuniq.p, ng, uoff.p);
-            k_fallback_sizes<<<nblk(ng, 256), 256, 0, st>>>(g_n.p, g_fb.p, ng, fsz.p);
-            k_scan_u32<<<1, 1024, 0, st>>>(fsz.p, ng, foff.p);
-            k_compact_uniq<<<ng, 128, 0, st>>>(st_hash.p, st_cnt.p, slot, g_nuniq.p, uoff.p, g_fb.p, g_src.p, nullptr, nullptr,
-                                                tmp_h.p, tmp_c.p);
-            ctx->launches += 5;
+            ctx->launches += 2;
             SYL_CUDA(cudaGetLastError());
-            SYL_CUDA(cudaMemcpyAsync(ctx->h_counters + CNT_UNIQ_TOTAL, uoff.p + ng, 4, cudaMemcpyDeviceToHost, st));
-            SYL_CUDA(cudaMemcpyAsync(ctx->h_counters + CNT_FALLBACK_TOTAL, foff.p + ng, 4, cudaMemcpyDeviceToHost, st));
         }
-        SYL_CUDA(cudaMemcpyAsync(ctx->h_counters, dc, 24, cudaMemcpyDeviceToHost, st));  // CNT_EVENTS, CNT_PENDING, CNT_DUPS
+        // CNT_EVENTS, CNT_PENDING, CNT_DUPS, CNT_PEND_MATE1, CNT_UNIQ_TOTAL, CNT_FALLBACK_TOTAL (all cleared in begin())
+        static_assert(CNT_UNIQ_TOTAL == 4 && CNT_FALLBACK_TOTAL == 5, "one copy of slots 0 .. 5");
+        SYL_CUDA(cudaMemcpyAsync(ctx->h_counters, dc, 6 * sizeof(uint64_t), cudaMemcpyDeviceToHost, st));
         SYL_CUDA(cudaStreamSynchronize(st));  // the one synchronisation of a sketch
         const uint64_t N_ovf = ctx->h_counters[CNT_EVENTS];
         if (N_ovf > cap) { *need_cap = N_ovf; return SYL_ERR_CAPACITY; }
         // the overflow list holds only events of groups past their slot, all of which are fallback groups (without
         // groups: every event)
-        const uint64_t U1 = ng ? (uint32_t)ctx->h_counters[CNT_UNIQ_TOTAL] : 0;
-        const uint64_t NF_slots = ng ? (uint32_t)ctx->h_counters[CNT_FALLBACK_TOTAL] : 0;
+        const uint64_t U1 = ng ? ctx->h_counters[CNT_UNIQ_TOTAL] : 0;
+        const uint64_t NF_slots = ng ? ctx->h_counters[CNT_FALLBACK_TOTAL] : 0;
         const uint64_t NF = NF_slots + N_ovf;
         uint64_t ndup = ctx->h_counters[CNT_DUPS];
         static const bool dbg = getenv("SYL_DEBUG_TIMING") != nullptr;
@@ -867,9 +917,12 @@ struct SampleBuilder {
         if (NF) {
             uint64_t nd2 = 0;
             SYL_TRY(fh.alloc(NF, st)); SYL_TRY(f_rf.alloc(NF, st)); SYL_TRY(f_p0.alloc(NF, st)); SYL_TRY(f_p1.alloc(NF, st));
-            if (ng) {
+            if (NF_slots) {  // the fallback groups' slotted events, compacted in group order
+                SYL_TRY(fsz.alloc(ng, st)); SYL_TRY(foff.alloc((uint64_t)ng + 1, st));
+                k_fallback_sizes<<<nblk(ng, 256), 256, 0, st>>>(g_n.p, g_fb.p, ng, fsz.p);
+                k_scan_u32<<<1, 1024, 0, st>>>(fsz.p, ng, foff.p);
                 k_gather_fallback<<<ng, 256, 0, st>>>(ev, slot, g_n.p, g_fb.p, foff.p, fh.p, f_rf.p, f_p0.p, f_p1.p);
-                ctx->launches++;
+                ctx->launches += 3;
             }
             if (N_ovf) {
                 k_unpack_events<<<nblk(N_ovf, 256), 256, 0, st>>>(ev + n_slots, N_ovf, fh.p + NF_slots, f_rf.p + NF_slots,
@@ -883,16 +936,19 @@ struct SampleBuilder {
         const uint64_t U = U1 + U2;
         SYL_TRY(hblock_alloc(ctx, (void **)&s->hash, std::max<uint64_t>(U, 1) * 8));
         SYL_TRY(hblock_alloc(ctx, (void **)&s->count, std::max<uint64_t>(U, 1) * 4));
-        if (ng && U2) {  // slot the generic path's pairs into their groups' positions, compact straight into the result
-            k_fallback_place<<<nblk(ng, 128), 128, 0, st>>>(g_fb.p, ng, g0, nbk, Mb, f_uq.p, U2, g_nuniq.p, g_src.p);
-            k_scan_u32<<<1, 1024, 0, st>>>(g_nuniq.p, ng, uoff.p);
+        if (ng) {
+            if (U2) {  // slot the generic path's pairs into the fallback groups' positions
+                k_fallback_place<<<nblk(ng, 128), 128, 0, st>>>(g_fb.p, ng, g0, nbk, Mb, f_uq.p, U2, g_nuniq.p, g_src.p);
+                k_scan_u32<<<1, 1024, 0, st>>>(g_nuniq.p, ng, uoff.p);
+                ctx->launches += 2;
+            }
             k_compact_uniq<<<ng, 128, 0, st>>>(st_hash.p, st_cnt.p, slot, g_nuniq.p, uoff.p, g_fb.p, g_src.p, f_uq.p, f_ct.p,
                                                 s->hash, s->count);
-            ctx->launches += 3;
+            ctx->launches++;
             SYL_CUDA(cudaGetLastError());
-        } else if (U) {  // the in-kernel uniques, or without groups the generic path's
-            SYL_CUDA(cudaMemcpyAsync(s->hash, ng ? tmp_h.p : f_uq.p, U * 8, cudaMemcpyDeviceToDevice, st));
-            SYL_CUDA(cudaMemcpyAsync(s->count, ng ? tmp_c.p : f_ct.p, U * 4, cudaMemcpyDeviceToDevice, st));
+        } else if (U) {  // without groups: the generic path's uniques
+            SYL_CUDA(cudaMemcpyAsync(s->hash, f_uq.p, U * 8, cudaMemcpyDeviceToDevice, st));
+            SYL_CUDA(cudaMemcpyAsync(s->count, f_ct.p, U * 4, cudaMemcpyDeviceToDevice, st));
         }
         if (NF) SYL_CUDA(cudaStreamSynchronize(st));  // f_uq / f_ct go out of scope
         s->n = U;

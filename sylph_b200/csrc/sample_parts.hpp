@@ -22,7 +22,11 @@ constexpr uint64_t SAMPLE_MAX_EVENTS = 0xFFFFFFFEull;  // a part's event array (
 
 // Device bytes per entry of the post-pass arrays (sample.cu, SampleBuilder):
 constexpr uint64_t SP_EVENT_BYTES = 32 + 4;          // begin(): EventRec + pending index, per slot and per overflow entry
-constexpr uint64_t SP_STAGE_BYTES = 8 + 4 + 8 + 4;   // finish(): staged and compacted (hash, count), per slot
+// finish(): the staged (hash, count) pairs k_group_dedup writes, 8 + 4 B per slot (the exact-size result is
+// SP_RESULT_BYTES).  The plan reserves twice that, as when the uniques were staged and then compacted into a second
+// array: the planned part sizes, and with them the parts a budget yields, stay as they were, 12 B per slot (about 19 B
+// per expected event) on the safe side.
+constexpr uint64_t SP_STAGE_BYTES = 8 + 4 + 8 + 4;
 constexpr uint64_t SP_GROUP_BYTES = 4 + 6 * 4 + 1;   // g_cnt; g_nuniq, g_n, uoff, fsz, foff, g_src; g_fb
 // the generic path per event handed to it: the event's four words, two index and two key buffers of the radix sorts,
 // the sorts' alternate buffers, uniques, run offsets and lengths, counts and the two-slot dedup set
