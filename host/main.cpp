@@ -23,6 +23,8 @@
 #include <thread>
 #include <vector>
 
+#include <unistd.h>
+
 #include "../include/sylph_b200.h"
 #include "fastx.hpp"
 #include "inspect.hpp"
@@ -82,10 +84,11 @@ struct Args {
     std::vector<int> devices;  // --devices: one context per entry (a device may repeat); empty = {device}
     // test hooks (INTEGRATION.md), read once from the environment: small values make the split paths run on small inputs
     uint64_t batch_bases = 1ull << 30;  // SYL_DRIVER_BATCH_BASES: a genome batch closes once it holds this many bases
-    uint64_t samples_per_call = 0;      // SYL_DRIVER_SAMPLES_PER_CALL: cap on samples per syl_query / syl_profile call (0 = none)
+    uint64_t samples_per_call = 0;      // SYL_DRIVER_SAMPLES_PER_CALL: cap on samples per host batch of query / profile (0 = none)
     uint64_t rows0 = 0;                 // SYL_DRIVER_ROWS: initial row-buffer length (0 = sized from the call)
     uint64_t shard_entries = 0;         // SYL_DRIVER_SHARD_ENTRIES: query / profile through db shards of this many entries
     uint64_t max_db_entries = 0;        // --max-db-entries: the same, as an option
+    uint64_t max_sample_bytes = 0;      // --max-sample-bytes: host bytes of one batch of query / profile samples (0 = default)
 };
 
 static uint64_t env_u64(const char *name, uint64_t dflt) {
@@ -185,6 +188,12 @@ static Args parse(int argc, char **argv) {
         else if (s == "-u" || s == "--estimate-unknown") a.estimate_unknown = true;
         else if (s == "-I" || s == "--read-seq-id") a.read_seq_id = std::stod(need(i));
         else if (s == "--max-db-entries") a.max_db_entries = std::max<uint64_t>(1, std::stoull(need(i)));  // driver-only
+        else if (s == "--max-sample-bytes") {  // driver-only
+            const std::string v = need(i);
+            if (v.empty() || v.size() > 19 || v.find_first_not_of("0123456789") != std::string::npos || std::stoull(v) == 0)
+                die("--max-sample-bytes " + v + ": not a positive number of bytes");
+            a.max_sample_bytes = std::stoull(v);
+        }
         else if (a.cmd == "sketch" && (s == "-S" || s == "--sample-names")) {
             while (i + 1 < argc && argv[i + 1][0] != '-') a.sample_names.push_back(argv[++i]);
         }
@@ -734,14 +743,65 @@ static int cmd_contain(const std::vector<syl_ctx *> &ctxs, const Args &a, bool p
     p.estimate_unknown = a.estimate_unknown ? 1 : 0; p.read_seq_id = a.read_seq_id;
     std::vector<std::string> names(n_samples);
     RowPrinter printer(o, pseudotax, names, gs);
+    // Each context queries its block of samples in host batches of at most --max-sample-bytes (default: a quarter of
+    // physical memory shared by the contexts), one syl_*_host_samples call per batch; the library stages each batch
+    // through the device in pieces that fit it, so the device never holds more than one batch's share.  The reference
+    // walks the samples in chunks too (src/contain.rs:239-263).
+    uint64_t max_bytes = a.max_sample_bytes;
+    if (!max_bytes) {
+        const long pages = sysconf(_SC_PHYS_PAGES), page = sysconf(_SC_PAGE_SIZE);
+        max_bytes = std::max<uint64_t>(1, (uint64_t)std::max(pages, 1L) * (uint64_t)std::max(page, 1L) / 4 / ctxs.size());
+    }
     run_workers(ctxs.size(), [&](size_t w) {
         syl_ctx *ctx = ctxs[w];
+        const ContextDb &db = dbs[w];
         const size_t s_begin = block[w], s_end = block[w + 1];
-        std::vector<syl_sample *> samples;
-        std::vector<size_t> ids;  // global index of each sample of `samples`
-        // a raw read file is sketched on the context that queries it
+        // one host batch: the samples' pairs back to back, in the order they were added
+        std::vector<uint64_t> hashes, off{0}, cs;
+        std::vector<uint32_t> counts;
+        std::vector<double> mrl;
+        std::vector<size_t> ids;  // global index of each sample of the batch
+        int batch_k = (int)gs[0].k;
+        auto flush = [&]() {
+            if (ids.empty()) return;
+            check_abort();
+            const syl_host_samples hs{hashes.data(), counts.data(), off.data(), cs.data(), mrl.data(), (uint32_t)ids.size(), batch_k};
+            std::vector<syl_ani_row> rows(a.rows0 ? a.rows0 : std::max<size_t>(1024, std::min<size_t>(gs.size() * ids.size(), 1u << 22)));
+            uint64_t n = 0;
+            for (;;) {
+                const int rc = (pseudotax ? syl_profile_host_samples : syl_query_host_samples)(ctx, db.db, db.shards, &hs, &p, rows.data(),
+                                                                                                rows.size(), &n);
+                if (rc == SYL_ERR_CAPACITY) { rows.resize(n); continue; }  // shards: the retry copies out the kept rows
+                check(rc, pseudotax ? "syl_profile_host_samples" : "syl_query_host_samples");
+                break;
+            }
+            rows.resize(n);
+            size_t i = 0;
+            for (uint32_t s = 0; s < ids.size(); s++) {
+                size_t j = i;
+                while (j < rows.size() && rows[j].sample == s) j++;
+                printer.done(ids[s], std::vector<syl_ani_row>(rows.begin() + i, rows.begin() + j), true);
+                i = j;
+            }
+            hashes.clear(); counts.clear(); off.assign(1, 0); cs.clear(); mrl.clear(); ids.clear();
+        };
+        // a sample joins the batch unless the batch holds samples and would pass the byte or sample cap with it
+        auto add = [&](size_t id, const uint64_t *h, const uint32_t *c, uint64_t n, int k, uint64_t sc, double m) {
+            const uint64_t bytes = 12 * (hashes.size() + n) + 24 * (ids.size() + 1);
+            if (!ids.empty() && (bytes > max_bytes || k != batch_k || (a.samples_per_call && ids.size() >= a.samples_per_call))) flush();
+            batch_k = k;
+            hashes.insert(hashes.end(), h, h + n);
+            counts.insert(counts.end(), c, c + n);
+            off.push_back(hashes.size());
+            cs.push_back(sc);
+            mrl.push_back(m);
+            ids.push_back(id);
+        };
+        // a raw read file is sketched on the context that queries it and copied out to the host batch
         std::vector<std::string> my_reads(read_files.begin() + std::min(s_begin, n_reads), read_files.begin() + std::min(s_end, n_reads));
         ParseQueue queue(my_reads, false);
+        std::vector<uint64_t> h;
+        std::vector<uint32_t> c;
         for (;;) {
             check_abort();
             ParsedFile pf;
@@ -754,8 +814,12 @@ static int cmd_contain(const std::vector<syl_ctx *> &ctxs, const Args &a, bool p
             syl_sample *s = nullptr;
             check(syl_sketch_reads(ctx, SYL_MEM_HOST, r.bases.data(), r.bases.size(), r.offsets.data(), r.n(), (int)gs[0].k, a.c, 0,
                                    SYL_SEM_AVX2, &s), "syl_sketch_reads");
-            samples.push_back(s);
-            ids.push_back(id);
+            h.resize(syl_sample_size(s));
+            c.resize(h.size());
+            check(syl_sample_download(ctx, s, h.data(), c.data()), "syl_sample_download");
+            const double m = syl_sample_mean_read_length(s);
+            syl_sample_free(s);
+            add(id, h.data(), c.data(), h.size(), (int)gs[0].k, a.c, m);
         }
         for (size_t id = std::max(s_begin, n_reads); id < s_end; id++) {
             check_abort();
@@ -766,43 +830,10 @@ static int cmd_contain(const std::vector<syl_ctx *> &ctxs, const Args &a, bool p
                 printer.done(id, {}, false);
                 continue;
             }
-            syl_sample *s = nullptr;
-            check(syl_sample_upload(ctx, SYL_MEM_HOST, sk.hashes.data(), sk.counts.data(), sk.hashes.size(), (int)sk.k, sk.c, &s), "syl_sample_upload");
-            syl_sample_set_mean_read_length(s, sk.mean_read_length);
-            samples.push_back(s);
-            ids.push_back(id);
             names[id] = sk.has_sample_name ? sk.sample_name : sk.file_name;
+            add(id, sk.hashes.data(), sk.counts.data(), sk.hashes.size(), (int)sk.k, sk.c, sk.mean_read_length);
         }
-        // sample batches sized so that samples x genomes stays below the library's per-call limits (2^31 pairs,
-        // 8 GB of per-pair histograms = 2^23 pairs); the reference walks the samples in chunks too (src/contain.rs:239-263).
-        // Shards take every sample in one call (the library batches them per shard), so each shard is built once.
-        const ContextDb &db = dbs[w];
-        size_t per_call = std::max<size_t>(1, std::min<size_t>(samples.size(), (size_t)((1ull << 22) / std::max<size_t>(gs.size(), 1))));
-        if (a.samples_per_call) per_call = std::min<size_t>(per_call, a.samples_per_call);
-        if (db.shards) per_call = std::max<size_t>(1, samples.size());
-        for (size_t s0 = 0; s0 < samples.size(); s0 += per_call) {
-            check_abort();
-            const size_t ns = std::min(per_call, samples.size() - s0);
-            std::vector<syl_ani_row> rows(a.rows0 ? a.rows0 : std::max<size_t>(1024, std::min<size_t>(gs.size() * ns, 1u << 22)));
-            uint64_t n = 0;
-            for (;;) {
-                int rc = db.shards ? (pseudotax ? syl_profile_shards : syl_query_shards)(ctx, db.shards, samples.data() + s0, (uint32_t)ns, &p,
-                                                                                          rows.data(), rows.size(), &n)
-                                   : (pseudotax ? syl_profile : syl_query)(ctx, db.db, samples.data() + s0, (uint32_t)ns, &p, rows.data(), rows.size(), &n);
-                if (rc == SYL_ERR_CAPACITY) { rows.resize(n); continue; }  // shards: the retry copies out the kept rows
-                check(rc, db.shards ? (pseudotax ? "syl_profile_shards" : "syl_query_shards") : (pseudotax ? "syl_profile" : "syl_query"));
-                break;
-            }
-            rows.resize(n);
-            size_t i = 0;
-            for (uint32_t s = 0; s < ns; s++) {
-                size_t j = i;
-                while (j < rows.size() && rows[j].sample == s) j++;
-                printer.done(ids[s0 + s], std::vector<syl_ani_row>(rows.begin() + i, rows.begin() + j), true);
-                i = j;
-            }
-        }
-        for (syl_sample *s : samples) syl_sample_free(s);
+        flush();
     });
     if (o != stdout) fclose(o);
     for (ContextDb &db : dbs) {

@@ -193,7 +193,10 @@ int syl_ctx_ingest_ring_bytes(const syl_ctx *ctx, uint64_t *device_bytes, uint64
  * host ASCII fed again for every part).  The parts' sketches wait in host memory and are assembled into the same
  * sketch, num_dup_removed and mean_read_length as one pass gives.  A budget that even 64 parts exceed is SYL_ERR_OOM
  * before anything is allocated; the message names the bytes needed.
- * syl_ctx_set_sample_memory: max_bytes of device memory a sketch call may use (block-cache blocks plus staging rings);
+ * syl_ctx_set_sample_memory: max_bytes of device memory a sketch call may use (block-cache blocks plus staging rings),
+ *   and that a host-samples query or profile (section 7) may use in block-cache blocks (its batch slots, sort and join
+ *   scratch, and with shards the largest shard's build; the staging rings, which that call shares with the sketch
+ *   calls and leaves allocated, are not counted against it);
  *   0 (the default) = the device's free memory at call time plus what the ctx holds in cached free blocks and rings
  *   (a sample whose one pass needs less than half of the free memory the ctx saw at its last look takes one pass
  *   without looking again).
@@ -437,6 +440,49 @@ int syl_query_shards(syl_ctx *ctx, syl_db_shards *s, const syl_sample *const *sa
 int syl_profile_shards(syl_ctx *ctx, syl_db_shards *s, const syl_sample *const *samples, uint32_t n_samples,
                        const syl_contain_params *p, syl_ani_row *rows, uint64_t cap, uint64_t *n_rows);
 void syl_db_shards_free(syl_db_shards *s);
+
+/* ------------------------------------------------------------------------------------------
+ * (7) Query and profile samples from HOST memory, any number of them, in bounded device memory: e.g. every deserialised
+ *     .sylsp of a study (the reference reads, sketches and profiles samples one chunk at a time, src/contain.rs:239-269).
+ *
+ * syl_host_samples: sample i holds the pairs hash[off[i] .. off[i + 1]) / count[...], in any order (as a .sylsp map),
+ * with distinct hashes; c[i] and mean_read_length[i] are its sketch parameter and mean read length (-u reads it); k is
+ * every sample's.  The arrays are borrowed for the duration of the call, in pinned or pageable host memory.
+ *
+ * syl_query_host_samples / syl_profile_host_samples take exactly one of db or shards (else SYL_ERR_ARG) and return the
+ * rows, order and values of syl_query / syl_profile (syl_query_shards / syl_profile_shards) on handles made with
+ * syl_sample_upload + syl_sample_set_mean_read_length from the same arrays; row.sample is the index into s.  The
+ * arguments are checked as there, before anything is allocated; offsets that do not start at 0 or decrease and device
+ * pointers are SYL_ERR_ARG.  SYL_ERR_CAPACITY: with a db, resize and call again; with shards, the handle keeps the rows
+ * as in section (6), keyed on the array pointers and n_samples.
+ *
+ * The samples are cut into contiguous batches, each the longest run that fits half the device budget of
+ * syl_ctx_set_sample_memory and at most 2^22 (sample, genome) pairs (with shards: pairs of the largest shard).  A batch
+ * costs its slot (12 bytes per k-mer), its share of the sort's second buffer (24 bytes per k-mer over both slots) and
+ * its joins' scratch (about 1 KB per pair, 16 bytes per k-mer of its largest sample per sample, 200 KB per sample);
+ * with shards the budget also covers the largest shard's build (16 bytes per entry).  The default budget is the free
+ * memory once the ctx's staging ring exists, plus the ctx's cached free blocks.  A sample that does not fit alone
+ * is SYL_ERR_OOM before anything is allocated, with the bytes it needs in the message.  Each batch crosses the link in
+ * one pass on the ctx's host-ingest copy stream (pageable arrays through its pinned ring) and is sorted there by one
+ * segmented sort, while the previous batch is joined on the ctx stream.  With shards, each shard is built once per
+ * call: every batch is joined with it before the next one is built (profile: then its survivor indexes, each joined
+ * with samples of one batch, staged again unless a slot still holds them, while the index is gathered and built).
+ * SYL_SAMPLE_BATCH=N (test hook, read per call) caps a batch at N samples.
+ * ---------------------------------------------------------------------------------------- */
+typedef struct {
+    const uint64_t *hash;            /* all samples' k-mers back to back */
+    const uint32_t *count;
+    const uint64_t *off;             /* n_samples + 1 monotone offsets, off[0] == 0 */
+    const uint64_t *c;               /* per sample */
+    const double *mean_read_length;  /* per sample */
+    uint32_t n_samples;
+    int k;
+} syl_host_samples;
+
+int syl_query_host_samples(syl_ctx *ctx, const syl_db *db, syl_db_shards *shards, const syl_host_samples *s,
+                           const syl_contain_params *p, syl_ani_row *rows, uint64_t cap, uint64_t *n_rows);
+int syl_profile_host_samples(syl_ctx *ctx, const syl_db *db, syl_db_shards *shards, const syl_host_samples *s,
+                             const syl_contain_params *p, syl_ani_row *rows, uint64_t cap, uint64_t *n_rows);
 
 #ifdef __cplusplus
 }

@@ -32,6 +32,13 @@ class AniRow(C.Structure):
     ]
 
 
+class HostSamples(C.Structure):
+    _fields_ = [
+        ("hash", C.c_void_p), ("count", C.c_void_p), ("off", C.c_void_p), ("c", C.c_void_p),
+        ("mean_read_length", C.c_void_p), ("n_samples", C.c_uint32), ("k", C.c_int),
+    ]
+
+
 assert C.sizeof(Survivor) == 16
 assert C.sizeof(AniRow) == 144
 
@@ -109,6 +116,8 @@ SIGNATURES = {
     "syl_query_shards": (_i, [_vp, _vp, _pp, _u32, C.POINTER(ContainParams), _vp, _u64, _pu64]),
     "syl_profile_shards": (_i, [_vp, _vp, _pp, _u32, C.POINTER(ContainParams), _vp, _u64, _pu64]),
     "syl_db_shards_free": (None, [_vp]),
+    "syl_query_host_samples": (_i, [_vp, _vp, _vp, C.POINTER(HostSamples), C.POINTER(ContainParams), _vp, _u64, _pu64]),
+    "syl_profile_host_samples": (_i, [_vp, _vp, _vp, C.POINTER(HostSamples), C.POINTER(ContainParams), _vp, _u64, _pu64]),
 }
 
 

@@ -360,6 +360,43 @@ class Context:
         params = params or contain_params(pseudotax=True)
         return self._pairs(_lib.lib().syl_profile, db, samples, params, cap)
 
+    def _host_samples(self, fn, db, hashes, counts, off, c, mean_read_length, k, params, cap):
+        off = np.ascontiguousarray(off, dtype=np.uint64)
+        if off.ndim != 1 or off.size < 1:
+            raise ValueError("off must hold n_samples + 1 offsets")
+        n = off.size - 1
+        keep = [a if isinstance(a, np.ndarray) and a.flags.c_contiguous and a.dtype == t else np.ascontiguousarray(a, dtype=t)
+                for a, t in ((hashes, np.uint64), (counts, np.uint32))]
+        cs = np.ascontiguousarray(np.broadcast_to(np.asarray(c, dtype=np.uint64), (n,)))
+        mrl = np.ascontiguousarray(np.broadcast_to(np.asarray(mean_read_length, dtype=np.float64), (n,)))
+        s = _lib.HostSamples(keep[0].ctypes.data, keep[1].ctypes.data, off.ctypes.data, cs.ctypes.data, mrl.ctypes.data, n,
+                             int(params.k if k is None else k))
+        one, shards = (db._h, None) if isinstance(db, Db) else (None, db._h)
+        if cap is None:
+            cap = max(4096, 1024 * max(n, 1))
+        while True:
+            rows = np.empty(cap, dtype=ANI_ROW_DTYPE)
+            n_rows = C.c_uint64(0)
+            rc = fn(self._h, one, shards, C.byref(s), C.byref(params), rows.ctypes.data_as(C.c_void_p), cap, C.byref(n_rows))
+            if rc == _lib.SYL_ERR_CAPACITY:
+                cap = n_rows.value
+                continue
+            _lib.check(rc)
+            return rows[: n_rows.value].copy()
+
+    def query_host_samples(self, db, hashes, counts, off, c, mean_read_length, params=None, cap=None, k=None):
+        """`sylph query` of samples in host memory (syl_query_host_samples): sample i holds hashes / counts
+        [off[i], off[i + 1]) in any order; c and mean_read_length per sample (or one value for all).  db is a Db or a
+        DbShards.  The samples are staged on the device in batches that fit the sample memory budget
+        (set_sample_memory), so any number of them may be given.  Same rows as query() on uploaded samples."""
+        params = params or contain_params(pseudotax=False)
+        return self._host_samples(_lib.lib().syl_query_host_samples, db, hashes, counts, off, c, mean_read_length, k, params, cap)
+
+    def profile_host_samples(self, db, hashes, counts, off, c, mean_read_length, params=None, cap=None, k=None):
+        """`sylph profile` of samples in host memory (syl_profile_host_samples); see query_host_samples."""
+        params = params or contain_params(pseudotax=True)
+        return self._host_samples(_lib.lib().syl_profile_host_samples, db, hashes, counts, off, c, mean_read_length, k, params, cap)
+
 
 class ProfileJob:
     """One in-flight `profile` over a genome-sharded db (syl_profile_job): see include/sylph_b200.h section (5).

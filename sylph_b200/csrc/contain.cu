@@ -32,11 +32,14 @@
 #include <cmath>
 #include <cstdio>
 #include <cstring>
+#include <functional>
 #include <new>
 #include <vector>
 
 #include "common.cuh"
 #include "crmath.cuh"
+#include "ingest.hpp"
+#include "sample_batches.hpp"
 #include "shard_cut.hpp"
 
 struct syl_db {
@@ -1082,13 +1085,16 @@ __global__ void k_sum_counts(const uint32_t *__restrict__ count, uint64_t n, uns
     if ((threadIdx.x & 31) == 0 && acc) atomicAdd(out, acc);
 }
 
-// -u: sample meta (sum of the counts is computed on the device once per sample handle)
-static int sample_metas(syl_ctx *ctx, const syl_sample *const *samples, uint32_t n, std::vector<SampleMeta> &out) {
+// Device handles as the views the joins take, and what -u needs to know of them (the sum of the counts is computed on the
+// device once per handle, and only for -u).
+static int handle_views(syl_ctx *ctx, const syl_sample *const *samples, uint32_t n, bool unknown, std::vector<SampleView> &views,
+                        std::vector<SampleMeta> &metas) {
     cudaStream_t st = ctx->stream;
-    out.resize(n);
+    views.resize(n);
+    metas.resize(n);
     for (uint32_t i = 0; i < n; i++) {
         syl_sample *s = const_cast<syl_sample *>(samples[i]);
-        if (!s->sum_counts_valid) {
+        if (unknown && !s->sum_counts_valid) {
             unsigned long long *d = reinterpret_cast<unsigned long long *>(ctx->d_counters + CNT_SUM_COUNTS);
             SYL_CUDA(cudaMemsetAsync(d, 0, 8, st));
             if (s->n) k_sum_counts<<<ctx->num_sms * 4, 256, 0, st>>>(s->count, s->n, d);
@@ -1097,7 +1103,8 @@ static int sample_metas(syl_ctx *ctx, const syl_sample *const *samples, uint32_t
             s->sum_counts = ctx->h_counters[CNT_SUM_COUNTS];
             s->sum_counts_valid = true;
         }
-        out[i] = {s->mean_read_length, s->c, s->sum_counts};
+        views[i] = {s->hash, s->count, s->n};
+        metas[i] = {s->mean_read_length, s->c, s->sum_counts};
     }
     return SYL_OK;
 }
@@ -1198,7 +1205,7 @@ static int enqueue_stats(syl_profile_job *j, const StatParams &P, bool pass2, vo
 
 // stage 1: allocate, pass 1 (P1 = the pass-1 parameters: profile skips the bootstrap there).  csr: the CSR formulation
 // (single GPU only); otherwise histograms beyond 8 GB are SYL_ERR_UNSUPPORTED.
-static int job_begin(syl_ctx *ctx, const syl_db *db, const syl_sample *const *samples, uint32_t n_samples,
+static int job_begin(syl_ctx *ctx, const syl_db *db, const SampleView *views, const SampleMeta *metas, uint32_t n_samples,
                      const syl_contain_params *p, bool profile, bool csr, uint32_t world, uint32_t rank, uint64_t R,
                      syl_profile_job **out) {
     cudaStream_t st = ctx->stream;
@@ -1210,18 +1217,15 @@ static int job_begin(syl_ctx *ctx, const syl_db *db, const syl_sample *const *sa
     pp.pseudotax = profile ? 1 : 0;
     j->P = make_params(&pp);
     j->redundant_ani = pp.redundant_ani;
-    if (p->estimate_unknown) { j->read_seq_id = p->read_seq_id; SYL_TRY(sample_metas(ctx, samples, n_samples, j->metas)); }
+    if (p->estimate_unknown) { j->read_seq_id = p->read_seq_id; j->metas.assign(metas, metas + n_samples); }
     j->R = R ? ((R + 255) & ~255ull) : default_rows_per_rank(n_samples, db->n_genomes, world);
     j->tbytes = table_bytes(j->R);
     if (j->R * BOOT_ITERS >= 0xFFFF0000ull) { set_error("row capacity too large for the bootstrap work counter"); return SYL_ERR_ARG; }
     const uint64_t NP = (uint64_t)j->S * j->G;
     if (NP >= 0x7FFFFFFFull) { set_error("samples x genomes exceeds 2^31 pairs per call; split the sample batch"); return SYL_ERR_ARG; }
     if (!csr && !histograms_fit(NP)) { set_error("pair histograms exceed 8 GB; split the sample batch"); return SYL_ERR_UNSUPPORTED; }
-    std::vector<SampleView> hv(n_samples);
-    for (uint32_t i = 0; i < n_samples; i++) {
-        hv[i] = {samples[i]->hash, samples[i]->count, samples[i]->n};
-        j->max_n = std::max<uint64_t>(j->max_n, samples[i]->n);
-    }
+    std::vector<SampleView> hv(views, views + n_samples);
+    for (const SampleView &v : hv) j->max_n = std::max<uint64_t>(j->max_n, v.n);
     const uint64_t HN = std::max<uint64_t>((uint64_t)j->S * j->max_n, 1);
     SYL_TRY(j->views.alloc(n_samples, st));
     if (csr) {
@@ -1445,13 +1449,16 @@ static int job_finish(syl_profile_job *j, std::vector<syl_ani_row> &out, uint64_
 // single-GPU driver of the stages for syl_query / syl_profile.  The CSR formulation is taken up front when
 // SYL_CONTAIN_CSR is set (read per call) or the per-pair histograms would exceed 8 GB, and after a histogram
 // run that met a count >= COV_BINS; a row table that is too small is redone with the size it needed.
-static int contain_fast(syl_ctx *ctx, const syl_db *db, const syl_sample *const *samples, uint32_t n_samples,
-                        const syl_contain_params *p, bool profile, std::vector<syl_ani_row> &out) {
+// `overlap`, when given, runs once, after the first attempt's stages are enqueued and before its result is awaited (the
+// host samples stage their next batch there).
+static int contain_fast(syl_ctx *ctx, const syl_db *db, const SampleView *views, const SampleMeta *metas, uint32_t n_samples,
+                        const syl_contain_params *p, bool profile, std::vector<syl_ani_row> &out,
+                        const std::function<int()> &overlap = {}) {
     uint64_t R = 0;
     bool csr = getenv("SYL_CONTAIN_CSR") != nullptr || !histograms_fit((uint64_t)n_samples * db->n_genomes);
     for (int attempt = 0; attempt < 4; attempt++) {  // one formulation switch + capacity retries
         syl_profile_job *j = nullptr;
-        SYL_TRY(job_begin(ctx, db, samples, n_samples, p, profile, csr, 1, 0, R, &j));
+        SYL_TRY(job_begin(ctx, db, views, metas, n_samples, p, profile, csr, 1, 0, R, &j));
         int rc = SYL_OK;
         if (profile) {
             rc = job_rank(j);
@@ -1459,6 +1466,7 @@ static int contain_fast(syl_ctx *ctx, const syl_db *db, const syl_sample *const 
         } else {
             rc = job_bootstrap(j, j->tab1.p);
         }
+        if (rc == SYL_OK && attempt == 0 && overlap) rc = overlap();
         uint64_t need = 0;
         if (rc == SYL_OK) rc = job_finish(j, out, &need);
         syl_profile_job_free(j);
@@ -1469,23 +1477,21 @@ static int contain_fast(syl_ctx *ctx, const syl_db *db, const syl_sample *const 
     return SYL_ERR_CAPACITY;
 }
 
-// The arguments of a query or profile call against a database of k-mer size k and sketch parameter c that has_tracked
-// k-mers or not; *n_rows is 0 once they are not NULL.
-static int check_contain_args(syl_ctx *ctx, int k, uint64_t c, bool has_tracked, bool profile, const syl_sample *const *samples,
-                              uint32_t n_samples, const syl_contain_params *p, syl_ani_row *rows, uint64_t cap, uint64_t *n_rows) {
-    if (!ctx || !p || !n_rows || (n_samples && !samples) || (cap && !rows)) { set_error("NULL argument"); return SYL_ERR_ARG; }
-    *n_rows = 0;
-    for (uint32_t i = 0; i < n_samples; i++) {
-        if (!samples[i]) { set_error("NULL sample"); return SYL_ERR_ARG; }
-        if (samples[i]->k != k) {  // src/contain.rs:608-615 (log::error + exit(1))
-            set_error("k parameter for reads != k parameter for genome");
-            return SYL_ERR_ARG;
-        }
-        if (c < samples[i]->c) {   // src/contain.rs:616-623
-            set_error("c parameter for reads > c parameter for genome");
-            return SYL_ERR_ARG;
-        }
+// k and c of one sample against a database of k-mer size k and sketch parameter c
+static int check_sample_kc(int k, uint64_t c, int sk, uint64_t sc) {
+    if (sk != k) {  // src/contain.rs:608-615 (log::error + exit(1))
+        set_error("k parameter for reads != k parameter for genome");
+        return SYL_ERR_ARG;
     }
+    if (c < sc) {   // src/contain.rs:616-623
+        set_error("c parameter for reads > c parameter for genome");
+        return SYL_ERR_ARG;
+    }
+    return SYL_OK;
+}
+
+// The parameters of a query or profile call against a database of k-mer size k that has_tracked k-mers or not
+static int check_params(int k, bool has_tracked, bool profile, const syl_contain_params *p) {
     if (p->k != k) { set_error("params.k != db k"); return SYL_ERR_ARG; }
     if (p->estimate_unknown && !(p->read_seq_id > 0.)) {
         set_error("-u without --read-seq-id: the automatic read-identity estimate depends on hash-map iteration order (src/contain.rs:901-951)");
@@ -1496,6 +1502,19 @@ static int check_contain_args(syl_ctx *ctx, int k, uint64_t c, bool has_tracked,
         return SYL_ERR_ARG;
     }
     return SYL_OK;
+}
+
+// The arguments of a query or profile call against a database of k-mer size k and sketch parameter c that has_tracked
+// k-mers or not; *n_rows is 0 once they are not NULL.
+static int check_contain_args(syl_ctx *ctx, int k, uint64_t c, bool has_tracked, bool profile, const syl_sample *const *samples,
+                              uint32_t n_samples, const syl_contain_params *p, syl_ani_row *rows, uint64_t cap, uint64_t *n_rows) {
+    if (!ctx || !p || !n_rows || (n_samples && !samples) || (cap && !rows)) { set_error("NULL argument"); return SYL_ERR_ARG; }
+    *n_rows = 0;
+    for (uint32_t i = 0; i < n_samples; i++) {
+        if (!samples[i]) { set_error("NULL sample"); return SYL_ERR_ARG; }
+        SYL_TRY(check_sample_kc(k, c, samples[i]->k, samples[i]->c));
+    }
+    return check_params(k, has_tracked, profile, p);
 }
 
 // the rows of a call into the caller's buffer of cap rows; *n_rows is their number even when they do not fit
@@ -1821,7 +1840,7 @@ struct syl_db_shards {
         uint64_t call = 0;        // 0: nothing kept
         bool profile = false;
         syl_contain_params p{};
-        std::vector<const syl_sample *> samples;
+        std::vector<const void *> key;  // the samples of the call (handle pointers, or host arrays and their count)
         std::vector<syl_ani_row> rows;
     } kept;
     uint64_t *pinned = nullptr;   // staging of the survivor k-mers (grow-only)
@@ -1868,12 +1887,195 @@ static int shard_build(const syl_db_shards *s, uint64_t a, uint64_t b, syl_db **
     return db_build(s->ctx, in, s->gn_size ? s->gn_size + a : nullptr, s->tracked_off ? 1 : 0, s->k, s->c, (uint32_t)a, out);
 }
 
-// Pass 1 (syl_query) of samples[0, S) against every shard in turn: each shard's index is built once, joined with all
-// samples in batches of at most PAIRS_PER_CALL pairs, and freed before the next one is built.  rows: by shard, then by
-// (sample, genome); row.genome is the global index.
-static int shards_sweep(syl_db_shards *s, const syl_sample *const *samples, uint32_t S, const syl_contain_params *p,
-                        std::vector<syl_ani_row> &rows) {
+// ---- the samples of a call, batch by batch --------------------------------------------------------
+
+// The samples of a call as the joins take them, in batches of samples [first[b], first[b + 1]): device handles (views
+// into their own arrays) or host arrays staged batch by batch into device slots (HostSamples).
+struct SampleSource {
+    std::vector<SampleMeta> metas;  // per sample
+    virtual ~SampleSource() = default;
+    // the batches of a join against an index of G genomes
+    virtual void batches(uint64_t G, std::vector<uint32_t> &first) const = 0;
+    // the most samples x genomes of a survivor join from sample s0 on, and whether such a batch must end before sample i
+    virtual uint64_t survivor_pairs(uint32_t) const { return PAIRS_PER_CALL; }
+    virtual bool cut_before(uint32_t) const { return false; }
+    // views of samples [s0, s1), inside one batch, ready for work enqueued on the ctx stream from now on
+    virtual int views(uint32_t s0, uint32_t s1, std::vector<SampleView> &v) = 0;
+    // stage samples [s0, s1) ahead of their views() (host samples), while the last views are joined
+    virtual int prefetch(uint32_t, uint32_t) { return SYL_OK; }
+    // the joins of the last views() are enqueued on the ctx stream
+    virtual void done() {}
+};
+
+// Device handles: batches of at most PAIRS_PER_CALL pairs.
+struct HandleSamples : SampleSource {
+    std::vector<SampleView> all;
+    void batches(uint64_t G, std::vector<uint32_t> &first) const override {
+        const uint32_t S = (uint32_t)all.size();
+        const uint32_t per = (uint32_t)std::max<uint64_t>(1, std::min<uint64_t>(S, PAIRS_PER_CALL / std::max<uint64_t>(G, 1)));
+        first.clear();
+        for (uint32_t s0 = 0; s0 < S; s0 += per) first.push_back(s0);
+        first.push_back(S);
+    }
+    int views(uint32_t s0, uint32_t s1, std::vector<SampleView> &v) override {
+        v.assign(all.begin() + s0, all.begin() + s1);
+        return SYL_OK;
+    }
+};
+
+// Device bytes of one result row in the joins: two row tables, the bootstrap's results and its histogram
+constexpr uint64_t ROW_BYTES = 2 * sizeof(syl_ani_row) + BOOT_ITERS * 17 + 17 * 4 + 8;
+
+// Host samples (syl_host_samples), staged on the device batch by batch (sample_batches.hpp).  Two slots each hold one
+// batch (hash, count and rebased offsets), filled on the ingest copy stream and sorted there by hash within each sample
+// (one segmented sort per batch, into the slot or the shared second buffer, whichever it ends in), while the ctx stream
+// joins the other slot.  Events order the two streams; the host waits only where the joins already do.
+struct HostSamples : SampleSource {
+    syl_ctx *ctx;
+    const syl_host_samples *in;
+    bool pinned_hash = false, pinned_count = false;
+    std::vector<uint32_t> plan;  // batch b: samples [plan[b], plan[b + 1])
+    uint64_t plan_G = 0;
+    struct Slot {
+        DevBuf<uint64_t> hash, off;
+        DevBuf<uint32_t> count;
+        std::vector<uint64_t> h_off;  // the slot's offsets, rebased to its first sample
+        uint32_t s0 = 0, s1 = 0;
+        bool full = false;
+        cudaEvent_t staged = nullptr, used = nullptr;
+    } slot[2];
+    DevBuf<uint64_t> alt_hash;
+    DevBuf<uint32_t> alt_count;
+    DevBuf<uint8_t> tmp;
+    cudaStream_t cs = nullptr;
+    int cur = -1;  // slot of the last views()
+
+    HostSamples(syl_ctx *c, const syl_host_samples *s) : ctx(c), in(s) {}
+    ~HostSamples() override {
+        if (cs) cudaStreamSynchronize(cs);  // the slots go back to the ctx cache, whose users run on the ctx stream
+        for (Slot &sl : slot)
+            for (cudaEvent_t e : {sl.staged, sl.used})
+                if (e) cudaEventDestroy(e);
+    }
+    void batches(uint64_t, std::vector<uint32_t> &first) const override { first = plan; }
+    uint32_t batch_of(uint32_t i) const { return (uint32_t)(std::upper_bound(plan.begin(), plan.end(), i) - plan.begin() - 1); }
+    uint64_t survivor_pairs(uint32_t s0) const override {
+        const uint32_t b = batch_of(s0);
+        return std::min<uint64_t>(PAIRS_PER_CALL, std::max<uint64_t>(plan_G, 1) * (plan[b + 1] - plan[b]));
+    }
+    bool cut_before(uint32_t i) const override { return std::binary_search(plan.begin(), plan.end(), i); }
+    int find(uint32_t s0, uint32_t s1) const {
+        for (int k = 0; k < 2; k++)
+            if (slot[k].full && slot[k].s0 <= s0 && s1 <= slot[k].s1) return k;
+        return -1;
+    }
+    // slots and sort storage for the largest batch of the plan; the copy stream starts behind the ctx stream's work so far
+    int init() {
+        uint64_t kmers = 0, S = 0;
+        size_t tb = 0;
+        for (size_t b = 0; b + 1 < plan.size(); b++) {
+            const uint64_t n = in->off[plan[b + 1]] - in->off[plan[b]], m = plan[b + 1] - plan[b];
+            kmers = std::max(kmers, n);
+            S = std::max(S, m);
+            cub::DoubleBuffer<uint64_t> dk(nullptr, nullptr);
+            cub::DoubleBuffer<uint32_t> dv(nullptr, nullptr);
+            size_t t = 0;
+            SYL_CUDA(cub::DeviceSegmentedSort::SortPairs(nullptr, t, dk, dv, (int)n, (int)m, (const uint64_t *)nullptr,
+                                                         (const uint64_t *)nullptr, ctx->stream));
+            tb = std::max(tb, t);
+        }
+        SYL_TRY(ingest_copy_stream(ctx, &cs));
+        cudaStream_t st = ctx->stream;
+        for (Slot &sl : slot) {
+            SYL_TRY(sl.hash.alloc(kmers, st)); SYL_TRY(sl.count.alloc(kmers, st)); SYL_TRY(sl.off.alloc(S + 1, st));
+            SYL_CUDA(cudaEventCreateWithFlags(&sl.staged, cudaEventDisableTiming));
+            SYL_CUDA(cudaEventCreateWithFlags(&sl.used, cudaEventDisableTiming));
+        }
+        SYL_TRY(alt_hash.alloc(kmers, st)); SYL_TRY(alt_count.alloc(kmers, st)); SYL_TRY(tmp.alloc(tb, st));
+        SYL_CUDA(cudaEventRecord(slot[0].used, st));  // cached blocks may still be in use by earlier work on the ctx stream
+        SYL_CUDA(cudaStreamWaitEvent(cs, slot[0].used, 0));
+        return SYL_OK;
+    }
+    // samples [s0, s1) into slot k, once the joins of its last batch are done
+    int stage(int k, uint32_t s0, uint32_t s1) {
+        if (!cs) SYL_TRY(init());
+        Slot &sl = slot[k];
+        SYL_CUDA(cudaStreamWaitEvent(cs, sl.used, 0));
+        const uint64_t a = in->off[s0], n = in->off[s1] - a;
+        sl.h_off.resize(s1 - s0 + 1);
+        for (uint32_t i = s0; i <= s1; i++) sl.h_off[i - s0] = in->off[i] - a;
+        SYL_TRY(ingest_copy(ctx, sl.off.p, sl.h_off.data(), sl.h_off.size() * 8, false));
+        SYL_TRY(ingest_copy(ctx, sl.hash.p, in->hash + a, n * 8, pinned_hash));
+        SYL_TRY(ingest_copy(ctx, sl.count.p, in->count + a, n * 4, pinned_count));
+        if (n) {
+            cub::DoubleBuffer<uint64_t> dk(sl.hash.p, alt_hash.p);
+            cub::DoubleBuffer<uint32_t> dv(sl.count.p, alt_count.p);
+            size_t tb = tmp.cap_bytes;
+            SYL_CUDA(cub::DeviceSegmentedSort::SortPairs(tmp.p, tb, dk, dv, (int)n, (int)(s1 - s0), sl.off.p, sl.off.p + 1, cs));
+            ctx->launches += 4;
+            if (dk.selector) sl.hash.swap(alt_hash);
+            if (dv.selector) sl.count.swap(alt_count);
+        }
+        SYL_CUDA(cudaEventRecord(sl.staged, cs));
+        sl.s0 = s0;
+        sl.s1 = s1;
+        sl.full = true;
+        return SYL_OK;
+    }
+    int prefetch(uint32_t s0, uint32_t s1) override {
+        if (find(s0, s1) >= 0) return SYL_OK;
+        return stage(cur < 0 ? 0 : 1 - cur, s0, s1);
+    }
+    int views(uint32_t s0, uint32_t s1, std::vector<SampleView> &v) override {
+        int k = find(s0, s1);
+        if (k < 0) {
+            k = cur < 0 ? 0 : 1 - cur;
+            SYL_TRY(stage(k, s0, s1));
+        }
+        const Slot &sl = slot[k];
+        SYL_CUDA(cudaStreamWaitEvent(ctx->stream, sl.staged, 0));
+        v.resize(s1 - s0);
+        for (uint32_t i = s0; i < s1; i++) {
+            const uint64_t o = sl.h_off[i - sl.s0];
+            v[i - s0] = {sl.hash.p + o, sl.count.p + o, sl.h_off[i + 1 - sl.s0] - o};
+        }
+        cur = k;
+        return SYL_OK;
+    }
+    void done() override {
+        if (cur >= 0) cudaEventRecord(slot[cur].used, ctx->stream);
+    }
+};
+
+// Every sample of `src` against db, in the batches of `first`: the next batch is staged while one is joined, and `then`
+// (samples [then[0], then[1]), if given) while the last one is.  Rows appended with the call's sample indices.
+static int join_batches(syl_ctx *ctx, const syl_db *db, SampleSource &src, const std::vector<uint32_t> &first,
+                        const uint32_t *then, const syl_contain_params *p, bool profile, std::vector<syl_ani_row> &rows) {
+    std::vector<SampleView> v;
+    for (size_t b = 0; b + 1 < first.size(); b++) {
+        const uint32_t s0 = first[b], s1 = first[b + 1];
+        SYL_TRY(src.views(s0, s1, v));
+        std::function<int()> next;
+        if (b + 2 < first.size()) next = [&] { return src.prefetch(s1, first[b + 2]); };
+        else if (then) next = [&] { return src.prefetch(then[0], then[1]); };
+        std::vector<syl_ani_row> part;
+        const int rc = contain_fast(ctx, db, v.data(), src.metas.data() + s0, s1 - s0, p, profile, part, next);
+        src.done();
+        SYL_TRY(rc);
+        for (syl_ani_row &r : part) {
+            r.sample += s0;
+            rows.push_back(r);
+        }
+    }
+    return SYL_OK;
+}
+
+// Pass 1 (syl_query) of every sample of src against every shard in turn: each shard's index is built once, joined with
+// all samples batch by batch, and freed before the next one is built.  rows: by shard, then by (sample, genome);
+// row.genome is the global index.
+static int shards_sweep(syl_db_shards *s, SampleSource &src, const syl_contain_params *p, std::vector<syl_ani_row> &rows) {
     syl_ctx *ctx = s->ctx;
+    std::vector<uint32_t> first, next;
     for (size_t i = 0; i + 1 < s->first.size(); i++) {
         const uint64_t a = s->first[i], G = s->first[i + 1] - a;
         // each shard's index and join scratch are allocated to that shard's size, not next to the previous shard's
@@ -1883,16 +2085,10 @@ static int shards_sweep(syl_db_shards *s, const syl_sample *const *samples, uint
         SYL_TRY(shard_build(s, a, s->first[i + 1], &db));
         const double build_ms = ms_since(t0);
         const auto t1 = std::chrono::steady_clock::now();
-        const uint32_t per = (uint32_t)std::max<uint64_t>(1, std::min<uint64_t>(S, PAIRS_PER_CALL / std::max<uint64_t>(G, 1)));
-        int rc = SYL_OK;
-        for (uint32_t s0 = 0; s0 < S && rc == SYL_OK; s0 += per) {
-            std::vector<syl_ani_row> part;
-            rc = contain_fast(ctx, db, samples + s0, std::min(per, S - s0), p, false, part);
-            for (syl_ani_row &r : part) {
-                r.sample += s0;
-                rows.push_back(r);
-            }
-        }
+        src.batches(G, first);
+        next.clear();
+        if (i + 2 < s->first.size()) src.batches(s->first[i + 2] - s->first[i + 1], next);
+        const int rc = join_batches(ctx, db, src, first, next.size() > 1 ? next.data() : nullptr, p, false, rows);
         static const bool dbg = getenv("SYL_DEBUG_TIMING") != nullptr;
         if (dbg)
             fprintf(stderr, "[db shard %zu/%zu] genomes %llu+%llu entries %llu: build %.1f ms, pass 1 %.1f ms\n", i + 1,
@@ -1903,11 +2099,14 @@ static int shards_sweep(syl_db_shards *s, const syl_sample *const *samples, uint
     return cache_trim(ctx);
 }
 
-// syl_profile of samples[s0, s1) on an index of the genomes `ids` (ascending global indices), gathered from the
+// syl_profile of samples[s0, s1) of src on an index of the genomes `ids` (ascending global indices), gathered from the
 // borrowed arrays into pinned staging; rows appended with global sample and genome indices.
-static int survivor_profile(syl_db_shards *s, const std::vector<uint32_t> &ids, const syl_sample *const *samples,
-                            uint32_t s0, uint32_t s1, const syl_contain_params *p, std::vector<syl_ani_row> &out) {
+static int survivor_profile(syl_db_shards *s, const std::vector<uint32_t> &ids, SampleSource &src, uint32_t s0, uint32_t s1,
+                            const syl_contain_params *p, std::vector<syl_ani_row> &out) {
     const auto t0 = std::chrono::steady_clock::now();
+    // host samples are staged on the copy stream while the index is gathered and built; the ctx stream waits for them
+    // only before the joins (views() below)
+    SYL_TRY(src.prefetch(s0, s1));
     const uint64_t n = ids.size();
     std::vector<uint64_t> ko(n + 1, 0), to(n + 1, 0), gsz(n, 0);
     for (uint64_t i = 0; i < n; i++) {
@@ -1934,8 +2133,11 @@ static int survivor_profile(syl_db_shards *s, const std::vector<uint32_t> &ids, 
                                 s->c, 0, &db));
     const double build_ms = ms_since(t0);
     const auto t1 = std::chrono::steady_clock::now();
+    std::vector<SampleView> v;
     std::vector<syl_ani_row> part;
-    const int rc = contain_fast(s->ctx, db, samples + s0, s1 - s0, p, true, part);
+    int rc = src.views(s0, s1, v);
+    if (rc == SYL_OK) rc = contain_fast(s->ctx, db, v.data(), src.metas.data() + s0, s1 - s0, p, true, part);
+    src.done();
     syl_db_free(db);
     SYL_TRY(rc);
     static const bool dbg = getenv("SYL_DEBUG_TIMING") != nullptr;
@@ -1954,9 +2156,10 @@ static int survivor_profile(syl_db_shards *s, const std::vector<uint32_t> &ids, 
 // abundances only ever see pass-1 survivors (src/contain.rs:284-334, 410-430).  So pass 1 runs per shard, without CIs
 // (never reported; the ANI gate comes before the bootstrap), and each batch of samples is profiled on an index of the
 // union of its survivors.  Ascending global order keeps the winner table's lowest-index tie rule.  A batch closes when
-// the union would pass the shard cap; one sample's survivors alone may take up to survivor_max entries.
-static int shards_profile(syl_db_shards *s, const syl_sample *const *samples, uint32_t S, const syl_contain_params *p,
-                          std::vector<syl_ani_row> &out) {
+// the union would pass the shard cap (or the source's pair or batch limits); one sample's survivors alone may take up
+// to survivor_max entries.
+static int shards_profile(syl_db_shards *s, SampleSource &src, const syl_contain_params *p, std::vector<syl_ani_row> &out) {
+    const uint32_t S = (uint32_t)src.metas.size();
     syl_contain_params p1 = *p;
     p1.no_ci = 1;
     p1.estimate_unknown = 0;
@@ -1965,7 +2168,7 @@ static int shards_profile(syl_db_shards *s, const syl_sample *const *samples, ui
     std::vector<std::vector<uint32_t>> surv(S);
     {
         std::vector<syl_ani_row> rows1;
-        SYL_TRY(shards_sweep(s, samples, S, &p1, rows1));
+        SYL_TRY(shards_sweep(s, src, &p1, rows1));
         for (const syl_ani_row &r : rows1) surv[r.sample].push_back(r.genome);
     }
     std::vector<uint8_t> in(s->G, 0);
@@ -1975,7 +2178,7 @@ static int shards_profile(syl_db_shards *s, const syl_sample *const *samples, ui
     auto flush = [&](uint32_t s1) -> int {
         if (!ids.empty()) {
             std::sort(ids.begin(), ids.end());
-            SYL_TRY(survivor_profile(s, ids, samples, s0, s1, p, out));
+            SYL_TRY(survivor_profile(s, ids, src, s0, s1, p, out));
             SYL_TRY(cache_trim(s->ctx));
         }
         for (uint32_t g : ids) in[g] = 0;
@@ -1997,7 +2200,8 @@ static int shards_profile(syl_db_shards *s, const syl_sample *const *samples, ui
             return SYL_ERR_UNSUPPORTED;
         }
         const uint64_t ng = ids.size() + addg;
-        if (i > s0 && (entries + add > s->cap || ng > SHARD_MAX_GENOMES || (uint64_t)(i - s0 + 1) * ng > PAIRS_PER_CALL)) {
+        if (i > s0 && (entries + add > s->cap || ng > SHARD_MAX_GENOMES || (uint64_t)(i - s0 + 1) * ng > src.survivor_pairs(s0) ||
+                       src.cut_before(i))) {
             SYL_TRY(flush(i));
             add = own;
         }
@@ -2008,27 +2212,23 @@ static int shards_profile(syl_db_shards *s, const syl_sample *const *samples, ui
     return flush(S);
 }
 
-// syl_query_shards / syl_profile_shards
-static int shards_call(syl_ctx *ctx, syl_db_shards *s, const syl_sample *const *samples, uint32_t n_samples,
-                       const syl_contain_params *p, bool profile, syl_ani_row *rows, uint64_t cap, uint64_t *n_rows) {
-    if (!s) { set_error("NULL argument"); return SYL_ERR_ARG; }
-    SYL_TRY(check_contain_args(ctx, s->k, s->c, s->tracked_off != nullptr, profile, samples, n_samples, p, rows, cap, n_rows));
-    if (ctx != s->ctx) { set_error("db shards used with another ctx than the one that created them"); return SYL_ERR_ARG; }
-    SYL_ENTER(ctx);
+// syl_query_shards / syl_profile_shards / syl_*_host_samples with shards, after the argument checks.  key: the samples
+// of the call, as the rows of a SYL_ERR_CAPACITY call are kept under.
+static int shards_call(syl_db_shards *s, SampleSource &src, const std::vector<const void *> &key, const syl_contain_params *p,
+                       bool profile, syl_ani_row *rows, uint64_t cap, uint64_t *n_rows) {
     const uint64_t call = ++s->calls;
     auto &kp = s->kept;
-    const bool retry = kp.call && kp.call + 1 == call && kp.profile == profile && !memcmp(&kp.p, p, sizeof *p) &&
-                       kp.samples == std::vector<const syl_sample *>(samples, samples + n_samples);
+    const bool retry = kp.call && kp.call + 1 == call && kp.profile == profile && !memcmp(&kp.p, p, sizeof *p) && kp.key == key;
     std::vector<syl_ani_row> out;
     if (retry) out.swap(kp.rows);
     kp.call = 0;
     std::vector<syl_ani_row>().swap(kp.rows);
-    kp.samples.clear();
-    if (!retry && s->G && n_samples) {
+    kp.key.clear();
+    if (!retry && s->G && !src.metas.empty()) {
         if (profile) {
-            SYL_TRY(shards_profile(s, samples, n_samples, p, out));
+            SYL_TRY(shards_profile(s, src, p, out));
         } else {
-            SYL_TRY(shards_sweep(s, samples, n_samples, p, out));
+            SYL_TRY(shards_sweep(s, src, p, out));
             std::sort(out.begin(), out.end(), [](const syl_ani_row &a, const syl_ani_row &b) {
                 return a.sample != b.sample ? a.sample < b.sample : a.genome < b.genome;
             });
@@ -2039,10 +2239,104 @@ static int shards_call(syl_ctx *ctx, syl_db_shards *s, const syl_sample *const *
         kp.call = call;
         kp.profile = profile;
         kp.p = *p;
-        kp.samples.assign(samples, samples + n_samples);
+        kp.key = key;
         kp.rows.swap(out);
     }
     return rc;
+}
+
+static int handle_shards_call(syl_ctx *ctx, syl_db_shards *s, const syl_sample *const *samples, uint32_t n_samples,
+                              const syl_contain_params *p, bool profile, syl_ani_row *rows, uint64_t cap, uint64_t *n_rows) {
+    if (!s) { set_error("NULL argument"); return SYL_ERR_ARG; }
+    SYL_TRY(check_contain_args(ctx, s->k, s->c, s->tracked_off != nullptr, profile, samples, n_samples, p, rows, cap, n_rows));
+    if (ctx != s->ctx) { set_error("db shards used with another ctx than the one that created them"); return SYL_ERR_ARG; }
+    SYL_ENTER(ctx);
+    HandleSamples src;
+    SYL_TRY(handle_views(ctx, samples, n_samples, p->estimate_unknown != 0, src.all, src.metas));
+    return shards_call(s, src, std::vector<const void *>(samples, samples + n_samples), p, profile, rows, cap, n_rows);
+}
+
+// syl_query_host_samples / syl_profile_host_samples
+static int host_samples_call(syl_ctx *ctx, const syl_db *db, syl_db_shards *sh, const syl_host_samples *s,
+                             const syl_contain_params *p, bool profile, syl_ani_row *rows, uint64_t cap, uint64_t *n_rows) {
+    if (!ctx || !s || !p || !n_rows || (cap && !rows)) { set_error("NULL argument"); return SYL_ERR_ARG; }
+    if ((db != nullptr) == (sh != nullptr)) { set_error("exactly one of db and shards must be given"); return SYL_ERR_ARG; }
+    *n_rows = 0;
+    const uint32_t S = s->n_samples;
+    if (!s->off || (S && (!s->c || !s->mean_read_length))) { set_error("NULL argument"); return SYL_ERR_ARG; }
+    if (s->off[0] != 0) { set_error(BAD_OFFSETS); return SYL_ERR_ARG; }
+    for (uint32_t i = 0; i < S; i++)
+        if (s->off[i + 1] < s->off[i]) { set_error(BAD_OFFSETS); return SYL_ERR_ARG; }
+    if (s->off[S] && (!s->hash || !s->count)) { set_error("off counts k-mers but hash or count is NULL"); return SYL_ERR_ARG; }
+    const int k = db ? db->k : sh->k;
+    const uint64_t c = db ? db->c : sh->c;
+    for (uint32_t i = 0; i < S; i++) SYL_TRY(check_sample_kc(k, c, s->k, s->c[i]));
+    SYL_TRY(check_params(k, db ? db->has_tracked != 0 : sh->tracked_off != nullptr, profile, p));
+    if (sh && ctx != sh->ctx) { set_error("db shards used with another ctx than the one that created them"); return SYL_ERR_ARG; }
+    SYL_ENTER(ctx);
+    HostSamples src(ctx, s);
+    for (int a = 0; a < 2 && s->off[S]; a++) {  // pinned arrays are copied as they are, pageable ones through the ring
+        cudaPointerAttributes at{};
+        const void *ptr = a ? (const void *)s->count : (const void *)s->hash;
+        bool pinned = false;
+        if (cudaPointerGetAttributes(&at, ptr) == cudaSuccess) {
+            if (at.type == cudaMemoryTypeDevice || at.type == cudaMemoryTypeManaged) { set_error("host samples: a device pointer was given"); return SYL_ERR_ARG; }
+            pinned = at.type == cudaMemoryTypeHost;
+        } else {
+            cudaGetLastError();
+        }
+        (a ? src.pinned_count : src.pinned_hash) = pinned;
+    }
+    // the plan: the device budget of syl_ctx_set_sample_memory (0: free memory once the ctx's staging ring exists, plus
+    // the ctx's cached free blocks), less the largest shard's build (16 bytes per entry)
+    cudaStream_t cs = nullptr;
+    SYL_TRY(ingest_copy_stream(ctx, &cs));
+    uint64_t budget = ctx->sample_budget, index = 0;
+    if (!budget) {
+        size_t free_b = 0, total_b = 0;
+        SYL_CUDA(cudaMemGetInfo(&free_b, &total_b));
+        budget = free_b;
+        for (const auto &b : ctx->free_blocks) budget += b.second;
+    }
+    if (sh) {
+        for (size_t i = 0; i + 1 < sh->first.size(); i++) {
+            const uint64_t a = sh->first[i], b = sh->first[i + 1];
+            src.plan_G = std::max(src.plan_G, b - a);
+            index = std::max(index, 16 * (sh->kmer_off[b] - sh->kmer_off[a] + (sh->tracked_off ? sh->tracked_off[b] - sh->tracked_off[a] : 0)));
+        }
+    } else {
+        src.plan_G = db->n_genomes;
+    }
+    uint32_t forced = 0;
+    if (const char *e = getenv("SYL_SAMPLE_BATCH")) forced = (uint32_t)std::max(0, atoi(e));
+    const BatchCost cost{36, 4 * 8 + sizeof(SampleView) + 96 * ROW_BYTES, 16, COV_BINS * 4 + 16, 256 * ROW_BYTES + (1u << 20)};
+    uint32_t bad = 0;
+    uint64_t need = 0;
+    const BatchPlanResult pr = plan_sample_batches(s->off, S, src.plan_G, budget > index ? budget - index : 0, PAIRS_PER_CALL,
+                                                   0x7FFFFFFFull, forced, cost, src.plan, &bad, &need);
+    if (pr == BATCH_TOO_MANY_KMERS) {
+        set_error("sample " + std::to_string(bad) + " holds " + std::to_string(need) + " k-mers, more than 2^31 - 1");
+        return SYL_ERR_UNSUPPORTED;
+    }
+    if (pr == BATCH_OOM) {
+        set_error("sample " + std::to_string(bad) + " needs " + std::to_string(need + index) + " bytes of device memory" +
+                  (index ? " (with the largest shard's build)" : "") + ", the budget is " + std::to_string(budget) + " bytes");
+        return SYL_ERR_OOM;
+    }
+    src.metas.resize(S);
+    for (uint32_t i = 0; i < S; i++) {
+        uint64_t sum = 0;
+        if (p->estimate_unknown)
+            for (uint64_t j = s->off[i]; j < s->off[i + 1]; j++) sum += s->count[j];
+        src.metas[i] = {s->mean_read_length[i], s->c[i], sum};
+    }
+    if (sh) {
+        const std::vector<const void *> key{s->hash, s->count, s->off, s->c, s->mean_read_length, (const void *)(uintptr_t)S};
+        return shards_call(sh, src, key, p, profile, rows, cap, n_rows);
+    }
+    std::vector<syl_ani_row> out;
+    if (db->n_genomes && S) SYL_TRY(join_batches(ctx, db, src, src.plan, nullptr, p, profile, out));
+    return copy_rows(out, rows, cap, n_rows);
 }
 
 }  // namespace syl
@@ -2149,8 +2443,11 @@ int syl_query(syl_ctx *ctx, const syl_db *db, const syl_sample *const *samples, 
     SYL_TRY(check_contain_args(ctx, db->k, db->c, db->has_tracked, false, samples, n_samples, p, rows, cap, n_rows));
     SYL_ENTER(ctx);
     if (db->n_genomes == 0 || n_samples == 0) return SYL_OK;
+    std::vector<SampleView> views;
+    std::vector<SampleMeta> metas;
+    SYL_TRY(handle_views(ctx, samples, n_samples, p->estimate_unknown != 0, views, metas));
     std::vector<syl_ani_row> out;
-    SYL_TRY(contain_fast(ctx, db, samples, n_samples, p, false, out));
+    SYL_TRY(contain_fast(ctx, db, views.data(), metas.data(), n_samples, p, false, out));
     return copy_rows(out, rows, cap, n_rows);
 }
 
@@ -2163,7 +2460,10 @@ int syl_profile_shard_begin(syl_ctx *ctx, const syl_db *db, const syl_sample *co
     if (world == 0 || rank >= world || n_samples == 0) { set_error("bad world / rank / sample count"); return SYL_ERR_ARG; }
     SYL_TRY(check_contain_args(ctx, db->k, db->c, db->has_tracked, true, samples, n_samples, p, nullptr, 0, &dummy));
     SYL_ENTER(ctx);
-    return job_begin(ctx, db, samples, n_samples, p, true, false, world, rank, rows_per_rank, out);
+    std::vector<SampleView> views;
+    std::vector<SampleMeta> metas;
+    SYL_TRY(handle_views(ctx, samples, n_samples, p->estimate_unknown != 0, views, metas));
+    return job_begin(ctx, db, views.data(), metas.data(), n_samples, p, true, false, world, rank, rows_per_rank, out);
 }
 
 int syl_profile_job_buffers(const syl_profile_job *j, void **d_table1, void **d_gathered1, uint64_t *table_bytes,
@@ -2212,8 +2512,11 @@ int syl_profile(syl_ctx *ctx, const syl_db *db, const syl_sample *const *samples
     SYL_TRY(check_contain_args(ctx, db->k, db->c, db->has_tracked, true, samples, n_samples, p, rows, cap, n_rows));
     SYL_ENTER(ctx);
     if (db->n_genomes == 0 || n_samples == 0) return SYL_OK;
+    std::vector<SampleView> views;
+    std::vector<SampleMeta> metas;
+    SYL_TRY(handle_views(ctx, samples, n_samples, p->estimate_unknown != 0, views, metas));
     std::vector<syl_ani_row> out;
-    SYL_TRY(contain_fast(ctx, db, samples, n_samples, p, true, out));
+    SYL_TRY(contain_fast(ctx, db, views.data(), metas.data(), n_samples, p, true, out));
     return copy_rows(out, rows, cap, n_rows);
 }
 
@@ -2272,12 +2575,22 @@ int syl_db_shards_range(const syl_db_shards *s, uint64_t i, uint64_t *first_geno
 
 int syl_query_shards(syl_ctx *ctx, syl_db_shards *s, const syl_sample *const *samples, uint32_t n_samples,
                      const syl_contain_params *p, syl_ani_row *rows, uint64_t cap, uint64_t *n_rows) {
-    return shards_call(ctx, s, samples, n_samples, p, false, rows, cap, n_rows);
+    return handle_shards_call(ctx, s, samples, n_samples, p, false, rows, cap, n_rows);
 }
 
 int syl_profile_shards(syl_ctx *ctx, syl_db_shards *s, const syl_sample *const *samples, uint32_t n_samples,
                        const syl_contain_params *p, syl_ani_row *rows, uint64_t cap, uint64_t *n_rows) {
-    return shards_call(ctx, s, samples, n_samples, p, true, rows, cap, n_rows);
+    return handle_shards_call(ctx, s, samples, n_samples, p, true, rows, cap, n_rows);
+}
+
+int syl_query_host_samples(syl_ctx *ctx, const syl_db *db, syl_db_shards *shards, const syl_host_samples *s,
+                           const syl_contain_params *p, syl_ani_row *rows, uint64_t cap, uint64_t *n_rows) {
+    return host_samples_call(ctx, db, shards, s, p, false, rows, cap, n_rows);
+}
+
+int syl_profile_host_samples(syl_ctx *ctx, const syl_db *db, syl_db_shards *shards, const syl_host_samples *s,
+                             const syl_contain_params *p, syl_ani_row *rows, uint64_t cap, uint64_t *n_rows) {
+    return host_samples_call(ctx, db, shards, s, p, true, rows, cap, n_rows);
 }
 
 void syl_db_shards_free(syl_db_shards *s) {

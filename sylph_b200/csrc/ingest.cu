@@ -1,6 +1,7 @@
 // ingest.cu — the host-memory feeder of ingest.hpp: packer pool, copy stream, pinned ring of packed chunks, two-slot
 // device ring of chunks shipped as they are, and the one-off buffer of a chunk larger than a ring slot.
 #include <cstdlib>
+#include <cstring>
 #include <memory>
 #include <string>
 #include <vector>
@@ -83,6 +84,7 @@ struct HostIngest {
     uint64_t cap_asc = 0, cap_aoff = 0;
     cudaEvent_t ev_a_copied[2] = {}, ev_a_used[2] = {};
     int a_slot = 0, a_last = -1;  // next ASCII slot; slot of the latest ASCII copy (-1: none yet)
+    int r_slot = 0;               // next packed-ring slot of ingest_copy's pageable pieces
 
     int init() {
         if (copy_stream) return SYL_OK;
@@ -367,6 +369,35 @@ int feed_host(syl_ctx *ctx, const Mate *m, int n_mates, const std::vector<Chunk>
                      (unsigned long long)ctx->ingest_chunks_ascii, chunks.size() - (size_t)ctx->ingest_chunks_ascii, I.pool->threads());
     if (rc != SYL_OK) I.drain(st);
     return rc;
+}
+
+int ingest_copy_stream(syl_ctx *ctx, cudaStream_t *cs) {
+    if (!ctx->ingest) ctx->ingest = new HostIngest();
+    HostIngest &I = *static_cast<HostIngest *>(ctx->ingest);
+    SYL_TRY(I.init());
+    SYL_TRY(I.ensure_packed(ctx->stream, {}, 1));
+    *cs = I.copy_stream;
+    return SYL_OK;
+}
+
+int ingest_copy(syl_ctx *ctx, void *dst, const void *src, uint64_t bytes, bool pinned) {
+    HostIngest &I = *static_cast<HostIngest *>(ctx->ingest);
+    ctx->ingest_h2d_bytes += bytes;
+    if (pinned) {
+        if (bytes) SYL_CUDA(cudaMemcpyAsync(dst, src, bytes, cudaMemcpyHostToDevice, I.copy_stream));
+        return SYL_OK;
+    }
+    const uint64_t piece = I.cap_words * 4;
+    for (uint64_t o = 0; o < bytes; o += piece) {
+        const int slot = I.r_slot;
+        I.r_slot = (I.r_slot + 1) % ING_SLOTS;
+        const uint64_t n = std::min(piece, bytes - o);
+        SYL_CUDA(cudaEventSynchronize(I.ev_copied[slot]));  // the slot's previous piece has crossed the link
+        memcpy(I.h_words[slot], static_cast<const uint8_t *>(src) + o, n);
+        SYL_CUDA(cudaMemcpyAsync(static_cast<uint8_t *>(dst) + o, I.h_words[slot], n, cudaMemcpyHostToDevice, I.copy_stream));
+        SYL_CUDA(cudaEventRecord(I.ev_copied[slot], I.copy_stream));
+    }
+    return SYL_OK;
 }
 
 uint64_t ring_bytes_after(const syl_ctx *ctx, const std::vector<Chunk> &chunks, int n_mates, bool ascii_only) {

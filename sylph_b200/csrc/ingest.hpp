@@ -64,4 +64,10 @@ int feed_host(syl_ctx *ctx, const Mate *m, int n_mates, const std::vector<Chunk>
 // kept until the ctx is destroyed; the ASCII ring of chunks taken from the back is counted whether or not it is used).
 uint64_t ring_bytes_after(const syl_ctx *ctx, const std::vector<Chunk> &chunks, int n_mates, bool ascii_only);
 
+// Whole host arrays to the device on the ctx's copy stream (host samples): *cs is that stream.  ingest_copy copies
+// `bytes` from src to dst on it, straight from pinned memory, from pageable memory through the pinned ring in slot-sized
+// pieces (a pageable cudaMemcpyAsync would wait for the copy stream and block the calling thread).
+int ingest_copy_stream(syl_ctx *ctx, cudaStream_t *cs);
+int ingest_copy(syl_ctx *ctx, void *dst, const void *src, uint64_t bytes, bool pinned);
+
 }  // namespace syl
