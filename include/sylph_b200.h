@@ -462,9 +462,12 @@ void syl_db_shards_free(syl_db_shards *s);
  * its joins' scratch (about 1 KB per pair, 16 bytes per k-mer of its largest sample per sample, 200 KB per sample);
  * with shards the budget also covers the largest shard's build (16 bytes per entry).  The default budget is the free
  * memory once the ctx's staging ring exists, plus the ctx's cached free blocks.  A sample that does not fit alone
- * is SYL_ERR_OOM before anything is allocated, with the bytes it needs in the message.  Each batch crosses the link in
- * one pass on the ctx's host-ingest copy stream (pageable arrays through its pinned ring) and is sorted there by one
- * segmented sort, while the previous batch is joined on the ctx stream.  With shards, each shard is built once per
+ * is SYL_ERR_OOM before anything is allocated, with the bytes it needs in the message.  The joins' allocations the plan
+ * does not charge (the CSR formulation's 4 bytes per hit, the row tables of samples with more than 96 rows) are held to
+ * the budget on top of what the ctx held in use when the call began: a batch whose joins would pass it is rerun as two
+ * halves, recursively, with the same rows, and a sample that does not fit alone is SYL_ERR_OOM, naming its bytes.
+ * Each batch crosses the link in one pass on the ctx's host-ingest copy stream (pageable arrays through its pinned
+ * ring) and is sorted there by one segmented sort, while the previous batch is joined on the ctx stream.  With shards, each shard is built once per
  * call: every batch is joined with it before the next one is built (profile: then its survivor indexes, each joined
  * with samples of one batch, staged again unless a slot still holds them, while the index is gathered and built).
  * SYL_SAMPLE_BATCH=N (test hook, read per call) caps a batch at N samples.

@@ -1046,6 +1046,31 @@ __global__ void k_join2_order(const SampleView *__restrict__ views, uint64_t G, 
 namespace syl {
 // what -u needs to know about a sample (src/contain.rs:377-408)
 struct SampleMeta { double mean_read_length; uint64_t c, sum_counts; };
+
+// Device bytes of one result row in the joins: two row tables, the bootstrap's results and its histogram
+constexpr uint64_t ROW_BYTES = 2 * sizeof(syl_ani_row) + BOOT_ITERS * 17 + 17 * 4 + 8;
+
+// What the joins of a host-sample batch may allocate beyond its plan (sample_batches.hpp charges neither): the CSR
+// formulation's hit values (4 bytes per hit) and the row tables of a capacity retry.  The ctx's held plus transient
+// device bytes stay within `limit` (0: unbounded, the handle path); a job that would pass it gives up with
+// SPLIT_BATCH and contain_fast reruns its samples as two halves.  `want` is the refused allocation, `s0` the call's
+// index of the job's first sample and `budget` the call's budget, for the error of a sample that does not fit alone.
+struct JoinRoom {
+    uint64_t limit = 0, budget = 0, want = 0;
+    uint32_t s0 = 0;
+};
+constexpr int SPLIT_BATCH = -1;  // internal status, never returned through the C ABI
+
+// SYL_OK when `bytes` more keep the ctx within room->limit (its cached free blocks are handed back first if they are
+// what stands in the way; that waits for the ctx stream), else SPLIT_BATCH
+static int take_room(syl_ctx *ctx, JoinRoom *room, uint64_t bytes) {
+    if (!room || !room->limit) return SYL_OK;
+    auto held = [ctx] { return (uint64_t)(ctx->cached_bytes + ctx->transient_bytes); };
+    if (held() + bytes > room->limit && !ctx->free_blocks.empty()) SYL_TRY(cache_trim(ctx));
+    if (held() + bytes <= room->limit) return SYL_OK;
+    room->want = bytes;
+    return SPLIT_BATCH;
+}
 }
 
 // One in-flight device-driven query / profile (C ABI: syl_profile_job).
@@ -1061,6 +1086,7 @@ struct syl_profile_job {
     uint64_t G = 0, R = 0, max_n = 0, tbytes = 0;
     int stage = 0;           // 1 pass 1 enqueued, 2 ranked, 3 pass 2 enqueued
     bool csr = false;        // CSR formulation (single GPU) instead of the per-pair count histograms
+    syl::JoinRoom *room = nullptr;  // bound on the CSR hit values (host-sample batches only)
     syl::DevBuf<syl::SampleView> views;
     syl::DevBuf<uint8_t> touched, tab1, gat1, tab2, gat2, res_ok, scan_tmp;
     syl::DevBuf<uint32_t> chist, lost, order, contain1, wbest, boot_rows, hist, reject, range_bounds;
@@ -1174,7 +1200,9 @@ static int csr_walks(syl_profile_job *j, bool pass2) {
     if (!pass2) {
         SYL_CUDA(cudaMemcpyAsync(ctx->h_counters + CNT_COVS_TOTAL, j->off.p + NP, 8, cudaMemcpyDeviceToHost, st));
         SYL_CUDA(cudaStreamSynchronize(st));
-        SYL_TRY(j->covs.alloc(std::max<uint64_t>(ctx->h_counters[CNT_COVS_TOTAL], 1), st));
+        const uint64_t total = std::max<uint64_t>(ctx->h_counters[CNT_COVS_TOTAL], 1);
+        SYL_TRY(take_room(ctx, j->room, (total * 4 + 255) & ~255ull));
+        SYL_TRY(j->covs.alloc(total, st));
     }
     join_walk<JOIN_CSR_FILL>(j, pass2);
     SYL_CUDA(cudaGetLastError());
@@ -1207,12 +1235,13 @@ static int enqueue_stats(syl_profile_job *j, const StatParams &P, bool pass2, vo
 // (single GPU only); otherwise histograms beyond 8 GB are SYL_ERR_UNSUPPORTED.
 static int job_begin(syl_ctx *ctx, const syl_db *db, const SampleView *views, const SampleMeta *metas, uint32_t n_samples,
                      const syl_contain_params *p, bool profile, bool csr, uint32_t world, uint32_t rank, uint64_t R,
-                     syl_profile_job **out) {
+                     syl_profile_job **out, JoinRoom *room = nullptr) {
     cudaStream_t st = ctx->stream;
     Handle<syl_profile_job> h(new (std::nothrow) syl_profile_job());
     if (!h) return SYL_ERR_OOM;
     syl_profile_job *j = h.get();
     j->ctx = ctx; j->db = db; j->profile = profile; j->csr = csr; j->S = n_samples; j->G = db->n_genomes; j->world = world; j->rank = rank;
+    j->room = room;
     syl_contain_params pp = *p;
     pp.pseudotax = profile ? 1 : 0;
     j->P = make_params(&pp);
@@ -1450,29 +1479,61 @@ static int job_finish(syl_profile_job *j, std::vector<syl_ani_row> &out, uint64_
 // SYL_CONTAIN_CSR is set (read per call) or the per-pair histograms would exceed 8 GB, and after a histogram
 // run that met a count >= COV_BINS; a row table that is too small is redone with the size it needed.
 // `overlap`, when given, runs once, after the first attempt's stages are enqueued and before its result is awaited (the
-// host samples stage their next batch there).
+// host samples stage their next batch there).  `room` (host-sample batches) bounds what the joins allocate beyond the
+// batch's plan: CSR hit values or a capacity retry's row tables that do not fit it rerun the samples as two halves on
+// the same views, recursively, and a single sample that does not fit is SYL_ERR_OOM.
 static int contain_fast(syl_ctx *ctx, const syl_db *db, const SampleView *views, const SampleMeta *metas, uint32_t n_samples,
                         const syl_contain_params *p, bool profile, std::vector<syl_ani_row> &out,
-                        const std::function<int()> &overlap = {}) {
+                        const std::function<int()> &overlap = {}, JoinRoom *room = nullptr) {
     uint64_t R = 0;
     bool csr = getenv("SYL_CONTAIN_CSR") != nullptr || !histograms_fit((uint64_t)n_samples * db->n_genomes);
+    bool overlapped = false;
     for (int attempt = 0; attempt < 4; attempt++) {  // one formulation switch + capacity retries
         syl_profile_job *j = nullptr;
-        SYL_TRY(job_begin(ctx, db, views, metas, n_samples, p, profile, csr, 1, 0, R, &j));
-        int rc = SYL_OK;
-        if (profile) {
-            rc = job_rank(j);
-            if (rc == SYL_OK) rc = job_pass2(j);
-        } else {
-            rc = job_bootstrap(j, j->tab1.p);
+        int rc = job_begin(ctx, db, views, metas, n_samples, p, profile, csr, 1, 0, R, &j, room);
+        if (rc == SYL_OK) {
+            if (profile) {
+                rc = job_rank(j);
+                if (rc == SYL_OK) rc = job_pass2(j);
+            } else {
+                rc = job_bootstrap(j, j->tab1.p);
+            }
+            if (rc == SYL_OK && !overlapped && overlap) { overlapped = true; rc = overlap(); }
+            uint64_t need = 0;
+            if (rc == SYL_OK) rc = job_finish(j, out, &need);
+            if (rc == SYL_ERR_CAPACITY) {
+                R = need + 256;
+                // the retry reuses this job's blocks and adds row tables for R rows (a few KB for rounding)
+                const int room_rc = take_room(ctx, room, ((R + 255) & ~255ull) * ROW_BYTES + 4096);
+                if (room_rc != SYL_OK) rc = room_rc;
+            }
+            syl_profile_job_free(j);
         }
-        if (rc == SYL_OK && attempt == 0 && overlap) rc = overlap();
-        uint64_t need = 0;
-        if (rc == SYL_OK) rc = job_finish(j, out, &need);
-        syl_profile_job_free(j);
-        if (rc == SYL_ERR_CAPACITY) { R = need + 256; out.clear(); continue; }
+        if (rc == SYL_ERR_CAPACITY) { out.clear(); continue; }
         if (rc == SYL_ERR_UNSUPPORTED && !csr) { csr = true; out.clear(); continue; }  // a count >= COV_BINS
-        return rc;
+        if (rc != SPLIT_BATCH) return rc;
+        out.clear();
+        if (n_samples == 1) {
+            set_error("sample " + std::to_string(room->s0) + " needs " + std::to_string(room->want) +
+                      " more bytes of device memory for its joins, the budget is " + std::to_string(room->budget) + " bytes");
+            return SYL_ERR_OOM;
+        }
+        SYL_TRY(cache_trim(ctx));  // the halves allocate to their own sizes, not next to this job's cached blocks
+        const uint32_t h = n_samples / 2;
+        static const bool dbg = getenv("SYL_DEBUG_TIMING") != nullptr;
+        if (dbg)
+            fprintf(stderr, "[join split] samples %u..%u: %llu bytes do not fit, halves of %u and %u samples\n", room->s0,
+                    room->s0 + n_samples, (unsigned long long)room->want, h, n_samples - h);
+        JoinRoom r0 = *room, r1 = *room;
+        r1.s0 += h;
+        std::vector<syl_ani_row> second;
+        SYL_TRY(contain_fast(ctx, db, views, metas, h, p, profile, out, overlapped ? std::function<int()>() : overlap, &r0));
+        SYL_TRY(contain_fast(ctx, db, views + h, metas + h, n_samples - h, p, profile, second, {}, &r1));
+        for (syl_ani_row &r : second) {
+            r.sample += h;
+            out.push_back(r);
+        }
+        return SYL_OK;
     }
     return SYL_ERR_CAPACITY;
 }
@@ -1893,6 +1954,7 @@ static int shard_build(const syl_db_shards *s, uint64_t a, uint64_t b, syl_db **
 // into their own arrays) or host arrays staged batch by batch into device slots (HostSamples).
 struct SampleSource {
     std::vector<SampleMeta> metas;  // per sample
+    JoinRoom room;                  // what the joins of a batch may take beyond its plan (handles: unbounded)
     virtual ~SampleSource() = default;
     // the batches of a join against an index of G genomes
     virtual void batches(uint64_t G, std::vector<uint32_t> &first) const = 0;
@@ -1922,9 +1984,6 @@ struct HandleSamples : SampleSource {
         return SYL_OK;
     }
 };
-
-// Device bytes of one result row in the joins: two row tables, the bootstrap's results and its histogram
-constexpr uint64_t ROW_BYTES = 2 * sizeof(syl_ani_row) + BOOT_ITERS * 17 + 17 * 4 + 8;
 
 // Host samples (syl_host_samples), staged on the device batch by batch (sample_batches.hpp).  Two slots each hold one
 // batch (hash, count and rebased offsets), filled on the ingest copy stream and sorted there by hash within each sample
@@ -2059,7 +2118,9 @@ static int join_batches(syl_ctx *ctx, const syl_db *db, SampleSource &src, const
         if (b + 2 < first.size()) next = [&] { return src.prefetch(s1, first[b + 2]); };
         else if (then) next = [&] { return src.prefetch(then[0], then[1]); };
         std::vector<syl_ani_row> part;
-        const int rc = contain_fast(ctx, db, v.data(), src.metas.data() + s0, s1 - s0, p, profile, part, next);
+        JoinRoom room = src.room;
+        room.s0 = s0;
+        const int rc = contain_fast(ctx, db, v.data(), src.metas.data() + s0, s1 - s0, p, profile, part, next, &room);
         src.done();
         SYL_TRY(rc);
         for (syl_ani_row &r : part) {
@@ -2135,8 +2196,10 @@ static int survivor_profile(syl_db_shards *s, const std::vector<uint32_t> &ids, 
     const auto t1 = std::chrono::steady_clock::now();
     std::vector<SampleView> v;
     std::vector<syl_ani_row> part;
+    JoinRoom room = src.room;
+    room.s0 = s0;
     int rc = src.views(s0, s1, v);
-    if (rc == SYL_OK) rc = contain_fast(s->ctx, db, v.data(), src.metas.data() + s0, s1 - s0, p, true, part);
+    if (rc == SYL_OK) rc = contain_fast(s->ctx, db, v.data(), src.metas.data() + s0, s1 - s0, p, true, part, {}, &room);
     src.done();
     syl_db_free(db);
     SYL_TRY(rc);
@@ -2298,6 +2361,11 @@ static int host_samples_call(syl_ctx *ctx, const syl_db *db, syl_db_shards *sh, 
         budget = free_b;
         for (const auto &b : ctx->free_blocks) budget += b.second;
     }
+    // the joins' allocations beyond the plan are held to the budget on top of the bytes the ctx holds in use now
+    uint64_t live = ctx->cached_bytes + ctx->transient_bytes;
+    for (const auto &b : ctx->free_blocks) live -= b.second;
+    src.room.limit = live + budget;
+    src.room.budget = budget;
     if (sh) {
         for (size_t i = 0; i + 1 < sh->first.size(); i++) {
             const uint64_t a = sh->first[i], b = sh->first[i + 1];
