@@ -16,7 +16,7 @@ OBJ = os.path.join(HERE, "build")
 SO = os.path.join(HERE, "libsylph_b200.so")
 HEADER = os.path.join(HERE, "..", "include", "sylph_b200.h")
 SOURCES = ["api.cu", "seed.cu", "seed_k31_sv.cu", "seed_k31_ev.cu", "seed_k21_sv.cu", "seed_k21_ev.cu", "ingest.cu",
-           "sample.cu", "genome.cu", "contain.cu", "host_pack.cpp"]
+           "sample.cu", "genome.cu", "db_index.cu", "contain.cu", "contain_calls.cu", "host_pack.cpp"]
 CXX_FLAGS = ["-O3", "-std=c++17", "-fPIC", "-pthread"]
 NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",

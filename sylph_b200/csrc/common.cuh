@@ -6,7 +6,9 @@
 #include <algorithm>
 #include <stdint.h>
 #include <stdio.h>
+#include <stdlib.h>
 
+#include <chrono>
 #include <memory>
 #include <new>
 #include <string>
@@ -44,6 +46,41 @@ void set_error(const std::string &msg);
         SYL_CUDA(cudaSetDevice(ctx->device));                                                    \
         ::syl::tl_ctx = ctx;                                                                     \
     } while (0)
+
+// ---- small host helpers -----------------------------------------------------------------------
+inline unsigned nblk(uint64_t n, int bs) { return (unsigned)((n + bs - 1) / bs); }
+
+// bits that hold every value up to maxval (at least 1)
+inline int bits_for(uint64_t maxval) {
+    int b = 1;
+    while (b < 64 && (maxval >> b)) b++;
+    return b;
+}
+
+// SYL_DEBUG_TIMING set: the host paths print where their time went (read once per process)
+inline bool debug_timing() {
+    static const bool on = getenv("SYL_DEBUG_TIMING") != nullptr;
+    return on;
+}
+inline double ms_since(std::chrono::steady_clock::time_point t) {
+    return std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t).count();
+}
+
+// What a caller's pointer points into.  Memory CUDA does not know (the query fails; its error is cleared) is pageable.
+enum class PtrKind { PAGEABLE, PINNED, DEVICE, MANAGED };
+inline PtrKind ptr_kind(const void *p) {
+    cudaPointerAttributes at{};
+    if (cudaPointerGetAttributes(&at, p) != cudaSuccess) {
+        cudaGetLastError();
+        return PtrKind::PAGEABLE;
+    }
+    switch (at.type) {
+        case cudaMemoryTypeHost: return PtrKind::PINNED;
+        case cudaMemoryTypeDevice: return PtrKind::DEVICE;
+        case cudaMemoryTypeManaged: return PtrKind::MANAGED;
+        default: return PtrKind::PAGEABLE;
+    }
+}
 
 // ---- context --------------------------------------------------------------------------------
 }  // namespace syl
@@ -176,7 +213,7 @@ static_assert(CNT_DUPS == CNT_EVENTS + 2 && CNT_PEND_MATE1 == CNT_EVENTS + 3 && 
               "slots cleared or copied as one range");
 
 // Owner of a half-built handle: frees it with the handle's free function unless release()d.  A half-built index is
-// freed once the ctx stream has drained (contain.cu).
+// freed once the ctx stream has drained (db_index.cu).
 struct HandleFree {
     void operator()(syl_sample *s) const { syl_sample_free(s); }
     void operator()(syl_genomes *g) const { syl_genomes_free(g); }

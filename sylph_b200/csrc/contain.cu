@@ -28,41 +28,16 @@
 #include <cub/cub.cuh>
 
 #include <algorithm>
-#include <chrono>
 #include <cmath>
 #include <cstdio>
-#include <cstring>
 #include <functional>
 #include <new>
 #include <vector>
 
-#include "common.cuh"
+#include "contain.hpp"
 #include "crmath.cuh"
-#include "ingest.hpp"
-#include "sample_batches.hpp"
-#include "shard_cut.hpp"
-
-struct syl_db {
-    int device = 0;
-    syl_ctx *owner = nullptr;       // arrays are blocks of this ctx's cache
-    cudaStream_t stream = nullptr;
-    uint64_t n_genomes = 0;
-    uint32_t genome_base = 0;
-    uint64_t N = 0;             // index entries (genome_kmers + tracked)
-    uint64_t *keys = nullptr;   // sorted ascending
-    uint32_t *gid = nullptr;    // (genome << 1) | is_tracked
-    uint32_t *bstart = nullptr; // NB + 1 bucket starts
-    uint64_t NB = 0, M = 0, maxkey = 0;
-    uint32_t *glen = nullptr;   // |genome_kmers| per genome (device)
-    std::vector<uint64_t> h_gn_size;
-    int has_tracked = 0;
-    int k = 31;
-    uint64_t c = 200;
-};
 
 namespace syl {
-
-static inline unsigned nblk(uint64_t n, int bs) { return (unsigned)((n + bs - 1) / bs); }
 
 // src/contain.rs:664-675 with src/constants.rs:3: largest cov with PoissonCDF(cov; m) < 0.9999999999
 // for integer medians m = 1..29 (statrs 0.16.1 cdf = Q(cov+1, m)); index 0 unused.
@@ -83,179 +58,6 @@ struct StatExtra {
     const uint32_t *contain1_in = nullptr;  // [S x G], pass 2 -> row.reserved
     const uint64_t *gn_size = nullptr;      // [G], pass 2 -> row.seq_abund
     uint64_t pair_stride = 0;               // G
-};
-
-// ---- index build ----------------------------------------------------------------------------
-//
-// The index is every entry (key, gid = genome << 1 | tracked) of the db in (key, tracked, genome) order: the order of a
-// stable sort of all genomes' k-mers in genome order followed by all tracked k-mers in genome order (entries equal in
-// key and gid cannot be told apart).  It is built without a global sort: a max pass fixes the bucket directory
-// (bucket_of below), a histogram pass counts each bucket, a scatter pass writes every entry into its bucket's segment
-// of the final arrays, and each bucket is then sorted on its own.  Every pass reads the input as CSR chunks
-// (DbChunk): a device source is one chunk, a host source is cut into chunks that are copied while the previous
-// chunk's kernels run, so the build needs device memory for the index and two staging chunks, not for a sort.
-
-__global__ void k_glen(const uint64_t *__restrict__ kmer_off, uint64_t n_genomes, uint32_t *__restrict__ glen) {
-    uint64_t g = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (g < n_genomes) glen[g] = (uint32_t)(kmer_off[g + 1] - kmer_off[g]);
-}
-
-__device__ __forceinline__ uint64_t bucket_of(uint64_t key, uint64_t M, uint64_t NB) {
-    uint64_t b = __umul64hi(key, M);
-    return b < NB ? b : NB - 1;
-}
-
-// One chunk of the build's input: up to two segments, each a run of entries of one part (0 = genome k-mers,
-// 1 = tracked k-mers).  Segment s holds keys[s][0 .. n[s]) of part part[s], its part-local entries p0[s] .. p0[s] + n[s];
-// off[s] is the slice of that part's offsets of genomes g0[s] .. g0[s] + n_off[s] - 1 (values part-local, as given).
-struct DbChunk {
-    const uint64_t *keys[2];
-    const uint64_t *off[2];
-    uint64_t n_off[2], g0[2], p0[2], n[2];
-    uint32_t part[2];
-};
-
-// (key, tracked, genome) order of an entry inside its key: the gid rotated so that the tracked bit leads (genome < 2^31 - 1)
-__device__ __forceinline__ uint32_t gid_rank(uint32_t gid) { return (gid >> 1) | (gid << 31); }
-__device__ __forceinline__ uint32_t rank_gid(uint32_t r) { return (r << 1) | (r >> 31); }
-__device__ __forceinline__ bool entry_less(uint64_t ka, uint32_t ra, uint64_t kb, uint32_t rb) {
-    return ka < kb || (ka == kb && ra < rb);
-}
-
-__device__ __forceinline__ uint64_t chunk_key(const DbChunk &c, uint64_t i) {
-    return i < c.n[0] ? c.keys[0][i] : c.keys[1][i - c.n[0]];
-}
-
-__global__ void __launch_bounds__(256) k_db_max(DbChunk c, unsigned long long *__restrict__ mx) {
-    uint64_t m = 0;
-    const uint64_t n = c.n[0] + c.n[1];
-    for (uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (uint64_t)gridDim.x * blockDim.x)
-        m = max(m, chunk_key(c, i));
-    for (int o = 16; o; o >>= 1) m = max(m, (uint64_t)__shfl_xor_sync(0xffffffffu, m, o));
-    if ((threadIdx.x & 31) == 0) atomicMax(mx, (unsigned long long)m);
-}
-
-// bucket b is counted in slot[b + 2]: the inclusive scan of the slots then leaves bucket b's start in slot[b + 1],
-// where k_db_scatter uses it as the bucket's cursor
-__global__ void __launch_bounds__(256) k_db_hist(DbChunk c, uint64_t M, uint64_t NB, uint32_t *__restrict__ slot) {
-    const uint64_t n = c.n[0] + c.n[1];
-    for (uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (uint64_t)gridDim.x * blockDim.x)
-        atomicAdd(slot + bucket_of(chunk_key(c, i), M, NB) + 2, 1u);
-}
-
-// every entry to the next free place of its bucket; afterwards slot[b + 1] has advanced to the start of bucket b + 1,
-// so slot[0 .. NB] is the bucket directory
-__global__ void __launch_bounds__(256) k_db_scatter(DbChunk c, uint64_t M, uint64_t NB, uint32_t *__restrict__ slot,
-                                                    uint64_t *__restrict__ keys, uint32_t *__restrict__ gid) {
-    const uint64_t n = c.n[0] + c.n[1];
-    for (uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (uint64_t)gridDim.x * blockDim.x) {
-        const bool s = i >= c.n[0];
-        const uint64_t j = s ? i - c.n[0] : i;
-        const uint64_t *off = s ? c.off[1] : c.off[0];
-        const uint64_t p = (s ? c.p0[1] : c.p0[0]) + j;
-        uint64_t lo = 0, hi = s ? c.n_off[1] : c.n_off[0];  // upper_bound(off, p) - 1 = the entry's genome in the slice
-        while (lo < hi) {
-            const uint64_t mid = (lo + hi) >> 1;
-            if (off[mid] > p) hi = mid; else lo = mid + 1;
-        }
-        const uint64_t genome = (s ? c.g0[1] : c.g0[0]) + lo - 1;
-        const uint64_t key = s ? c.keys[1][j] : c.keys[0][j];
-        const uint32_t at = atomicAdd(slot + bucket_of(key, M, NB) + 1, 1u);
-        keys[at] = key;
-        gid[at] = (uint32_t)(genome << 1) | (s ? c.part[1] : c.part[0]);
-    }
-}
-
-constexpr uint32_t DB_SMALL = 16;   // buckets up to this size are sorted by one thread
-constexpr uint32_t DB_MID = 2048;   // up to this size by one block in shared memory; larger ones one at a time (db_sort_large)
-constexpr uint32_t DB_SORT_TILE = 256;
-
-// Sorts every bucket of up to DB_MID entries in place by (key, tracked, genome) and lists the larger ones in large[]
-// as (start, size).  Block i looks at buckets DB_SORT_TILE * i ..: a thread per small bucket, then the block on each
-// middle-sized one (bitonic sort of the bucket padded to a power of two with entries above every real one).
-__global__ void __launch_bounds__(DB_SORT_TILE) k_db_sort_buckets(const uint32_t *__restrict__ bstart, uint64_t NB,
-                                                                  uint64_t *__restrict__ keys, uint32_t *__restrict__ gid,
-                                                                  uint2 *__restrict__ large, unsigned long long *__restrict__ n_large) {
-    __shared__ uint64_t sk[DB_MID];
-    __shared__ uint32_t sr[DB_MID];
-    __shared__ uint32_t mid_b[DB_SORT_TILE];
-    __shared__ uint32_t n_mid;
-    if (threadIdx.x == 0) n_mid = 0;
-    __syncthreads();
-    const uint64_t b = (uint64_t)blockIdx.x * DB_SORT_TILE + threadIdx.x;
-    if (b < NB) {
-        const uint32_t s = bstart[b], m = bstart[b + 1] - s;
-        if (m > DB_MID) {
-            large[atomicAdd(n_large, 1ull)] = make_uint2(s, m);
-        } else if (m > DB_SMALL) {
-            mid_b[atomicAdd(&n_mid, 1u)] = (uint32_t)(b - (uint64_t)blockIdx.x * DB_SORT_TILE);
-        } else if (m > 1) {
-            uint64_t k[DB_SMALL];
-            uint32_t r[DB_SMALL];
-            for (uint32_t i = 0; i < m; i++) {  // insertion sort
-                const uint64_t ki = keys[s + i];
-                const uint32_t ri = gid_rank(gid[s + i]);
-                uint32_t j = i;
-                for (; j > 0 && entry_less(ki, ri, k[j - 1], r[j - 1]); j--) { k[j] = k[j - 1]; r[j] = r[j - 1]; }
-                k[j] = ki;
-                r[j] = ri;
-            }
-            for (uint32_t i = 0; i < m; i++) { keys[s + i] = k[i]; gid[s + i] = rank_gid(r[i]); }
-        }
-    }
-    __syncthreads();
-    const uint32_t nm = n_mid;
-    for (uint32_t q = 0; q < nm; q++) {
-        const uint64_t bb = (uint64_t)blockIdx.x * DB_SORT_TILE + mid_b[q];
-        const uint32_t s = bstart[bb], m = bstart[bb + 1] - s;
-        uint32_t P = 32;
-        while (P < m) P <<= 1;
-        for (uint32_t i = threadIdx.x; i < P; i += DB_SORT_TILE) {
-            sk[i] = i < m ? keys[s + i] : ~0ull;
-            sr[i] = i < m ? gid_rank(gid[s + i]) : ~0u;  // real ranks are < 2^32 - 1
-        }
-        __syncthreads();
-        for (uint32_t kk = 2; kk <= P; kk <<= 1) {
-            for (uint32_t jj = kk >> 1; jj > 0; jj >>= 1) {
-                for (uint32_t i = threadIdx.x; i < P; i += DB_SORT_TILE) {
-                    const uint32_t x = i ^ jj;
-                    if (x > i) {
-                        const bool up = (i & kk) == 0;
-                        if (entry_less(sk[x], sr[x], sk[i], sr[i]) == up) {
-                            const uint64_t tk = sk[i]; sk[i] = sk[x]; sk[x] = tk;
-                            const uint32_t tr = sr[i]; sr[i] = sr[x]; sr[x] = tr;
-                        }
-                    }
-                }
-                __syncthreads();
-            }
-        }
-        for (uint32_t i = threadIdx.x; i < m; i += DB_SORT_TILE) { keys[s + i] = sk[i]; gid[s + i] = rank_gid(sr[i]); }
-        __syncthreads();
-    }
-}
-
-__global__ void k_gid_to_rank(const uint32_t *__restrict__ gid, uint32_t m, uint32_t *__restrict__ r) {
-    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i < m) r[i] = gid_rank(gid[i]);
-}
-
-__global__ void k_rank_to_gid(const uint32_t *__restrict__ r, uint32_t m, uint32_t *__restrict__ gid) {
-    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i < m) gid[i] = rank_gid(r[i]);
-}
-
-// SYL_ERR_ARG-worthy device offsets: off[0] != 0 or a decrease
-__global__ void k_check_offsets(const uint64_t *__restrict__ off, uint64_t n, unsigned long long *__restrict__ bad) {
-    const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (i < n && (i == 0 ? off[0] != 0 : off[i] < off[i - 1])) *bad = 1ull;
-}
-
-// ---- the join -------------------------------------------------------------------------------
-struct SampleView {
-    const uint64_t *hash;
-    const uint32_t *count;
-    uint64_t n;
 };
 
 // ---- per-genome statistics: one warp per genome ---------------------------------------------
@@ -453,7 +255,6 @@ k_stats(const uint32_t *__restrict__ cnt, const uint64_t *__restrict__ off, cons
 // k_stats that reads 1 KB per pair instead of selecting a median from a value list.  Values
 // >= COV_BINS (a genome covered 256x or deeper) are only counted in `ovf`; if there are any, the
 // call is redone in the CSR formulation.
-constexpr uint32_t COV_BINS = 256;
 
 // ---- thread -> (sample, key) mapping of the join kernels ---------------------------------------------------------
 // Plain form (rb == nullptr): grid (key blocks, samples), one key per thread.  With several samples that order walks
@@ -662,7 +463,6 @@ __device__ __forceinline__ uint64_t wyrand_at(uint64_t seed, uint64_t d) {
     return (s * t) ^ __umul64hi(s, t);
 }
 
-constexpr int BOOT_ITERS = 100;
 constexpr int BOOT_THREADS = 256;
 
 // 64 x 64 -> 128-bit product, xor of the two halves (WyRand's output function).  The 128-bit type
@@ -1041,26 +841,6 @@ __global__ void k_join2_order(const SampleView *__restrict__ views, uint64_t G, 
   });
 }
 
-}  // namespace syl
-
-namespace syl {
-// what -u needs to know about a sample (src/contain.rs:377-408)
-struct SampleMeta { double mean_read_length; uint64_t c, sum_counts; };
-
-// Device bytes of one result row in the joins: two row tables, the bootstrap's results and its histogram
-constexpr uint64_t ROW_BYTES = 2 * sizeof(syl_ani_row) + BOOT_ITERS * 17 + 17 * 4 + 8;
-
-// What the joins of a host-sample batch may allocate beyond its plan (sample_batches.hpp charges neither): the CSR
-// formulation's hit values (4 bytes per hit) and the row tables of a capacity retry.  The ctx's held plus transient
-// device bytes stay within `limit` (0: unbounded, the handle path); a job that would pass it gives up with
-// SPLIT_BATCH and contain_fast reruns its samples as two halves.  `want` is the refused allocation, `s0` the call's
-// index of the job's first sample and `budget` the call's budget, for the error of a sample that does not fit alone.
-struct JoinRoom {
-    uint64_t limit = 0, budget = 0, want = 0;
-    uint32_t s0 = 0;
-};
-constexpr int SPLIT_BATCH = -1;  // internal status, never returned through the C ABI
-
 // SYL_OK when `bytes` more keep the ctx within room->limit (its cached free blocks are handed back first if they are
 // what stands in the way; that waits for the ctx stream), else SPLIT_BATCH
 static int take_room(syl_ctx *ctx, JoinRoom *room, uint64_t bytes) {
@@ -1071,7 +851,8 @@ static int take_room(syl_ctx *ctx, JoinRoom *room, uint64_t bytes) {
     room->want = bytes;
     return SPLIT_BATCH;
 }
-}
+
+}  // namespace syl
 
 // One in-flight device-driven query / profile (C ABI: syl_profile_job).
 struct syl_profile_job {
@@ -1102,39 +883,6 @@ struct syl_profile_job {
 };
 
 namespace syl {
-
-__global__ void k_sum_counts(const uint32_t *__restrict__ count, uint64_t n, unsigned long long *__restrict__ out) {
-    unsigned long long acc = 0;
-    for (uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (uint64_t)gridDim.x * blockDim.x) acc += count[i];
-#pragma unroll
-    for (int d = 16; d >= 1; d >>= 1) acc += __shfl_xor_sync(0xffffffffu, acc, d);
-    if ((threadIdx.x & 31) == 0 && acc) atomicAdd(out, acc);
-}
-
-// Device handles as the views the joins take, and what -u needs to know of them (the sum of the counts is computed on the
-// device once per handle, and only for -u).
-static int handle_views(syl_ctx *ctx, const syl_sample *const *samples, uint32_t n, bool unknown, std::vector<SampleView> &views,
-                        std::vector<SampleMeta> &metas) {
-    cudaStream_t st = ctx->stream;
-    views.resize(n);
-    metas.resize(n);
-    for (uint32_t i = 0; i < n; i++) {
-        syl_sample *s = const_cast<syl_sample *>(samples[i]);
-        if (unknown && !s->sum_counts_valid) {
-            unsigned long long *d = reinterpret_cast<unsigned long long *>(ctx->d_counters + CNT_SUM_COUNTS);
-            SYL_CUDA(cudaMemsetAsync(d, 0, 8, st));
-            if (s->n) k_sum_counts<<<ctx->num_sms * 4, 256, 0, st>>>(s->count, s->n, d);
-            SYL_CUDA(cudaMemcpyAsync(ctx->h_counters + CNT_SUM_COUNTS, d, 8, cudaMemcpyDeviceToHost, st));
-            SYL_CUDA(cudaStreamSynchronize(st));
-            s->sum_counts = ctx->h_counters[CNT_SUM_COUNTS];
-            s->sum_counts_valid = true;
-        }
-        views[i] = {s->hash, s->count, s->n};
-        metas[i] = {s->mean_read_length, s->c, s->sum_counts};
-    }
-    return SYL_OK;
-}
-
 // estimate_true_cov (src/contain.rs:377-389) for the rows of one call (query: all rows; profile: the kept rows)
 static inline double unknown_multiplier(const SampleMeta &m, int k) { return m.mean_read_length / (m.mean_read_length - (double)k + 1.); }
 
@@ -1482,9 +1230,9 @@ static int job_finish(syl_profile_job *j, std::vector<syl_ani_row> &out, uint64_
 // host samples stage their next batch there).  `room` (host-sample batches) bounds what the joins allocate beyond the
 // batch's plan: CSR hit values or a capacity retry's row tables that do not fit it rerun the samples as two halves on
 // the same views, recursively, and a single sample that does not fit is SYL_ERR_OOM.
-static int contain_fast(syl_ctx *ctx, const syl_db *db, const SampleView *views, const SampleMeta *metas, uint32_t n_samples,
-                        const syl_contain_params *p, bool profile, std::vector<syl_ani_row> &out,
-                        const std::function<int()> &overlap = {}, JoinRoom *room = nullptr) {
+int contain_fast(syl_ctx *ctx, const syl_db *db, const SampleView *views, const SampleMeta *metas, uint32_t n_samples,
+                 const syl_contain_params *p, bool profile, std::vector<syl_ani_row> &out, const std::function<int()> &overlap,
+                 JoinRoom *room) {
     uint64_t R = 0;
     bool csr = getenv("SYL_CONTAIN_CSR") != nullptr || !histograms_fit((uint64_t)n_samples * db->n_genomes);
     bool overlapped = false;
@@ -1520,8 +1268,7 @@ static int contain_fast(syl_ctx *ctx, const syl_db *db, const SampleView *views,
         }
         SYL_TRY(cache_trim(ctx));  // the halves allocate to their own sizes, not next to this job's cached blocks
         const uint32_t h = n_samples / 2;
-        static const bool dbg = getenv("SYL_DEBUG_TIMING") != nullptr;
-        if (dbg)
+        if (debug_timing())
             fprintf(stderr, "[join split] samples %u..%u: %llu bytes do not fit, halves of %u and %u samples\n", room->s0,
                     room->s0 + n_samples, (unsigned long long)room->want, h, n_samples - h);
         JoinRoom r0 = *room, r1 = *room;
@@ -1538,957 +1285,11 @@ static int contain_fast(syl_ctx *ctx, const syl_db *db, const SampleView *views,
     return SYL_ERR_CAPACITY;
 }
 
-// k and c of one sample against a database of k-mer size k and sketch parameter c
-static int check_sample_kc(int k, uint64_t c, int sk, uint64_t sc) {
-    if (sk != k) {  // src/contain.rs:608-615 (log::error + exit(1))
-        set_error("k parameter for reads != k parameter for genome");
-        return SYL_ERR_ARG;
-    }
-    if (c < sc) {   // src/contain.rs:616-623
-        set_error("c parameter for reads > c parameter for genome");
-        return SYL_ERR_ARG;
-    }
-    return SYL_OK;
-}
-
-// The parameters of a query or profile call against a database of k-mer size k that has_tracked k-mers or not
-static int check_params(int k, bool has_tracked, bool profile, const syl_contain_params *p) {
-    if (p->k != k) { set_error("params.k != db k"); return SYL_ERR_ARG; }
-    if (p->estimate_unknown && !(p->read_seq_id > 0.)) {
-        set_error("-u without --read-seq-id: the automatic read-identity estimate depends on hash-map iteration order (src/contain.rs:901-951)");
-        return SYL_ERR_UNSUPPORTED;
-    }
-    if (profile && !has_tracked) {  // src/contain.rs:231-234
-        set_error("Attempting profiling, but the database was sketched with the --disable-profiling option");
-        return SYL_ERR_ARG;
-    }
-    return SYL_OK;
-}
-
-// The arguments of a query or profile call against a database of k-mer size k and sketch parameter c that has_tracked
-// k-mers or not; *n_rows is 0 once they are not NULL.
-static int check_contain_args(syl_ctx *ctx, int k, uint64_t c, bool has_tracked, bool profile, const syl_sample *const *samples,
-                              uint32_t n_samples, const syl_contain_params *p, syl_ani_row *rows, uint64_t cap, uint64_t *n_rows) {
-    if (!ctx || !p || !n_rows || (n_samples && !samples) || (cap && !rows)) { set_error("NULL argument"); return SYL_ERR_ARG; }
-    *n_rows = 0;
-    for (uint32_t i = 0; i < n_samples; i++) {
-        if (!samples[i]) { set_error("NULL sample"); return SYL_ERR_ARG; }
-        SYL_TRY(check_sample_kc(k, c, samples[i]->k, samples[i]->c));
-    }
-    return check_params(k, has_tracked, profile, p);
-}
-
-// the rows of a call into the caller's buffer of cap rows; *n_rows is their number even when they do not fit
-static int copy_rows(const std::vector<syl_ani_row> &out, syl_ani_row *rows, uint64_t cap, uint64_t *n_rows) {
-    *n_rows = out.size();
-    if (out.size() > cap) { set_error("row buffer too small"); return SYL_ERR_CAPACITY; }
-    std::copy(out.begin(), out.end(), rows);
-    return SYL_OK;
-}
-
-// ---- index build, host side -------------------------------------------------------------------
-
-// A large temporary of the index build: allocated outside the ctx's block cache (counted in its peak while it lives)
-// and returned to the driver once the ctx stream has drained, so the build leaves nothing but the index behind.
-struct BuildBuf {
-    syl_ctx *ctx;
-    void *p = nullptr;
-    size_t bytes = 0;
-    explicit BuildBuf(syl_ctx *c) : ctx(c) {}
-    BuildBuf(const BuildBuf &) = delete;
-    BuildBuf &operator=(const BuildBuf &) = delete;
-    ~BuildBuf() { release(); }
-    int alloc(size_t b) {
-        release();
-        b = (std::max<size_t>(b, 1) + 255) & ~(size_t)255;
-        cudaError_t e = cudaMalloc(&p, b);
-        if (e != cudaSuccess) {
-            p = nullptr;
-            set_error(std::string("cudaMalloc(") + std::to_string(b) + " B): " + cudaGetErrorString(e));
-            return e == cudaErrorMemoryAllocation ? SYL_ERR_OOM : SYL_ERR_CUDA;
-        }
-        bytes = b;
-        ctx->transient_bytes += b;
-        note_device_bytes(ctx);
-        return SYL_OK;
-    }
-    void release() {
-        if (!p) return;
-        cudaStreamSynchronize(ctx->stream);
-        cudaFree(p);
-        ctx->transient_bytes -= bytes;
-        p = nullptr;
-        bytes = 0;
-    }
-    template <typename T> T *as() const { return reinterpret_cast<T *>(p); }
-};
-
-// The build's input: part 0 = genome k-mers, part 1 = tracked k-mers, each CSR over the same G genomes
-// (off[part][0 .. G], validated: starts at 0, monotone).
-struct DbInput {
-    int mem;
-    const uint64_t *keys[2], *off[2];
-    uint64_t G, n[2];
-};
-
-static uint64_t db_chunk_entries() {  // SYL_DB_CHUNK overrides (tests; read per call)
-    if (const char *e = getenv("SYL_DB_CHUNK")) {
-        const long long v = atoll(e);
-        if (v >= 1) return (uint64_t)v;
-    }
-    return 1ull << 25;
-}
-
-// Hands the input to a pass chunk by chunk.  A device source is one chunk over the whole arrays.  A host source is
-// cut into chunks of at most C entries and, per segment, at most min(C, G) genome offsets; each chunk is copied on a
-// second stream into one of two staging buffers while the previous chunk's kernels run on the ctx stream.
-struct DbFeed {
-    syl_ctx *ctx;
-    const DbInput &in;
-    uint64_t C = 0, L = 0;
-    BuildBuf stage[2];
-    cudaStream_t cs = nullptr;
-    cudaEvent_t copied[2] = {}, done[2] = {};
-    DbFeed(syl_ctx *c, const DbInput &i) : ctx(c), in(i), stage{BuildBuf(c), BuildBuf(c)} {}
-    ~DbFeed() {
-        cudaStreamSynchronize(ctx->stream);
-        if (cs) { cudaStreamSynchronize(cs); cudaStreamDestroy(cs); }
-        for (int b = 0; b < 2; b++) {
-            if (copied[b]) cudaEventDestroy(copied[b]);
-            if (done[b]) cudaEventDestroy(done[b]);
-        }
-    }
-    int init() {
-        if (in.mem == SYL_MEM_DEVICE) return SYL_OK;
-        C = std::min<uint64_t>(db_chunk_entries(), in.n[0] + in.n[1]);
-        L = std::min<uint64_t>(C, in.G);
-        SYL_CUDA(cudaStreamCreateWithFlags(&cs, cudaStreamNonBlocking));
-        for (int b = 0; b < 2; b++) {
-            SYL_CUDA(cudaEventCreateWithFlags(&copied[b], cudaEventDisableTiming));
-            SYL_CUDA(cudaEventCreateWithFlags(&done[b], cudaEventDisableTiming));
-            SYL_TRY(stage[b].alloc((C + 2 * L) * 8));
-        }
-        return SYL_OK;
-    }
-    // the host chunk that starts at entry e of the concatenated parts; advances e past it
-    int plan(uint64_t &e, uint64_t p0[2], uint64_t p1[2], uint64_t glo[2], uint64_t ghi[2], uint32_t part[2]) const {
-        uint64_t budget = C;
-        int ns = 0;
-        while (budget && e < in.n[0] + in.n[1] && ns < 2) {
-            const uint32_t pt = e < in.n[0] ? 0 : 1;
-            const uint64_t *off = in.off[pt];
-            const uint64_t a = pt ? e - in.n[0] : e;
-            const uint64_t g = (uint64_t)(std::upper_bound(off, off + in.G + 1, a) - off) - 1;
-            uint64_t z = std::min(a + budget, in.n[pt]);
-            if (g + L <= in.G) z = std::min(z, off[g + L]);  // > a: genome g holds entry a
-            p0[ns] = a; p1[ns] = z; glo[ns] = g; part[ns] = pt;
-            ghi[ns] = (uint64_t)(std::upper_bound(off, off + in.G + 1, z - 1) - off) - 1;
-            ns++;
-            budget -= z - a;
-            e += z - a;
-            if (z < in.n[pt]) break;  // the chunk ends inside this part
-        }
-        return ns;
-    }
-    template <typename F> int pass(F launch) {
-        cudaStream_t st = ctx->stream;
-        if (in.mem == SYL_MEM_DEVICE) {
-            DbChunk c{};
-            int ns = 0;
-            for (uint32_t pt = 0; pt < 2; pt++) {
-                if (!in.n[pt]) continue;
-                c.keys[ns] = in.keys[pt]; c.off[ns] = in.off[pt]; c.n_off[ns] = in.G + 1;
-                c.g0[ns] = 0; c.p0[ns] = 0; c.n[ns] = in.n[pt]; c.part[ns] = pt;
-                ns++;
-            }
-            launch(c);
-            ctx->launches++;
-            SYL_CUDA(cudaGetLastError());
-            return SYL_OK;
-        }
-        uint64_t e = 0;
-        for (uint64_t i = 0; e < in.n[0] + in.n[1]; i++) {
-            const int b = (int)(i & 1);
-            uint64_t p0[2], p1[2], glo[2], ghi[2];
-            uint32_t part[2];
-            const int ns = plan(e, p0, p1, glo, ghi, part);
-            if (i >= 2) SYL_CUDA(cudaStreamWaitEvent(cs, done[b], 0));
-            uint64_t *kw = stage[b].as<uint64_t>(), *ow = kw + C;
-            DbChunk c{};
-            for (int s = 0; s < ns; s++) {
-                const uint64_t n = p1[s] - p0[s], no = ghi[s] - glo[s] + 1;
-                SYL_CUDA(cudaMemcpyAsync(kw, in.keys[part[s]] + p0[s], n * 8, cudaMemcpyHostToDevice, cs));
-                SYL_CUDA(cudaMemcpyAsync(ow, in.off[part[s]] + glo[s], no * 8, cudaMemcpyHostToDevice, cs));
-                c.keys[s] = kw; c.off[s] = ow; c.n_off[s] = no; c.g0[s] = glo[s]; c.p0[s] = p0[s]; c.n[s] = n; c.part[s] = part[s];
-                kw += n;
-                ow += no;
-            }
-            SYL_CUDA(cudaEventRecord(copied[b], cs));
-            SYL_CUDA(cudaStreamWaitEvent(st, copied[b], 0));
-            launch(c);
-            ctx->launches++;
-            SYL_CUDA(cudaGetLastError());
-            SYL_CUDA(cudaEventRecord(done[b], st));
-        }
-        return SYL_OK;
-    }
-};
-
-static unsigned db_grid(const syl_ctx *ctx, const DbChunk &c) {
-    return (unsigned)std::max<uint64_t>(1, std::min<uint64_t>(nblk(c.n[0] + c.n[1], 256), (uint64_t)ctx->num_sms * 16));
-}
-
-// Buckets of more than DB_MID entries, one at a time: two stable radix sorts (by rank, then by key) through temporaries
-// sized by the largest of them.
-static int db_sort_large(syl_ctx *ctx, syl_db *db, const std::vector<uint2> &large) {
-    cudaStream_t st = ctx->stream;
-    uint32_t mmax = 0;
-    for (const uint2 &l : large) mmax = std::max(mmax, l.y);
-    size_t t1 = 0, t2 = 0;
-    SYL_CUDA(cub::DeviceRadixSort::SortPairs(nullptr, t1, (const uint32_t *)nullptr, (uint32_t *)nullptr,
-                                             (const uint64_t *)nullptr, (uint64_t *)nullptr, mmax, 0, 32, st));
-    SYL_CUDA(cub::DeviceRadixSort::SortPairs(nullptr, t2, (const uint64_t *)nullptr, (uint64_t *)nullptr,
-                                             (const uint32_t *)nullptr, (uint32_t *)nullptr, mmax, 0, 64, st));
-    const size_t tb = std::max(t1, t2);
-    const size_t kb = ((size_t)mmax * 8 + 255) & ~(size_t)255, rb = ((size_t)mmax * 4 + 255) & ~(size_t)255;
-    BuildBuf buf(ctx);
-    SYL_TRY(buf.alloc(kb + 2 * rb + tb));
-    uint64_t *kalt = buf.as<uint64_t>();
-    uint32_t *ra = reinterpret_cast<uint32_t *>(buf.as<uint8_t>() + kb), *rb2 = reinterpret_cast<uint32_t *>(buf.as<uint8_t>() + kb + rb);
-    void *tmp = buf.as<uint8_t>() + kb + 2 * rb;
-    for (const uint2 &l : large) {
-        uint64_t *k = db->keys + l.x;
-        uint32_t *g = db->gid + l.x;
-        size_t t = tb;
-        k_gid_to_rank<<<nblk(l.y, 256), 256, 0, st>>>(g, l.y, ra);
-        SYL_CUDA(cub::DeviceRadixSort::SortPairs(tmp, t, ra, rb2, k, kalt, l.y, 0, 32, st));
-        t = tb;
-        SYL_CUDA(cub::DeviceRadixSort::SortPairs(tmp, t, kalt, k, rb2, ra, l.y, 0, 64, st));
-        k_rank_to_gid<<<nblk(l.y, 256), 256, 0, st>>>(ra, l.y, g);
-        ctx->launches += 4;
-    }
-    SYL_CUDA(cudaGetLastError());
-    return SYL_OK;
-}
-
-static const char *const BAD_OFFSETS = "offsets must start at 0 and be monotone";
-
-// CSR offsets of G genomes in host memory (tracked_off may be NULL): the chunk planner and the scatter's genome search
-// walk them, so they must start at 0 and never decrease
-static int check_host_offsets(const uint64_t *kmer_off, const uint64_t *tracked_off, uint64_t G) {
-    for (const uint64_t *o : {kmer_off, tracked_off}) {
-        if (!o) continue;
-        bool bad = o[0] != 0;
-        for (uint64_t i = 1; i <= G && !bad; i++) bad = o[i] < o[i - 1];
-        if (bad) { set_error(BAD_OFFSETS); return SYL_ERR_ARG; }
-    }
-    return SYL_OK;
-}
-
-static int check_db_size(uint64_t nk, uint64_t nt, uint64_t G) {
-    if (nk >= 0xFFFFFFFFull || nt >= 0xFFFFFFFFull || nk + nt >= 0xFFFFFFFFull) {
-        set_error("db shard holds more than 2^32-2 k-mers; shard the database");
-        return SYL_ERR_ARG;
-    }
-    if (G >= 0x7FFFFFFFull) { set_error("too many genomes in one db shard"); return SYL_ERR_ARG; }
-    return SYL_OK;
-}
-
-// a half-built index: its kernels may still be writing it
-void HandleFree::operator()(syl_db *db) const {
-    cudaStreamSynchronize(db->stream);
-    syl_db_free(db);
-}
-
-// The index of `in` (see "index build" above).  gn_size: G sizes in in.mem's memory, or NULL (zeros).
-static int db_build(syl_ctx *ctx, const DbInput &in, const uint64_t *gn_size, int has_tracked, int k, uint64_t c,
-                    uint32_t genome_base, syl_db **out) {
-    cudaStream_t st = ctx->stream;
-    const uint64_t G = in.G, N = in.n[0] + in.n[1];
-    Handle<syl_db> db = new_handle<syl_db>(ctx);
-    if (!db) return SYL_ERR_OOM;
-    db->n_genomes = G;
-    db->genome_base = genome_base;
-    db->N = N;
-    db->has_tracked = has_tracked;
-    db->k = k;
-    db->c = c;
-    SYL_TRY(hblock_alloc(ctx, (void **)&db->keys, std::max<uint64_t>(N, 1) * 8));
-    SYL_TRY(hblock_alloc(ctx, (void **)&db->gid, std::max<uint64_t>(N, 1) * 4));
-    SYL_TRY(hblock_alloc(ctx, (void **)&db->glen, std::max<uint64_t>(G, 1) * 4));
-    db->h_gn_size.assign(G, 0);
-    std::vector<uint32_t> h_glen;
-    if (G) {
-        if (in.mem == SYL_MEM_DEVICE) {
-            if (gn_size) SYL_CUDA(cudaMemcpyAsync(db->h_gn_size.data(), gn_size, G * 8, cudaMemcpyDeviceToHost, st));
-            k_glen<<<nblk(G, 256), 256, 0, st>>>(in.off[0], G, db->glen);
-            ctx->launches++;
-        } else {
-            if (gn_size) std::copy(gn_size, gn_size + G, db->h_gn_size.begin());
-            h_glen.resize(G);
-            for (uint64_t g = 0; g < G; g++) h_glen[g] = (uint32_t)(in.off[0][g + 1] - in.off[0][g]);
-            SYL_CUDA(cudaMemcpyAsync(db->glen, h_glen.data(), G * 4, cudaMemcpyHostToDevice, st));
-        }
-    }
-    uint64_t NB = 1024;
-    while (NB < N / 4) NB <<= 1;
-    db->NB = NB;
-    SYL_TRY(hblock_alloc(ctx, (void **)&db->bstart, (NB + 2) * 4));
-    SYL_CUDA(cudaMemsetAsync(db->bstart, 0, (NB + 2) * 4, st));
-    if (N) {
-        DbFeed feed(ctx, in);
-        SYL_TRY(feed.init());
-        unsigned long long *d_max = reinterpret_cast<unsigned long long *>(ctx->d_counters + CNT_MAX_KEY);
-        SYL_CUDA(cudaMemsetAsync(d_max, 0, 16, st));  // CNT_MAX_KEY, CNT_LARGE_BUCKETS
-        SYL_TRY(feed.pass([&](const DbChunk &ch) { k_db_max<<<db_grid(ctx, ch), 256, 0, st>>>(ch, d_max); }));
-        SYL_CUDA(cudaMemcpyAsync(ctx->h_counters + CNT_MAX_KEY, d_max, 8, cudaMemcpyDeviceToHost, st));
-        SYL_CUDA(cudaStreamSynchronize(st));
-        db->maxkey = ctx->h_counters[CNT_MAX_KEY];
-        unsigned __int128 m = ((unsigned __int128)NB << 64) / ((unsigned __int128)db->maxkey + 1);
-        db->M = m > (unsigned __int128)UINT64_MAX ? UINT64_MAX : (uint64_t)m;
-        const uint64_t M = db->M;
-        SYL_TRY(feed.pass([&](const DbChunk &ch) { k_db_hist<<<db_grid(ctx, ch), 256, 0, st>>>(ch, M, NB, db->bstart); }));
-        {
-            BuildBuf tmp(ctx);
-            size_t tb = 0;
-            SYL_CUDA(cub::DeviceScan::InclusiveSum(nullptr, tb, db->bstart, db->bstart, (int)(NB + 2), st));
-            SYL_TRY(tmp.alloc(tb));
-            SYL_CUDA(cub::DeviceScan::InclusiveSum(tmp.p, tb, db->bstart, db->bstart, (int)(NB + 2), st));
-            ctx->launches++;
-        }
-        SYL_TRY(feed.pass([&](const DbChunk &ch) {
-            k_db_scatter<<<db_grid(ctx, ch), 256, 0, st>>>(ch, M, NB, db->bstart, db->keys, db->gid);
-        }));
-        // everything below reads the index only: the staging buffers go before the large-bucket temporaries come
-        feed.stage[0].release();
-        feed.stage[1].release();
-        BuildBuf large(ctx);
-        SYL_TRY(large.alloc((N / (DB_MID + 1) + 1) * sizeof(uint2)));
-        unsigned long long *d_nl = reinterpret_cast<unsigned long long *>(ctx->d_counters + CNT_LARGE_BUCKETS);
-        k_db_sort_buckets<<<nblk(NB, DB_SORT_TILE), DB_SORT_TILE, 0, st>>>(db->bstart, NB, db->keys, db->gid,
-                                                                            large.as<uint2>(), d_nl);
-        ctx->launches++;
-        SYL_CUDA(cudaGetLastError());
-        SYL_CUDA(cudaMemcpyAsync(ctx->h_counters + CNT_LARGE_BUCKETS, d_nl, 8, cudaMemcpyDeviceToHost, st));
-        SYL_CUDA(cudaStreamSynchronize(st));
-        std::vector<uint2> h_large(ctx->h_counters[CNT_LARGE_BUCKETS]);
-        if (!h_large.empty()) {
-            SYL_CUDA(cudaMemcpyAsync(h_large.data(), large.p, h_large.size() * sizeof(uint2), cudaMemcpyDeviceToHost, st));
-            SYL_CUDA(cudaStreamSynchronize(st));
-            large.release();
-            SYL_TRY(db_sort_large(ctx, db.get(), h_large));
-        }
-    }
-    SYL_CUDA(cudaStreamSynchronize(st));
-    *out = db.release();
-    return SYL_OK;
-}
-
-}  // namespace syl
-
-// A database in borrowed host arrays, cut into index shards (syl_db_shards_*).
-struct syl_db_shards {
-    syl_ctx *ctx = nullptr;
-    const uint64_t *kmers = nullptr, *kmer_off = nullptr, *tracked = nullptr, *tracked_off = nullptr, *gn_size = nullptr;
-    uint64_t G = 0;
-    int k = 31;
-    uint64_t c = 200;
-    uint64_t cap = 0;             // entries per shard, and per survivor index of several samples
-    uint64_t survivor_max = 0;    // entries of one sample's survivor index
-    std::vector<uint64_t> first;  // shard i = genomes [first[i], first[i + 1])
-    uint64_t calls = 0;
-    struct {                      // the rows of the last call, when they did not fit the caller's buffer
-        uint64_t call = 0;        // 0: nothing kept
-        bool profile = false;
-        syl_contain_params p{};
-        std::vector<const void *> key;  // the samples of the call (handle pointers, or host arrays and their count)
-        std::vector<syl_ani_row> rows;
-    } kept;
-    uint64_t *pinned = nullptr;   // staging of the survivor k-mers (grow-only)
-    uint64_t pinned_n = 0;
-};
-
-namespace syl {
-
-constexpr uint64_t PAIRS_PER_CALL = 1ull << 22;  // (sample, genome) pairs per join: 4 GB of per-pair histograms
-
-// Entries per shard when the caller gives none: the device's free memory at 16 bytes per entry (the build's peak is
-// about 14), after an eighth of it and the histograms of PAIRS_PER_CALL pairs are set aside for the joins.
-static int default_shard_entries(uint64_t *out) {
-    size_t free_b = 0, total_b = 0;
-    SYL_CUDA(cudaMemGetInfo(&free_b, &total_b));
-    const uint64_t budget = free_b - free_b / 8, joins = PAIRS_PER_CALL * COV_BINS * 4;
-    const uint64_t e = budget > joins ? (budget - joins) / 16 : 0;
-    *out = std::min<uint64_t>(std::max<uint64_t>(e, 1ull << 20), SHARD_MAX_ENTRIES);
-    return SYL_OK;
-}
-
-static uint64_t shard_entries_env() {  // SYL_DB_SHARD_ENTRIES caps max_entries (tests; read per syl_db_shards_create)
-    if (const char *e = getenv("SYL_DB_SHARD_ENTRIES")) {
-        const long long v = atoll(e);
-        if (v >= 1) return (uint64_t)v;
-    }
-    return 0;
-}
-
-static double ms_since(std::chrono::steady_clock::time_point t) {
-    return std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t).count();
-}
-
-// The index of genomes [a, b) straight from the borrowed host arrays; only the offsets are copied (rebased to 0).
-static int shard_build(const syl_db_shards *s, uint64_t a, uint64_t b, syl_db **out) {
-    const uint64_t G = b - a;
-    std::vector<uint64_t> ko(G + 1), to(s->tracked_off ? G + 1 : 0);
-    for (uint64_t i = 0; i <= G; i++) ko[i] = s->kmer_off[a + i] - s->kmer_off[a];
-    for (uint64_t i = 0; i < to.size(); i++) to[i] = s->tracked_off[a + i] - s->tracked_off[a];
-    const uint64_t nt = to.empty() ? 0 : to[G];
-    const DbInput in{SYL_MEM_HOST,
-                     {ko[G] ? s->kmers + s->kmer_off[a] : nullptr, nt ? s->tracked + s->tracked_off[a] : nullptr},
-                     {ko.data(), to.empty() ? nullptr : to.data()}, G, {ko[G], nt}};
-    return db_build(s->ctx, in, s->gn_size ? s->gn_size + a : nullptr, s->tracked_off ? 1 : 0, s->k, s->c, (uint32_t)a, out);
-}
-
-// ---- the samples of a call, batch by batch --------------------------------------------------------
-
-// The samples of a call as the joins take them, in batches of samples [first[b], first[b + 1]): device handles (views
-// into their own arrays) or host arrays staged batch by batch into device slots (HostSamples).
-struct SampleSource {
-    std::vector<SampleMeta> metas;  // per sample
-    JoinRoom room;                  // what the joins of a batch may take beyond its plan (handles: unbounded)
-    virtual ~SampleSource() = default;
-    // the batches of a join against an index of G genomes
-    virtual void batches(uint64_t G, std::vector<uint32_t> &first) const = 0;
-    // the most samples x genomes of a survivor join from sample s0 on, and whether such a batch must end before sample i
-    virtual uint64_t survivor_pairs(uint32_t) const { return PAIRS_PER_CALL; }
-    virtual bool cut_before(uint32_t) const { return false; }
-    // views of samples [s0, s1), inside one batch, ready for work enqueued on the ctx stream from now on
-    virtual int views(uint32_t s0, uint32_t s1, std::vector<SampleView> &v) = 0;
-    // stage samples [s0, s1) ahead of their views() (host samples), while the last views are joined
-    virtual int prefetch(uint32_t, uint32_t) { return SYL_OK; }
-    // the joins of the last views() are enqueued on the ctx stream
-    virtual void done() {}
-};
-
-// Device handles: batches of at most PAIRS_PER_CALL pairs.
-struct HandleSamples : SampleSource {
-    std::vector<SampleView> all;
-    void batches(uint64_t G, std::vector<uint32_t> &first) const override {
-        const uint32_t S = (uint32_t)all.size();
-        const uint32_t per = (uint32_t)std::max<uint64_t>(1, std::min<uint64_t>(S, PAIRS_PER_CALL / std::max<uint64_t>(G, 1)));
-        first.clear();
-        for (uint32_t s0 = 0; s0 < S; s0 += per) first.push_back(s0);
-        first.push_back(S);
-    }
-    int views(uint32_t s0, uint32_t s1, std::vector<SampleView> &v) override {
-        v.assign(all.begin() + s0, all.begin() + s1);
-        return SYL_OK;
-    }
-};
-
-// Host samples (syl_host_samples), staged on the device batch by batch (sample_batches.hpp).  Two slots each hold one
-// batch (hash, count and rebased offsets), filled on the ingest copy stream and sorted there by hash within each sample
-// (one segmented sort per batch, into the slot or the shared second buffer, whichever it ends in), while the ctx stream
-// joins the other slot.  Events order the two streams; the host waits only where the joins already do.
-struct HostSamples : SampleSource {
-    syl_ctx *ctx;
-    const syl_host_samples *in;
-    bool pinned_hash = false, pinned_count = false;
-    std::vector<uint32_t> plan;  // batch b: samples [plan[b], plan[b + 1])
-    uint64_t plan_G = 0;
-    struct Slot {
-        DevBuf<uint64_t> hash, off;
-        DevBuf<uint32_t> count;
-        std::vector<uint64_t> h_off;  // the slot's offsets, rebased to its first sample
-        uint32_t s0 = 0, s1 = 0;
-        bool full = false;
-        cudaEvent_t staged = nullptr, used = nullptr;
-    } slot[2];
-    DevBuf<uint64_t> alt_hash;
-    DevBuf<uint32_t> alt_count;
-    DevBuf<uint8_t> tmp;
-    cudaStream_t cs = nullptr;
-    int cur = -1;  // slot of the last views()
-
-    HostSamples(syl_ctx *c, const syl_host_samples *s) : ctx(c), in(s) {}
-    ~HostSamples() override {
-        if (cs) cudaStreamSynchronize(cs);  // the slots go back to the ctx cache, whose users run on the ctx stream
-        for (Slot &sl : slot)
-            for (cudaEvent_t e : {sl.staged, sl.used})
-                if (e) cudaEventDestroy(e);
-    }
-    void batches(uint64_t, std::vector<uint32_t> &first) const override { first = plan; }
-    uint32_t batch_of(uint32_t i) const { return (uint32_t)(std::upper_bound(plan.begin(), plan.end(), i) - plan.begin() - 1); }
-    uint64_t survivor_pairs(uint32_t s0) const override {
-        const uint32_t b = batch_of(s0);
-        return std::min<uint64_t>(PAIRS_PER_CALL, std::max<uint64_t>(plan_G, 1) * (plan[b + 1] - plan[b]));
-    }
-    bool cut_before(uint32_t i) const override { return std::binary_search(plan.begin(), plan.end(), i); }
-    int find(uint32_t s0, uint32_t s1) const {
-        for (int k = 0; k < 2; k++)
-            if (slot[k].full && slot[k].s0 <= s0 && s1 <= slot[k].s1) return k;
-        return -1;
-    }
-    // slots and sort storage for the largest batch of the plan; the copy stream starts behind the ctx stream's work so far
-    int init() {
-        uint64_t kmers = 0, S = 0;
-        size_t tb = 0;
-        for (size_t b = 0; b + 1 < plan.size(); b++) {
-            const uint64_t n = in->off[plan[b + 1]] - in->off[plan[b]], m = plan[b + 1] - plan[b];
-            kmers = std::max(kmers, n);
-            S = std::max(S, m);
-            cub::DoubleBuffer<uint64_t> dk(nullptr, nullptr);
-            cub::DoubleBuffer<uint32_t> dv(nullptr, nullptr);
-            size_t t = 0;
-            SYL_CUDA(cub::DeviceSegmentedSort::SortPairs(nullptr, t, dk, dv, (int)n, (int)m, (const uint64_t *)nullptr,
-                                                         (const uint64_t *)nullptr, ctx->stream));
-            tb = std::max(tb, t);
-        }
-        SYL_TRY(ingest_copy_stream(ctx, &cs));
-        cudaStream_t st = ctx->stream;
-        for (Slot &sl : slot) {
-            SYL_TRY(sl.hash.alloc(kmers, st)); SYL_TRY(sl.count.alloc(kmers, st)); SYL_TRY(sl.off.alloc(S + 1, st));
-            SYL_CUDA(cudaEventCreateWithFlags(&sl.staged, cudaEventDisableTiming));
-            SYL_CUDA(cudaEventCreateWithFlags(&sl.used, cudaEventDisableTiming));
-        }
-        SYL_TRY(alt_hash.alloc(kmers, st)); SYL_TRY(alt_count.alloc(kmers, st)); SYL_TRY(tmp.alloc(tb, st));
-        SYL_CUDA(cudaEventRecord(slot[0].used, st));  // cached blocks may still be in use by earlier work on the ctx stream
-        SYL_CUDA(cudaStreamWaitEvent(cs, slot[0].used, 0));
-        return SYL_OK;
-    }
-    // samples [s0, s1) into slot k, once the joins of its last batch are done
-    int stage(int k, uint32_t s0, uint32_t s1) {
-        if (!cs) SYL_TRY(init());
-        Slot &sl = slot[k];
-        SYL_CUDA(cudaStreamWaitEvent(cs, sl.used, 0));
-        const uint64_t a = in->off[s0], n = in->off[s1] - a;
-        sl.h_off.resize(s1 - s0 + 1);
-        for (uint32_t i = s0; i <= s1; i++) sl.h_off[i - s0] = in->off[i] - a;
-        SYL_TRY(ingest_copy(ctx, sl.off.p, sl.h_off.data(), sl.h_off.size() * 8, false));
-        SYL_TRY(ingest_copy(ctx, sl.hash.p, in->hash + a, n * 8, pinned_hash));
-        SYL_TRY(ingest_copy(ctx, sl.count.p, in->count + a, n * 4, pinned_count));
-        if (n) {
-            cub::DoubleBuffer<uint64_t> dk(sl.hash.p, alt_hash.p);
-            cub::DoubleBuffer<uint32_t> dv(sl.count.p, alt_count.p);
-            size_t tb = tmp.cap_bytes;
-            SYL_CUDA(cub::DeviceSegmentedSort::SortPairs(tmp.p, tb, dk, dv, (int)n, (int)(s1 - s0), sl.off.p, sl.off.p + 1, cs));
-            ctx->launches += 4;
-            if (dk.selector) sl.hash.swap(alt_hash);
-            if (dv.selector) sl.count.swap(alt_count);
-        }
-        SYL_CUDA(cudaEventRecord(sl.staged, cs));
-        sl.s0 = s0;
-        sl.s1 = s1;
-        sl.full = true;
-        return SYL_OK;
-    }
-    int prefetch(uint32_t s0, uint32_t s1) override {
-        if (find(s0, s1) >= 0) return SYL_OK;
-        return stage(cur < 0 ? 0 : 1 - cur, s0, s1);
-    }
-    int views(uint32_t s0, uint32_t s1, std::vector<SampleView> &v) override {
-        int k = find(s0, s1);
-        if (k < 0) {
-            k = cur < 0 ? 0 : 1 - cur;
-            SYL_TRY(stage(k, s0, s1));
-        }
-        const Slot &sl = slot[k];
-        SYL_CUDA(cudaStreamWaitEvent(ctx->stream, sl.staged, 0));
-        v.resize(s1 - s0);
-        for (uint32_t i = s0; i < s1; i++) {
-            const uint64_t o = sl.h_off[i - sl.s0];
-            v[i - s0] = {sl.hash.p + o, sl.count.p + o, sl.h_off[i + 1 - sl.s0] - o};
-        }
-        cur = k;
-        return SYL_OK;
-    }
-    void done() override {
-        if (cur >= 0) cudaEventRecord(slot[cur].used, ctx->stream);
-    }
-};
-
-// Every sample of `src` against db, in the batches of `first`: the next batch is staged while one is joined, and `then`
-// (samples [then[0], then[1]), if given) while the last one is.  Rows appended with the call's sample indices.
-static int join_batches(syl_ctx *ctx, const syl_db *db, SampleSource &src, const std::vector<uint32_t> &first,
-                        const uint32_t *then, const syl_contain_params *p, bool profile, std::vector<syl_ani_row> &rows) {
-    std::vector<SampleView> v;
-    for (size_t b = 0; b + 1 < first.size(); b++) {
-        const uint32_t s0 = first[b], s1 = first[b + 1];
-        SYL_TRY(src.views(s0, s1, v));
-        std::function<int()> next;
-        if (b + 2 < first.size()) next = [&] { return src.prefetch(s1, first[b + 2]); };
-        else if (then) next = [&] { return src.prefetch(then[0], then[1]); };
-        std::vector<syl_ani_row> part;
-        JoinRoom room = src.room;
-        room.s0 = s0;
-        const int rc = contain_fast(ctx, db, v.data(), src.metas.data() + s0, s1 - s0, p, profile, part, next, &room);
-        src.done();
-        SYL_TRY(rc);
-        for (syl_ani_row &r : part) {
-            r.sample += s0;
-            rows.push_back(r);
-        }
-    }
-    return SYL_OK;
-}
-
-// Pass 1 (syl_query) of every sample of src against every shard in turn: each shard's index is built once, joined with
-// all samples batch by batch, and freed before the next one is built.  rows: by shard, then by (sample, genome);
-// row.genome is the global index.
-static int shards_sweep(syl_db_shards *s, SampleSource &src, const syl_contain_params *p, std::vector<syl_ani_row> &rows) {
-    syl_ctx *ctx = s->ctx;
-    std::vector<uint32_t> first, next;
-    for (size_t i = 0; i + 1 < s->first.size(); i++) {
-        const uint64_t a = s->first[i], G = s->first[i + 1] - a;
-        // each shard's index and join scratch are allocated to that shard's size, not next to the previous shard's
-        SYL_TRY(cache_trim(ctx));
-        const auto t0 = std::chrono::steady_clock::now();
-        syl_db *db = nullptr;
-        SYL_TRY(shard_build(s, a, s->first[i + 1], &db));
-        const double build_ms = ms_since(t0);
-        const auto t1 = std::chrono::steady_clock::now();
-        src.batches(G, first);
-        next.clear();
-        if (i + 2 < s->first.size()) src.batches(s->first[i + 2] - s->first[i + 1], next);
-        const int rc = join_batches(ctx, db, src, first, next.size() > 1 ? next.data() : nullptr, p, false, rows);
-        static const bool dbg = getenv("SYL_DEBUG_TIMING") != nullptr;
-        if (dbg)
-            fprintf(stderr, "[db shard %zu/%zu] genomes %llu+%llu entries %llu: build %.1f ms, pass 1 %.1f ms\n", i + 1,
-                    s->first.size() - 1, (unsigned long long)a, (unsigned long long)G, (unsigned long long)db->N, build_ms, ms_since(t1));
-        syl_db_free(db);
-        SYL_TRY(rc);
-    }
-    return cache_trim(ctx);
-}
-
-// syl_profile of samples[s0, s1) of src on an index of the genomes `ids` (ascending global indices), gathered from the
-// borrowed arrays into pinned staging; rows appended with global sample and genome indices.
-static int survivor_profile(syl_db_shards *s, const std::vector<uint32_t> &ids, SampleSource &src, uint32_t s0, uint32_t s1,
-                            const syl_contain_params *p, std::vector<syl_ani_row> &out) {
-    const auto t0 = std::chrono::steady_clock::now();
-    // host samples are staged on the copy stream while the index is gathered and built; the ctx stream waits for them
-    // only before the joins (views() below)
-    SYL_TRY(src.prefetch(s0, s1));
-    const uint64_t n = ids.size();
-    std::vector<uint64_t> ko(n + 1, 0), to(n + 1, 0), gsz(n, 0);
-    for (uint64_t i = 0; i < n; i++) {
-        const uint32_t g = ids[i];
-        ko[i + 1] = ko[i] + s->kmer_off[g + 1] - s->kmer_off[g];
-        to[i + 1] = to[i] + s->tracked_off[g + 1] - s->tracked_off[g];
-        if (s->gn_size) gsz[i] = s->gn_size[g];
-    }
-    const uint64_t nk = ko[n], nt = to[n];
-    if (nk + nt > s->pinned_n) {
-        if (s->pinned) cudaFreeHost(s->pinned);
-        s->pinned = nullptr;
-        s->pinned_n = 0;
-        SYL_CUDA(cudaHostAlloc((void **)&s->pinned, (nk + nt) * 8, cudaHostAllocDefault));
-        s->pinned_n = nk + nt;
-    }
-    for (uint64_t i = 0; i < n; i++) {
-        const uint32_t g = ids[i];
-        std::copy(s->kmers + s->kmer_off[g], s->kmers + s->kmer_off[g + 1], s->pinned + ko[i]);
-        std::copy(s->tracked + s->tracked_off[g], s->tracked + s->tracked_off[g + 1], s->pinned + nk + to[i]);
-    }
-    syl_db *db = nullptr;
-    SYL_TRY(syl_db_build_arrays(s->ctx, SYL_MEM_HOST, s->pinned, ko.data(), s->pinned + nk, to.data(), gsz.data(), n, s->k,
-                                s->c, 0, &db));
-    const double build_ms = ms_since(t0);
-    const auto t1 = std::chrono::steady_clock::now();
-    std::vector<SampleView> v;
-    std::vector<syl_ani_row> part;
-    JoinRoom room = src.room;
-    room.s0 = s0;
-    int rc = src.views(s0, s1, v);
-    if (rc == SYL_OK) rc = contain_fast(s->ctx, db, v.data(), src.metas.data() + s0, s1 - s0, p, true, part, {}, &room);
-    src.done();
-    syl_db_free(db);
-    SYL_TRY(rc);
-    static const bool dbg = getenv("SYL_DEBUG_TIMING") != nullptr;
-    if (dbg)
-        fprintf(stderr, "[survivor index] samples %u..%u genomes %llu entries %llu: gather+build %.1f ms, profile %.1f ms\n", s0, s1,
-                (unsigned long long)n, (unsigned long long)(nk + nt), build_ms, ms_since(t1));
-    for (syl_ani_row &r : part) {
-        r.sample += s0;
-        r.genome = ids[r.genome];
-        out.push_back(r);
-    }
-    return SYL_OK;
-}
-
-// Profile over all shards, equal to syl_profile on one db of every genome: the winner table, pass 2, derep and the
-// abundances only ever see pass-1 survivors (src/contain.rs:284-334, 410-430).  So pass 1 runs per shard, without CIs
-// (never reported; the ANI gate comes before the bootstrap), and each batch of samples is profiled on an index of the
-// union of its survivors.  Ascending global order keeps the winner table's lowest-index tie rule.  A batch closes when
-// the union would pass the shard cap (or the source's pair or batch limits); one sample's survivors alone may take up
-// to survivor_max entries.
-static int shards_profile(syl_db_shards *s, SampleSource &src, const syl_contain_params *p, std::vector<syl_ani_row> &out) {
-    const uint32_t S = (uint32_t)src.metas.size();
-    syl_contain_params p1 = *p;
-    p1.no_ci = 1;
-    p1.estimate_unknown = 0;
-    p1.read_seq_id = -1.;
-    if (p1.minimum_ani < 0.) p1.minimum_ani = 95.;  // profile's gate in a query-mode pass (make_params)
-    std::vector<std::vector<uint32_t>> surv(S);
-    {
-        std::vector<syl_ani_row> rows1;
-        SYL_TRY(shards_sweep(s, src, &p1, rows1));
-        for (const syl_ani_row &r : rows1) surv[r.sample].push_back(r.genome);
-    }
-    std::vector<uint8_t> in(s->G, 0);
-    std::vector<uint32_t> ids;
-    uint64_t entries = 0;
-    uint32_t s0 = 0;
-    auto flush = [&](uint32_t s1) -> int {
-        if (!ids.empty()) {
-            std::sort(ids.begin(), ids.end());
-            SYL_TRY(survivor_profile(s, ids, src, s0, s1, p, out));
-            SYL_TRY(cache_trim(s->ctx));
-        }
-        for (uint32_t g : ids) in[g] = 0;
-        ids.clear();
-        entries = 0;
-        s0 = s1;
-        return SYL_OK;
-    };
-    for (uint32_t i = 0; i < S; i++) {
-        uint64_t own = 0, add = 0, addg = 0;
-        for (uint32_t g : surv[i]) {
-            const uint64_t e = genome_entries(s->kmer_off, s->tracked_off, g);
-            own += e;
-            if (!in[g]) { add += e; addg++; }
-        }
-        if (own > s->survivor_max) {
-            set_error("the pass-1 survivors of sample " + std::to_string(i) + " hold " + std::to_string(own) +
-                      " index entries, more than one survivor index takes (" + std::to_string(s->survivor_max) + ")");
-            return SYL_ERR_UNSUPPORTED;
-        }
-        const uint64_t ng = ids.size() + addg;
-        if (i > s0 && (entries + add > s->cap || ng > SHARD_MAX_GENOMES || (uint64_t)(i - s0 + 1) * ng > src.survivor_pairs(s0) ||
-                       src.cut_before(i))) {
-            SYL_TRY(flush(i));
-            add = own;
-        }
-        for (uint32_t g : surv[i])
-            if (!in[g]) { in[g] = 1; ids.push_back(g); }
-        entries += add;
-    }
-    return flush(S);
-}
-
-// syl_query_shards / syl_profile_shards / syl_*_host_samples with shards, after the argument checks.  key: the samples
-// of the call, as the rows of a SYL_ERR_CAPACITY call are kept under.
-static int shards_call(syl_db_shards *s, SampleSource &src, const std::vector<const void *> &key, const syl_contain_params *p,
-                       bool profile, syl_ani_row *rows, uint64_t cap, uint64_t *n_rows) {
-    const uint64_t call = ++s->calls;
-    auto &kp = s->kept;
-    const bool retry = kp.call && kp.call + 1 == call && kp.profile == profile && !memcmp(&kp.p, p, sizeof *p) && kp.key == key;
-    std::vector<syl_ani_row> out;
-    if (retry) out.swap(kp.rows);
-    kp.call = 0;
-    std::vector<syl_ani_row>().swap(kp.rows);
-    kp.key.clear();
-    if (!retry && s->G && !src.metas.empty()) {
-        if (profile) {
-            SYL_TRY(shards_profile(s, src, p, out));
-        } else {
-            SYL_TRY(shards_sweep(s, src, p, out));
-            std::sort(out.begin(), out.end(), [](const syl_ani_row &a, const syl_ani_row &b) {
-                return a.sample != b.sample ? a.sample < b.sample : a.genome < b.genome;
-            });
-        }
-    }
-    const int rc = copy_rows(out, rows, cap, n_rows);
-    if (rc == SYL_ERR_CAPACITY) {
-        kp.call = call;
-        kp.profile = profile;
-        kp.p = *p;
-        kp.key = key;
-        kp.rows.swap(out);
-    }
-    return rc;
-}
-
-static int handle_shards_call(syl_ctx *ctx, syl_db_shards *s, const syl_sample *const *samples, uint32_t n_samples,
-                              const syl_contain_params *p, bool profile, syl_ani_row *rows, uint64_t cap, uint64_t *n_rows) {
-    if (!s) { set_error("NULL argument"); return SYL_ERR_ARG; }
-    SYL_TRY(check_contain_args(ctx, s->k, s->c, s->tracked_off != nullptr, profile, samples, n_samples, p, rows, cap, n_rows));
-    if (ctx != s->ctx) { set_error("db shards used with another ctx than the one that created them"); return SYL_ERR_ARG; }
-    SYL_ENTER(ctx);
-    HandleSamples src;
-    SYL_TRY(handle_views(ctx, samples, n_samples, p->estimate_unknown != 0, src.all, src.metas));
-    return shards_call(s, src, std::vector<const void *>(samples, samples + n_samples), p, profile, rows, cap, n_rows);
-}
-
-// syl_query_host_samples / syl_profile_host_samples
-static int host_samples_call(syl_ctx *ctx, const syl_db *db, syl_db_shards *sh, const syl_host_samples *s,
-                             const syl_contain_params *p, bool profile, syl_ani_row *rows, uint64_t cap, uint64_t *n_rows) {
-    if (!ctx || !s || !p || !n_rows || (cap && !rows)) { set_error("NULL argument"); return SYL_ERR_ARG; }
-    if ((db != nullptr) == (sh != nullptr)) { set_error("exactly one of db and shards must be given"); return SYL_ERR_ARG; }
-    *n_rows = 0;
-    const uint32_t S = s->n_samples;
-    if (!s->off || (S && (!s->c || !s->mean_read_length))) { set_error("NULL argument"); return SYL_ERR_ARG; }
-    if (s->off[0] != 0) { set_error(BAD_OFFSETS); return SYL_ERR_ARG; }
-    for (uint32_t i = 0; i < S; i++)
-        if (s->off[i + 1] < s->off[i]) { set_error(BAD_OFFSETS); return SYL_ERR_ARG; }
-    if (s->off[S] && (!s->hash || !s->count)) { set_error("off counts k-mers but hash or count is NULL"); return SYL_ERR_ARG; }
-    const int k = db ? db->k : sh->k;
-    const uint64_t c = db ? db->c : sh->c;
-    for (uint32_t i = 0; i < S; i++) SYL_TRY(check_sample_kc(k, c, s->k, s->c[i]));
-    SYL_TRY(check_params(k, db ? db->has_tracked != 0 : sh->tracked_off != nullptr, profile, p));
-    if (sh && ctx != sh->ctx) { set_error("db shards used with another ctx than the one that created them"); return SYL_ERR_ARG; }
-    SYL_ENTER(ctx);
-    HostSamples src(ctx, s);
-    for (int a = 0; a < 2 && s->off[S]; a++) {  // pinned arrays are copied as they are, pageable ones through the ring
-        cudaPointerAttributes at{};
-        const void *ptr = a ? (const void *)s->count : (const void *)s->hash;
-        bool pinned = false;
-        if (cudaPointerGetAttributes(&at, ptr) == cudaSuccess) {
-            if (at.type == cudaMemoryTypeDevice || at.type == cudaMemoryTypeManaged) { set_error("host samples: a device pointer was given"); return SYL_ERR_ARG; }
-            pinned = at.type == cudaMemoryTypeHost;
-        } else {
-            cudaGetLastError();
-        }
-        (a ? src.pinned_count : src.pinned_hash) = pinned;
-    }
-    // the plan: the device budget of syl_ctx_set_sample_memory (0: free memory once the ctx's staging ring exists, plus
-    // the ctx's cached free blocks), less the largest shard's build (16 bytes per entry)
-    cudaStream_t cs = nullptr;
-    SYL_TRY(ingest_copy_stream(ctx, &cs));
-    uint64_t budget = ctx->sample_budget, index = 0;
-    if (!budget) {
-        size_t free_b = 0, total_b = 0;
-        SYL_CUDA(cudaMemGetInfo(&free_b, &total_b));
-        budget = free_b;
-        for (const auto &b : ctx->free_blocks) budget += b.second;
-    }
-    // the joins' allocations beyond the plan are held to the budget on top of the bytes the ctx holds in use now
-    uint64_t live = ctx->cached_bytes + ctx->transient_bytes;
-    for (const auto &b : ctx->free_blocks) live -= b.second;
-    src.room.limit = live + budget;
-    src.room.budget = budget;
-    if (sh) {
-        for (size_t i = 0; i + 1 < sh->first.size(); i++) {
-            const uint64_t a = sh->first[i], b = sh->first[i + 1];
-            src.plan_G = std::max(src.plan_G, b - a);
-            index = std::max(index, 16 * (sh->kmer_off[b] - sh->kmer_off[a] + (sh->tracked_off ? sh->tracked_off[b] - sh->tracked_off[a] : 0)));
-        }
-    } else {
-        src.plan_G = db->n_genomes;
-    }
-    uint32_t forced = 0;
-    if (const char *e = getenv("SYL_SAMPLE_BATCH")) forced = (uint32_t)std::max(0, atoi(e));
-    const BatchCost cost{36, 4 * 8 + sizeof(SampleView) + 96 * ROW_BYTES, 16, COV_BINS * 4 + 16, 256 * ROW_BYTES + (1u << 20)};
-    uint32_t bad = 0;
-    uint64_t need = 0;
-    const BatchPlanResult pr = plan_sample_batches(s->off, S, src.plan_G, budget > index ? budget - index : 0, PAIRS_PER_CALL,
-                                                   0x7FFFFFFFull, forced, cost, src.plan, &bad, &need);
-    if (pr == BATCH_TOO_MANY_KMERS) {
-        set_error("sample " + std::to_string(bad) + " holds " + std::to_string(need) + " k-mers, more than 2^31 - 1");
-        return SYL_ERR_UNSUPPORTED;
-    }
-    if (pr == BATCH_OOM) {
-        set_error("sample " + std::to_string(bad) + " needs " + std::to_string(need + index) + " bytes of device memory" +
-                  (index ? " (with the largest shard's build)" : "") + ", the budget is " + std::to_string(budget) + " bytes");
-        return SYL_ERR_OOM;
-    }
-    src.metas.resize(S);
-    for (uint32_t i = 0; i < S; i++) {
-        uint64_t sum = 0;
-        if (p->estimate_unknown)
-            for (uint64_t j = s->off[i]; j < s->off[i + 1]; j++) sum += s->count[j];
-        src.metas[i] = {s->mean_read_length[i], s->c[i], sum};
-    }
-    if (sh) {
-        const std::vector<const void *> key{s->hash, s->count, s->off, s->c, s->mean_read_length, (const void *)(uintptr_t)S};
-        return shards_call(sh, src, key, p, profile, rows, cap, n_rows);
-    }
-    std::vector<syl_ani_row> out;
-    if (db->n_genomes && S) SYL_TRY(join_batches(ctx, db, src, src.plan, nullptr, p, profile, out));
-    return copy_rows(out, rows, cap, n_rows);
-}
-
 }  // namespace syl
 
 using namespace syl;
 
 extern "C" {
-
-int syl_db_build(syl_ctx *ctx, const syl_genomes *g, uint32_t genome_base, syl_db **out) {
-    if (!ctx || !g || !out) { set_error("NULL argument"); return SYL_ERR_ARG; }
-    *out = nullptr;
-    SYL_ENTER(ctx);
-    const uint64_t nt = g->has_tracked ? g->total_tracked : 0;
-    SYL_TRY(check_db_size(g->total_kmers, nt, g->n));
-    const DbInput in{SYL_MEM_DEVICE, {g->kmers, g->tracked}, {g->kmer_off, g->tracked_off}, g->n, {g->total_kmers, nt}};
-    return db_build(ctx, in, g->gn_size, g->has_tracked, g->k, g->c, genome_base, out);
-}
-
-int syl_db_build_arrays(syl_ctx *ctx, int mem, const uint64_t *kmers, const uint64_t *kmer_off, const uint64_t *tracked,
-                        const uint64_t *tracked_off, const uint64_t *gn_size, uint64_t n_genomes, int k, uint64_t c,
-                        uint32_t genome_base, syl_db **out) {
-    if (!ctx || !kmer_off || !out) { set_error("NULL argument"); return SYL_ERR_ARG; }
-    *out = nullptr;
-    if (mem != SYL_MEM_HOST && mem != SYL_MEM_DEVICE) { set_error("bad mem"); return SYL_ERR_ARG; }
-    SYL_ENTER(ctx);
-    cudaStream_t st = ctx->stream;
-    if (n_genomes >= 0x7FFFFFFFull) return check_db_size(0, 0, n_genomes);
-    uint64_t nk = 0, nt = 0;
-    if (mem == SYL_MEM_HOST) {
-        nk = kmer_off[n_genomes];
-        nt = tracked_off ? tracked_off[n_genomes] : 0;
-    } else {
-        SYL_CUDA(cudaMemcpyAsync(ctx->h_counters + CNT_KMER_TOTAL, kmer_off + n_genomes, 8, cudaMemcpyDeviceToHost, st));
-        if (tracked_off) SYL_CUDA(cudaMemcpyAsync(ctx->h_counters + CNT_TRACKED_TOTAL, tracked_off + n_genomes, 8, cudaMemcpyDeviceToHost, st));
-        SYL_CUDA(cudaStreamSynchronize(st));
-        nk = ctx->h_counters[CNT_KMER_TOTAL];
-        nt = tracked_off ? ctx->h_counters[CNT_TRACKED_TOTAL] : 0;
-    }
-    SYL_TRY(check_db_size(nk, nt, n_genomes));
-    SYL_TRY(check_kmer_arrays(kmers, nk, tracked, nt));
-    if (mem == SYL_MEM_HOST) {
-        SYL_TRY(check_host_offsets(kmer_off, tracked_off, n_genomes));
-    } else {
-        unsigned long long *d_bad = reinterpret_cast<unsigned long long *>(ctx->d_counters + CNT_BAD_OFFSETS);
-        SYL_CUDA(cudaMemsetAsync(d_bad, 0, 8, st));
-        for (const uint64_t *o : {kmer_off, tracked_off}) {
-            if (!o) continue;
-            k_check_offsets<<<nblk(n_genomes + 1, 256), 256, 0, st>>>(o, n_genomes + 1, d_bad);
-            ctx->launches++;
-        }
-        SYL_CUDA(cudaGetLastError());
-        SYL_CUDA(cudaMemcpyAsync(ctx->h_counters + CNT_BAD_OFFSETS, d_bad, 8, cudaMemcpyDeviceToHost, st));
-        SYL_CUDA(cudaStreamSynchronize(st));
-        if (ctx->h_counters[CNT_BAD_OFFSETS]) { set_error(BAD_OFFSETS); return SYL_ERR_ARG; }
-    }
-    const DbInput in{mem, {kmers, tracked}, {kmer_off, tracked_off}, n_genomes, {nk, nt}};
-    return db_build(ctx, in, gn_size, tracked_off ? 1 : 0, k, c, genome_base, out);
-}
-
-int syl_db_download(syl_ctx *ctx, const syl_db *db, uint64_t *keys, uint32_t *gid, uint32_t *bstart, uint64_t *n_entries,
-                    uint64_t *n_buckets) {
-    if (!ctx || !db) { set_error("NULL argument"); return SYL_ERR_ARG; }
-    if (n_entries) *n_entries = db->N;
-    if (n_buckets) *n_buckets = db->NB;
-    SYL_ENTER(ctx);
-    cudaStream_t st = ctx->stream;
-    if (keys && db->N) SYL_CUDA(cudaMemcpyAsync(keys, db->keys, db->N * 8, cudaMemcpyDeviceToHost, st));
-    if (gid && db->N) SYL_CUDA(cudaMemcpyAsync(gid, db->gid, db->N * 4, cudaMemcpyDeviceToHost, st));
-    if (bstart) SYL_CUDA(cudaMemcpyAsync(bstart, db->bstart, (db->NB + 1) * 4, cudaMemcpyDeviceToHost, st));
-    SYL_CUDA(cudaStreamSynchronize(st));
-    return SYL_OK;
-}
-
-uint64_t syl_db_num_genomes(const syl_db *db) { return db ? db->n_genomes : 0; }
-
-void syl_db_free(syl_db *db) {
-    if (!db) return;
-    cudaSetDevice(db->device);
-    hblock_free(db->owner, db->keys);
-    hblock_free(db->owner, db->gid);
-    hblock_free(db->owner, db->bstart);
-    hblock_free(db->owner, db->glen);
-    delete db;
-}
 
 void syl_contain_params_default(syl_contain_params *p, int k, int pseudotax) {
     if (!p) return;
@@ -2503,20 +1304,6 @@ void syl_contain_params_default(syl_contain_params *p, int k, int pseudotax) {
     p->min_count_correct = 3.;
     p->minimum_ani = -1.;
     p->redundant_ani = 99.;
-}
-
-int syl_query(syl_ctx *ctx, const syl_db *db, const syl_sample *const *samples, uint32_t n_samples,
-              const syl_contain_params *p, syl_ani_row *rows, uint64_t cap, uint64_t *n_rows) {
-    if (!db) { set_error("NULL argument"); return SYL_ERR_ARG; }
-    SYL_TRY(check_contain_args(ctx, db->k, db->c, db->has_tracked, false, samples, n_samples, p, rows, cap, n_rows));
-    SYL_ENTER(ctx);
-    if (db->n_genomes == 0 || n_samples == 0) return SYL_OK;
-    std::vector<SampleView> views;
-    std::vector<SampleMeta> metas;
-    SYL_TRY(handle_views(ctx, samples, n_samples, p->estimate_unknown != 0, views, metas));
-    std::vector<syl_ani_row> out;
-    SYL_TRY(contain_fast(ctx, db, views.data(), metas.data(), n_samples, p, false, out));
-    return copy_rows(out, rows, cap, n_rows);
 }
 
 int syl_profile_shard_begin(syl_ctx *ctx, const syl_db *db, const syl_sample *const *samples, uint32_t n_samples,
@@ -2572,99 +1359,6 @@ int syl_profile_shard_finish(syl_profile_job *j, syl_ani_row *rows, uint64_t cap
 
 void syl_profile_job_free(syl_profile_job *j) {
     delete j;  // the scratch blocks go back to the owning ctx's cache (DevBuf::owner)
-}
-
-int syl_profile(syl_ctx *ctx, const syl_db *db, const syl_sample *const *samples, uint32_t n_samples,
-                const syl_contain_params *p, syl_ani_row *rows, uint64_t cap, uint64_t *n_rows) {
-    if (!db) { set_error("NULL argument"); return SYL_ERR_ARG; }
-    SYL_TRY(check_contain_args(ctx, db->k, db->c, db->has_tracked, true, samples, n_samples, p, rows, cap, n_rows));
-    SYL_ENTER(ctx);
-    if (db->n_genomes == 0 || n_samples == 0) return SYL_OK;
-    std::vector<SampleView> views;
-    std::vector<SampleMeta> metas;
-    SYL_TRY(handle_views(ctx, samples, n_samples, p->estimate_unknown != 0, views, metas));
-    std::vector<syl_ani_row> out;
-    SYL_TRY(contain_fast(ctx, db, views.data(), metas.data(), n_samples, p, true, out));
-    return copy_rows(out, rows, cap, n_rows);
-}
-
-int syl_db_shards_create(syl_ctx *ctx, const uint64_t *kmers, const uint64_t *kmer_off, const uint64_t *tracked,
-                         const uint64_t *tracked_off, const uint64_t *gn_size, uint64_t n_genomes, int k, uint64_t c,
-                         uint64_t max_entries, syl_db_shards **out) {
-    if (!ctx || !kmer_off || !out) { set_error("NULL argument"); return SYL_ERR_ARG; }
-    *out = nullptr;
-    if (n_genomes > 0xFFFFFFFFull) { set_error("more than 2^32 genomes: row.genome is 32 bits"); return SYL_ERR_ARG; }
-    SYL_ENTER(ctx);
-    for (const uint64_t *a : {kmers, kmer_off, tracked, tracked_off, gn_size}) {  // the sweep reads them on the host
-        cudaPointerAttributes at{};
-        if (!a) continue;
-        if (cudaPointerGetAttributes(&at, a) != cudaSuccess) {
-            cudaGetLastError();
-            continue;
-        }
-        if (at.type == cudaMemoryTypeDevice) { set_error("db shards borrow host arrays; a device pointer was given"); return SYL_ERR_ARG; }
-    }
-    SYL_TRY(check_host_offsets(kmer_off, tracked_off, n_genomes));
-    SYL_TRY(check_kmer_arrays(kmers, kmer_off[n_genomes], tracked, tracked_off ? tracked_off[n_genomes] : 0));
-    uint64_t dflt = 0;
-    SYL_TRY(default_shard_entries(&dflt));
-    uint64_t cap = max_entries ? std::min(max_entries, SHARD_MAX_ENTRIES) : dflt;
-    if (const uint64_t e = shard_entries_env()) cap = std::min(cap, e);
-    std::vector<uint64_t> first;
-    uint64_t big = 0;
-    if (!cut_shards(kmer_off, tracked_off, n_genomes, cap, first, &big)) {
-        set_error("genome " + std::to_string(big) + " alone holds more than 2^32-3 index entries");
-        return SYL_ERR_ARG;
-    }
-    syl_db_shards *s = new (std::nothrow) syl_db_shards();
-    if (!s) return SYL_ERR_OOM;
-    s->ctx = ctx;
-    s->kmers = kmers; s->kmer_off = kmer_off; s->tracked = tracked; s->tracked_off = tracked_off; s->gn_size = gn_size;
-    s->G = n_genomes;
-    s->k = k;
-    s->c = c;
-    s->cap = cap;
-    s->survivor_max = std::max(cap, dflt);
-    s->first.swap(first);
-    *out = s;
-    return SYL_OK;
-}
-
-uint64_t syl_db_shards_count(const syl_db_shards *s) { return s && !s->first.empty() ? s->first.size() - 1 : 0; }
-
-int syl_db_shards_range(const syl_db_shards *s, uint64_t i, uint64_t *first_genome, uint64_t *n_genomes, uint64_t *n_entries) {
-    if (!s || i >= syl_db_shards_count(s)) { set_error("NULL handle or shard index out of range"); return SYL_ERR_ARG; }
-    const uint64_t a = s->first[i], b = s->first[i + 1];
-    if (first_genome) *first_genome = a;
-    if (n_genomes) *n_genomes = b - a;
-    if (n_entries) *n_entries = s->kmer_off[b] - s->kmer_off[a] + (s->tracked_off ? s->tracked_off[b] - s->tracked_off[a] : 0);
-    return SYL_OK;
-}
-
-int syl_query_shards(syl_ctx *ctx, syl_db_shards *s, const syl_sample *const *samples, uint32_t n_samples,
-                     const syl_contain_params *p, syl_ani_row *rows, uint64_t cap, uint64_t *n_rows) {
-    return handle_shards_call(ctx, s, samples, n_samples, p, false, rows, cap, n_rows);
-}
-
-int syl_profile_shards(syl_ctx *ctx, syl_db_shards *s, const syl_sample *const *samples, uint32_t n_samples,
-                       const syl_contain_params *p, syl_ani_row *rows, uint64_t cap, uint64_t *n_rows) {
-    return handle_shards_call(ctx, s, samples, n_samples, p, true, rows, cap, n_rows);
-}
-
-int syl_query_host_samples(syl_ctx *ctx, const syl_db *db, syl_db_shards *shards, const syl_host_samples *s,
-                           const syl_contain_params *p, syl_ani_row *rows, uint64_t cap, uint64_t *n_rows) {
-    return host_samples_call(ctx, db, shards, s, p, false, rows, cap, n_rows);
-}
-
-int syl_profile_host_samples(syl_ctx *ctx, const syl_db *db, syl_db_shards *shards, const syl_host_samples *s,
-                             const syl_contain_params *p, syl_ani_row *rows, uint64_t cap, uint64_t *n_rows) {
-    return host_samples_call(ctx, db, shards, s, p, true, rows, cap, n_rows);
-}
-
-void syl_db_shards_free(syl_db_shards *s) {
-    if (!s) return;
-    if (s->pinned) cudaFreeHost(s->pinned);
-    delete s;
 }
 
 }  // extern "C"

@@ -30,13 +30,6 @@ int seed_device(syl_ctx *ctx, const uint8_t *d_bases, const uint32_t *d_packed, 
 
 namespace syl {
 
-static inline unsigned nblk(uint64_t n, int bs) { return (unsigned)((n + bs - 1) / bs); }
-static inline int bits_for(uint64_t maxval) {
-    int b = 1;
-    while (b < 64 && (maxval >> b)) b++;
-    return b;
-}
-
 __global__ void k_split(const syl_survivor *__restrict__ sv, uint64_t n, uint64_t *__restrict__ key,
                         uint64_t *__restrict__ hash) {
     uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;

@@ -14,8 +14,6 @@ namespace syl {
 constexpr uint64_t ING_SLICE = 256ull << 10;       // bases per work item
 constexpr uint64_t ING_OSLICE = 64ull << 10;       // offsets per work item
 
-static inline unsigned nblk(uint64_t n, int bs) { return (unsigned)((n + bs - 1) / bs); }
-
 __global__ void k_off32_to_64(const uint32_t *__restrict__ in, uint64_t n, uint64_t *__restrict__ out) {
     const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (i < n) out[i] = in[i];
@@ -274,11 +272,7 @@ int feed_host(syl_ctx *ctx, const Mate *m, int n_mates, const std::vector<Chunk>
     // is in flight, a chunk nobody has started is taken from the BACK and shipped as ASCII (4x the bytes, but the
     // link would idle otherwise).  Needs pinned caller memory (a pageable copy would block this thread).
     bool steal_ok = true;
-    for (int i = 0; i < n_mates; i++) {
-        cudaPointerAttributes pa;
-        if (cudaPointerGetAttributes(&pa, m[i].bases) == cudaSuccess) steal_ok = steal_ok && pa.type == cudaMemoryTypeHost;
-        else { cudaGetLastError(); steal_ok = false; }
-    }
+    for (int i = 0; i < n_mates; i++) steal_ok = steal_ok && ptr_kind(m[i].bases) == PtrKind::PINNED;
     {
         const char *e = getenv("SYL_HOST_INGEST");
         if (e && std::string(e) == "packed-only") steal_ok = false;
@@ -364,8 +358,7 @@ int feed_host(syl_ctx *ctx, const Mate *m, int n_mates, const std::vector<Chunk>
     }
     I.pool->open_gate((int64_t)1 << 60);  // all remaining items (skipped chunks included) drain
     I.pool->finish();
-    static const bool dbg = getenv("SYL_DEBUG_TIMING") != nullptr;
-    if (dbg) fprintf(stderr, "[host ingest] %zu chunks: %llu shipped as ASCII, %zu packed by %d threads\n", chunks.size(),
+    if (debug_timing()) fprintf(stderr, "[host ingest] %zu chunks: %llu shipped as ASCII, %zu packed by %d threads\n", chunks.size(),
                      (unsigned long long)ctx->ingest_chunks_ascii, chunks.size() - (size_t)ctx->ingest_chunks_ascii, I.pool->threads());
     if (rc != SYL_OK) I.drain(st);
     return rc;

@@ -681,14 +681,6 @@ __global__ void k_fallback_sizes(const uint32_t *__restrict__ g_n, const uint8_t
     if (g < ng) fsz[g] = g_fallback[g] ? g_n[g] : 0u;
 }
 
-static inline unsigned nblk(uint64_t n, int bs) { return (unsigned)((n + bs - 1) / bs); }
-
-static inline int bits_for(uint64_t maxval) {
-    int b = 1;
-    while (b < 64 && (maxval >> b)) b++;
-    return b;
-}
-
 // Accumulates events over one or more seeding batches, then finishes into a syl_sample.
 // Nothing in begin() / add() synchronises with the host: the event array is sized up front from the
 // expected number of survivors, the seeding kernel appends at a running device counter, and every
@@ -906,8 +898,7 @@ struct SampleBuilder {
         const uint64_t NF_slots = ng ? ctx->h_counters[CNT_FALLBACK_TOTAL] : 0;
         const uint64_t NF = NF_slots + N_ovf;
         uint64_t ndup = ctx->h_counters[CNT_DUPS];
-        static const bool dbg = getenv("SYL_DEBUG_TIMING") != nullptr;
-        if (dbg) fprintf(stderr, "[sample post-pass] groups %u of %u slots, overflow list %llu (cap %llu): in-kernel uniques %llu, events handed to the generic path %llu (%.2f %% of the slotted events)\n",
+        if (debug_timing()) fprintf(stderr, "[sample post-pass] groups %u of %u slots, overflow list %llu (cap %llu): in-kernel uniques %llu, events handed to the generic path %llu (%.2f %% of the slotted events)\n",
                          ng, slot, (unsigned long long)N_ovf, (unsigned long long)cap, (unsigned long long)U1, (unsigned long long)NF,
                          n_slots ? 100.0 * (double)NF_slots / (double)n_slots : 0.);
         // the generic path: fallback groups (heavy-hitter k-mers, duplicate-heavy replays) and the overflow list
@@ -1056,7 +1047,6 @@ static int sketch_reads_impl(syl_ctx *ctx, int mem, bool packed, const Mate *m, 
     }
     // the mean length of mate 1 (for pairs src/sketch.rs:824-826)
     const double mean_read_length = n_reads ? (double)m[0].nb / (double)n_reads : 0.;
-    static const bool dbg = getenv("SYL_DEBUG_TIMING") != nullptr;
     auto now = []() { return std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now().time_since_epoch()).count(); };
     uint64_t h2d = staged_bytes, n_packed = 0, n_ascii = 0;  // host ingest of the parts so far
     std::vector<uint64_t> all_hash;  // the sketches of the parts so far (P > 1)
@@ -1092,7 +1082,7 @@ static int sketch_reads_impl(syl_ctx *ctx, int mem, bool packed, const Mate *m, 
             const double t1 = now();
             uint64_t need = 0;
             rc = b.finish(&ps, &need);
-            if (dbg) fprintf(stderr, "[%s] feed %.2f ms, finish %.2f ms (attempt %d)%s\n",
+            if (debug_timing()) fprintf(stderr, "[%s] feed %.2f ms, finish %.2f ms (attempt %d)%s\n",
                              n_mates == 2 ? "syl_sketch_read_pairs" : "syl_sketch_reads", t1 - t0, now() - t1, attempt,
                              P > 1 ? (", part " + std::to_string(p + 1) + "/" + std::to_string(P)).c_str() : "");
             if (rc == SYL_ERR_CAPACITY) cap_override = need + 16;  // more events than estimated: redo with the exact size

@@ -39,7 +39,7 @@ from oracle import pyref as R
 
 K = 31
 MAX_KEY = 2**64 - 2       # largest legal key: u64::MAX is the oracle's empty-slot marker
-COV_BINS = 256            # contain.cu: a count >= 256 sends the call through the CSR formulation
+COV_BINS = 256            # contain.hpp: a count >= 256 sends the call through the CSR formulation
 BOOT_PYREF_MAX = 5000     # pyref bootstraps rows up to this many genome k-mers (100 * n Python draws)
 REPLAY_MAX = 20000        # SYL_BOOT_REPLAY: one thread replays 100 * n draws per row
 LOW, HIGH, LAMBDA = 0, 1, 2

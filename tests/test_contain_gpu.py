@@ -244,7 +244,7 @@ def deep_coverage_case(ctx, depth):
 def test_deep_coverage_uploaded_sample(ctx, depth):
     """Coverage around the 256-bin limit of the per-pair count histograms: up to 255 the histogram
     formulation of get_stats answers, from 256 on the call is redone in the CSR formulation
-    (contain.cu COV_BINS); medians >= 30 take the no-cutoff branch (src/contain.rs:664)."""
+    (contain.hpp COV_BINS); medians >= 30 take the no-cutoff branch (src/contain.rs:664)."""
     g, d, (sh, sc), smp = deep_coverage_case(ctx, depth)
     db = ctx.build_db(g)
     exp = oracle_rows(d, (sh, sc), False)

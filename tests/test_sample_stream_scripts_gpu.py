@@ -43,7 +43,7 @@ MEMS = {"pageable": (False, False), "pinned": (True, True), "hash_pinned": (True
 
 
 def row_bytes():
-    """contain.cu ROW_BYTES: two row tables, the bootstrap's results and its histogram"""
+    """contain.hpp ROW_BYTES: two row tables, the bootstrap's results and its histogram"""
     from sylph_b200.api import ANI_ROW_DTYPE
     return 2 * ANI_ROW_DTYPE.itemsize + 100 * 17 + 17 * 4 + 8
 
