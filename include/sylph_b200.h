@@ -39,7 +39,7 @@
 extern "C" {
 #endif
 
-#define SYL_ABI_VERSION 2
+#define SYL_ABI_VERSION 3
 
 enum {
     SYL_OK = 0,
@@ -261,9 +261,6 @@ int syl_genomes_upload(syl_ctx *ctx, int mem, const uint64_t *kmers, const uint6
 /* Concatenate batches (database build in chunks): genome i of part p becomes genome
  * (sum of earlier parts' counts) + i.  All parts must agree on k, c and has_tracked. */
 int syl_genomes_concat(syl_ctx *ctx, const syl_genomes *const *parts, uint32_t n_parts, syl_genomes **out);
-/* New batch holding genomes idx[0..n) of g (host index array), e.g. the pass-1 survivors of a
- * shard that are gathered into a small survivor database for the multi-GPU profile. */
-int syl_genomes_select(syl_ctx *ctx, const syl_genomes *g, const uint32_t *idx, uint32_t n, syl_genomes **out);
 uint64_t syl_genomes_count(const syl_genomes *g);
 uint64_t syl_genomes_total_kmers(const syl_genomes *g);
 uint64_t syl_genomes_total_tracked(const syl_genomes *g);
@@ -383,14 +380,20 @@ int syl_profile(syl_ctx *ctx, const syl_db *db, const syl_sample *const *samples
  *     rows_per_rank == 0 takes the default, 256 + 96 * n_samples rounded up to a multiple of 256 when world > 1:
  *     it does not depend on the shard, so every rank's table has the same size.  A rank whose shard holds no
  *     genome runs every stage (zeroed table headers, no winner candidates) and takes part in every collective.
- *     SYL_ERR_CAPACITY from finish: redo with rows_per_rank >= *need_rows_per_rank (same verdict on every
- *     rank).  SYL_ERR_UNSUPPORTED: a k-mer count >= 256 was met (every rank sees it); use the gathered-
- *     survivor path (sylph_b200/dist.py profile_sharded_gather).  world == 1 is allowed (no collectives).
+ *
+ *     Each rank picks its own join formulation in begin: the per-pair count histograms, or the CSR formulation
+ *     when csr != 0, when SYL_CONTAIN_CSR is set or when its shard's histograms would exceed 8 GB (samples x
+ *     shard genomes > 2^23 pairs).  Both write the same row tables, so ranks may run different formulations.
+ *     CSR adds one host synchronisation inside begin, before the first collective.
+ *
+ *     SYL_ERR_CAPACITY from finish: redo with rows_per_rank >= *need_rows_per_rank.  SYL_ERR_UNSUPPORTED from
+ *     finish: a histogram rank met a k-mer count >= 256; redo the job with csr = 1.  Both verdicts come from the
+ *     gathered table headers, so every rank reaches the same one.  world == 1 is allowed (no collectives).
  * ---------------------------------------------------------------------------------------- */
 typedef struct syl_profile_job syl_profile_job;
 int syl_profile_shard_begin(syl_ctx *ctx, const syl_db *db, const syl_sample *const *samples, uint32_t n_samples,
                             const syl_contain_params *p, uint32_t world, uint32_t rank, uint64_t rows_per_rank,
-                            syl_profile_job **out);
+                            int csr, syl_profile_job **out);
 int syl_profile_job_buffers(const syl_profile_job *job, void **d_table1, void **d_gathered1, uint64_t *table_bytes,
                             void **d_winner, uint64_t *winner_elems, void **d_table2, void **d_gathered2);
 int syl_profile_shard_rank(syl_profile_job *job);

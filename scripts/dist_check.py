@@ -1,6 +1,6 @@
 """Run under torchrun (N ranks, one GPU each): query / profile over a genome-sharded db must equal the single-GPU
-result on the whole db — for the three-collective profile (dist.profile_sharded) and for the gathered-survivor
-formulation (dist.profile_sharded_gather).  The samples' communities are spread over ALL shards.
+result on the whole db — for the three-collective profile (dist.profile_sharded) in the formulation each rank picks
+and with every rank in the CSR formulation (SYL_CONTAIN_CSR=1).  The samples' communities are spread over ALL shards.
   python -m torch.distributed.run --nnodes=1 --nproc-per-node 2 --master-addr 127.0.0.1 --master-port 29511 scripts/dist_check.py
 """
 import os
@@ -48,7 +48,11 @@ def main():
             samples.append(ctx.sketch_sequences(rb, ro, c=c))
         q = D.query_sharded(ctx, db, samples)
         p = D.profile_sharded(ctx, genomes, db, samples, b0)
-        pg = D.profile_sharded_gather(ctx, genomes, db, samples, b0)
+        prev = os.environ.get("SYL_CONTAIN_CSR")
+        os.environ["SYL_CONTAIN_CSR"] = "1"         # read by the library per call
+        pc = D.profile_sharded(ctx, genomes, db, samples, b0)
+        if prev is None:
+            del os.environ["SYL_CONTAIN_CSR"]
         if rank == 0:  # single-GPU reference with the whole db
             fb, fo = synth.db_chunk(0, G, glen, device="cuda")
             fg = ctx.sketch_genomes(fb, fo, torch.arange(G + 1, dtype=torch.int64, device="cuda"), c=c)
@@ -56,7 +60,7 @@ def main():
             q1 = ctx.query(fdb, samples, contain_params(pseudotax=False))
             p1 = ctx.profile(fdb, samples, contain_params(pseudotax=True))
             shards_hit = len(set(int(g) * world // G for g in p1["genome"]))
-            for name, a, b in (("query", q, q1), ("profile (3 collectives)", p, p1), ("profile (gathered survivors)", pg, p1)):
+            for name, a, b in (("query", q, q1), ("profile (3 collectives)", p, p1), ("profile (3 collectives, CSR)", pc, p1)):
                 same = same_rows(a, b)
                 print("G=%d c=%d %s: sharded(%d ranks) rows=%d single rows=%d genomes from %d shards equal=%s"
                       % (G, c, name, world, len(a), len(b), shards_hit, same), flush=True)

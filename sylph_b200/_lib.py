@@ -86,7 +86,6 @@ SIGNATURES = {
     "syl_sketch_genomes_packed2": (_i, [_vp, _i, _vp, _u64, _vp, _u64, _vp, _u64, _i, _u64, _u64, _i, _i, _i, _pp]),
     "syl_genomes_upload": (_i, [_vp, _i, _vp, _vp, _vp, _vp, _vp, _u64, _i, _u64, _pp]),
     "syl_genomes_concat": (_i, [_vp, _pp, _u32, _pp]),
-    "syl_genomes_select": (_i, [_vp, _vp, _vp, _u32, _pp]),
     "syl_genomes_count": (_u64, [_vp]),
     "syl_genomes_total_kmers": (_u64, [_vp]),
     "syl_genomes_total_tracked": (_u64, [_vp]),
@@ -104,7 +103,7 @@ SIGNATURES = {
     "syl_contain_params_default": (None, [C.POINTER(ContainParams), _i, _i]),
     "syl_query": (_i, [_vp, _vp, _pp, _u32, C.POINTER(ContainParams), _vp, _u64, _pu64]),
     "syl_profile": (_i, [_vp, _vp, _pp, _u32, C.POINTER(ContainParams), _vp, _u64, _pu64]),
-    "syl_profile_shard_begin": (_i, [_vp, _vp, _pp, _u32, C.POINTER(ContainParams), _u32, _u32, _u64, _pp]),
+    "syl_profile_shard_begin": (_i, [_vp, _vp, _pp, _u32, C.POINTER(ContainParams), _u32, _u32, _u64, _i, _pp]),
     "syl_profile_job_buffers": (_i, [_vp, _pp, _pp, _pu64, _pp, _pu64, _pp, _pp]),
     "syl_profile_shard_rank": (_i, [_vp]),
     "syl_profile_shard_pass2": (_i, [_vp]),

@@ -287,12 +287,6 @@ class Context:
         _lib.check(_lib.lib().syl_genomes_concat(self._h, arr, len(parts), C.byref(h)))
         return Genomes(self, h)
 
-    def select_genomes(self, genomes, idx):
-        a = np.ascontiguousarray(idx, dtype=np.uint32)
-        h = C.c_void_p()
-        _lib.check(_lib.lib().syl_genomes_select(self._h, genomes._h, a.ctypes.data_as(C.c_void_p), len(a), C.byref(h)))
-        return Genomes(self, h)
-
     # ---- (4) containment ---------------------------------------------------------------------
     def build_db(self, genomes, genome_base=0):
         """Index a batch of genome sketches for probing (syl_db_build)."""
@@ -345,14 +339,15 @@ class Context:
         params = params or contain_params(pseudotax=False)
         return self._pairs(_lib.lib().syl_query, db, samples, params, cap)
 
-    def profile_shard_begin(self, db, samples, params=None, world=1, rank=0, rows_per_rank=0):
-        """Stage 1 of `profile` over a genome-sharded db (pass 1 on this rank's shard) -> ProfileJob."""
+    def profile_shard_begin(self, db, samples, params=None, world=1, rank=0, rows_per_rank=0, csr=False):
+        """Stage 1 of `profile` over a genome-sharded db (pass 1 on this rank's shard) -> ProfileJob.  csr=True forces
+        the CSR formulation (needed after finish reported SYL_ERR_UNSUPPORTED)."""
         _CTX_STREAM[0] = self._stream
         params = params or contain_params(pseudotax=True)
         arr = (C.c_void_p * max(len(samples), 1))(*[s._h for s in samples])
         h = C.c_void_p()
         _lib.check(_lib.lib().syl_profile_shard_begin(self._h, db._h, arr, len(samples), C.byref(params), int(world), int(rank),
-                                                      int(rows_per_rank), C.byref(h)))
+                                                      int(rows_per_rank), int(bool(csr)), C.byref(h)))
         return ProfileJob(self, h, int(world))
 
     def profile(self, db, samples, params=None, cap=None):

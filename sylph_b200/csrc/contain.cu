@@ -732,13 +732,14 @@ static StatParams make_params(const syl_contain_params *p) {
 //   [N ranks: the caller all-gathers the pass-2 row tables — collective 3]
 //   finish      D2H of the table(s), derep_if_reassign_threshold (:353-375), abundances (:319-326), sort
 // Single GPU: the winner minimum is taken inside k_join2_order and nothing is gathered.  A coverage
-// count >= COV_BINS or more rows than the table holds is reported in the header; contain_fast then
+// count >= COV_BINS or more rows than the table holds is reported in the header; the caller then
 // redoes the call in the CSR formulation or with a larger table.
-// CSR formulation (single GPU only): k_join_hist<probe only> records the equal ranges and
-// k_join2_order<.., CSR_*> walks them twice per pass (count hits per pair, CUB scan, scatter the hits'
-// sample counts), with no winner in pass 1; k_stats replaces k_stats_hist; ranking, bootstrap and finish
-// are shared.  Sizing the value array after the pass-1 scan costs a second host synchronisation; pass 2
-// needs none, because its hits are a subset of pass 1's (same ranges, winners only).
+// CSR formulation: k_join_hist<probe only> records the equal ranges and k_join2_order<.., CSR_*> walks
+// them twice per pass (count hits per pair, CUB scan, scatter the hits' sample counts), with no winner in
+// pass 1; k_stats replaces k_stats_hist; ranking, bootstrap and finish are shared.  Sizing the value
+// array after the pass-1 scan costs a second host synchronisation, inside stage 1 (before any collective);
+// pass 2 needs none, because its hits are a subset of pass 1's (same ranges, winners only).  Both
+// formulations write the same row tables, so the ranks of a sharded profile may each run either one.
 constexpr uint32_t ORD_NONE = 0x7F7F7F7Fu;  // memset-able; valid as int32 for the MIN all-reduce
 
 struct ShardTable { unsigned long long n_rows, n_boot, ovf, pad; };
@@ -866,7 +867,7 @@ struct syl_profile_job {
     uint32_t S = 0, world = 1, rank = 0;
     uint64_t G = 0, R = 0, max_n = 0, tbytes = 0;
     int stage = 0;           // 1 pass 1 enqueued, 2 ranked, 3 pass 2 enqueued
-    bool csr = false;        // CSR formulation (single GPU) instead of the per-pair count histograms
+    bool csr = false;        // CSR formulation instead of the per-pair count histograms
     syl::JoinRoom *room = nullptr;  // bound on the CSR hit values (host-sample batches only)
     syl::DevBuf<syl::SampleView> views;
     syl::DevBuf<uint8_t> touched, tab1, gat1, tab2, gat2, res_ok, scan_tmp;
@@ -919,15 +920,13 @@ static int clear_pairs(syl_profile_job *j) {
 
 // One walk over the equal ranges in j->hits into OUT.  Pass 1 walks only in the CSR formulation (the histogram one
 // accumulates inside the probe) and counts every kept hit.  Pass 2 counts the winner's hits, with the winner taken in
-// the walk on one GPU and from the all-reduced wbest across ranks (histogram formulation only).
+// the walk on one GPU and from the all-reduced wbest across ranks.
 template <JoinOut OUT>
 static void join_walk(syl_profile_job *j, bool pass2) {
     const syl_db *db = j->db;
     if (!j->max_n || !db->N) return;
-    auto k = k_join2_order<WIN_FUSED, OUT>;
-    if constexpr (OUT == JOIN_HIST) {
-        if (j->world > 1) k = k_join2_order<WIN_GIVEN, OUT>;
-    } else {
+    auto k = j->world > 1 ? k_join2_order<WIN_GIVEN, OUT> : k_join2_order<WIN_FUSED, OUT>;
+    if constexpr (OUT != JOIN_HIST) {
         if (!pass2) k = k_join2_order<WIN_NONE, OUT>;
     }
     KernelTimer kt(j->ctx, pass2 ? SYL_KERNEL_JOIN2 : SYL_KERNEL_JOIN);
@@ -979,8 +978,10 @@ static int enqueue_stats(syl_profile_job *j, const StatParams &P, bool pass2, vo
     return SYL_OK;
 }
 
-// stage 1: allocate, pass 1 (P1 = the pass-1 parameters: profile skips the bootstrap there).  csr: the CSR formulation
-// (single GPU only); otherwise histograms beyond 8 GB are SYL_ERR_UNSUPPORTED.
+// stage 1: allocate, pass 1 (P1 = the pass-1 parameters: profile skips the bootstrap there).  The one place that picks
+// the formulation: CSR when the caller asks for it (a histogram run met a count >= COV_BINS), when SYL_CONTAIN_CSR is
+// set (read per call) or when this job's per-pair histograms would exceed 8 GB.  The choice is local to the job: the
+// ranks of a sharded profile may pick differently.
 static int job_begin(syl_ctx *ctx, const syl_db *db, const SampleView *views, const SampleMeta *metas, uint32_t n_samples,
                      const syl_contain_params *p, bool profile, bool csr, uint32_t world, uint32_t rank, uint64_t R,
                      syl_profile_job **out, JoinRoom *room = nullptr) {
@@ -988,6 +989,8 @@ static int job_begin(syl_ctx *ctx, const syl_db *db, const SampleView *views, co
     Handle<syl_profile_job> h(new (std::nothrow) syl_profile_job());
     if (!h) return SYL_ERR_OOM;
     syl_profile_job *j = h.get();
+    const uint64_t NP = (uint64_t)n_samples * db->n_genomes;
+    csr = csr || getenv("SYL_CONTAIN_CSR") != nullptr || !histograms_fit(NP);
     j->ctx = ctx; j->db = db; j->profile = profile; j->csr = csr; j->S = n_samples; j->G = db->n_genomes; j->world = world; j->rank = rank;
     j->room = room;
     syl_contain_params pp = *p;
@@ -998,9 +1001,7 @@ static int job_begin(syl_ctx *ctx, const syl_db *db, const SampleView *views, co
     j->R = R ? ((R + 255) & ~255ull) : default_rows_per_rank(n_samples, db->n_genomes, world);
     j->tbytes = table_bytes(j->R);
     if (j->R * BOOT_ITERS >= 0xFFFF0000ull) { set_error("row capacity too large for the bootstrap work counter"); return SYL_ERR_ARG; }
-    const uint64_t NP = (uint64_t)j->S * j->G;
     if (NP >= 0x7FFFFFFFull) { set_error("samples x genomes exceeds 2^31 pairs per call; split the sample batch"); return SYL_ERR_ARG; }
-    if (!csr && !histograms_fit(NP)) { set_error("pair histograms exceed 8 GB; split the sample batch"); return SYL_ERR_UNSUPPORTED; }
     std::vector<SampleView> hv(views, views + n_samples);
     for (const SampleView &v : hv) j->max_n = std::max<uint64_t>(j->max_n, v.n);
     const uint64_t HN = std::max<uint64_t>((uint64_t)j->S * j->max_n, 1);
@@ -1223,9 +1224,9 @@ static int job_finish(syl_profile_job *j, std::vector<syl_ani_row> &out, uint64_
     return SYL_OK;
 }
 
-// single-GPU driver of the stages for syl_query / syl_profile.  The CSR formulation is taken up front when
-// SYL_CONTAIN_CSR is set (read per call) or the per-pair histograms would exceed 8 GB, and after a histogram
-// run that met a count >= COV_BINS; a row table that is too small is redone with the size it needed.
+// single-GPU driver of the stages for syl_query / syl_profile.  A histogram run that met a count >= COV_BINS is redone
+// in the CSR formulation (job_begin may also take it up front); a row table that is too small is redone with the size
+// it needed.
 // `overlap`, when given, runs once, after the first attempt's stages are enqueued and before its result is awaited (the
 // host samples stage their next batch there).  `room` (host-sample batches) bounds what the joins allocate beyond the
 // batch's plan: CSR hit values or a capacity retry's row tables that do not fit it rerun the samples as two halves on
@@ -1234,7 +1235,7 @@ int contain_fast(syl_ctx *ctx, const syl_db *db, const SampleView *views, const 
                  const syl_contain_params *p, bool profile, std::vector<syl_ani_row> &out, const std::function<int()> &overlap,
                  JoinRoom *room) {
     uint64_t R = 0;
-    bool csr = getenv("SYL_CONTAIN_CSR") != nullptr || !histograms_fit((uint64_t)n_samples * db->n_genomes);
+    bool csr = false;
     bool overlapped = false;
     for (int attempt = 0; attempt < 4; attempt++) {  // one formulation switch + capacity retries
         syl_profile_job *j = nullptr;
@@ -1307,7 +1308,7 @@ void syl_contain_params_default(syl_contain_params *p, int k, int pseudotax) {
 }
 
 int syl_profile_shard_begin(syl_ctx *ctx, const syl_db *db, const syl_sample *const *samples, uint32_t n_samples,
-                            const syl_contain_params *p, uint32_t world, uint32_t rank, uint64_t rows_per_rank,
+                            const syl_contain_params *p, uint32_t world, uint32_t rank, uint64_t rows_per_rank, int csr,
                             syl_profile_job **out) {
     uint64_t dummy = 0;
     if (!out || !db) { set_error("NULL argument"); return SYL_ERR_ARG; }
@@ -1318,7 +1319,7 @@ int syl_profile_shard_begin(syl_ctx *ctx, const syl_db *db, const syl_sample *co
     std::vector<SampleView> views;
     std::vector<SampleMeta> metas;
     SYL_TRY(handle_views(ctx, samples, n_samples, p->estimate_unknown != 0, views, metas));
-    return job_begin(ctx, db, views.data(), metas.data(), n_samples, p, true, false, world, rank, rows_per_rank, out);
+    return job_begin(ctx, db, views.data(), metas.data(), n_samples, p, true, csr != 0, world, rank, rows_per_rank, out);
 }
 
 int syl_profile_job_buffers(const syl_profile_job *j, void **d_table1, void **d_gathered1, uint64_t *table_bytes,

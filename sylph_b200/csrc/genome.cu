@@ -93,18 +93,6 @@ __global__ void k_add_offset(const uint64_t *__restrict__ src, uint64_t n, uint6
     if (i < n) dst[i] = src[i] + add;
 }
 
-// block i copies genome i's k-mer and tracked ranges: src4 = {src_k, dst_k, src_t, dst_t} starts
-__global__ void k_copy_ranges(const uint64_t *__restrict__ src4, const uint64_t *__restrict__ kmers,
-                              const uint64_t *__restrict__ tracked, uint64_t *__restrict__ okmers,
-                              uint64_t *__restrict__ otracked, const uint64_t *__restrict__ okoff,
-                              const uint64_t *__restrict__ otoff) {
-    const uint64_t i = blockIdx.x;
-    const uint64_t sk = src4[4 * i], dk = src4[4 * i + 1], st = src4[4 * i + 2], dt = src4[4 * i + 3];
-    const uint64_t nk = okoff[i + 1] - okoff[i], nt = otoff[i + 1] - otoff[i];
-    for (uint64_t j = threadIdx.x; j < nk; j += blockDim.x) okmers[dk + j] = kmers[sk + j];
-    for (uint64_t j = threadIdx.x; j < nt; j += blockDim.x) otracked[dt + j] = tracked[st + j];
-}
-
 // the arrays of a handle from new_handle: blocks of its owner's cache
 static int genomes_alloc(syl_genomes *g, uint64_t n_genomes, uint64_t nk, uint64_t nt) {
     SYL_TRY(hblock_alloc(g->owner, (void **)&g->kmers, std::max<uint64_t>(nk, 1) * 8));
@@ -602,46 +590,6 @@ int syl_genomes_concat(syl_ctx *ctx, const syl_genomes *const *parts, uint32_t n
     if (n_parts) { g->k = parts[0]->k; g->c = parts[0]->c; g->has_tracked = parts[0]->has_tracked; }
     SYL_TRY(genomes_concat_into(ctx, parts, n_parts, g.get()));
     *out = g.release();
-    return SYL_OK;
-}
-
-int syl_genomes_select(syl_ctx *ctx, const syl_genomes *g, const uint32_t *idx, uint32_t n, syl_genomes **out) {
-    if (!ctx || !g || !out || (n && !idx)) { set_error("NULL argument"); return SYL_ERR_ARG; }
-    *out = nullptr;
-    SYL_ENTER(ctx);
-    cudaStream_t st = ctx->stream;
-    std::vector<uint64_t> koff(g->n + 1), toff(g->n + 1), gs(std::max<uint64_t>(g->n, 1));
-    SYL_CUDA(cudaMemcpyAsync(koff.data(), g->kmer_off, (g->n + 1) * 8, cudaMemcpyDeviceToHost, st));
-    SYL_CUDA(cudaMemcpyAsync(toff.data(), g->tracked_off, (g->n + 1) * 8, cudaMemcpyDeviceToHost, st));
-    if (g->n) SYL_CUDA(cudaMemcpyAsync(gs.data(), g->gn_size, g->n * 8, cudaMemcpyDeviceToHost, st));
-    SYL_CUDA(cudaStreamSynchronize(st));
-    std::vector<uint64_t> nko(n + 1, 0), nto(n + 1, 0), ngs(std::max<uint32_t>(n, 1)), src(4 * (uint64_t)std::max<uint32_t>(n, 1));
-    for (uint32_t i = 0; i < n; i++) {
-        if (idx[i] >= g->n) { set_error("genome index out of range"); return SYL_ERR_ARG; }
-        const uint64_t a = idx[i];
-        nko[i + 1] = nko[i] + (koff[a + 1] - koff[a]);
-        nto[i + 1] = nto[i] + (toff[a + 1] - toff[a]);
-        ngs[i] = gs[a];
-        src[4 * i] = koff[a]; src[4 * i + 1] = nko[i]; src[4 * i + 2] = toff[a]; src[4 * i + 3] = nto[i];
-    }
-    Handle<syl_genomes> o = new_handle<syl_genomes>(ctx);
-    if (!o) return SYL_ERR_OOM;
-    o->k = g->k; o->c = g->c; o->has_tracked = g->has_tracked;
-    SYL_TRY(genomes_alloc(o.get(), n, nko[n], nto[n]));
-    DevBuf<uint64_t> d_src;
-    SYL_TRY(d_src.alloc(4 * (uint64_t)std::max<uint32_t>(n, 1), st));
-    SYL_CUDA(cudaMemcpyAsync(o->kmer_off, nko.data(), (n + 1) * 8, cudaMemcpyHostToDevice, st));
-    SYL_CUDA(cudaMemcpyAsync(o->tracked_off, nto.data(), (n + 1) * 8, cudaMemcpyHostToDevice, st));
-    if (n) {
-        SYL_CUDA(cudaMemcpyAsync(o->gn_size, ngs.data(), (size_t)n * 8, cudaMemcpyHostToDevice, st));
-        SYL_CUDA(cudaMemcpyAsync(d_src.p, src.data(), (size_t)n * 32, cudaMemcpyHostToDevice, st));
-        k_copy_ranges<<<n, 256, 0, st>>>(d_src.p, g->kmers, g->tracked, o->kmers,
-                                         o->tracked, o->kmer_off, o->tracked_off);
-        ctx->launches++;
-        SYL_CUDA(cudaGetLastError());
-    }
-    SYL_CUDA(cudaStreamSynchronize(st));
-    *out = o.release();
     return SYL_OK;
 }
 

@@ -9,9 +9,11 @@ CPU tests).  The path shards naturally:
                 pass 1 per shard -> all_gather of the per-rank row tables
                 order of the survivors + per-key local winner -> all_reduce(MIN) of the winner array
                 pass 2 per shard + bootstrap -> all_gather of the pass-2 row tables -> host finish
-              profile_sharded_gather is the round-1 formulation (pass-1 survivors' sketches gathered into a
-              small survivor db on every rank); it remains as the fallback for samples with k-mer counts
-              >= 256 (CSR formulation) and as an independent cross-check in the tests.
+              every rank picks its own join formulation; a k-mer count >= 256 makes every rank redo the job
+              in the CSR formulation.
+  sketches  : gather_survivor_genomes (with all_gather_bytes / all_gather_device) gathers genome sketches of
+              every rank into one database, identical on every rank; bench.py's multi-GPU parity step gathers
+              the whole database with it to compare the sharded profile with a single-GPU one.
 
 torch is plumbing here (process group, collectives); all compute goes through the C ABI.
 """
@@ -124,7 +126,7 @@ def gather_survivor_genomes(sub, global_ids):
 def profile_sharded(ctx, genomes, db, samples, genome_base, params=None, rows_per_rank=0):
     """`sylph profile` over a genome-sharded db: three collectives (module docstring).  Returns all rows on
     every rank, per sample sorted by rel_abund descending; row.genome is the GLOBAL genome id.
-    `genomes` / `genome_base` are only used by the fallback (profile_sharded_gather)."""
+    `genomes` and `genome_base` are unused; they stay because existing callers (bench.py) pass them."""
     import torch
     import torch.distributed as dist
     from . import _lib
@@ -141,8 +143,9 @@ def profile_sharded(ctx, genomes, db, samples, genome_base, params=None, rows_pe
             ctx.sync()
             torch.cuda.current_stream().synchronize()
 
-    for _ in range(4):
-        job = ctx.profile_shard_begin(db, samples, params, world, rank, rows_per_rank)
+    csr = False
+    for _ in range(4):   # one formulation switch + capacity retries, as in the single-GPU driver
+        job = ctx.profile_shard_begin(db, samples, params, world, rank, rows_per_rank, csr)
         try:
             b = job.buffers()
             if world > 1:
@@ -164,51 +167,12 @@ def profile_sharded(ctx, genomes, db, samples, genome_base, params=None, rows_pe
             job.free()
         if rc == _lib.SYL_OK:
             return rows
-        if rc == _lib.SYL_ERR_CAPACITY:          # same verdict on every rank: redo with a larger row table
+        # every rank reaches the same verdict (the table headers were gathered)
+        if rc == _lib.SYL_ERR_CAPACITY:          # redo with a larger row table
             rows_per_rank = need + 256
-            continue
-        return profile_sharded_gather(ctx, genomes, db, samples, genome_base, params)   # SYL_ERR_UNSUPPORTED
+        elif rc == _lib.SYL_ERR_UNSUPPORTED and not csr:   # a count >= 256: redo in the CSR formulation
+            csr = True
+        else:
+            _lib.check(rc)
     raise RuntimeError("profile_sharded: row table kept overflowing")
 
-
-def profile_sharded_gather(ctx, genomes, db, samples, genome_base, params=None):
-    """Round-1 formulation of the sharded profile: pass 1 per shard, the pass-1 survivors' sketches are
-    gathered into a small survivor db on every rank, the exact two-pass profile of sample s runs on rank
-    s % world, rows all-gathered.  ~14 collectives; handles every input (CSR formulation included)."""
-    import torch.distributed as dist
-    rank = dist.get_rank() if dist.is_initialized() else 0
-    world = dist.get_world_size() if dist.is_initialized() else 1
-    params = params or contain_params(pseudotax=True)
-    params.pseudotax = 1
-    p1 = contain_params(k=params.k, pseudotax=True)
-    for f, _ in params._fields_:
-        setattr(p1, f, getattr(params, f))
-    p1.no_ci = 1                                                # pass-1 CIs are never reported
-    rows1 = ctx.query(db, samples, p1)                          # pass 1 on the shard (profile ANI gate)
-    local_ids = np.unique(rows1["genome"].astype(np.int64) - int(genome_base)).astype(np.uint32)
-    sub = ctx.select_genomes(genomes, local_ids)
-    on_gpu = dist.is_initialized() and dist.get_backend() == "nccl"
-    merged, gids = gather_survivor_genomes(sub.device_tensors() if on_gpu else sub.download(),
-                                           local_ids.astype(np.uint64) + np.uint64(genome_base))
-    if on_gpu:
-        import torch
-        torch.cuda.current_stream().synchronize()  # the gathered copies are complete before `sub` goes away
-    sub.free()
-    out = np.zeros(0, dtype=ANI_ROW_DTYPE)
-    if len(gids):
-        g = ctx.upload_genomes(merged["kmers"], merged["kmer_off"], merged["tracked"], merged["tracked_off"],
-                               merged["gn_size"], k=params.k, c=genomes.c)
-        sdb = ctx.build_db(g)
-        mine = [i for i in range(len(samples)) if i % world == rank]
-        if mine:
-            out = ctx.profile(sdb, [samples[i] for i in mine], params)
-            out["sample"] = np.array(mine, dtype=np.uint32)[out["sample"]]
-            out["genome"] = gids[out["genome"]].astype(np.uint32)
-        sdb.free()
-        g.free()
-    parts = [p for p in all_gather_bytes(out) if len(p)]
-    if not parts:
-        return np.zeros(0, dtype=ANI_ROW_DTYPE)
-    rows = np.concatenate(parts)
-    order = np.lexsort((-rows["rel_abund"], rows["sample"]))  # stable: per sample by abundance desc
-    return rows[order]

@@ -23,7 +23,7 @@ def test_header_symbols_all_exported_and_bound():
     for n in names:
         assert hasattr(lib, n), "library does not export " + n
         assert n in _lib.SIGNATURES, "python binding misses " + n
-    assert lib.syl_abi_version() == 2
+    assert lib.syl_abi_version() == 3
 
 
 def test_struct_layouts_match_header():

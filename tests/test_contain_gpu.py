@@ -321,29 +321,36 @@ def test_estimate_unknown_with_read_seq_id(ctx, pseudotax):
     assert e.value.code == 5                                          # SYL_ERR_UNSUPPORTED
 
 
-def test_sharded_profile_deep_coverage_on_one_gpu(ctx):
-    """A count >= 256 makes the three-collective sharded profile (world = 1) report SYL_ERR_UNSUPPORTED;
-    profile_sharded then takes profile_sharded_gather, whose query / profile calls run the CSR formulation.
-    The result must equal syl_profile field for field."""
+def test_sharded_profile_deep_coverage_on_one_gpu(ctx, contain_mode):
+    """A count >= 256 makes a histogram job of the three-collective sharded profile (world = 1) report
+    SYL_ERR_UNSUPPORTED; a job with csr = 1, or any job under SYL_CONTAIN_CSR ("synchronous"), returns syl_profile's
+    rows, and so does profile_sharded, which redoes the job with csr = 1.  Field for field."""
     from sylph_b200 import _lib
     from sylph_b200 import dist as D
     from sylph_b200.api import contain_params
     g, _, _, smp = deep_coverage_case(ctx, 700)
     db = ctx.build_db(g)
     P = contain_params(pseudotax=True)
-    job = ctx.profile_shard_begin(db, [smp], P, 1, 0, 0)
-    try:
-        job.rank()
-        job.pass2()
-        _, rc, _ = job.finish()
-    finally:
-        job.free()
-    assert rc == _lib.SYL_ERR_UNSUPPORTED
     exp = ctx.profile(db, [smp], P)
-    rows = D.profile_sharded(ctx, g, db, [smp], 0, P)
-    assert len(exp) >= 1 and len(rows) == len(exp)
-    for f in rows.dtype.names:
-        assert np.array_equal(rows[f], exp[f]), f
+    assert len(exp) >= 1
+    results = [D.profile_sharded(ctx, g, db, [smp], 0, P)]
+    for csr in (False, True):
+        job = ctx.profile_shard_begin(db, [smp], P, 1, 0, 0, csr=csr)
+        try:
+            job.rank()
+            job.pass2()
+            rows, rc, _ = job.finish()
+        finally:
+            job.free()
+        if csr or contain_mode == "synchronous":
+            assert rc == _lib.SYL_OK, csr
+            results.append(rows)
+        else:
+            assert rc == _lib.SYL_ERR_UNSUPPORTED
+    for got in results:
+        assert len(got) == len(exp)
+        for f in got.dtype.names:
+            assert np.array_equal(got[f], exp[f]), f
 
 
 @pytest.mark.parametrize("pseudotax", [False, True])

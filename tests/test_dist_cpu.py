@@ -94,14 +94,14 @@ class _FakeJob:
     """Stand-in for api.ProfileJob on CPU tensors: records the order of the stages and checks, stage by stage, that the
     collective before it delivered every rank's contribution (what the library's kernels rely on)."""
 
-    def __init__(self, ctx, rows_per_rank):
+    def __init__(self, ctx, rows_per_rank, csr):
         import torch
-        self.ctx, self.R = ctx, rows_per_rank if rows_per_rank else 4
+        self.ctx, self.R, self.csr = ctx, rows_per_rank if rows_per_rank else 4, csr
         w, r = ctx.world, ctx.rank
         self.b = dict(table1=torch.full((8,), 10 + r, dtype=torch.uint8), gathered1=torch.zeros(8 * w, dtype=torch.uint8),
                       winner=torch.full((5,), 1000, dtype=torch.int32), table2=torch.zeros(8, dtype=torch.uint8),
                       gathered2=torch.zeros(8 * w, dtype=torch.uint8))
-        ctx.log.append("begin(R=%d)" % self.R)
+        ctx.log.append("begin(R=%d, csr=%d)" % (self.R, self.csr))
 
     def buffers(self):
         return self.b
@@ -128,7 +128,7 @@ class _FakeJob:
         w = self.ctx.world
         assert self.b["gathered2"].view(w, 8)[:, 0].tolist() == [50 + i for i in range(w)]   # every rank's pass-2 table
         self.ctx.log.append("finish")
-        if self.ctx.mode == "unsupported":
+        if self.ctx.mode == "unsupported" and not self.csr:     # a count >= 256 in the histogram formulation
             return None, _lib.SYL_ERR_UNSUPPORTED, 0
         if self.R < 300:                                   # same verdict on every rank (the headers were gathered)
             return None, _lib.SYL_ERR_CAPACITY, 300
@@ -144,9 +144,9 @@ class _FakeCtx:
     def __init__(self, rank, world, mode):
         self.rank, self.world, self.mode, self.log, self._stream = rank, world, mode, [], 0
 
-    def profile_shard_begin(self, db, samples, params, world, rank, rows_per_rank):
+    def profile_shard_begin(self, db, samples, params, world, rank, rows_per_rank, csr):
         assert (world, rank) == (self.world, self.rank)
-        return _FakeJob(self, rows_per_rank)
+        return _FakeJob(self, rows_per_rank, csr)
 
     def sync(self):
         pass
@@ -164,16 +164,13 @@ def _worker_profile(rank, world, port, q):
         rows = D.profile_sharded(ctx, None, None, [], 0, params=object())
         assert len(rows) == world
         stage = ["rank", "pass2", "finish", "free"]
-        assert ctx.log == ["begin(R=4)"] + stage + ["begin(R=556)"] + stage, ctx.log
-        # 2. the >= 256-count case: every rank falls back to the gathered-survivor formulation
+        assert ctx.log == ["begin(R=4, csr=0)"] + stage + ["begin(R=556, csr=0)"] + stage, ctx.log
+        # 2. the >= 256-count case: every rank redoes the job in the CSR formulation, through the same collectives,
+        #    and keeps that formulation for the row-table retry that follows
         ctx = _FakeCtx(rank, world, "unsupported")
-        called = []
-        orig = D.profile_sharded_gather
-        D.profile_sharded_gather = lambda *a, **k: called.append(1) or "fallback"
-        try:
-            assert D.profile_sharded(ctx, None, None, [], 0, params=object()) == "fallback" and called == [1]
-        finally:
-            D.profile_sharded_gather = orig
+        rows = D.profile_sharded(ctx, None, None, [], 0, params=object())
+        assert len(rows) == world
+        assert ctx.log == (["begin(R=4, csr=0)"] + stage + ["begin(R=4, csr=1)"] + stage + ["begin(R=556, csr=1)"] + stage), ctx.log
         q.put((rank, "ok"))
     except Exception as e:  # pragma: no cover
         import traceback
@@ -185,7 +182,8 @@ def _worker_profile(rank, world, port, q):
 @pytest.mark.parametrize("world", [2, 3])
 def test_gloo_profile_sharded_control_flow(world):
     """The three collectives of the sharded profile sit between the library's stages in the right order, move every
-    rank's table / the minimum of the winner orders, and all ranks take the same retry / fallback decision."""
+    rank's table / the minimum of the winner orders, and all ranks take the same retry decisions (a larger row table, the
+    CSR formulation)."""
     import torch.multiprocessing as mp
     ctx = mp.get_context("spawn")
     q = ctx.Queue()

@@ -192,14 +192,15 @@ class Sharded:
         self.ranks = []
 
     def log_jobs(self):
-        """Wrap every rank's profile_shard_begin: -> per rank, one dict per job (R = table rows, rc / need of finish)."""
+        """Wrap every rank's profile_shard_begin: -> per rank, one dict per job (R = table rows, csr = the formulation the
+        caller asked for, rc / need of finish)."""
         logs = [[] for _ in self.ranks]
         for rk, log in zip(self.ranks, logs):
             begin = rk.ctx.profile_shard_begin
 
-            def logged(*a, _begin=begin, _log=log, **k):
-                job = _begin(*a, **k)
-                entry = {"R": (job.buffers()["table1"].numel() - TABLE_HEADER) // ROW_BYTES}
+            def logged(db, samples, params, world, rank, rows_per_rank, csr, _begin=begin, _log=log):
+                job = _begin(db, samples, params, world, rank, rows_per_rank, csr)
+                entry = {"R": (job.buffers()["table1"].numel() - TABLE_HEADER) // ROW_BYTES, "csr": csr}
                 _log.append(entry)
                 finish = job.finish
 
@@ -233,7 +234,7 @@ def params(pseudotax, kw):
     return contain_params(pseudotax=pseudotax, **kw)
 
 
-def run_sharded(monkeypatch, sh, kw=None, rows_per_rank=0, which=("query", "profile", "gather")):
+def run_sharded(monkeypatch, sh, kw=None, rows_per_rank=0, which=("query", "profile")):
     """The sharded calls on every rank -> {call: rows}, after checking that every rank returned the same rows."""
     from sylph_b200 import dist as D
     kw = kw or {}
@@ -244,8 +245,6 @@ def run_sharded(monkeypatch, sh, kw=None, rows_per_rank=0, which=("query", "prof
             out["query"] = D.query_sharded(rk.ctx, rk.db, rk.samples, params(False, kw))
         if "profile" in which:
             out["profile"] = D.profile_sharded(rk.ctx, rk.g, rk.db, rk.samples, rk.base, params(True, kw), rows_per_rank)
-        if "gather" in which:
-            out["gather"] = D.profile_sharded_gather(rk.ctx, rk.g, rk.db, rk.samples, rk.base, params(True, kw))
         return out
 
     res, grp = run_ranks(monkeypatch, sh.world, rank_fn)
@@ -300,6 +299,19 @@ class Whole:
         self.g.free()
 
 
+def with_csr(values):
+    """parameter sets (value, csr): every value as it is, then every value again with the id suffix -csr, where the
+    test sets SYL_CONTAIN_CSR=1 and every rank runs the CSR formulation"""
+    return [pytest.param(v, False, id=str(v)) for v in values] + [pytest.param(v, True, id="%s-csr" % v) for v in values]
+
+
+def set_csr(monkeypatch, csr):
+    if csr:
+        monkeypatch.setenv("SYL_CONTAIN_CSR", "1")
+    else:
+        monkeypatch.delenv("SYL_CONTAIN_CSR", raising=False)
+
+
 # ---- synthetic communities spread over every shard (scripts/dist_check.py) ----------------------------------------
 
 G_SYN, GLEN_SYN, C_SYN = 200, 50000, 20
@@ -337,10 +349,11 @@ def syn(ctx):
     whole.close()
 
 
-@pytest.mark.parametrize("world", [2, 3, 4, 8])
-def test_communities_over_every_shard(ctx, syn, monkeypatch, world):
+@pytest.mark.parametrize("world,csr", with_csr([2, 3, 4, 8]))
+def test_communities_over_every_shard(ctx, syn, monkeypatch, world, csr):
     """G = 200 at c = 20, three samples whose communities span every shard, shard_range splits; the shards are
     sketched by their own ranks.  The profile keeps genomes of every shard."""
+    set_csr(monkeypatch, csr)
     sh = Sharded(shard_cuts(G_SYN, world), lambda c, b0, b1: synth_genomes(c, b0, b1, GLEN_SYN, C_SYN), syn.samples)
     try:
         got, grp = run_sharded(monkeypatch, sh)
@@ -350,6 +363,60 @@ def test_communities_over_every_shard(ctx, syn, monkeypatch, world):
     shards = {int(np.searchsorted(sh.cuts, g, side="right")) - 1 for g in got["profile"]["genome"]}
     assert shards == set(range(world))
     assert [n for n, _ in grp.calls[0]].count("all_reduce") == 1        # one pass of the three-collective profile
+
+
+def test_mixed_formulations(ctx, syn, monkeypatch):
+    """The odd ranks ask for the CSR formulation and the even ranks run the histograms: the ranks' row tables meet in
+    the same collectives and give ctx.profile's rows."""
+    world = 4
+    sh = Sharded(shard_cuts(G_SYN, world), lambda cx, b0, b1: upload(cx, csr_slice(syn.d, b0, b1), C_SYN), syn.samples)
+    logs = sh.log_jobs()
+    for r in range(1, world, 2):
+        begin = sh.ranks[r].ctx.profile_shard_begin
+        sh.ranks[r].ctx.profile_shard_begin = lambda *a, _begin=begin: _begin(*a[:6], True)
+    try:
+        got, _ = run_sharded(monkeypatch, sh, which=("profile",))
+    finally:
+        sh.close()
+    assert syn.check(got) > 20
+    assert [[e["csr"] for e in lg] for lg in logs] == [[r % 2 == 1] for r in range(world)]
+
+
+HIST_PAIRS = (8 << 30) // (S.COV_BINS * 4)      # the most (sample, genome) pairs whose count histograms fit 8 GB
+
+
+def test_one_rank_past_the_histogram_limit(ctx, syn, monkeypatch):
+    """64 samples (the `syn` ones, small ones and empty ones).  Rank 0 holds 100 `syn` genomes and enough filler genomes
+    to pass the 8 GB histogram limit, rank 1 the other 100 `syn` genomes: rank 0 runs the CSR formulation, rank 1 the
+    histograms, with no error and no retry.  Each filler genome has one kept and one tracked k-mer above the FracMinHash
+    threshold, so no sample hits it.  The rows equal ctx.profile on the concatenated db and the oracle."""
+    from sylph_b200 import _lib
+    from sylph_b200 import synth
+    from sylph_b200.dist import _merge_csr
+    n_samples, half = 64, G_SYN // 2
+    n_fill = HIST_PAIRS // n_samples + 1 - half          # rank 0: 131 073 genomes
+    assert n_samples * (half + n_fill) > HIST_PAIRS >= n_samples * half
+    lo = np.uint64((2**64 - 1) // C_SYN + 1)            # sample hashes stay below (2^64 - 1) / c
+    fill = dict(kmers=lo + np.arange(0, 2 * n_fill, 2, dtype=np.uint64), kmer_off=np.arange(n_fill + 1, dtype=np.uint64),
+                tracked=lo + np.arange(1, 2 * n_fill, 2, dtype=np.uint64), tracked_off=np.arange(n_fill + 1, dtype=np.uint64),
+                gn_size=np.full(n_fill, 100000, np.uint64))
+    parts = [csr_slice(syn.d, 0, half), fill, csr_slice(syn.d, half, G_SYN)]
+    d = _merge_csr({k: [p[k] for p in parts] for k in fill})
+    small = [synth_sample(ctx, 300, synth.SEED_READS + 0x60 + i, 10, G_SYN, GLEN_SYN, C_SYN) for i in range(5)]
+    empty = SampleData(np.zeros(0, np.uint64), np.zeros(0, np.uint32), C_SYN)
+    samples = syn.samples + small + [empty] * (n_samples - len(syn.samples) - len(small))
+    whole = Whole(ctx, d, C_SYN, samples)
+    sh = Sharded([0, half + n_fill, G_SYN + n_fill], lambda cx, b0, b1: upload(cx, csr_slice(d, b0, b1), C_SYN), samples)
+    logs = sh.log_jobs()
+    try:
+        got, _ = run_sharded(monkeypatch, sh, which=("profile",))
+        assert whole.check(got) > 20
+    finally:
+        sh.close()
+        whole.close()
+    assert [[(e["csr"], e["rc"]) for e in lg] for lg in logs] == [[(False, _lib.SYL_OK)]] * 2
+    genomes = got["profile"]["genome"]
+    assert (genomes < half).any() and (genomes >= half + n_fill).any() and not ((genomes >= half) & (genomes < half + n_fill)).any()
 
 
 def parent_default_rows(S, G):
@@ -443,11 +510,12 @@ def empty_genomes(ctx, kind, b):
     return ctx.upload_genomes(z, np.zeros(1, np.uint64), z, np.zeros(1, np.uint64), z, c=200)
 
 
-@pytest.mark.parametrize("kind", ["sketch", "upload"])
+@pytest.mark.parametrize("kind,csr", with_csr(["sketch", "upload"]))
 @pytest.mark.parametrize("cuts", [[0, 1, 2, 3, 3], [0, 0, 3], [0, 3, 3], [0, 1, 1, 3]], ids=["W4", "0|3", "3|0", "1|0|2"])
-def test_empty_shards(ctx, ecoli, monkeypatch, cuts, kind):
+def test_empty_shards(ctx, ecoli, monkeypatch, cuts, kind, csr):
     """The three config-1 E. coli genomes and o157_reads with a rank that holds no genome: that rank runs every stage
     and every collective the others run, and all ranks return the single-GPU rows."""
+    set_csr(monkeypatch, csr)
     if cuts == [0, 1, 2, 3, 3]:
         assert cuts == shard_cuts(3, 4)
 
@@ -483,12 +551,15 @@ def scripted(ctx, names, sel):
 
 
 def run_scripted(ctx, monkeypatch, names, sel, cuts, kws):
+    """every parameter set in `kws`, in the formulation each rank picks and with SYL_CONTAIN_CSR=1"""
     d, samples, whole = scripted(ctx, names, sel)
     sh = Sharded(cuts, lambda cx, b0, b1: upload(cx, csr_slice(d, b0, b1), 1), samples)
     try:
-        for kw in kws:
-            got, _ = run_sharded(monkeypatch, sh, kw)
-            assert whole.check(got, kw) > 0, kw
+        for csr in (False, True):
+            set_csr(monkeypatch, csr)
+            for kw in kws:
+                got, _ = run_sharded(monkeypatch, sh, kw)
+                assert whole.check(got, kw) > 0, (kw, csr)
     finally:
         sh.close()
         whole.close()
@@ -511,9 +582,10 @@ def test_scripted_shard_range(ctx, monkeypatch, name, world):
     run_scripted(ctx, monkeypatch, [name], sel, shard_cuts(len(sel), world), S.params_for(name))
 
 
-def test_scripted_big_falls_back_on_every_rank(ctx, monkeypatch):
+def test_scripted_big_is_redone_in_csr_on_every_rank(ctx, monkeypatch):
     """`big` (counts >= 256) on two ranks and the `median` genomes, which see no count >= 256, on a third: every rank's
-    finish returns SYL_ERR_UNSUPPORTED, and the gathered-survivor fallback gives ctx.profile's rows."""
+    first finish returns SYL_ERR_UNSUPPORTED, every rank redoes the job with csr set and gets ctx.profile's rows.  The
+    redo runs the same three collectives again and moves no sketch."""
     from sylph_b200 import _lib
     w = S.world()
     big, med = w.local["big"], w.local["median"]
@@ -524,12 +596,14 @@ def test_scripted_big_falls_back_on_every_rank(ctx, monkeypatch):
     sh = Sharded(cuts, lambda cx, b0, b1: upload(cx, csr_slice(d, b0, b1), 1), samples)
     logs = sh.log_jobs()
     try:
-        got, _ = run_sharded(monkeypatch, sh, which=("profile", "gather"))
+        got, grp = run_sharded(monkeypatch, sh, which=("profile",))
         assert whole.check(got) > 5
     finally:
         sh.close()
         whole.close()
-    assert [[e["rc"] for e in lg] for lg in logs] == [[_lib.SYL_ERR_UNSUPPORTED]] * 3
+    assert [[(e["csr"], e["rc"]) for e in lg] for lg in logs] == [[(False, _lib.SYL_ERR_UNSUPPORTED), (True, _lib.SYL_OK)]] * 3
+    for r in range(3):
+        assert [n for n, _ in grp.calls[r]] == ["all_gather_into_tensor", "all_reduce", "all_gather_into_tensor"] * 2, r
 
 
 # ---- parameters -----------------------------------------------------------------------------------------------------
