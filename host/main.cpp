@@ -665,16 +665,42 @@ static int cmd_contain(const std::vector<syl_ctx *> &ctxs, const Args &a, bool p
         std::vector<uint64_t>().swap(g.tracked);
     }
     const bool has_tr = gs[0].has_tracked;
+    // samples: raw reads, then sketches, cut into one contiguous block per context
+    if (!read_files.empty() && a.c > gs[0].c) {
+        for (const std::string &f : read_files) warn(f + " error: value of -c for contain is greater than the smallest value of -c for a genome sketch. Continuing without sketching.");
+        read_files.clear();
+    }
+    if (!read_files.empty() && a.k != gs[0].k) {  // src/contain.rs:578-584: raw reads are sketched with -k or not at all
+        for (const std::string &f : read_files)
+            warn(f + " -k " + std::to_string(a.k) + " is not equal to -k " + std::to_string(gs[0].k) + " found in sketches. Continuing without sketching.");
+        read_files.clear();
+    }
+    const size_t n_reads = read_files.size(), n_samples = n_reads + sample_files.size();
+    std::vector<uint64_t> weight(n_samples);
+    for (size_t i = 0; i < n_samples; i++)
+        weight[i] = i < n_reads ? sample_weight(read_files[i], false, a.c) : sample_weight(sample_files[i - n_reads], true, a.c);
+    const std::vector<size_t> block = sample_blocks(weight, ctxs.size());
     // one index while the db fits one (fewer than 2^32-2 entries and 2^31-1 genomes) and no cap is set; otherwise db
     // shards that every query / profile call sweeps once, reading the flat arrays from host memory
     uint64_t shard_cap = a.max_db_entries;
     if (a.shard_entries) shard_cap = shard_cap ? std::min(shard_cap, a.shard_entries) : a.shard_entries;
     const bool sharded = shard_cap || nk + (has_tr ? nt : 0) >= 0xFFFFFFFEull || gs.size() >= 0x7FFFFFFFull;
+    // a context whose block of samples the library would scan past the genome k-mers (syl_db_scan_plan) takes shards
+    // too: its calls then build no index at all
+    std::vector<char> scans(ctxs.size(), 0);
+    for (size_t w = 0; w < ctxs.size() && !sharded; w++) {
+        uint64_t sk = 0;
+        for (size_t i = block[w]; i < block[w + 1]; i++) sk += weight[i];
+        int scan = 0;
+        check(syl_db_scan_plan(ctxs[w], nk, has_tr ? nt : 0, gs.size(), (uint32_t)(block[w + 1] - block[w]), sk, &scan), "syl_db_scan_plan");
+        scans[w] = scan != 0;
+    }
+    const bool any_scan = std::count(scans.begin(), scans.end(), 1) > 0;
     // every context builds its own index (or shards) from the same host arrays, which stay alive until all have
     std::vector<ContextDb> dbs(ctxs.size());
     run_workers(ctxs.size(), [&](size_t w) {
         syl_ctx *ctx = ctxs[w];
-        if (!sharded) {
+        if (!sharded && !scans[w]) {
             check(syl_db_build_arrays(ctx, SYL_MEM_HOST, kmers.data(), koff.data(), has_tr ? tracked.data() : nullptr,
                                       has_tr ? toff.data() : nullptr, gsz.data(), gs.size(), (int)gs[0].k, db_c, 0, &dbs[w].db),
                   "syl_db_build_arrays");
@@ -700,10 +726,10 @@ static int cmd_contain(const std::vector<syl_ctx *> &ctxs, const Args &a, bool p
             create(std::max<uint64_t>(1, largest / share));
         }
     });
-    if (!sharded) {
+    if (!sharded && !any_scan) {
         std::vector<uint64_t>().swap(kmers);
         std::vector<uint64_t>().swap(tracked);
-    } else {
+    } else if (sharded) {
         const uint64_t n_shards = syl_db_shards_count(dbs[0].shards);
         for (uint64_t i = 0; i < n_shards; i++) {
             uint64_t g0 = 0, ng = 0, ne = 0;
@@ -712,22 +738,6 @@ static int cmd_contain(const std::vector<syl_ctx *> &ctxs, const Args &a, bool p
                  std::to_string(g0 + ng) + ", " + std::to_string(ne) + " index entries.");
         }
     }
-    // samples: raw reads, then sketches, cut into one contiguous block per context
-    if (!read_files.empty() && a.c > gs[0].c) {
-        for (const std::string &f : read_files) warn(f + " error: value of -c for contain is greater than the smallest value of -c for a genome sketch. Continuing without sketching.");
-        read_files.clear();
-    }
-    if (!read_files.empty() && a.k != gs[0].k) {  // src/contain.rs:578-584: raw reads are sketched with -k or not at all
-        for (const std::string &f : read_files)
-            warn(f + " -k " + std::to_string(a.k) + " is not equal to -k " + std::to_string(gs[0].k) + " found in sketches. Continuing without sketching.");
-        read_files.clear();
-    }
-    const size_t n_reads = read_files.size(), n_samples = n_reads + sample_files.size();
-    std::vector<uint64_t> weight(n_samples);
-    if (ctxs.size() > 1)
-        for (size_t i = 0; i < n_samples; i++)
-            weight[i] = i < n_reads ? sample_weight(read_files[i], false, a.c) : sample_weight(sample_files[i - n_reads], true, a.c);
-    const std::vector<size_t> block = sample_blocks(weight, ctxs.size());
     FILE *o = a.out_file.empty() ? stdout : fopen(a.out_file.c_str(), "w");
     if (!o) die("cannot open output file " + a.out_file);
     if (!pseudotax)  // src/contain.rs:461-480

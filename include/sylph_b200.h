@@ -91,7 +91,8 @@ enum {
     SYL_KERNEL_BOOT = 5,        /* bootstrap: k_boot_iter_p (+ k_boot_seq, k_boot_final) */
     SYL_KERNEL_GENOME_POST = 6, /* genome-sketch post-pass (everything after k_seed) */
     SYL_KERNEL_PACK = 7,        /* ASCII -> 2-bit packing on the device (unused by the host-packed path) */
-    SYL_KERNEL_COUNT = 8
+    SYL_KERNEL_SCAN = 8,        /* scan formulation of pass 1 (db shards): k_scan (+ the sample tables, k_table_*) */
+    SYL_KERNEL_COUNT = 9
 };
 int syl_ctx_kernel_time(syl_ctx *ctx, int which, double *total_ms, uint64_t *launches, int reset);
 /* Device memory of the ctx.  held: bytes of every block the ctx's block cache has allocated (blocks of live
@@ -443,6 +444,22 @@ int syl_query_shards(syl_ctx *ctx, syl_db_shards *s, const syl_sample *const *sa
 int syl_profile_shards(syl_ctx *ctx, syl_db_shards *s, const syl_sample *const *samples, uint32_t n_samples,
                        const syl_contain_params *p, syl_ani_row *rows, uint64_t cap, uint64_t *n_rows);
 void syl_db_shards_free(syl_db_shards *s);
+/* Scan instead of build.  A call of few samples on a large syl_db_shards handle does not build any index: its pass 1
+ * streams the genome k-mers (never the tracked ones) from the borrowed host arrays to the device in chunks of whole
+ * genomes, on the ctx's host-ingest copy stream (pageable arrays through its pinned ring) into two device buffers,
+ * chunk i + 1 while chunk i is scanned, and every genome k-mer probes a lookup table of every sample (about 6 bytes of
+ * device memory per sample k-mer).  The rows, their order and the capacity protocol are those of the build path,
+ * bit for bit; profile's pass 2 runs on the survivor indexes as above.  A call scans when all its samples fit one
+ * sample batch, the database holds at least 2^28 index entries, and the measured cost model of DESIGN.md §10 puts
+ * the scan below the build (it depends on whether the genome k-mers are in pinned memory, and on whether all samples'
+ * tables fit the L2 cache).  SYL_DB_SCAN=0|1 (read per call) forces the build or the scan, the scan only where the
+ * samples fit one batch (host samples that do not are swept shard by shard, as without the switch);
+ * SYL_DB_SCAN_CHUNK=N (test hook, read per call) sets the genome k-mers per chunk (default 2^25).
+ * syl_db_scan_plan sets *scan to what a call of n_samples samples holding sample_kmers k-mers together would do on a
+ * handle of n_genomes genomes holding n_kmers genome k-mers and n_tracked tracked k-mers (1: scan, 0: build), taking
+ * the samples as equal host samples for the batch condition and the database as pageable host arrays. */
+int syl_db_scan_plan(syl_ctx *ctx, uint64_t n_kmers, uint64_t n_tracked, uint64_t n_genomes, uint32_t n_samples,
+                     uint64_t sample_kmers, int *scan);
 
 /* ------------------------------------------------------------------------------------------
  * (7) Query and profile samples from HOST memory, any number of them, in bounded device memory: e.g. every deserialised

@@ -115,6 +115,7 @@ SIGNATURES = {
     "syl_query_shards": (_i, [_vp, _vp, _pp, _u32, C.POINTER(ContainParams), _vp, _u64, _pu64]),
     "syl_profile_shards": (_i, [_vp, _vp, _pp, _u32, C.POINTER(ContainParams), _vp, _u64, _pu64]),
     "syl_db_shards_free": (None, [_vp]),
+    "syl_db_scan_plan": (_i, [_vp, _u64, _u64, _u64, _u32, _u64, C.POINTER(C.c_int)]),
     "syl_query_host_samples": (_i, [_vp, _vp, _vp, C.POINTER(HostSamples), C.POINTER(ContainParams), _vp, _u64, _pu64]),
     "syl_profile_host_samples": (_i, [_vp, _vp, _vp, C.POINTER(HostSamples), C.POINTER(ContainParams), _vp, _u64, _pu64]),
 }

@@ -92,7 +92,7 @@ class Context:
         _lib.check(_lib.lib().syl_ctx_seed_kernel_time(self._h, C.byref(ms), C.byref(n), C.byref(b), int(reset)))
         return ms.value, n.value, b.value
 
-    KERNELS = {"seed": 0, "group_dedup": 1, "join": 2, "join2": 3, "stats": 4, "boot": 5, "genome_post": 6, "pack": 7}
+    KERNELS = {"seed": 0, "group_dedup": 1, "join": 2, "join2": 3, "stats": 4, "boot": 5, "genome_post": 6, "pack": 7, "scan": 8}
 
     def ingest_stats(self):
         """-> (h2d_bytes, chunks_packed, chunks_ascii) of the last host-memory sketch_sequences,
@@ -307,6 +307,14 @@ class Context:
         _lib.check(_lib.lib().syl_db_build_arrays(self._h, mem, pk, pko, pt, pto, pg, nko - 1, k, c, int(genome_base),
                                                   C.byref(h)))
         return Db(self, h)
+
+    def db_scan_plan(self, n_kmers, n_tracked, n_genomes, n_samples, sample_kmers):
+        """-> True when a call of n_samples samples holding sample_kmers k-mers together on a db_shards handle of that
+        shape would stream the genome k-mers past the samples instead of building an index (syl_db_scan_plan)"""
+        scan = C.c_int(0)
+        _lib.check(_lib.lib().syl_db_scan_plan(self._h, int(n_kmers), int(n_tracked), int(n_genomes), int(n_samples),
+                                               int(sample_kmers), C.byref(scan)))
+        return bool(scan.value)
 
     def db_shards(self, kmers, kmer_off, tracked=None, tracked_off=None, gn_size=None, k=31, c=200, max_entries=0):
         """A database larger than one index, in host memory (syl_db_shards_create): cut into shards of at most

@@ -36,6 +36,7 @@
 
 #include "contain.hpp"
 #include "crmath.cuh"
+#include "scan_plan.hpp"
 
 namespace syl {
 
@@ -384,6 +385,114 @@ __global__ void k_join_hist(const SampleView *__restrict__ views, uint64_t G,
         walk_range(gid, lo, e, [&](const uint32_t g) { out.hit<JOIN_HIST>(row + g, c); });
     }
   });
+}
+
+// ---- scan formulation of pass 1 (the join the reference does, src/contain.rs:632-652) ---------------------------------
+// For a call of few samples against a database in host memory, building the index costs far more than the joins.  The
+// scan streams the genome k-mers of a chunk of whole genomes instead, and each one probes every sample's lookup table
+// (scan_plan.hpp): the same (sample key, genome k-mer) hits as the index join, so the same per-pair outputs.
+
+// tables[s].M, and the directory of an empty sample
+__global__ void k_table_params(SampleTable *__restrict__ tables, uint32_t S) {
+    const uint32_t s = blockIdx.x * blockDim.x + threadIdx.x;
+    if (s >= S) return;
+    SampleTable &t = tables[s];
+    t.M = table_mult(t.n ? t.hash[t.n - 1] : 0, t.NB);
+    if (!t.n) { const_cast<uint32_t *>(t.dir)[0] = 0; const_cast<uint32_t *>(t.dir)[1] = 0; }
+}
+
+// grid (key blocks, samples s0 ..): fingerprints and directory entries of every key
+__global__ void k_table_fill(const SampleTable *__restrict__ tables, uint32_t s0) {
+    const SampleTable t = tables[s0 + blockIdx.y];
+    const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= t.n) return;
+    const_cast<uint32_t *>(t.fp)[i] = (uint32_t)t.hash[i];
+    table_dir_entries(t.hash, t.n, i, t.M, t.NB, const_cast<uint32_t *>(t.dir));
+}
+
+constexpr int SCAN_THREADS = 256;
+constexpr int SCAN_PER_THREAD = 4;  // k-mers per thread: two 128-bit loads, four independent probe chains per sample
+
+// One thread per SCAN_PER_THREAD consecutive k-mers of the chunk (coalesced 128-bit loads).  A k-mer's genome is the last
+// g with off[g] <= its index (empty genomes share their successor's offset).  Every k-mer probes every sample's table;
+// a hit with a non-zero count (src/contain.rs:634-636) goes to pair (s, g) as in the index join.
+template <JoinOut OUT>
+__global__ void __launch_bounds__(SCAN_THREADS)
+k_scan(const ScanChunk ch, uint32_t S, uint64_t G, const PairOut out) {
+    const uint64_t i0 = ((uint64_t)blockIdx.x * SCAN_THREADS + threadIdx.x) * SCAN_PER_THREAD;
+    if (i0 >= ch.n) return;
+    uint64_t kq[SCAN_PER_THREAD];
+    const int nk = ch.n - i0 < SCAN_PER_THREAD ? (int)(ch.n - i0) : SCAN_PER_THREAD;
+    if (nk == SCAN_PER_THREAD) {
+        const ulonglong2 *p = reinterpret_cast<const ulonglong2 *>(ch.kmers + i0);
+        const ulonglong2 a = p[0], b = p[1];
+        kq[0] = a.x; kq[1] = a.y; kq[2] = b.x; kq[3] = b.y;
+    } else {
+#pragma unroll
+        for (int q = 0; q < SCAN_PER_THREAD; q++) kq[q] = q < nk ? ch.kmers[i0 + q] : 0;
+    }
+    uint64_t lo = 0, hi = G;  // off[lo] <= i0 < off[hi]
+    while (hi - lo > 1) {
+        const uint64_t mid = (lo + hi) >> 1;
+        if (ch.off[mid] <= i0) lo = mid; else hi = mid;
+    }
+    uint32_t g[SCAN_PER_THREAD];
+#pragma unroll
+    for (int q = 0; q < SCAN_PER_THREAD; q++) {
+        if (q < nk) while (ch.off[lo + 1] <= i0 + q) lo++;
+        g[q] = (uint32_t)lo;
+    }
+    for (uint32_t s = 0; s < S; s++) {
+        const SampleTable t = ch.tables[s];
+        const uint64_t row = (uint64_t)s * G;
+        uint32_t b0[SCAN_PER_THREAD], b1[SCAN_PER_THREAD];
+#pragma unroll
+        for (int q = 0; q < SCAN_PER_THREAD; q++) {
+            const uint64_t b = table_bucket(kq[q], t.M, t.NB);
+            b0[q] = q < nk ? t.dir[b] : 0;
+            b1[q] = q < nk ? t.dir[b + 1] : 0;
+        }
+#pragma unroll
+        for (int q = 0; q < SCAN_PER_THREAD; q++) {
+            for (uint32_t j = b0[q]; j < b1[q]; j++) {
+                if (t.fp[j] != (uint32_t)kq[q] || t.hash[j] != kq[q]) continue;
+                const uint32_t c = t.count[j];
+                if (c) out.hit<OUT>(row + g[q], c);
+            }
+        }
+    }
+}
+
+int build_tables(syl_ctx *ctx, const SampleView *views, uint32_t S, DevBuf<SampleTable> &tables, DevBuf<uint32_t> &dir,
+                 DevBuf<uint32_t> &fp, std::vector<SampleTable> &h) {
+    cudaStream_t st = ctx->stream;
+    uint64_t nd = 0, nf = 0, max_n = 0;
+    for (uint32_t s = 0; s < S; s++) {
+        nd += table_buckets(views[s].n) + 1;
+        nf += views[s].n;
+        max_n = std::max(max_n, views[s].n);
+    }
+    SYL_TRY(tables.alloc(S, st)); SYL_TRY(dir.alloc(nd, st)); SYL_TRY(fp.alloc(nf, st));
+    h.resize(S);
+    nd = nf = 0;
+    for (uint32_t s = 0; s < S; s++) {
+        const uint64_t NB = table_buckets(views[s].n);
+        h[s] = SampleTable{views[s].hash, views[s].count, fp.p + nf, dir.p + nd, views[s].n, NB, 0};
+        nd += NB + 1;
+        nf += views[s].n;
+    }
+    if (!S) return SYL_OK;
+    // a pageable source is staged by the driver before cudaMemcpyAsync returns
+    SYL_CUDA(cudaMemcpyAsync(tables.p, h.data(), S * sizeof(SampleTable), cudaMemcpyHostToDevice, st));
+    KernelTimer kt(ctx, SYL_KERNEL_SCAN);
+    k_table_params<<<nblk(S, 128), 128, 0, st>>>(tables.p, S);
+    ctx->launches++;
+    for (uint32_t s0 = 0; s0 < S && max_n; s0 += 65535) {
+        k_table_fill<<<dim3(nblk(max_n, 256), std::min<uint32_t>(S - s0, 65535)), 256, 0, st>>>(tables.p, s0);
+        ctx->launches++;
+    }
+    SYL_CUDA(cudaGetLastError());
+    return SYL_OK;
 }
 
 // one warp per (sample, genome); lane l owns the bins [8l, 8l+8)
@@ -881,6 +990,7 @@ struct syl_profile_job {
     syl::DevBuf<double> res_ani, res_lambda;
     syl::DevBuf<uint64_t> gn_size;
     std::vector<uint8_t> h_tab;
+    syl::ScanChunk scan{};   // scan.kmers != nullptr: pass 1 by the scan formulation
 };
 
 namespace syl {
@@ -924,6 +1034,14 @@ static int clear_pairs(syl_profile_job *j) {
 template <JoinOut OUT>
 static void join_walk(syl_profile_job *j, bool pass2) {
     const syl_db *db = j->db;
+    if (j->scan.kmers) {
+        if (!j->max_n || !j->scan.n) return;
+        KernelTimer kt(j->ctx, SYL_KERNEL_SCAN);
+        k_scan<OUT><<<nblk(j->scan.n, (uint64_t)SCAN_THREADS * SCAN_PER_THREAD), SCAN_THREADS, 0, j->ctx->stream>>>(j->scan, j->S, j->G,
+                                                                                                            pair_out(j, pass2));
+        j->ctx->launches++;
+        return;
+    }
     if (!j->max_n || !db->N) return;
     auto k = j->world > 1 ? k_join2_order<WIN_GIVEN, OUT> : k_join2_order<WIN_FUSED, OUT>;
     if constexpr (OUT != JOIN_HIST) {
@@ -984,15 +1102,18 @@ static int enqueue_stats(syl_profile_job *j, const StatParams &P, bool pass2, vo
 // ranks of a sharded profile may pick differently.
 static int job_begin(syl_ctx *ctx, const syl_db *db, const SampleView *views, const SampleMeta *metas, uint32_t n_samples,
                      const syl_contain_params *p, bool profile, bool csr, uint32_t world, uint32_t rank, uint64_t R,
-                     syl_profile_job **out, JoinRoom *room = nullptr) {
+                     syl_profile_job **out, JoinRoom *room = nullptr, const ScanChunk *scan = nullptr) {
     cudaStream_t st = ctx->stream;
     Handle<syl_profile_job> h(new (std::nothrow) syl_profile_job());
     if (!h) return SYL_ERR_OOM;
+    // the scan formulation is pass 1 of a query: pass 2 walks the winners of recorded index ranges, which a scan has not
+    if (scan && profile) { set_error("the scan formulation runs query calls only"); return SYL_ERR_ARG; }
     syl_profile_job *j = h.get();
     const uint64_t NP = (uint64_t)n_samples * db->n_genomes;
     csr = csr || getenv("SYL_CONTAIN_CSR") != nullptr || !histograms_fit(NP);
     j->ctx = ctx; j->db = db; j->profile = profile; j->csr = csr; j->S = n_samples; j->G = db->n_genomes; j->world = world; j->rank = rank;
     j->room = room;
+    if (scan) j->scan = *scan;
     syl_contain_params pp = *p;
     pp.pseudotax = profile ? 1 : 0;
     j->P = make_params(&pp);
@@ -1004,7 +1125,7 @@ static int job_begin(syl_ctx *ctx, const syl_db *db, const SampleView *views, co
     if (NP >= 0x7FFFFFFFull) { set_error("samples x genomes exceeds 2^31 pairs per call; split the sample batch"); return SYL_ERR_ARG; }
     std::vector<SampleView> hv(views, views + n_samples);
     for (const SampleView &v : hv) j->max_n = std::max<uint64_t>(j->max_n, v.n);
-    const uint64_t HN = std::max<uint64_t>((uint64_t)j->S * j->max_n, 1);
+    const uint64_t HN = scan ? 1 : std::max<uint64_t>((uint64_t)j->S * j->max_n, 1);  // the scan records no ranges
     SYL_TRY(j->views.alloc(n_samples, st));
     if (csr) {
         SYL_TRY(j->cnt.alloc(NP + 1, st)); SYL_TRY(j->cursor.alloc(NP, st)); SYL_TRY(j->off.alloc(NP + 1, st));
@@ -1032,7 +1153,7 @@ static int job_begin(syl_ctx *ctx, const syl_db *db, const SampleView *views, co
     SYL_CUDA(cudaMemsetAsync(j->tab1.p, 0, sizeof(ShardTable), st));
     j->jgrid = dim3(nblk(std::max<uint64_t>(j->max_n, 1), 128), (unsigned)j->S);
     static const bool tile_env_off = getenv("SYL_JOIN_PLAIN") != nullptr;
-    if (j->S > 1 && j->max_n && db->N && !tile_env_off) {
+    if (j->S > 1 && j->max_n && db->N && !tile_env_off && !scan) {
         // ~100 keys of the largest sample per (range, sample) block; ranges are equal numbers of db buckets
         const uint64_t R = std::min<uint64_t>(std::max<uint64_t>(j->max_n / 100, 1), std::max<uint64_t>(db->NB, 1));
         const uint64_t bpr = (db->NB + R - 1) / R;
@@ -1045,7 +1166,8 @@ static int job_begin(syl_ctx *ctx, const syl_db *db, const SampleView *views, co
             j->jgrid = dim3((unsigned)(R * j->S), 1);
         }
     }
-    if (j->max_n && db->N) {
+    if (scan && !csr) join_walk<JOIN_HIST>(j, false);
+    if (j->max_n && db->N && !scan) {
         KernelTimer kt(ctx, SYL_KERNEL_JOIN);
         const auto probe = csr ? k_join_hist<true> : k_join_hist<false>;
         probe<<<j->jgrid, 128, 0, st>>>(j->views.p, j->G, db->keys, db->gid, db->N, db->bstart, db->M, db->NB, db->maxkey,
@@ -1233,13 +1355,13 @@ static int job_finish(syl_profile_job *j, std::vector<syl_ani_row> &out, uint64_
 // the same views, recursively, and a single sample that does not fit is SYL_ERR_OOM.
 int contain_fast(syl_ctx *ctx, const syl_db *db, const SampleView *views, const SampleMeta *metas, uint32_t n_samples,
                  const syl_contain_params *p, bool profile, std::vector<syl_ani_row> &out, const std::function<int()> &overlap,
-                 JoinRoom *room) {
+                 JoinRoom *room, const ScanChunk *scan) {
     uint64_t R = 0;
     bool csr = false;
     bool overlapped = false;
     for (int attempt = 0; attempt < 4; attempt++) {  // one formulation switch + capacity retries
         syl_profile_job *j = nullptr;
-        int rc = job_begin(ctx, db, views, metas, n_samples, p, profile, csr, 1, 0, R, &j, room);
+        int rc = job_begin(ctx, db, views, metas, n_samples, p, profile, csr, 1, 0, R, &j, room, scan);
         if (rc == SYL_OK) {
             if (profile) {
                 rc = job_rank(j);
@@ -1275,8 +1397,10 @@ int contain_fast(syl_ctx *ctx, const syl_db *db, const SampleView *views, const 
         JoinRoom r0 = *room, r1 = *room;
         r1.s0 += h;
         std::vector<syl_ani_row> second;
-        SYL_TRY(contain_fast(ctx, db, views, metas, h, p, profile, out, overlapped ? std::function<int()>() : overlap, &r0));
-        SYL_TRY(contain_fast(ctx, db, views + h, metas + h, n_samples - h, p, profile, second, {}, &r1));
+        ScanChunk s1{};
+        if (scan) { s1 = *scan; s1.tables += h; }
+        SYL_TRY(contain_fast(ctx, db, views, metas, h, p, profile, out, overlapped ? std::function<int()>() : overlap, &r0, scan));
+        SYL_TRY(contain_fast(ctx, db, views + h, metas + h, n_samples - h, p, profile, second, {}, &r1, scan ? &s1 : nullptr));
         for (syl_ani_row &r : second) {
             r.sample += h;
             out.push_back(r);

@@ -76,9 +76,29 @@ struct JoinRoom {
 };
 constexpr int SPLIT_BATCH = -1;  // internal status, never returned through the C ABI
 
+// The scan formulation of pass 1 (a query without an index): the genome k-mers of a chunk of whole genomes, on the
+// device, probe every sample's lookup table (scan_plan.hpp has its layout).  The chunk's genomes are the db's of the
+// call (n_genomes, genome_base, glen; it holds no index, N == 0); off = its n_genomes + 1 k-mer offsets, rebased to 0.
+struct SampleTable {
+    const uint64_t *hash;
+    const uint32_t *count, *fp, *dir;
+    uint64_t n, NB, M;
+};
+struct ScanChunk {
+    const uint64_t *kmers, *off;
+    uint64_t n;
+    const SampleTable *tables;  // one per sample of the call
+};
+
+// the lookup tables of samples views[0 .. S) into tables (device, S entries), dir and fp (scan_plan.hpp), on the ctx
+// stream; the host array `h` (S entries) is filled as well
+int build_tables(syl_ctx *ctx, const SampleView *views, uint32_t S, DevBuf<SampleTable> &tables, DevBuf<uint32_t> &dir,
+                 DevBuf<uint32_t> &fp, std::vector<SampleTable> &h);
+
+// scan != nullptr: pass 1 of a query by the scan formulation (with profile: SYL_ERR_ARG)
 int contain_fast(syl_ctx *ctx, const syl_db *db, const SampleView *views, const SampleMeta *metas, uint32_t n_samples,
                  const syl_contain_params *p, bool profile, std::vector<syl_ani_row> &out,
-                 const std::function<int()> &overlap = {}, JoinRoom *room = nullptr);
+                 const std::function<int()> &overlap = {}, JoinRoom *room = nullptr, const ScanChunk *scan = nullptr);
 
 // ---- the calls (contain_calls.cu) -----------------------------------------------------------
 

@@ -13,6 +13,7 @@
 #include "contain.hpp"
 #include "ingest.hpp"
 #include "sample_batches.hpp"
+#include "scan_plan.hpp"
 #include "shard_cut.hpp"
 
 // A database in borrowed host arrays, cut into index shards (syl_db_shards_*).
@@ -160,6 +161,7 @@ static int shard_build(const syl_db_shards *s, uint64_t a, uint64_t b, syl_db **
 struct SampleSource {
     std::vector<SampleMeta> metas;  // per sample
     JoinRoom room;                  // what the joins of a batch may take beyond its plan (handles: unbounded)
+    bool scan = false;              // pass 1 of a shards call by the scan formulation (decided at the call's entry)
     virtual ~SampleSource() = default;
     // the batches of a join against an index of G genomes
     virtual void batches(uint64_t G, std::vector<uint32_t> &first) const = 0;
@@ -338,11 +340,140 @@ static int join_batches(syl_ctx *ctx, const syl_db *db, SampleSource &src, const
     return SYL_OK;
 }
 
+// Whether a call of this shape scans (scan_plan.hpp), with SYL_DB_SCAN (read per call) forcing either path where the
+// samples fit one batch
+static bool plan_scan(const ScanShape &shape) { return scan_decision(shape, scan_forced(getenv("SYL_DB_SCAN"))); }
+
+// Genomes of one scan chunk at most: a chunk's joins hold at most PAIRS_PER_CALL (sample, genome) pairs
+static uint64_t scan_chunk_genomes(uint32_t S) { return std::max<uint64_t>(PAIRS_PER_CALL / std::max<uint32_t>(S, 1), 1); }
+
+static uint64_t scan_chunk_env() {  // SYL_DB_SCAN_CHUNK: genome k-mers per scan chunk (tests; read per call)
+    if (const char *e = getenv("SYL_DB_SCAN_CHUNK")) {
+        const long long v = atoll(e);
+        if (v >= 1) return (uint64_t)v;
+    }
+    return SCAN_CHUNK;
+}
+
+// Pass 1 (syl_query) of all samples of src (one batch) by the scan formulation: the genome k-mers cross the link chunk by
+// chunk (whole genomes) on the ingest copy stream into two device buffers, chunk i + 1 while chunk i is scanned, and
+// each chunk is a query of its genomes (contain_fast with the chunk).  rows: by chunk, then by (sample, genome);
+// row.genome is the global index.  Its blocks go back to the ctx cache when it returns.  src holds all samples in one
+// batch (scan_one_batch).
+static int scan_sweep(syl_db_shards *s, SampleSource &src, const syl_contain_params *p, std::vector<syl_ani_row> &rows) {
+    syl_ctx *ctx = s->ctx;
+    cudaStream_t st = ctx->stream;
+    const uint32_t S = (uint32_t)src.metas.size();
+    SYL_TRY(cache_trim(ctx));
+    const auto t0 = std::chrono::steady_clock::now();
+    // kernel milliseconds of SYL_DEBUG_TIMING's line (with syl_ctx_enable_timing; else they stay 0)
+    double scan0 = 0., stats0 = 0., scan1 = 0., stats1 = 0.;
+    if (debug_timing()) {
+        SYL_TRY(syl_ctx_kernel_time(ctx, SYL_KERNEL_SCAN, &scan0, nullptr, 0));
+        SYL_TRY(syl_ctx_kernel_time(ctx, SYL_KERNEL_STATS, &stats0, nullptr, 0));
+    }
+    const uint64_t h2d0 = ctx->ingest_h2d_bytes;
+    std::vector<SampleView> v;
+    SYL_TRY(src.views(0, S, v));
+    DevBuf<SampleTable> tables;
+    DevBuf<uint32_t> dir, fp;
+    std::vector<SampleTable> ht;
+    int rc = build_tables(ctx, v.data(), S, tables, dir, fp, ht);
+    std::vector<uint64_t> first;
+    cut_scan_chunks(s->kmer_off, s->G, scan_chunk_env(), scan_chunk_genomes(S), first);
+    const size_t nc = first.size() - 1;
+    uint64_t max_n = 0, max_g = 0;
+    for (size_t i = 0; i < nc; i++) {
+        max_n = std::max(max_n, s->kmer_off[first[i + 1]] - s->kmer_off[first[i]]);
+        max_g = std::max(max_g, first[i + 1] - first[i]);
+    }
+    struct Slot {
+        DevBuf<uint64_t> kmers, off;
+        DevBuf<uint32_t> glen;
+        cudaEvent_t staged = nullptr, used = nullptr;
+    } slot[2];
+    cudaStream_t cs = nullptr;
+    const bool pinned = s->kmers && ptr_kind(s->kmers) == PtrKind::PINNED;
+    std::vector<uint64_t> h_off;
+    std::vector<uint32_t> h_glen;
+    // chunk i into slot i % 2 on the copy stream, once the scan of the chunk before it in that slot is done
+    auto stage = [&](size_t i) -> int {
+        Slot &sl = slot[i % 2];
+        const uint64_t a = first[i], G = first[i + 1] - a, k0 = s->kmer_off[a];
+        SYL_CUDA(cudaStreamWaitEvent(cs, sl.used, 0));
+        h_off.resize(G + 1);
+        h_glen.resize(G);
+        for (uint64_t g = 0; g <= G; g++) h_off[g] = s->kmer_off[a + g] - k0;
+        for (uint64_t g = 0; g < G; g++) h_glen[g] = (uint32_t)(h_off[g + 1] - h_off[g]);
+        SYL_TRY(ingest_copy(ctx, sl.off.p, h_off.data(), (G + 1) * 8, false));  // pageable: staged before it returns
+        SYL_TRY(ingest_copy(ctx, sl.glen.p, h_glen.data(), G * 4, false));
+        SYL_TRY(ingest_copy(ctx, sl.kmers.p, s->kmers + k0, h_off[G] * 8, pinned));
+        SYL_CUDA(cudaEventRecord(sl.staged, cs));
+        return SYL_OK;
+    };
+    if (rc == SYL_OK) rc = ingest_copy_stream(ctx, &cs);
+    for (Slot &sl : slot) {
+        if (rc == SYL_OK) rc = sl.kmers.alloc(max_n, st);
+        if (rc == SYL_OK) rc = sl.off.alloc(max_g + 1, st);
+        if (rc == SYL_OK) rc = sl.glen.alloc(max_g, st);
+        if (rc == SYL_OK && cudaEventCreateWithFlags(&sl.staged, cudaEventDisableTiming) != cudaSuccess) rc = SYL_ERR_CUDA;
+        if (rc == SYL_OK && cudaEventCreateWithFlags(&sl.used, cudaEventDisableTiming) != cudaSuccess) rc = SYL_ERR_CUDA;
+        if (rc == SYL_OK && cudaEventRecord(sl.used, st) != cudaSuccess) rc = SYL_ERR_CUDA;  // cached blocks: earlier work
+    }
+    if (rc == SYL_OK && nc) rc = stage(0);
+    for (size_t i = 0; i < nc && rc == SYL_OK; i++) {
+        Slot &sl = slot[i % 2];
+        if (cudaStreamWaitEvent(st, sl.staged, 0) != cudaSuccess) { rc = SYL_ERR_CUDA; break; }
+        syl_db db;
+        db.device = ctx->device;
+        db.n_genomes = first[i + 1] - first[i];
+        db.genome_base = (uint32_t)first[i];
+        db.glen = sl.glen.p;
+        db.k = s->k;
+        db.c = s->c;
+        db.has_tracked = s->tracked_off ? 1 : 0;
+        const ScanChunk ch{sl.kmers.p, sl.off.p, s->kmer_off[first[i + 1]] - s->kmer_off[first[i]], tables.p};
+        bool next_staged = i + 1 >= nc;
+        std::function<int()> next;
+        if (!next_staged) next = [&] { next_staged = true; return stage(i + 1); };
+        std::vector<syl_ani_row> part;
+        JoinRoom room = src.room;
+        room.s0 = 0;
+        rc = contain_fast(ctx, &db, v.data(), src.metas.data(), S, p, false, part, next, &room, &ch);
+        if (rc == SYL_OK && cudaEventRecord(sl.used, st) != cudaSuccess) rc = SYL_ERR_CUDA;
+        if (rc == SYL_OK && !next_staged) rc = stage(i + 1);
+        rows.insert(rows.end(), part.begin(), part.end());
+    }
+    src.done();
+    if (cs) cudaStreamSynchronize(cs);  // the slots go back to the ctx cache, whose users run on the ctx stream
+    cudaStreamSynchronize(st);
+    for (Slot &sl : slot)
+        for (cudaEvent_t e : {sl.staged, sl.used})
+            if (e) cudaEventDestroy(e);
+    if (rc == SYL_OK && debug_timing()) {
+        SYL_TRY(syl_ctx_kernel_time(ctx, SYL_KERNEL_SCAN, &scan1, nullptr, 0));
+        SYL_TRY(syl_ctx_kernel_time(ctx, SYL_KERNEL_STATS, &stats1, nullptr, 0));
+        fprintf(stderr, "[db scan] samples %u chunks %zu genome k-mers %llu: H2D %llu bytes (%s), scan %.1f ms, stats %.1f ms, pass 1 %.1f ms\n",
+                S, nc, (unsigned long long)s->kmer_off[s->G], (unsigned long long)(ctx->ingest_h2d_bytes - h2d0),
+                pinned ? "pinned" : "pageable", scan1 - scan0, stats1 - stats0, ms_since(t0));
+    }
+    return rc;
+}
+
+static ScanShape shards_shape(const syl_db_shards *s, uint32_t S, uint64_t sample_kmers, bool one_batch) {
+    const bool pinned = s->kmers && ptr_kind(s->kmers) == PtrKind::PINNED;
+    return ScanShape{s->kmer_off[s->G], s->tracked_off ? s->tracked_off[s->G] : 0, s->G, S, sample_kmers, one_batch, pinned};
+}
+
 // Pass 1 (syl_query) of every sample of src against every shard in turn: each shard's index is built once, joined with
-// all samples batch by batch, and freed before the next one is built.  rows: by shard, then by (sample, genome);
-// row.genome is the global index.
+// all samples batch by batch, and freed before the next one is built; or, when the call scans (src.scan), scan_sweep.
+// rows: by shard, then by (sample, genome); row.genome is the global index.
 static int shards_sweep(syl_db_shards *s, SampleSource &src, const syl_contain_params *p, std::vector<syl_ani_row> &rows) {
     syl_ctx *ctx = s->ctx;
+    if (src.scan) {
+        SYL_TRY(scan_sweep(s, src, p, rows));
+        return cache_trim(ctx);  // the scan's blocks are back in the cache once scan_sweep has returned
+    }
     std::vector<uint32_t> first, next;
     for (size_t i = 0; i + 1 < s->first.size(); i++) {
         const uint64_t a = s->first[i], G = s->first[i + 1] - a;
@@ -543,7 +674,50 @@ static int handle_call(syl_ctx *ctx, const syl_db *db, syl_db_shards *sh, const 
     SYL_ENTER(ctx);
     HandleSamples src(db ? UINT64_MAX : PAIRS_PER_CALL);  // one index: all samples in one join (contain_fast sizes it)
     SYL_TRY(handle_views(ctx, samples, n, p->estimate_unknown != 0, src.all, src.metas));
+    if (sh) {  // handles are resident already: the scan takes them all at once
+        uint64_t kmers = 0;
+        for (const SampleView &v : src.all) kmers += v.n;
+        src.scan = plan_scan(shards_shape(sh, n, kmers, true));
+    }
     return contain_call(ctx, db, sh, src, std::vector<const void *>(samples, samples + n), p, profile, rows, cap, n_rows);
+}
+
+// the device budget of host samples: syl_ctx_set_sample_memory's, or (0) free memory plus the ctx's cached free blocks
+static int sample_budget(syl_ctx *ctx, uint64_t *budget) {
+    *budget = ctx->sample_budget;
+    if (!*budget) {
+        size_t free_b = 0, total_b = 0;
+        SYL_CUDA(cudaMemGetInfo(&free_b, &total_b));
+        *budget = free_b;
+        for (const auto &b : ctx->free_blocks) *budget += b.second;
+    }
+    return SYL_OK;
+}
+
+// the batches of host samples (sample_batches.hpp) against G genomes per join, within `budget`; SYL_SAMPLE_BATCH=N
+// (read per call) caps a batch at N samples
+static BatchPlanResult plan_host_batches(const uint64_t *off, uint32_t S, uint64_t G, uint64_t budget, std::vector<uint32_t> &plan,
+                                         uint32_t *bad, uint64_t *need) {
+    uint32_t forced = 0;
+    if (const char *e = getenv("SYL_SAMPLE_BATCH")) forced = (uint32_t)std::max(0, atoi(e));
+    const BatchCost cost{36, 4 * 8 + sizeof(SampleView) + 96 * ROW_BYTES, 16, COV_BINS * 4 + 16, 256 * ROW_BYTES + (1u << 20)};
+    return plan_sample_batches(off, S, G, budget, PAIRS_PER_CALL, 0x7FFFFFFFull, forced, cost, plan, bad, need);
+}
+
+// Whether S host samples of `kmers` k-mers together, the largest n_max, fit the one batch a scan call stages them in:
+// the batch cost of plan_host_batches against a scan chunk's genomes, plus the samples' tables (6 bytes per k-mer), within
+// the sample budget less the two staging chunks; SYL_SAMPLE_BATCH=N below S says no.  The decision of the call and of
+// syl_db_scan_plan.
+static int scan_one_batch(syl_ctx *ctx, uint32_t S, uint64_t kmers, uint64_t n_max, bool *one) {
+    uint64_t budget = 0;
+    SYL_TRY(sample_budget(ctx, &budget));
+    const uint64_t staging = 2 * (8 * scan_chunk_env() + 12 * scan_chunk_genomes(S)), tables = 6 * kmers + 256 * (uint64_t)S;
+    uint32_t forced = 0;
+    if (const char *e = getenv("SYL_SAMPLE_BATCH")) forced = (uint32_t)std::max(0, atoi(e));
+    const BatchCost cost{36, 4 * 8 + sizeof(SampleView) + 96 * ROW_BYTES, 16, COV_BINS * 4 + 16, 256 * ROW_BYTES + (1u << 20)};
+    const unsigned __int128 bytes = (unsigned __int128)2 * batch_bytes(cost, kmers, S, n_max, scan_chunk_genomes(S)) + staging + tables;
+    *one = S && kmers <= 0x7FFFFFFFull && bytes <= budget && (!forced || S <= forced);
+    return SYL_OK;
 }
 
 // syl_query_host_samples / syl_profile_host_samples
@@ -571,19 +745,24 @@ static int host_samples_call(syl_ctx *ctx, const syl_db *db, syl_db_shards *sh, 
     // the ctx's cached free blocks), less the largest shard's build (16 bytes per entry)
     cudaStream_t cs = nullptr;
     SYL_TRY(ingest_copy_stream(ctx, &cs));
-    uint64_t budget = ctx->sample_budget, index = 0;
-    if (!budget) {
-        size_t free_b = 0, total_b = 0;
-        SYL_CUDA(cudaMemGetInfo(&free_b, &total_b));
-        budget = free_b;
-        for (const auto &b : ctx->free_blocks) budget += b.second;
-    }
+    uint64_t budget = 0, index = 0;
+    SYL_TRY(sample_budget(ctx, &budget));
     // the joins' allocations beyond the plan are held to the budget on top of the bytes the ctx holds in use now
     uint64_t live = ctx->cached_bytes + ctx->transient_bytes;
     for (const auto &b : ctx->free_blocks) live -= b.second;
     src.room.limit = live + budget;
     src.room.budget = budget;
-    if (sh) {
+    if (sh) {  // a scan stages all samples as one batch and builds no index
+        uint64_t n_max = 0;
+        for (uint32_t i = 0; i < S; i++) n_max = std::max<uint64_t>(n_max, s->off[i + 1] - s->off[i]);
+        bool one = false;
+        SYL_TRY(scan_one_batch(ctx, S, s->off[S], n_max, &one));
+        src.scan = plan_scan(shards_shape(sh, S, s->off[S], one));
+    }
+    if (src.scan) {
+        src.plan = {0, S};
+        src.plan_G = scan_chunk_genomes(S);
+    } else if (sh) {
         for (size_t i = 0; i + 1 < sh->first.size(); i++) {
             const uint64_t a = sh->first[i], b = sh->first[i + 1];
             src.plan_G = std::max(src.plan_G, b - a);
@@ -592,13 +771,10 @@ static int host_samples_call(syl_ctx *ctx, const syl_db *db, syl_db_shards *sh, 
     } else {
         src.plan_G = db->n_genomes;
     }
-    uint32_t forced = 0;
-    if (const char *e = getenv("SYL_SAMPLE_BATCH")) forced = (uint32_t)std::max(0, atoi(e));
-    const BatchCost cost{36, 4 * 8 + sizeof(SampleView) + 96 * ROW_BYTES, 16, COV_BINS * 4 + 16, 256 * ROW_BYTES + (1u << 20)};
     uint32_t bad = 0;
     uint64_t need = 0;
-    const BatchPlanResult pr = plan_sample_batches(s->off, S, src.plan_G, budget > index ? budget - index : 0, PAIRS_PER_CALL,
-                                                   0x7FFFFFFFull, forced, cost, src.plan, &bad, &need);
+    const BatchPlanResult pr = src.scan ? BATCH_OK
+                                        : plan_host_batches(s->off, S, src.plan_G, budget > index ? budget - index : 0, src.plan, &bad, &need);
     if (pr == BATCH_TOO_MANY_KMERS) {
         set_error("sample " + std::to_string(bad) + " holds " + std::to_string(need) + " k-mers, more than 2^31 - 1");
         return SYL_ERR_UNSUPPORTED;
@@ -699,6 +875,18 @@ int syl_query_host_samples(syl_ctx *ctx, const syl_db *db, syl_db_shards *shards
 int syl_profile_host_samples(syl_ctx *ctx, const syl_db *db, syl_db_shards *shards, const syl_host_samples *s,
                              const syl_contain_params *p, syl_ani_row *rows, uint64_t cap, uint64_t *n_rows) {
     return host_samples_call(ctx, db, shards, s, p, true, rows, cap, n_rows);
+}
+
+int syl_db_scan_plan(syl_ctx *ctx, uint64_t n_kmers, uint64_t n_tracked, uint64_t n_genomes, uint32_t n_samples,
+                     uint64_t sample_kmers, int *scan) {
+    if (!ctx || !scan) { set_error("NULL argument"); return SYL_ERR_ARG; }
+    *scan = 0;
+    SYL_ENTER(ctx);
+    // one batch as the call decides it, for n_samples equal host samples of sample_kmers k-mers together
+    bool one = false;
+    SYL_TRY(scan_one_batch(ctx, n_samples, sample_kmers, n_samples ? (sample_kmers + n_samples - 1) / n_samples : 0, &one));
+    *scan = plan_scan(ScanShape{n_kmers, n_tracked, n_genomes, n_samples, sample_kmers, one, false}) ? 1 : 0;
+    return SYL_OK;
 }
 
 void syl_db_shards_free(syl_db_shards *s) {

@@ -16,11 +16,11 @@ inline uint64_t genome_entries(const uint64_t *kmer_off, const uint64_t *tracked
 }
 
 // Cut genomes [0, G) into contiguous shards, greedily in genome order: shard i is [first[i], first[i + 1]), holds at most
-// `cap` entries (capped at SHARD_MAX_ENTRIES) and SHARD_MAX_GENOMES genomes.  A genome with more than `cap` entries is a
+// `cap` entries (capped at SHARD_MAX_ENTRIES) and `max_genomes` genomes.  A genome with more than `cap` entries is a
 // shard of its own.  Offsets must be monotone.  Returns false, with *bad = the genome, when a genome alone holds more
 // than SHARD_MAX_ENTRIES entries.  G == 0 gives no shard (first = {0}).
 inline bool cut_shards(const uint64_t *kmer_off, const uint64_t *tracked_off, uint64_t G, uint64_t cap,
-                       std::vector<uint64_t> &first, uint64_t *bad) {
+                       std::vector<uint64_t> &first, uint64_t *bad, uint64_t max_genomes = SHARD_MAX_GENOMES) {
     if (cap == 0 || cap > SHARD_MAX_ENTRIES) cap = SHARD_MAX_ENTRIES;
     first.assign(1, 0);
     uint64_t n = 0, g0 = 0;
@@ -30,7 +30,7 @@ inline bool cut_shards(const uint64_t *kmer_off, const uint64_t *tracked_off, ui
             *bad = g;
             return false;
         }
-        if (g > g0 && (n + e > cap || g - g0 >= SHARD_MAX_GENOMES)) {
+        if (g > g0 && (n + e > cap || g - g0 >= max_genomes)) {
             first.push_back(g);
             g0 = g;
             n = 0;
