@@ -297,7 +297,8 @@ int syl_db_build(syl_ctx *ctx, const syl_genomes *g, uint32_t genome_base, syl_d
  * plus temporaries it frees before returning: from host memory two staging chunks of SYL_DB_CHUNK entries each
  * (default 2^25; 8 bytes per entry plus 16 per genome up to the chunk size), and for buckets of more than 2048 entries
  * (a key shared by that many genomes) about 16 bytes per entry of the largest one.  Host input is read three times,
- * chunk by chunk, each chunk copied while the previous one is processed. */
+ * chunk by chunk, each chunk copied straight from the arrays on the ctx's copy stream (the one its host-memory staging
+ * shares; no staging ring is allocated) while the previous one is processed. */
 int syl_db_build_arrays(syl_ctx *ctx, int mem, const uint64_t *kmers, const uint64_t *kmer_off, const uint64_t *tracked,
                         const uint64_t *tracked_off, const uint64_t *gn_size, uint64_t n_genomes, int k, uint64_t c,
                         uint32_t genome_base, syl_db **out);
@@ -446,7 +447,7 @@ int syl_profile_shards(syl_ctx *ctx, syl_db_shards *s, const syl_sample *const *
 void syl_db_shards_free(syl_db_shards *s);
 /* Scan instead of build.  A call of few samples on a large syl_db_shards handle does not build any index: its pass 1
  * streams the genome k-mers (never the tracked ones) from the borrowed host arrays to the device in chunks of whole
- * genomes, on the ctx's host-ingest copy stream (pageable arrays through its pinned ring) into two device buffers,
+ * genomes, on the ctx's copy stream (pageable arrays through its pinned ring) into two device buffers,
  * chunk i + 1 while chunk i is scanned, and every genome k-mer probes a lookup table of every sample (about 6 bytes of
  * device memory per sample k-mer).  The rows, their order and the capacity protocol are those of the build path,
  * bit for bit; profile's pass 2 runs on the survivor indexes as above.  A call scans when all its samples fit one
@@ -486,7 +487,7 @@ int syl_db_scan_plan(syl_ctx *ctx, uint64_t n_kmers, uint64_t n_tracked, uint64_
  * does not charge (the CSR formulation's 4 bytes per hit, the row tables of samples with more than 96 rows) are held to
  * the budget on top of what the ctx held in use when the call began: a batch whose joins would pass it is rerun as two
  * halves, recursively, with the same rows, and a sample that does not fit alone is SYL_ERR_OOM, naming its bytes.
- * Each batch crosses the link in one pass on the ctx's host-ingest copy stream (pageable arrays through its pinned
+ * Each batch crosses the link in one pass on the ctx's copy stream (pageable arrays through its pinned
  * ring) and is sorted there by one segmented sort, while the previous batch is joined on the ctx stream.  With shards, each shard is built once per
  * call: every batch is joined with it before the next one is built (profile: then its survivor indexes, each joined
  * with samples of one batch, staged again unless a slot still holds them, while the index is gathered and built).

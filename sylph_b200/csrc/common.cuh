@@ -104,8 +104,8 @@ struct syl_ctx {
     uint64_t kernel_launches[SYL_KERNEL_COUNT] = {};
     uint64_t seed_bases = 0;
     uint64_t ingest_h2d_bytes = 0, ingest_chunks_packed = 0, ingest_chunks_ascii = 0;  // last host-memory sketch
-    // HostIngest (ingest.cu) of the host-memory read and genome paths: packer pool, copy stream, pinned ring of packed
-    // chunks and two-slot device ring of ASCII chunks (lazily allocated, reused across calls)
+    // HostIngest (ingest.cu): the copy stream of all host staging, and the host-memory read and genome paths' packer
+    // pool, pinned ring of packed chunks and two-slot device ring of ASCII chunks (lazily allocated, reused across calls)
     void *ingest = nullptr;
     // grow-only cache of scratch blocks: all work of a ctx is ordered on ONE stream, so a block can
     // be handed to the next user as soon as the previous user's kernels are enqueued; steady-state

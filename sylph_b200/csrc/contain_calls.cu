@@ -195,9 +195,9 @@ struct HandleSamples : SampleSource {
 };
 
 // Host samples (syl_host_samples), staged on the device batch by batch (sample_batches.hpp).  Two slots each hold one
-// batch (hash, count and rebased offsets), filled on the ingest copy stream and sorted there by hash within each sample
+// batch (hash, count and rebased offsets), filled on the ctx's copy stream and sorted there by hash within each sample
 // (one segmented sort per batch, into the slot or the shared second buffer, whichever it ends in), while the ctx stream
-// joins the other slot.  Events order the two streams; the host waits only where the joins already do.
+// joins the other slot.  A SlotHandoff orders the two streams; the host waits only where the joins already do.
 struct HostSamples : SampleSource {
     syl_ctx *ctx;
     const syl_host_samples *in;
@@ -210,21 +210,14 @@ struct HostSamples : SampleSource {
         std::vector<uint64_t> h_off;  // the slot's offsets, rebased to its first sample
         uint32_t s0 = 0, s1 = 0;
         bool full = false;
-        cudaEvent_t staged = nullptr, used = nullptr;
     } slot[2];
     DevBuf<uint64_t> alt_hash;
     DevBuf<uint32_t> alt_count;
     DevBuf<uint8_t> tmp;
-    cudaStream_t cs = nullptr;
+    SlotHandoff<2> handoff;  // after the buffers it orders (ingest.hpp)
     int cur = -1;  // slot of the last views()
 
     HostSamples(syl_ctx *c, const syl_host_samples *s) : ctx(c), in(s) {}
-    ~HostSamples() override {
-        if (cs) cudaStreamSynchronize(cs);  // the slots go back to the ctx cache, whose users run on the ctx stream
-        for (Slot &sl : slot)
-            for (cudaEvent_t e : {sl.staged, sl.used})
-                if (e) cudaEventDestroy(e);
-    }
     void batches(uint64_t, std::vector<uint32_t> &first) const override { first = plan; }
     uint32_t batch_of(uint32_t i) const { return (uint32_t)(std::upper_bound(plan.begin(), plan.end(), i) - plan.begin() - 1); }
     uint64_t survivor_pairs(uint32_t s0) const override {
@@ -252,23 +245,20 @@ struct HostSamples : SampleSource {
                                                          (const uint64_t *)nullptr, ctx->stream));
             tb = std::max(tb, t);
         }
+        cudaStream_t cs = nullptr, st = ctx->stream;
         SYL_TRY(ingest_copy_stream(ctx, &cs));
-        cudaStream_t st = ctx->stream;
+        SYL_TRY(handoff.init(cs, st));
         for (Slot &sl : slot) {
             SYL_TRY(sl.hash.alloc(kmers, st)); SYL_TRY(sl.count.alloc(kmers, st)); SYL_TRY(sl.off.alloc(S + 1, st));
-            SYL_CUDA(cudaEventCreateWithFlags(&sl.staged, cudaEventDisableTiming));
-            SYL_CUDA(cudaEventCreateWithFlags(&sl.used, cudaEventDisableTiming));
         }
         SYL_TRY(alt_hash.alloc(kmers, st)); SYL_TRY(alt_count.alloc(kmers, st)); SYL_TRY(tmp.alloc(tb, st));
-        SYL_CUDA(cudaEventRecord(slot[0].used, st));  // cached blocks may still be in use by earlier work on the ctx stream
-        SYL_CUDA(cudaStreamWaitEvent(cs, slot[0].used, 0));
-        return SYL_OK;
+        return handoff.fence();
     }
     // samples [s0, s1) into slot k, once the joins of its last batch are done
     int stage(int k, uint32_t s0, uint32_t s1) {
-        if (!cs) SYL_TRY(init());
+        if (!handoff.cs) SYL_TRY(init());
         Slot &sl = slot[k];
-        SYL_CUDA(cudaStreamWaitEvent(cs, sl.used, 0));
+        SYL_TRY(handoff.before_copy(k));
         const uint64_t a = in->off[s0], n = in->off[s1] - a;
         sl.h_off.resize(s1 - s0 + 1);
         for (uint32_t i = s0; i <= s1; i++) sl.h_off[i - s0] = in->off[i] - a;
@@ -279,12 +269,12 @@ struct HostSamples : SampleSource {
             cub::DoubleBuffer<uint64_t> dk(sl.hash.p, alt_hash.p);
             cub::DoubleBuffer<uint32_t> dv(sl.count.p, alt_count.p);
             size_t tb = tmp.cap_bytes;
-            SYL_CUDA(cub::DeviceSegmentedSort::SortPairs(tmp.p, tb, dk, dv, (int)n, (int)(s1 - s0), sl.off.p, sl.off.p + 1, cs));
+            SYL_CUDA(cub::DeviceSegmentedSort::SortPairs(tmp.p, tb, dk, dv, (int)n, (int)(s1 - s0), sl.off.p, sl.off.p + 1, handoff.cs));
             ctx->launches += 4;
             if (dk.selector) sl.hash.swap(alt_hash);
             if (dv.selector) sl.count.swap(alt_count);
         }
-        SYL_CUDA(cudaEventRecord(sl.staged, cs));
+        SYL_TRY(handoff.copied_in(k));
         sl.s0 = s0;
         sl.s1 = s1;
         sl.full = true;
@@ -301,7 +291,7 @@ struct HostSamples : SampleSource {
             SYL_TRY(stage(k, s0, s1));
         }
         const Slot &sl = slot[k];
-        SYL_CUDA(cudaStreamWaitEvent(ctx->stream, sl.staged, 0));
+        SYL_TRY(handoff.take(k));
         v.resize(s1 - s0);
         for (uint32_t i = s0; i < s1; i++) {
             const uint64_t o = sl.h_off[i - sl.s0];
@@ -311,7 +301,7 @@ struct HostSamples : SampleSource {
         return SYL_OK;
     }
     void done() override {
-        if (cur >= 0) cudaEventRecord(slot[cur].used, ctx->stream);
+        if (cur >= 0) handoff.done(cur);
     }
 };
 
@@ -356,7 +346,7 @@ static uint64_t scan_chunk_env() {  // SYL_DB_SCAN_CHUNK: genome k-mers per scan
 }
 
 // Pass 1 (syl_query) of all samples of src (one batch) by the scan formulation: the genome k-mers cross the link chunk by
-// chunk (whole genomes) on the ingest copy stream into two device buffers, chunk i + 1 while chunk i is scanned, and
+// chunk (whole genomes) on the ctx's copy stream into two device buffers, chunk i + 1 while chunk i is scanned, and
 // each chunk is a query of its genomes (contain_fast with the chunk).  rows: by chunk, then by (sample, genome);
 // row.genome is the global index.  Its blocks go back to the ctx cache when it returns.  src holds all samples in one
 // batch (scan_one_batch).
@@ -378,7 +368,7 @@ static int scan_sweep(syl_db_shards *s, SampleSource &src, const syl_contain_par
     DevBuf<SampleTable> tables;
     DevBuf<uint32_t> dir, fp;
     std::vector<SampleTable> ht;
-    int rc = build_tables(ctx, v.data(), S, tables, dir, fp, ht);
+    SYL_TRY(build_tables(ctx, v.data(), S, tables, dir, fp, ht));
     std::vector<uint64_t> first;
     cut_scan_chunks(s->kmer_off, s->G, scan_chunk_env(), scan_chunk_genomes(S), first);
     const size_t nc = first.size() - 1;
@@ -387,12 +377,17 @@ static int scan_sweep(syl_db_shards *s, SampleSource &src, const syl_contain_par
         max_n = std::max(max_n, s->kmer_off[first[i + 1]] - s->kmer_off[first[i]]);
         max_g = std::max(max_g, first[i + 1] - first[i]);
     }
-    struct Slot {
-        DevBuf<uint64_t> kmers, off;
-        DevBuf<uint32_t> glen;
-        cudaEvent_t staged = nullptr, used = nullptr;
-    } slot[2];
+    struct Slot { DevBuf<uint64_t> kmers, off; DevBuf<uint32_t> glen; } slot[2];
+    SlotHandoff<2> handoff;  // after the slots (ingest.hpp)
     cudaStream_t cs = nullptr;
+    SYL_TRY(ingest_copy_stream(ctx, &cs));
+    for (Slot &sl : slot) {
+        SYL_TRY(sl.kmers.alloc(max_n, st));
+        SYL_TRY(sl.off.alloc(max_g + 1, st));
+        SYL_TRY(sl.glen.alloc(max_g, st));
+    }
+    SYL_TRY(handoff.init(cs, st));
+    SYL_TRY(handoff.fence());  // cached blocks: earlier work
     const bool pinned = s->kmers && ptr_kind(s->kmers) == PtrKind::PINNED;
     std::vector<uint64_t> h_off;
     std::vector<uint32_t> h_glen;
@@ -400,7 +395,7 @@ static int scan_sweep(syl_db_shards *s, SampleSource &src, const syl_contain_par
     auto stage = [&](size_t i) -> int {
         Slot &sl = slot[i % 2];
         const uint64_t a = first[i], G = first[i + 1] - a, k0 = s->kmer_off[a];
-        SYL_CUDA(cudaStreamWaitEvent(cs, sl.used, 0));
+        SYL_TRY(handoff.before_copy(i % 2));
         h_off.resize(G + 1);
         h_glen.resize(G);
         for (uint64_t g = 0; g <= G; g++) h_off[g] = s->kmer_off[a + g] - k0;
@@ -408,22 +403,12 @@ static int scan_sweep(syl_db_shards *s, SampleSource &src, const syl_contain_par
         SYL_TRY(ingest_copy(ctx, sl.off.p, h_off.data(), (G + 1) * 8, false));  // pageable: staged before it returns
         SYL_TRY(ingest_copy(ctx, sl.glen.p, h_glen.data(), G * 4, false));
         SYL_TRY(ingest_copy(ctx, sl.kmers.p, s->kmers + k0, h_off[G] * 8, pinned));
-        SYL_CUDA(cudaEventRecord(sl.staged, cs));
-        return SYL_OK;
+        return handoff.copied_in(i % 2);
     };
-    if (rc == SYL_OK) rc = ingest_copy_stream(ctx, &cs);
-    for (Slot &sl : slot) {
-        if (rc == SYL_OK) rc = sl.kmers.alloc(max_n, st);
-        if (rc == SYL_OK) rc = sl.off.alloc(max_g + 1, st);
-        if (rc == SYL_OK) rc = sl.glen.alloc(max_g, st);
-        if (rc == SYL_OK && cudaEventCreateWithFlags(&sl.staged, cudaEventDisableTiming) != cudaSuccess) rc = SYL_ERR_CUDA;
-        if (rc == SYL_OK && cudaEventCreateWithFlags(&sl.used, cudaEventDisableTiming) != cudaSuccess) rc = SYL_ERR_CUDA;
-        if (rc == SYL_OK && cudaEventRecord(sl.used, st) != cudaSuccess) rc = SYL_ERR_CUDA;  // cached blocks: earlier work
-    }
-    if (rc == SYL_OK && nc) rc = stage(0);
-    for (size_t i = 0; i < nc && rc == SYL_OK; i++) {
+    if (nc) SYL_TRY(stage(0));
+    for (size_t i = 0; i < nc; i++) {
         Slot &sl = slot[i % 2];
-        if (cudaStreamWaitEvent(st, sl.staged, 0) != cudaSuccess) { rc = SYL_ERR_CUDA; break; }
+        SYL_TRY(handoff.take(i % 2));
         syl_db db;
         db.device = ctx->device;
         db.n_genomes = first[i + 1] - first[i];
@@ -439,25 +424,21 @@ static int scan_sweep(syl_db_shards *s, SampleSource &src, const syl_contain_par
         std::vector<syl_ani_row> part;
         JoinRoom room = src.room;
         room.s0 = 0;
-        rc = contain_fast(ctx, &db, v.data(), src.metas.data(), S, p, false, part, next, &room, &ch);
-        if (rc == SYL_OK && cudaEventRecord(sl.used, st) != cudaSuccess) rc = SYL_ERR_CUDA;
-        if (rc == SYL_OK && !next_staged) rc = stage(i + 1);
+        SYL_TRY(contain_fast(ctx, &db, v.data(), src.metas.data(), S, p, false, part, next, &room, &ch));
+        SYL_TRY(handoff.done(i % 2));
+        if (!next_staged) SYL_TRY(stage(i + 1));
         rows.insert(rows.end(), part.begin(), part.end());
     }
     src.done();
-    if (cs) cudaStreamSynchronize(cs);  // the slots go back to the ctx cache, whose users run on the ctx stream
-    cudaStreamSynchronize(st);
-    for (Slot &sl : slot)
-        for (cudaEvent_t e : {sl.staged, sl.used})
-            if (e) cudaEventDestroy(e);
-    if (rc == SYL_OK && debug_timing()) {
+    cudaStreamSynchronize(st);  // the handoff drains the copy stream as it returns
+    if (debug_timing()) {
         SYL_TRY(syl_ctx_kernel_time(ctx, SYL_KERNEL_SCAN, &scan1, nullptr, 0));
         SYL_TRY(syl_ctx_kernel_time(ctx, SYL_KERNEL_STATS, &stats1, nullptr, 0));
         fprintf(stderr, "[db scan] samples %u chunks %zu genome k-mers %llu: H2D %llu bytes (%s), scan %.1f ms, stats %.1f ms, pass 1 %.1f ms\n",
                 S, nc, (unsigned long long)s->kmer_off[s->G], (unsigned long long)(ctx->ingest_h2d_bytes - h2d0),
                 pinned ? "pinned" : "pageable", scan1 - scan0, stats1 - stats0, ms_since(t0));
     }
-    return rc;
+    return SYL_OK;
 }
 
 static ScanShape shards_shape(const syl_db_shards *s, uint32_t S, uint64_t sample_kmers, bool one_batch) {
@@ -694,14 +675,15 @@ static int sample_budget(syl_ctx *ctx, uint64_t *budget) {
     return SYL_OK;
 }
 
-// the batches of host samples (sample_batches.hpp) against G genomes per join, within `budget`; SYL_SAMPLE_BATCH=N
-// (read per call) caps a batch at N samples
+// What a batch of host samples costs (sample_batches.hpp), and SYL_SAMPLE_BATCH=N (read per call): at most N samples
+// per batch (0: no cap)
+constexpr BatchCost HOST_BATCH_COST{36, 4 * 8 + sizeof(SampleView) + 96 * ROW_BYTES, 16, COV_BINS * 4 + 16, 256 * ROW_BYTES + (1u << 20)};
+static uint32_t sample_batch_env() { const char *e = getenv("SYL_SAMPLE_BATCH"); return e ? (uint32_t)std::max(0, atoi(e)) : 0; }
+
+// the batches of host samples against G genomes per join, within `budget`
 static BatchPlanResult plan_host_batches(const uint64_t *off, uint32_t S, uint64_t G, uint64_t budget, std::vector<uint32_t> &plan,
                                          uint32_t *bad, uint64_t *need) {
-    uint32_t forced = 0;
-    if (const char *e = getenv("SYL_SAMPLE_BATCH")) forced = (uint32_t)std::max(0, atoi(e));
-    const BatchCost cost{36, 4 * 8 + sizeof(SampleView) + 96 * ROW_BYTES, 16, COV_BINS * 4 + 16, 256 * ROW_BYTES + (1u << 20)};
-    return plan_sample_batches(off, S, G, budget, PAIRS_PER_CALL, 0x7FFFFFFFull, forced, cost, plan, bad, need);
+    return plan_sample_batches(off, S, G, budget, PAIRS_PER_CALL, 0x7FFFFFFFull, sample_batch_env(), HOST_BATCH_COST, plan, bad, need);
 }
 
 // Whether S host samples of `kmers` k-mers together, the largest n_max, fit the one batch a scan call stages them in:
@@ -712,10 +694,8 @@ static int scan_one_batch(syl_ctx *ctx, uint32_t S, uint64_t kmers, uint64_t n_m
     uint64_t budget = 0;
     SYL_TRY(sample_budget(ctx, &budget));
     const uint64_t staging = 2 * (8 * scan_chunk_env() + 12 * scan_chunk_genomes(S)), tables = 6 * kmers + 256 * (uint64_t)S;
-    uint32_t forced = 0;
-    if (const char *e = getenv("SYL_SAMPLE_BATCH")) forced = (uint32_t)std::max(0, atoi(e));
-    const BatchCost cost{36, 4 * 8 + sizeof(SampleView) + 96 * ROW_BYTES, 16, COV_BINS * 4 + 16, 256 * ROW_BYTES + (1u << 20)};
-    const unsigned __int128 bytes = (unsigned __int128)2 * batch_bytes(cost, kmers, S, n_max, scan_chunk_genomes(S)) + staging + tables;
+    const uint32_t forced = sample_batch_env();
+    const unsigned __int128 bytes = (unsigned __int128)2 * batch_bytes(HOST_BATCH_COST, kmers, S, n_max, scan_chunk_genomes(S)) + staging + tables;
     *one = S && kmers <= 0x7FFFFFFFull && bytes <= budget && (!forced || S <= forced);
     return SYL_OK;
 }

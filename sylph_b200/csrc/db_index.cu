@@ -7,6 +7,7 @@
 #include <vector>
 
 #include "contain.hpp"
+#include "ingest.hpp"
 
 namespace syl {
 
@@ -217,34 +218,24 @@ static uint64_t db_chunk_entries() {  // SYL_DB_CHUNK overrides (tests; read per
 }
 
 // Hands the input to a pass chunk by chunk.  A device source is one chunk over the whole arrays.  A host source is
-// cut into chunks of at most C entries and, per segment, at most min(C, G) genome offsets; each chunk is copied on a
-// second stream into one of two staging buffers while the previous chunk's kernels run on the ctx stream.
+// cut into chunks of at most C entries and, per segment, at most min(C, G) genome offsets; each chunk is copied on the
+// ctx's copy stream (ingest.hpp), straight from the caller's arrays, into one of two staging buffers while the previous
+// chunk's kernels run on the ctx stream.
 struct DbFeed {
     syl_ctx *ctx;
     const DbInput &in;
     uint64_t C = 0, L = 0;
     BuildBuf stage[2];
-    cudaStream_t cs = nullptr;
-    cudaEvent_t copied[2] = {}, done[2] = {};
+    SlotHandoff<2> handoff;  // after the staging buffers (ingest.hpp); those are not cached blocks, so no fence
     DbFeed(syl_ctx *c, const DbInput &i) : ctx(c), in(i), stage{BuildBuf(c), BuildBuf(c)} {}
-    ~DbFeed() {
-        cudaStreamSynchronize(ctx->stream);
-        if (cs) { cudaStreamSynchronize(cs); cudaStreamDestroy(cs); }
-        for (int b = 0; b < 2; b++) {
-            if (copied[b]) cudaEventDestroy(copied[b]);
-            if (done[b]) cudaEventDestroy(done[b]);
-        }
-    }
     int init() {
         if (in.mem == SYL_MEM_DEVICE) return SYL_OK;
         C = std::min<uint64_t>(db_chunk_entries(), in.n[0] + in.n[1]);
         L = std::min<uint64_t>(C, in.G);
-        SYL_CUDA(cudaStreamCreateWithFlags(&cs, cudaStreamNonBlocking));
-        for (int b = 0; b < 2; b++) {
-            SYL_CUDA(cudaEventCreateWithFlags(&copied[b], cudaEventDisableTiming));
-            SYL_CUDA(cudaEventCreateWithFlags(&done[b], cudaEventDisableTiming));
-            SYL_TRY(stage[b].alloc((C + 2 * L) * 8));
-        }
+        cudaStream_t cs = nullptr;
+        SYL_TRY(ctx_copy_stream(ctx, &cs));
+        SYL_TRY(handoff.init(cs, ctx->stream));
+        for (int b = 0; b < 2; b++) SYL_TRY(stage[b].alloc((C + 2 * L) * 8));
         return SYL_OK;
     }
     // the host chunk that starts at entry e of the concatenated parts; advances e past it
@@ -268,7 +259,6 @@ struct DbFeed {
         return ns;
     }
     template <typename F> int pass(F launch) {
-        cudaStream_t st = ctx->stream;
         if (in.mem == SYL_MEM_DEVICE) {
             DbChunk c{};
             int ns = 0;
@@ -289,23 +279,23 @@ struct DbFeed {
             uint64_t p0[2], p1[2], glo[2], ghi[2];
             uint32_t part[2];
             const int ns = plan(e, p0, p1, glo, ghi, part);
-            if (i >= 2) SYL_CUDA(cudaStreamWaitEvent(cs, done[b], 0));
+            SYL_TRY(handoff.before_copy(b));
             uint64_t *kw = stage[b].as<uint64_t>(), *ow = kw + C;
             DbChunk c{};
             for (int s = 0; s < ns; s++) {
                 const uint64_t n = p1[s] - p0[s], no = ghi[s] - glo[s] + 1;
-                SYL_CUDA(cudaMemcpyAsync(kw, in.keys[part[s]] + p0[s], n * 8, cudaMemcpyHostToDevice, cs));
-                SYL_CUDA(cudaMemcpyAsync(ow, in.off[part[s]] + glo[s], no * 8, cudaMemcpyHostToDevice, cs));
+                SYL_CUDA(cudaMemcpyAsync(kw, in.keys[part[s]] + p0[s], n * 8, cudaMemcpyHostToDevice, handoff.cs));
+                SYL_CUDA(cudaMemcpyAsync(ow, in.off[part[s]] + glo[s], no * 8, cudaMemcpyHostToDevice, handoff.cs));
                 c.keys[s] = kw; c.off[s] = ow; c.n_off[s] = no; c.g0[s] = glo[s]; c.p0[s] = p0[s]; c.n[s] = n; c.part[s] = part[s];
                 kw += n;
                 ow += no;
             }
-            SYL_CUDA(cudaEventRecord(copied[b], cs));
-            SYL_CUDA(cudaStreamWaitEvent(st, copied[b], 0));
+            SYL_TRY(handoff.copied_in(b));
+            SYL_TRY(handoff.take(b));
             launch(c);
             ctx->launches++;
             SYL_CUDA(cudaGetLastError());
-            SYL_CUDA(cudaEventRecord(done[b], st));
+            SYL_TRY(handoff.done(b));
         }
         return SYL_OK;
     }

@@ -68,39 +68,27 @@ void plan_chunks(const Mate *m, int n_mates, uint64_t n_reads, uint64_t max_base
 }
 
 struct HostIngest {
+    // the ctx's copy stream (ingest.hpp); destroyed after the handoffs below have drained it
+    std::unique_ptr<CUstream_st, cudaError_t (*)(cudaStream_t)> copy_stream{nullptr, cudaStreamDestroy};
     std::unique_ptr<PackPool> pool;
-    cudaStream_t copy_stream = nullptr;  // the H2D copies of both rings
     // packed ring: words and chunk-relative u32 offsets, written by the pool
     uint32_t *h_words[ING_SLOTS] = {}, *h_off[ING_SLOTS] = {};  // pinned
     uint32_t *d_words[ING_SLOTS] = {}, *d_off32[ING_SLOTS] = {};
     uint64_t *d_off64[ING_SLOTS] = {};
     uint64_t cap_words = 0, cap_recs = 0;
-    cudaEvent_t ev_copied[ING_SLOTS] = {}, ev_used[ING_SLOTS] = {};
     // ASCII ring: bases (or caller 2-bit words) and u64 offsets copied from caller memory as they are
     uint8_t *d_asc[2] = {};
     uint64_t *d_aoff[2] = {};
     uint64_t cap_asc = 0, cap_aoff = 0;
-    cudaEvent_t ev_a_copied[2] = {}, ev_a_used[2] = {};
     int a_slot = 0, a_last = -1;  // next ASCII slot; slot of the latest ASCII copy (-1: none yet)
     int r_slot = 0;               // next packed-ring slot of ingest_copy's pageable pieces
+    SlotHandoff<ING_SLOTS> packed;  // the packed ring's slots (also ingest_copy's pinned pieces)
+    SlotHandoff<2> ascii;           // the ASCII ring's slots
 
-    int init() {
-        if (copy_stream) return SYL_OK;
-        SYL_CUDA(cudaStreamCreateWithFlags(&copy_stream, cudaStreamNonBlocking));
-        for (int i = 0; i < ING_SLOTS; i++) {
-            SYL_CUDA(cudaEventCreateWithFlags(&ev_copied[i], cudaEventDisableTiming));
-            SYL_CUDA(cudaEventCreateWithFlags(&ev_used[i], cudaEventDisableTiming));
-        }
-        for (int i = 0; i < 2; i++) {
-            SYL_CUDA(cudaEventCreateWithFlags(&ev_a_copied[i], cudaEventDisableTiming));
-            SYL_CUDA(cudaEventCreateWithFlags(&ev_a_used[i], cudaEventDisableTiming));
-        }
-        return SYL_OK;
-    }
     // the two streams that use the ring buffers: idle before a buffer is freed, and after a failed call
     void drain(cudaStream_t st) {
         cudaStreamSynchronize(st);
-        cudaStreamSynchronize(copy_stream);
+        cudaStreamSynchronize(copy_stream.get());
     }
     void free_packed() {
         for (int i = 0; i < ING_SLOTS; i++) {
@@ -177,7 +165,7 @@ struct HostIngest {
         a_slot ^= 1;
         const uint64_t no = c.n_off();
         const bool words = m[0].packed != nullptr;
-        cudaStreamWaitEvent(copy_stream, ev_a_used[slot], 0);
+        ascii.before_copy(slot);
         Mate bt[2] = {};
         for (int i = 0; i < n_mates; i++) {
             const void *src = words ? (const void *)(m[0].packed + word0(c)) : (const void *)(m[i].bases + c.base[i]);
@@ -185,8 +173,8 @@ struct HostIngest {
             uint8_t *dst = d_asc[slot] + (i ? mate2_at(c.nb[0]) : 0);
             if (words) bt[i] = {nullptr, reinterpret_cast<const uint32_t *>(dst), c.nb[i] + c.base[i] % 16, d_aoff[slot], word0(c) * 16};
             else bt[i] = {dst, nullptr, c.nb[i], d_aoff[slot] + i * no, c.base[i]};
-            if ((bytes && cudaMemcpyAsync(dst, src, bytes, cudaMemcpyHostToDevice, copy_stream) != cudaSuccess) ||
-                cudaMemcpyAsync((void *)bt[i].off, m[i].off + c.r0, no * 8, cudaMemcpyHostToDevice, copy_stream) != cudaSuccess) {
+            if ((bytes && cudaMemcpyAsync(dst, src, bytes, cudaMemcpyHostToDevice, copy_stream.get()) != cudaSuccess) ||
+                cudaMemcpyAsync((void *)bt[i].off, m[i].off + c.r0, no * 8, cudaMemcpyHostToDevice, copy_stream.get()) != cudaSuccess) {
                 set_error("H2D copy failed");
                 return SYL_ERR_CUDA;
             }
@@ -194,10 +182,10 @@ struct HostIngest {
         }
         if (words) ctx->ingest_chunks_packed++;
         else ctx->ingest_chunks_ascii++;
-        cudaEventRecord(ev_a_copied[slot], copy_stream);
-        cudaStreamWaitEvent(ctx->stream, ev_a_copied[slot], 0);
+        ascii.copied_in(slot);
+        ascii.take(slot);
         const int rc = sink(bt, ci);
-        cudaEventRecord(ev_a_used[slot], ctx->stream);
+        ascii.done(slot);
         a_last = slot;
         return rc;
     }
@@ -205,15 +193,6 @@ struct HostIngest {
         pool.reset();
         free_packed();
         free_ascii();
-        for (int i = 0; i < ING_SLOTS; i++) {
-            if (ev_copied[i]) cudaEventDestroy(ev_copied[i]);
-            if (ev_used[i]) cudaEventDestroy(ev_used[i]);
-        }
-        for (int i = 0; i < 2; i++) {
-            if (ev_a_copied[i]) cudaEventDestroy(ev_a_copied[i]);
-            if (ev_a_used[i]) cudaEventDestroy(ev_a_used[i]);
-        }
-        if (copy_stream) cudaStreamDestroy(copy_stream);
     }
 };
 
@@ -252,10 +231,9 @@ static int ship_own(syl_ctx *ctx, const Mate &m, const Chunk &c, size_t ci, cons
 }
 
 int feed_host(syl_ctx *ctx, const Mate *m, int n_mates, const std::vector<Chunk> &chunks, bool ascii_only, const ChunkSink &sink) {
-    if (!ctx->ingest) ctx->ingest = new HostIngest();
+    cudaStream_t st = ctx->stream, cs = nullptr;
+    SYL_TRY(ctx_copy_stream(ctx, &cs));
     HostIngest &I = *static_cast<HostIngest *>(ctx->ingest);
-    SYL_TRY(I.init());
-    cudaStream_t st = ctx->stream, cs = I.copy_stream;
     const bool words = m[0].packed != nullptr;
     if (ascii_only || words) {
         SYL_TRY(I.ensure_ascii(st, chunks, n_mates, words, words ? ING_CHUNK / 4 : ING_ASCII_CHUNK));
@@ -305,7 +283,7 @@ int feed_host(syl_ctx *ctx, const Mate *m, int n_mates, const std::vector<Chunk>
         if (chunks[(size_t)f].own) {  // ---- a chunk of its own (no pool items): in order, from the front
             rc = ship_own(ctx, m[0], chunks[(size_t)f], (size_t)f, sink);
             // every chunk up to f is done; the packed ones have crossed the link once the last of them has
-            if (last_packed >= 0) cudaEventSynchronize(I.ev_copied[last_packed % ING_SLOTS]);
+            if (last_packed >= 0) cudaEventSynchronize(I.packed.copied[last_packed % ING_SLOTS]);
             I.pool->open_gate(f + ING_SLOTS);
             f++;
             continue;
@@ -316,23 +294,23 @@ int feed_host(syl_ctx *ctx, const Mate *m, int n_mates, const std::vector<Chunk>
             const Chunk &c = chunks[ci];
             const int slot = (int)(ci % ING_SLOTS);
             const uint64_t nw = (footprint(c, n_mates) + 15) / 16, no = n_mates * c.n_off();  // both mates in one copy each
-            cudaStreamWaitEvent(cs, I.ev_used[slot], 0);  // the seeding of the previous chunk in this slot is done
+            I.packed.before_copy(slot);  // the seeding of the previous chunk in this slot is done
             if (cudaMemcpyAsync(I.d_words[slot], I.h_words[slot], nw * 4, cudaMemcpyHostToDevice, cs) != cudaSuccess ||
                 cudaMemcpyAsync(I.d_off32[slot], I.h_off[slot], no * 4, cudaMemcpyHostToDevice, cs) != cudaSuccess) {
                 rc = SYL_ERR_CUDA; set_error("H2D copy failed"); break;
             }
             ctx->ingest_h2d_bytes += nw * 4 + no * 4;
-            cudaEventRecord(I.ev_copied[slot], cs);
-            cudaStreamWaitEvent(st, I.ev_copied[slot], 0);
+            I.packed.copied_in(slot);
+            I.packed.take(slot);
             k_off32_to_64<<<nblk(no, 256), 256, 0, st>>>(I.d_off32[slot], no, I.d_off64[slot]);
             ctx->launches++;
             Mate bt[2] = {};
             for (int i = 0; i < n_mates; i++)
                 bt[i] = {nullptr, I.d_words[slot] + (i ? mate2_at(c.nb[0]) / 16 : 0), c.nb[i], I.d_off64[slot] + i * c.n_off(), 0};
             rc = sink(bt, ci);
-            cudaEventRecord(I.ev_used[slot], st);
+            I.packed.done(slot);
             if (last_packed >= 0) {  // the pinned buffers of the previous packed chunk have crossed the link: refill them
-                cudaEventSynchronize(I.ev_copied[last_packed % ING_SLOTS]);
+                cudaEventSynchronize(I.packed.copied[last_packed % ING_SLOTS]);
                 I.pool->open_gate(last_packed + ING_SLOTS);
             }
             last_packed = f;
@@ -341,7 +319,7 @@ int feed_host(syl_ctx *ctx, const Mate *m, int n_mates, const std::vector<Chunk>
             steal_turn = true;
             continue;
         }
-        const bool ascii_busy = !force_steal && I.a_last >= 0 && cudaEventQuery(I.ev_a_copied[I.a_last]) == cudaErrorNotReady;
+        const bool ascii_busy = !force_steal && I.a_last >= 0 && cudaEventQuery(I.ascii.copied[I.a_last]) == cudaErrorNotReady;
         if (steal_ok && !ascii_busy && (!force_steal || steal_turn) && bk > f && !chunks[(size_t)bk].own &&
             I.pool->try_skip_chunk((uint32_t)bk)) {  // ---- ASCII chunk from the back
             rc = I.ship_ascii(ctx, m, n_mates, chunks[(size_t)bk], (size_t)bk, sink);
@@ -364,20 +342,30 @@ int feed_host(syl_ctx *ctx, const Mate *m, int n_mates, const std::vector<Chunk>
     return rc;
 }
 
-int ingest_copy_stream(syl_ctx *ctx, cudaStream_t *cs) {
+// the one place that creates the ctx's ingest state, its copy stream and the handoffs of both rings
+int ctx_copy_stream(syl_ctx *ctx, cudaStream_t *cs) {
     if (!ctx->ingest) ctx->ingest = new HostIngest();
     HostIngest &I = *static_cast<HostIngest *>(ctx->ingest);
-    SYL_TRY(I.init());
-    SYL_TRY(I.ensure_packed(ctx->stream, {}, 1));
-    *cs = I.copy_stream;
+    if (!I.copy_stream) {
+        SYL_CUDA(cudaStreamCreateWithFlags(cs, cudaStreamNonBlocking));
+        I.copy_stream.reset(*cs);
+        SYL_TRY(I.packed.init(*cs, ctx->stream));
+        SYL_TRY(I.ascii.init(*cs, ctx->stream));
+    }
+    *cs = I.copy_stream.get();
     return SYL_OK;
+}
+
+int ingest_copy_stream(syl_ctx *ctx, cudaStream_t *cs) {
+    SYL_TRY(ctx_copy_stream(ctx, cs));
+    return static_cast<HostIngest *>(ctx->ingest)->ensure_packed(ctx->stream, {}, 1);
 }
 
 int ingest_copy(syl_ctx *ctx, void *dst, const void *src, uint64_t bytes, bool pinned) {
     HostIngest &I = *static_cast<HostIngest *>(ctx->ingest);
     ctx->ingest_h2d_bytes += bytes;
     if (pinned) {
-        if (bytes) SYL_CUDA(cudaMemcpyAsync(dst, src, bytes, cudaMemcpyHostToDevice, I.copy_stream));
+        if (bytes) SYL_CUDA(cudaMemcpyAsync(dst, src, bytes, cudaMemcpyHostToDevice, I.copy_stream.get()));
         return SYL_OK;
     }
     const uint64_t piece = I.cap_words * 4;
@@ -385,10 +373,10 @@ int ingest_copy(syl_ctx *ctx, void *dst, const void *src, uint64_t bytes, bool p
         const int slot = I.r_slot;
         I.r_slot = (I.r_slot + 1) % ING_SLOTS;
         const uint64_t n = std::min(piece, bytes - o);
-        SYL_CUDA(cudaEventSynchronize(I.ev_copied[slot]));  // the slot's previous piece has crossed the link
+        SYL_CUDA(cudaEventSynchronize(I.packed.copied[slot]));  // the slot's previous piece has crossed the link
         memcpy(I.h_words[slot], static_cast<const uint8_t *>(src) + o, n);
-        SYL_CUDA(cudaMemcpyAsync(static_cast<uint8_t *>(dst) + o, I.h_words[slot], n, cudaMemcpyHostToDevice, I.copy_stream));
-        SYL_CUDA(cudaEventRecord(I.ev_copied[slot], I.copy_stream));
+        SYL_CUDA(cudaMemcpyAsync(static_cast<uint8_t *>(dst) + o, I.h_words[slot], n, cudaMemcpyHostToDevice, I.copy_stream.get()));
+        SYL_TRY(I.packed.copied_in(slot));
     }
     return SYL_OK;
 }

@@ -64,10 +64,49 @@ int feed_host(syl_ctx *ctx, const Mate *m, int n_mates, const std::vector<Chunk>
 // kept until the ctx is destroyed; the ASCII ring of chunks taken from the back is counted whether or not it is used).
 uint64_t ring_bytes_after(const syl_ctx *ctx, const std::vector<Chunk> &chunks, int n_mates, bool ascii_only);
 
-// Whole host arrays to the device on the ctx's copy stream (host samples): *cs is that stream.  ingest_copy copies
-// `bytes` from src to dst on it, straight from pinned memory, from pageable memory through the pinned ring in slot-sized
-// pieces (a pageable cudaMemcpyAsync would wait for the copy stream and block the calling thread).
+// Host input staged into device slots while the ctx stream works on earlier ones (both rings above, host samples, scan
+// and index-build chunks) crosses the link on the ctx's ONE copy stream, and a SlotHandoff hands each slot between the
+// two streams.  ctx_copy_stream: *cs is that stream, created on first use with no ring; ingest_copy_stream: the same
+// once the pinned ring exists.  ingest_copy copies `bytes` from src to dst on it, straight from pinned memory, from
+// pageable memory through the pinned ring in slot-sized pieces (a pageable cudaMemcpyAsync would wait for the copy
+// stream and block the calling thread).
+int ctx_copy_stream(syl_ctx *ctx, cudaStream_t *cs);
 int ingest_copy_stream(syl_ctx *ctx, cudaStream_t *cs);
 int ingest_copy(syl_ctx *ctx, void *dst, const void *src, uint64_t bytes, bool pinned);
+
+// The handoff of N device slots between the copy stream cs, which fills them, and the ctx stream st, which reads them.
+// Per use of slot k: before_copy(k) (cs waits until st is done with k's last contents; a slot never used is free), the
+// copies, copied_in(k) (on cs), take(k) (st waits for the copy; a slot may be staged well before it is taken), st's
+// work on it, done(k) (on st).  fence(): cs waits once for st's work so far, for slots made of ctx-cache blocks.  The
+// slots' buffers and which slot comes next stay with the user.  Declare it AFTER the slot buffers: its destructor
+// drains cs, so the copies into cached blocks have run before those blocks go back to the ctx cache.
+template <int N>
+struct SlotHandoff {
+    cudaStream_t cs = nullptr, st = nullptr;
+    cudaEvent_t copied[N] = {}, used[N] = {};  // a host that waits on or polls the copy into slot k reads copied[k]
+    SlotHandoff() = default;
+    SlotHandoff(const SlotHandoff &) = delete;
+    SlotHandoff &operator=(const SlotHandoff &) = delete;
+    ~SlotHandoff() {
+        if (cs) cudaStreamSynchronize(cs);
+        for (int k = 0; k < N; k++)
+            for (cudaEvent_t e : {copied[k], used[k]})
+                if (e) cudaEventDestroy(e);
+    }
+    int init(cudaStream_t copy_stream, cudaStream_t ctx_stream) {
+        cs = copy_stream;
+        st = ctx_stream;
+        for (int k = 0; k < N; k++) {
+            SYL_CUDA(cudaEventCreateWithFlags(&copied[k], cudaEventDisableTiming));
+            SYL_CUDA(cudaEventCreateWithFlags(&used[k], cudaEventDisableTiming));
+        }
+        return SYL_OK;
+    }
+    int fence() { SYL_CUDA(cudaEventRecord(used[0], st)); SYL_CUDA(cudaStreamWaitEvent(cs, used[0], 0)); return SYL_OK; }
+    int before_copy(int k) { SYL_CUDA(cudaStreamWaitEvent(cs, used[k], 0)); return SYL_OK; }
+    int copied_in(int k) { SYL_CUDA(cudaEventRecord(copied[k], cs)); return SYL_OK; }
+    int take(int k) { SYL_CUDA(cudaStreamWaitEvent(st, copied[k], 0)); return SYL_OK; }
+    int done(int k) { SYL_CUDA(cudaEventRecord(used[k], st)); return SYL_OK; }
+};
 
 }  // namespace syl

@@ -272,6 +272,7 @@ def test_build_memory_is_bounded(monkeypatch, big_db):
     try:
         held0, peak0 = ctx.device_bytes(reset_peak=True)
         assert held0 == 0 and peak0 == 0
+        stats0 = ctx.ingest_stats()
         db1 = ctx.build_db_arrays(*_args(big_db))
         held, peak = ctx.device_bytes(reset_peak=True)
         assert peak <= index + staging + small, (peak, index + staging + small)
@@ -280,6 +281,9 @@ def test_build_memory_is_bounded(monkeypatch, big_db):
         held2, peak2 = ctx.device_bytes()
         assert held2 <= 2 * index + (1 << 20), (held2, 2 * index)
         assert peak2 <= index + held + staging + small
+        # the chunks cross on the ctx's copy stream, straight from the arrays: no staging ring, no ingest bytes counted
+        assert ctx.ingest_ring_bytes() == (0, 0)
+        assert ctx.ingest_stats() == stats0
         db2.free()
         db1.free()
         assert ctx.device_bytes()[0] == held2      # freed handles return their blocks to the ctx cache

@@ -1,8 +1,9 @@
 """GPU: query and profile samples from host memory (syl_query_host_samples / syl_profile_host_samples).  Rows equal
 the handle path's (syl_sample_upload + syl_query / syl_profile, or the _shards calls) bit for bit, at one sample per
 batch, three per batch and the budget's own batches, on one index and on forced shards, for query, profile and profile
--u -I 98, with samples of c below the db's, empty samples and unsorted input, from pinned and pageable arrays.  Also: the
-capacity protocol on both db kinds, every argument error, the device-memory bound, and one build per shard per call."""
+-u -I 98, with samples of c below the db's, empty samples and unsorted input, from pinned and pageable arrays.  Also:
+shard builds in small chunks against one-sample batches, equal to the one-index call in both formulations; the capacity
+protocol on both db kinds, every argument error, the device-memory bound, and one build per shard per call."""
 import os
 import subprocess
 import sys
@@ -104,6 +105,29 @@ def test_rows_equal_handle_path(ctx, world, monkeypatch, batch, kind):
     finally:
         if kind == "shards":
             target.free()
+
+
+@pytest.mark.parametrize("csr", [False, True], ids=["hist", "csr"])
+def test_shard_builds_share_the_copy_stream_with_batches(ctx, world, monkeypatch, csr):
+    """index chunks of 4096 entries and one sample per batch: each shard build's chunk copies and the staging of the next
+    batch take turns on the ctx's copy stream; rows equal the one-index call's, from pageable and pinned arrays"""
+    for v in ("SYL_DB_SHARD_ENTRIES", "SYL_CONTAIN_CSR", "SYL_BOOT_REPLAY"):
+        monkeypatch.delenv(v, raising=False)
+    monkeypatch.setenv("SYL_DB_CHUNK", "4096")
+    monkeypatch.setenv("SYL_SAMPLE_BATCH", "1")
+    if csr:
+        monkeypatch.setenv("SYL_CONTAIN_CSR", "1")
+    d, hs = world["d"], world["hs"]
+    sh = ctx.db_shards(d["kmers"], d["kmer_off"], d["tracked"], d["tracked_off"], d["gn_size"], c=200,
+                       max_entries=cap_for("uneven", d))
+    try:
+        assert len(sh) >= 2 and all(e > 4 * 4096 for _, _, e in sh.ranges())
+        for mode in MODES:
+            want = run_handles(ctx, world["db"], world["handles"], mode, False)
+            for arrays, what in (((hs["hashes"], hs["counts"]), "pageable"), (world["pinned"], "pinned")):
+                same(run_host(ctx, sh, hs, arrays, mode), want, (csr, mode, what))
+    finally:
+        sh.free()
 
 
 @pytest.mark.parametrize("kind", ["one", "shards"])
