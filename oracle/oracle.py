@@ -28,6 +28,8 @@ class Params(C.Structure):
         ("no_adj", C.c_int),
         ("mean_coverage", C.c_int),
         ("redundant_ani", C.c_double),
+        ("cr_math", C.c_int),                        # 1: the ANI's pow / exp correctly rounded (sylph_oracle.h)
+        ("cr_undecided", C.POINTER(C.c_uint64)),     # set per call by _decided
     ]
 
 
@@ -58,8 +60,10 @@ class AniResult(C.Structure):
 
 
 def default_params(k=31, pseudotax=False, **kw):
+    """the reference's defaults; cr_math=1 rounds the ANI's pow / exp correctly (as the device does) instead of
+    calling glibc"""
     p = Params(k=k, min_number_kmers=50.0, min_count_correct=3.0, minimum_ani=-1.0,
-               pseudotax=int(pseudotax), no_ci=0, no_adj=0, mean_coverage=0, redundant_ani=99.0)
+               pseudotax=int(pseudotax), no_ci=0, no_adj=0, mean_coverage=0, redundant_ani=99.0, cr_math=0)
     for a, b in kw.items():
         setattr(p, a, b)
     return p
@@ -254,10 +258,24 @@ class Sample:
             self._h = None
 
 
+def _decided(params, call):
+    """call(params) with a private undecided-call counter under cr_math; raises if any ANI call fell within 2^-100 of
+    a rounding midpoint, where the correctly rounded value is not known from the quad result"""
+    if not params.cr_math:
+        return call(params)
+    n = C.c_uint64(0)
+    p = Params.from_buffer_copy(params)
+    p.cr_undecided = C.pointer(n)
+    out = call(p)
+    if n.value:
+        raise ValueError("%d ANI pow / exp calls lie too close to a rounding midpoint to be rounded correctly" % n.value)
+    return out
+
+
 def get_stats(params, genome_kmers, sample, genome_index=0):
     g = np.ascontiguousarray(genome_kmers, dtype=np.uint64)
     r = AniResult()
-    ok = lib().syo_get_stats(C.byref(params), _ptr(g), len(g), sample._h, genome_index, C.byref(r))
+    ok = _decided(params, lambda p: lib().syo_get_stats(C.byref(p), _ptr(g), len(g), sample._h, genome_index, C.byref(r)))
     return r if ok else None
 
 
@@ -275,11 +293,12 @@ def contain_sample(params, kmers, kmer_off, tracked, tracked_off, gn_size, sampl
     n = len(kmer_off) - 1
     out = (AniResult * max(n, 1))()
     if unknown is not None:
-        m = lib().syo_contain_sample_unknown(C.byref(params), _ptr(kmers), _ptr(kmer_off), _ptr(tr), _ptr(tro), _ptr(gs), n,
-                                             sample._h, nthreads, out, max(n, 1), C.byref(unknown))
+        m = _decided(params, lambda p: lib().syo_contain_sample_unknown(
+            C.byref(p), _ptr(kmers), _ptr(kmer_off), _ptr(tr), _ptr(tro), _ptr(gs), n, sample._h, nthreads, out, max(n, 1),
+            C.byref(unknown)))
     else:
-        m = lib().syo_contain_sample(C.byref(params), _ptr(kmers), _ptr(kmer_off), _ptr(tr), _ptr(tro), _ptr(gs), n,
-                                     sample._h, nthreads, out, max(n, 1))
+        m = _decided(params, lambda p: lib().syo_contain_sample(
+            C.byref(p), _ptr(kmers), _ptr(kmer_off), _ptr(tr), _ptr(tro), _ptr(gs), n, sample._h, nthreads, out, max(n, 1)))
     assert m >= 0
     return [out[i] for i in range(m)]
 

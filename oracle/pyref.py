@@ -4,7 +4,9 @@ TEST INFRASTRUCTURE ONLY.  Written from SURVEY.md §8 / the reference sources wi
 oracle/sylph_oracle.c, so that the C oracle is cross-checked by a second implementation
 (tests/test_oracle_cpu.py).  Every function cites the reference file:line it follows.
 """
+import decimal
 import math
+from decimal import Decimal
 
 MASK64 = (1 << 64) - 1
 
@@ -218,13 +220,49 @@ def ratio_lambda(full, min_count_correct):
     return cp1 / cc * (most + 1)
 
 
-def ani_from_lambda(lam, k, full):
+# ---- the ANI's pow / exp, correctly rounded --------------------------------------------------------------------------
+_CTX = decimal.Context(prec=50)
+_EXACT = decimal.Context(prec=1200)   # a double and a midpoint between two doubles in decimal without rounding
+
+
+def _nearest(v):
+    """the double nearest the 50-digit Decimal v; refuses a v within 1e-40 (relative) of a midpoint between two
+    doubles, where 50 digits cannot decide the rounding"""
+    y = float(v)
+    for nb in (math.nextafter(y, math.inf), math.nextafter(y, -math.inf)):
+        mid = _EXACT.divide(_EXACT.add(Decimal(y), Decimal(nb)), 2)
+        if _EXACT.abs(_EXACT.subtract(v, mid)) <= _EXACT.multiply(_EXACT.abs(v), Decimal("1e-40")):
+            raise ValueError("too close to a rounding midpoint: %s" % v)
+    return y
+
+
+def cr_pow(x, c):
+    """x ** c (doubles) correctly rounded"""
+    return _nearest(_CTX.power(Decimal(x), Decimal(c)))
+
+
+def cr_exp(z):
+    """exp(z) correctly rounded"""
+    return _nearest(_CTX.exp(Decimal(z)))
+
+
+def ani_pow(x, c, cr_math):
+    """the reference's ANI pow (src/contain.rs:657, :836): glibc's (Python's float power), or correctly rounded"""
+    return cr_pow(x, c) if cr_math else x ** c
+
+
+def ani_exp(z, cr_math):
+    """the reference's ANI exp (src/contain.rs:833)"""
+    return cr_exp(z) if cr_math else math.exp(z)
+
+
+def ani_from_lambda(lam, k, full, cr_math=False):
     """src/contain.rs:817-847"""
     if lam is None:
         return None
     contain = sum(1 for x in full if x != 0)
-    adj = contain / (1.0 - math.exp(-lam)) / len(full)
-    ani = adj ** (1.0 / k)
+    adj = contain / (1.0 - ani_exp(-lam, cr_math)) / len(full)
+    ani = ani_pow(adj, 1.0 / k, cr_math)
     if ani < 0 or math.isnan(ani):
         return None
     return ani
@@ -254,7 +292,7 @@ class WyRand:
         return hi
 
 
-def bootstrap_interval(full, k, min_count_correct):
+def bootstrap_interval(full, k, min_count_correct, cr_math=False):
     """src/contain.rs:849-898"""
     rng = WyRand(7)
     res_a, res_l = [], []
@@ -262,7 +300,7 @@ def bootstrap_interval(full, k, min_count_correct):
     for _ in range(100):
         rv = [full[rng.usize(n)] for _ in range(n)]
         lam = ratio_lambda(rv, min_count_correct)
-        ani = ani_from_lambda(lam, k, rv)
+        ani = ani_from_lambda(lam, k, rv, cr_math)
         if ani is not None and lam is not None:
             res_a.append(ani)
             res_l.append(lam)
@@ -275,9 +313,10 @@ def bootstrap_interval(full, k, min_count_correct):
 
 
 def get_stats(genome_kmers, sample, k=31, min_number_kmers=50.0, min_count_correct=3.0, min_ani=0.90, no_ci=False,
-              winner=None, genome_id=None, mean_coverage=False, no_adj=False):
+              winner=None, genome_id=None, mean_coverage=False, no_adj=False, cr_math=False):
     """src/contain.rs:601-814 (pass 1 when winner is None) -> dict or None.  mean_coverage: the final coverage of a
-    median >= 15 is the mean too (:722); no_adj: the final ANI is the naive one (:740)."""
+    median >= 15 is the mean too (:722); no_adj: the final ANI is the naive one (:740); cr_math: the ANI's pow / exp
+    correctly rounded instead of glibc's."""
     if len(genome_kmers) < min_number_kmers:
         return None
     covs, lost = [], 0
@@ -292,7 +331,7 @@ def get_stats(genome_kmers, sample, k=31, min_number_kmers=50.0, min_count_corre
     if not covs:
         return None
     n = len(genome_kmers)
-    naive = (len(covs) / n) ** (1.0 / k)
+    naive = ani_pow(len(covs) / n, 1.0 / k, cr_math)
     covs.sort()
     median = covs[len(covs) // 2]
     max_cov = float("inf")
@@ -312,27 +351,29 @@ def get_stats(genome_kmers, sample, k=31, min_number_kmers=50.0, min_count_corre
         lam = ratio_lambda(full, min_count_correct)
         status = "LOW" if lam is None else "LAMBDA"
     final_cov = lam if lam is not None else (geq1 if median < 15 or mean_coverage else float(median))
-    est = ani_from_lambda(lam, k, full)
+    est = ani_from_lambda(lam, k, full, cr_math)
     final_ani = naive if (lam is None or est is None or no_adj) else est
     if final_ani < min_ani:
         return None
     ci = None
     if not no_ci and lam is not None:
-        ci = bootstrap_interval(full, k, min_count_correct)
+        ci = bootstrap_interval(full, k, min_count_correct, cr_math)
     return dict(naive_ani=naive, final_est_ani=final_ani, final_est_cov=final_cov, mean_cov=geq1, median_cov=float(median),
                 contain=len(covs), glen=n, status=status, lam=lam, ci=ci, kmers_lost=lost if winner is not None else None)
 
 
 def contain_sample(genomes, sample, k=31, pseudotax=False, min_number_kmers=50.0, min_count_correct=3.0,
-                   minimum_ani=None, redundant_ani=99.0, no_ci=False, unknown=None, mean_coverage=False, no_adj=False):
+                   minimum_ani=None, redundant_ani=99.0, no_ci=False, unknown=None, mean_coverage=False, no_adj=False,
+                   cr_math=False):
     """Inner body of contain() for one sample (src/contain.rs:284-334), written from the reference
     source only.  genomes: list of dict(kmers=[..], tracked=[..], gn_size=int); sample: dict hash->count.
     Pass-1 results are taken in genome-index order (the reference's order is thread-timing dependent).
     unknown = (read_seq_id percent, mean_read_length, sample c): -u with --read-seq-id (:274-279, :377-408).
+    cr_math: the ANI's pow / exp correctly rounded; the k-mer identity and the derep threshold stay on glibc.
     -> list of dicts (get_stats fields + genome, rel_abund, seq_abund) in output order."""
     min_ani = minimum_ani / 100.0 if minimum_ani is not None else (0.95 if pseudotax else 0.90)  # :746-748
     kw = dict(k=k, min_number_kmers=min_number_kmers, min_count_correct=min_count_correct, min_ani=min_ani, no_ci=no_ci,
-              mean_coverage=mean_coverage, no_adj=no_adj)
+              mean_coverage=mean_coverage, no_adj=no_adj, cr_math=cr_math)
     res = []
     for gi, g in enumerate(genomes):  # :286-292
         r = get_stats(g["kmers"], sample, **kw)

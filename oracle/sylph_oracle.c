@@ -6,6 +6,7 @@
 #include "sylph_oracle.h"
 
 #include <math.h>
+#include <quadmath.h>
 #include <stdio.h>
 #include <stdlib.h>
 #include <string.h>
@@ -733,14 +734,35 @@ done:
     return ok;
 }
 
+/* The double nearest the 113-bit q; a q within 2^-100 (relative) of a midpoint between two doubles is counted in
+ * *p->cr_undecided, since libquadmath's own error could then decide the rounding (tests/cpp/crmath_check.cpp
+ * round_quad). */
+static double cr_round(const syo_params *p, __float128 q) {
+    const double y = (double)q;
+    const double up = nextafter(y, INFINITY), dn = nextafter(y, 0.);
+    const __float128 tol = fabsq(q) * (__float128)0x1p-100;
+    if ((fabsq(q - ((__float128)y + (__float128)up) / 2) <= tol || fabsq(q - ((__float128)y + (__float128)dn) / 2) <= tol) &&
+        p->cr_undecided)
+        __atomic_fetch_add(p->cr_undecided, 1, __ATOMIC_RELAXED);
+    return y;
+}
+
+/* the reference's ANI pow / exp: glibc, or correctly rounded under p->cr_math */
+static double ani_pow(const syo_params *p, double x, double c) {
+    return p->cr_math ? cr_round(p, powq((__float128)x, (__float128)c)) : pow(x, c);
+}
+static double ani_exp(const syo_params *p, double z) {
+    return p->cr_math ? cr_round(p, expq((__float128)z)) : exp(z);
+}
+
 /* src/contain.rs:817-847 */
-static int ani_from_lambda(int has_lambda, double lambda, double k, const uint32_t *full, size_t n,
+static int ani_from_lambda(const syo_params *p, int has_lambda, double lambda, double k, const uint32_t *full, size_t n,
                            double *ani_out) {
     if (!has_lambda) return 0;
     size_t contain = 0;
     for (size_t i = 0; i < n; i++) if (full[i] != 0) contain++;
-    double adj = (double)contain / (1. - exp(-lambda)) / (double)n;
-    double ani = pow(adj, 1. / k);
+    double adj = (double)contain / (1. - ani_exp(p, -lambda)) / (double)n;
+    double ani = ani_pow(p, adj, 1. / k);
     if (ani < 0. || isnan(ani)) return 0;
     *ani_out = ani;
     return 1;
@@ -784,7 +806,7 @@ static int dbl_cmp(const void *a, const void *b) {
 }
 
 /* src/contain.rs:849-898 */
-static int bootstrap_interval(const uint32_t *full, size_t n, double k, double min_count_correct,
+static int bootstrap_interval(const syo_params *p, const uint32_t *full, size_t n, double k, double min_count_correct,
                               double ci[4]) {
     wyrand rng = {7}; /* fastrand::seed(7) :854 */
     const int iters = 100;
@@ -795,7 +817,7 @@ static int bootstrap_interval(const uint32_t *full, size_t n, double k, double m
         for (size_t j = 0; j < n; j++) rv[j] = full[wy_mod(&rng, (uint64_t)n)];
         double lam = 0., ani = 0.;
         int hl = ratio_lambda(rv, n, min_count_correct, &lam);
-        int ha = ani_from_lambda(hl, lam, k, rv, n, &ani);
+        int ha = ani_from_lambda(p, hl, lam, k, rv, n, &ani);
         if (ha && hl && !isnan(ani) && !isnan(lam)) {
             res_ani[suc] = ani;
             res_lambda[suc] = lam;
@@ -868,7 +890,7 @@ static int get_stats(const syo_params *p, const uint64_t *gk, size_t n, const sy
     }
     if (contain == 0) { free(covs); return 0; } /* :654 */
     double k = (double)p->k;
-    double naive_ani = pow((double)contain / (double)n, 1. / k);
+    double naive_ani = ani_pow(p, (double)contain / (double)n, 1. / k);
     qsort(covs, contain, sizeof(uint32_t), u32_cmp);
     double median = (double)covs[contain / 2];
     double max_cov = 1.7976931348623157e308; /* f64::MAX */
@@ -897,13 +919,13 @@ static int get_stats(const syo_params *p, const uint64_t *gk, size_t n, const sy
     else final_cov = p->mean_coverage ? geq1_mean : median;
     int has_lambda = status == SYO_LAMBDA_VALUE;
     double est_ani = 0.;
-    int has_est = ani_from_lambda(has_lambda, final_cov, k, full, nfull, &est_ani);
+    int has_est = ani_from_lambda(p, has_lambda, final_cov, k, full, nfull, &est_ani);
     double final_ani = (!has_lambda || !has_est || p->no_adj) ? naive_ani : est_ani;
     double min_ani = p->minimum_ani >= 0. ? p->minimum_ani / 100. : (p->pseudotax ? 0.95 : 0.90);
     if (final_ani < min_ani) { free(covs); free(full); return 0; }
     memset(out, 0, sizeof(*out));
     if (!p->no_ci && has_lambda)
-        out->ci_valid = (uint32_t)bootstrap_interval(full, nfull, k, p->min_count_correct, out->ci);
+        out->ci_valid = (uint32_t)bootstrap_interval(p, full, nfull, k, p->min_count_correct, out->ci);
     out->genome = genome_index;
     out->lambda_status = status;
     out->contain = contain;

@@ -85,6 +85,15 @@ typedef struct {
     int no_adj;
     int mean_coverage;
     double redundant_ani; /* src/cmdline.rs:119 default 99 */
+    /* 0: the reference's ANI calls on glibc (its pow is 0.52 ulp, so about 1 in 1000 results is one ulp off).
+     * 1: those calls correctly rounded: the naive ANI's pow (src/contain.rs:657) and ani_from_lambda's exp and pow
+     * (:833-836, which the final ANI and every bootstrap replicate go through) as libquadmath's powq / expq rounded
+     * to the nearest double.  Every other libm call (the -u k-mer identity, the derep threshold, the Poisson CDF)
+     * stays on glibc in both modes. */
+    int cr_math;
+    /* cr_math: if not NULL, counts the calls whose 113-bit value lies within 2^-100 (relative) of a midpoint between
+     * two doubles, where the quad value cannot decide the rounding (atomically; pass 1 runs on several threads) */
+    uint64_t *cr_undecided;
 } syo_params;
 
 enum { SYO_LAMBDA_LOW = 0, SYO_LAMBDA_HIGH = 1, SYO_LAMBDA_VALUE = 2 };

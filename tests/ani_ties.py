@@ -5,35 +5,18 @@ The reference computes (src/contain.rs:817-847, src/inference.rs:207-242, glibc 
   naive     RN(pow(RN(n / gl), RN(1 / k)))
   adjusted  x1 = RN(exp(-lambda)), RN(pow(RN(RN(nz / RN(1 - x1)) / nfull), RN(1 / k))), lambda = RN(RN(cp1 / cm) * (mode + 1))
 The cr_* functions evaluate the same expressions with every transcendental call correctly rounded (Python decimal at
-50 digits, then the nearest double); the glibc_* functions with Python's float arithmetic, which calls glibc.  The
-device (sylph_b200/csrc/crmath.cuh) is correctly rounded, so on every pinned input glibc must be too (checked by
-tests/test_ani_ties_cpu.py): a pin never rests on a glibc misrounding.
+50 digits, then the nearest double, oracle/pyref.py); the glibc_* functions with Python's float arithmetic, which calls
+glibc.  The device (sylph_b200/csrc/crmath.cuh) is correctly rounded.
 
-The pins were picked by scripts/find_ani_ties.py on an H100 among inputs where CUDA's own pow / exp (torch float64)
-and glibc disagree, so a device that rounds like CUDA's pow fails them; see the pin tables below.
+GATES, WINNER_PAIRS and TIE_PAIRS rest on inputs where glibc is correctly rounded too (checked by
+tests/test_ani_ties_cpu.py); they were picked by scripts/find_ani_ties.py on an H100 among inputs where CUDA's own
+pow / exp (torch float64) and glibc disagree, so a device that rounds like CUDA's pow fails them.  The MISROUNDED pins
+are the other way round: glibc is one ulp off there (found by scripts/find_glibc_misroundings.py), and the device must
+print the correctly rounded ANI and the rows and winners that follow from it, not the glibc reference's.
 """
-import decimal
 import math
-from decimal import Decimal
 
-_CTX = decimal.Context(prec=50)
-
-
-def _nearest(v):
-    """the double nearest the 50-digit Decimal v; refuses a v within 1e-40 (relative) of a rounding midpoint"""
-    y = float(v)
-    for nb in (math.nextafter(y, math.inf), math.nextafter(y, -math.inf)):
-        mid = (Decimal(y) + Decimal(nb)) / 2
-        assert abs(v - mid) > abs(v) * Decimal("1e-40"), ("too close to a midpoint", v)
-    return y
-
-
-def cr_pow(x, c):
-    return _nearest(_CTX.power(Decimal(x), Decimal(c)))
-
-
-def cr_exp(z):
-    return _nearest(_CTX.exp(Decimal(z)))
+from oracle.pyref import cr_exp, cr_pow  # noqa: F401  (50-digit decimal, nearest double, a midpoint refused)
 
 
 def ratio_lambda(hist):
@@ -106,7 +89,7 @@ def calls_of(spec, k):
         return [("pow", spec[1] / spec[2], 1.0 / k)]
     lam = ratio_lambda(hist_of(spec))
     nz = spec[1] + spec[2]
-    return [("exp", -lam), ("pow", nz / (1.0 - math.exp(-lam)) / (nz + spec[3]), 1.0 / k)]
+    return [("exp", -lam), ("pow", nz / (1.0 - cr_exp(-lam)) / (nz + spec[3]), 1.0 / k)]
 
 
 class Case:
@@ -171,10 +154,43 @@ TIE_PAIRS = [
 ]
 
 
-def pinned_specs():
-    for k, spec, *_ in GATES:
+# ---- pins where glibc misrounds (scripts/find_glibc_misroundings.py) ------------------------------------------------
+# (k, spec, glibc's ANI, the correctly rounded ANI): one ulp apart either way, from the naive ANI's pow and from the
+# adjusted ANI's exp / pow
+MISROUNDED = [
+    (21, ("naive", 78, 79), float.fromhex("0x1.ffb0835fb1302p-1"), float.fromhex("0x1.ffb0835fb1303p-1")),
+    (21, ("naive", 71, 358), float.fromhex("0x1.da094e0e32ae4p-1"), float.fromhex("0x1.da094e0e32ae3p-1")),
+    (21, ("adj", 17, 10, 169), float.fromhex("0x1.da21ff355a7d8p-1"), float.fromhex("0x1.da21ff355a7d7p-1")),
+    (21, ("adj", 17, 15, 39), float.fromhex("0x1.f15cc12c4dbeep-1"), float.fromhex("0x1.f15cc12c4dbefp-1")),
+    (31, ("naive", 120, 151), float.fromhex("0x1.fc3804b0174d2p-1"), float.fromhex("0x1.fc3804b0174d3p-1")),
+    (31, ("naive", 246, 271), float.fromhex("0x1.fe6768b75ae50p-1"), float.fromhex("0x1.fe6768b75ae4fp-1")),
+    (31, ("adj", 14, 13, 91), float.fromhex("0x1.eae46448b4ba6p-1"), float.fromhex("0x1.eae46448b4ba5p-1")),
+    (31, ("adj", 19, 10, 91), float.fromhex("0x1.efe481cefeebap-1"), float.fromhex("0x1.efe481cefeebbp-1")),
+]
+
+# (k, spec, p): glibc's ANI is the double below the correctly rounded ANI a, and RN(p / 100) == a.  At -m p correct
+# rounding keeps the row (a >= a) and the glibc reference drops it
+MISROUNDED_GATES = [
+    (21, ("naive", 78, 79), float.fromhex("0x1.8fc1e6a2c26dap+6")),
+    (21, ("adj", 17, 15, 39), float.fromhex("0x1.849076ea9cbd3p+6")),
+    (31, ("naive", 120, 151), float.fromhex("0x1.8d0bc3a992345p+6")),
+    (31, ("adj", 19, 10, 91), float.fromhex("0x1.836a8569b7282p+6")),
+]
+
+# (k, spec A, spec B, winner under glibc, winner correctly rounded): genome 0 = A, genome 1 = B, B = A's counts scaled
+# (the same rational ANI input rounded along another path), so the two ANIs are equal or adjacent doubles and one glibc
+# misrounding reverses the pass-2 winner of the k-mers they share
+MISROUNDED_WINNERS = [
+    (21, ("adj", 65, 60, 1540), ("adj", 13, 12, 308), 0, 1),   # glibc: equal ANIs, A first; correct: B one ulp above
+    (31, ("adj", 39, 36, 798), ("adj", 13, 12, 266), 1, 0),    # glibc: B one ulp above; correct: equal ANIs
+]
+
+
+def pinned_specs(misrounded=True):
+    """(k, spec) of every pin; misrounded=False: only those glibc rounds correctly"""
+    for k, spec, *_ in GATES + (MISROUNDED if misrounded else []):
         yield k, spec
-    for k, a, b in WINNER_PAIRS + TIE_PAIRS:
+    for k, a, b, *_ in WINNER_PAIRS + TIE_PAIRS + (MISROUNDED_WINNERS if misrounded else []):
         yield k, a
         yield k, b
 

@@ -90,8 +90,8 @@ def pair_sketch(path1, path2, name, k=31, c=200, no_dedup=False):
 
 def contain(genomes, samples, pseudotax, min_ani=-1., min_number_kmers=50., min_count_correct=3., redundant_ani=99.,
             no_ci=False, no_adj=False, mean_cov=False, read_seq_id=None):
-    """Expected rows of query / profile: per sample in the given order, the oracle's rows sorted as the reference
-    sorts them (src/contain.rs:329-334).  samples: dicts in the .sylsp layout; the printed sample name is
+    """Expected rows of query / profile: per sample in the given order, the oracle's rows (with the ANI's pow / exp
+    correctly rounded, as the product computes them) sorted as the reference sorts them (src/contain.rs:329-334).  samples: dicts in the .sylsp layout; the printed sample name is
     sample_name if set, else file_name.  -> list of (sample_index, sort_key, row_fields)"""
     from oracle import oracle as O
     k = int(genomes[0]["k"])
@@ -103,7 +103,7 @@ def contain(genomes, samples, pseudotax, min_ani=-1., min_number_kmers=50., min_
     gsz = np.array([g["gn_size"] for g in genomes], np.uint64)
     p = O.default_params(k=k, pseudotax=pseudotax, minimum_ani=float(min_ani), min_number_kmers=float(min_number_kmers),
                          min_count_correct=float(min_count_correct), redundant_ani=float(redundant_ani), no_ci=int(no_ci),
-                         no_adj=int(no_adj), mean_coverage=int(mean_cov))
+                         no_adj=int(no_adj), mean_coverage=int(mean_cov), cr_math=1)
     out = []
     for si, s in enumerate(samples):
         u = None if read_seq_id is None else O.Unknown(read_seq_id, s["mean_read_length"], int(s["c"]))

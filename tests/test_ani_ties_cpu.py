@@ -93,7 +93,7 @@ def test_crmath_log_table_and_ln2():
     assert (float.fromhex(ln2.group(1)), float.fromhex(ln2.group(2))) == split(ctx.ln(Decimal(2)))
 
 
-@pytest.mark.parametrize("k,spec", list(T.pinned_specs()), ids=lambda v: str(v))
+@pytest.mark.parametrize("k,spec", list(T.pinned_specs(misrounded=False)), ids=lambda v: str(v))
 def test_pin_oracle_and_pyref_reproduce_the_ani(k, spec):
     """The oracle's and pyref's rows for the pinned genome carry its glibc ANI bit for bit, and glibc's value is the
     correctly rounded one at every pow / exp call along the way."""
@@ -129,3 +129,65 @@ def test_pairs_are_adjacent_or_equal():
         assert math.nextafter(T.glibc_ani(a, k), math.inf) == T.glibc_ani(b, k), (k, a, b)
     for k, a, b in T.TIE_PAIRS:
         assert T.glibc_ani(a, k) == T.glibc_ani(b, k) and a != b, (k, a, b)
+
+
+def misrounded_call(spec, k):
+    """the pow / exp calls along spec's ANI where glibc and the decimal reference differ"""
+    return [c for c in T.calls_of(spec, k) if (c[1] ** c[2] if c[0] == "pow" else math.exp(c[1])) != decimal_of(c)]
+
+
+@pytest.mark.parametrize("pin", T.MISROUNDED, ids=lambda m: "k%d_%s" % (m[0], "_".join(map(str, m[1]))))
+def test_misrounded_pin_against_decimal_and_glibc(crmath_exe, pin):
+    """glibc's ANI and the correctly rounded one are the pinned adjacent doubles, a glibc call along the way is the
+    misrounded one, and crmath.cuh's host build rounds every call as decimal does.  The oracle and pyref print
+    glibc's ANI in their default mode and the correctly rounded one in their correctly rounded mode."""
+    from oracle import oracle as O
+    from oracle import pyref as R
+    k, spec, a_glibc, a_cr = pin
+    assert T.glibc_ani(spec, k) == a_glibc and T.cr_ani(spec, k) == a_cr
+    assert a_glibc in (math.nextafter(a_cr, math.inf), math.nextafter(a_cr, -math.inf))
+    assert misrounded_call(spec, k)
+    calls = T.calls_of(spec, k)
+    assert cr_eval(crmath_exe, calls) == [decimal_of(c) for c in calls]
+    case = T.Case([spec])
+    d = case.db
+    for cr, a in ((0, a_glibc), (1, a_cr)):
+        rows = O.contain_sample(O.default_params(k=k, minimum_ani=0.0, no_ci=1, cr_math=cr), d["kmers"], d["kmer_off"],
+                                d["tracked"], d["tracked_off"], d["gn_size"], O.Sample(case.hash, case.count))
+        assert len(rows) == 1 and rows[0].final_est_ani == a
+        r = R.get_stats(d["kmers"].tolist(), case.sample, k=k, min_ani=0.0, no_ci=True, cr_math=bool(cr))
+        assert r["final_est_ani"] == a
+
+
+@pytest.mark.parametrize("gate", T.MISROUNDED_GATES, ids=lambda g: "k%d_%s" % (g[0], "_".join(map(str, g[1]))))
+def test_misrounded_gate_keeps_only_the_correctly_rounded_row(gate):
+    """RN(p / 100) is the correctly rounded ANI and glibc's ANI the double below it: at -m p the correctly rounded
+    oracle keeps the row and the glibc oracle drops it."""
+    from oracle import oracle as O
+    k, spec, p = gate
+    a = T.cr_ani(spec, k)
+    assert p / 100.0 == a and T.glibc_ani(spec, k) == math.nextafter(a, -math.inf)
+    case = T.Case([spec])
+    d = case.db
+    for cr in (0, 1):
+        rows = O.contain_sample(O.default_params(k=k, minimum_ani=p, cr_math=cr), d["kmers"], d["kmer_off"], d["tracked"],
+                                d["tracked_off"], d["gn_size"], O.Sample(case.hash, case.count))
+        assert len(rows) == cr
+
+
+@pytest.mark.parametrize("pair", T.MISROUNDED_WINNERS, ids=lambda w: "k%d_%s_%s" % (w[0], w[1][1], w[2][1]))
+def test_misrounded_winner_differs(pair):
+    """A (genome 0) and B: the pass-2 winner is the pinned one in each mode (the greater ANI, A on equal ANIs), in
+    the decimal / glibc restatement and in the oracle."""
+    from oracle import oracle as O
+    k, a, b, win_glibc, win_cr = pair
+    assert win_glibc != win_cr
+    for ani, win in (((T.glibc_ani(a, k), T.glibc_ani(b, k)), win_glibc), ((T.cr_ani(a, k), T.cr_ani(b, k)), win_cr)):
+        assert abs(ani[0] - ani[1]) <= math.ulp(ani[0])
+        assert (0 if ani[0] >= ani[1] else 1) == win
+    case = T.Case([a, b], shared=3)
+    d = case.db
+    for cr, win in ((0, win_glibc), (1, win_cr)):
+        rows = O.contain_sample(O.default_params(k=k, pseudotax=True, minimum_ani=0.0, cr_math=cr), d["kmers"],
+                                d["kmer_off"], d["tracked"], d["tracked_off"], d["gn_size"], O.Sample(case.hash, case.count))
+        assert {r.genome: r.kmers_lost for r in rows} == {win: 0, 1 - win: 3}

@@ -1,12 +1,13 @@
 """ANI near-ties on the device (tests/ani_ties.py): the -m gate at a pinned ANI and one ulp either side, the profile
 winner between genomes whose ANIs are adjacent doubles or equal (both genome orders), and the query order of those
-genomes; in both formulations (per-pair count histograms, CSR).  Every pinned ANI is correctly rounded in glibc too, so
-the device's rows must equal the oracle's bit for bit, ANIs included."""
+genomes; in both formulations (per-pair count histograms, CSR).  The device's rows equal the correctly rounded oracle's
+bit for bit.  On the MISROUNDED pins glibc is one ulp off, and the glibc oracle (the reference's arithmetic) prints
+another ANI, drops the row at the gate, or gives the shared k-mers to the other genome: the device must not."""
 import numpy as np
 import pytest
 
 from tests import ani_ties as T
-from tests.test_contain_gpu import compare, sort_query_rows
+from tests.contain_compare import compare, cr_params, sort_query_rows
 
 pytestmark = pytest.mark.gpu
 
@@ -19,7 +20,16 @@ def formulation(request, monkeypatch):
     return request.param
 
 
+def glibc_rows(case, k, pseudotax, **P):
+    """the oracle's rows with the reference's glibc pow / exp"""
+    from oracle import oracle as O
+    d = case.db
+    return O.contain_sample(O.default_params(k=k, pseudotax=pseudotax, **P), d["kmers"], d["kmer_off"], d["tracked"],
+                            d["tracked_off"], d["gn_size"], O.Sample(case.hash, case.count))
+
+
 def run(ctx, case, k, pseudotax, **P):
+    """the device's rows of case == the correctly rounded oracle's -> (rows, oracle rows)"""
     from oracle import oracle as O
     from sylph_b200.api import contain_params
     d = case.db
@@ -33,11 +43,9 @@ def run(ctx, case, k, pseudotax, **P):
         smp.free()
         db.free()
         g.free()
-    exp = O.contain_sample(O.default_params(k=k, pseudotax=pseudotax, **P), d["kmers"], d["kmer_off"], d["tracked"],
+    exp = O.contain_sample(cr_params(k=k, pseudotax=pseudotax, **P), d["kmers"], d["kmer_off"], d["tracked"],
                            d["tracked_off"], d["gn_size"], O.Sample(case.hash, case.count))
     compare(rows, exp, pseudotax)
-    for r, e in zip(rows, exp):   # pinned inputs: glibc is correctly rounded there, so no ulp of slack
-        assert float(r["naive_ani"]) == e.naive_ani and float(r["final_est_ani"]) == e.final_est_ani
     return rows, exp
 
 
@@ -95,3 +103,48 @@ def test_query_order_of_near_tied_genomes(ctx, formulation, pair, swap):
     want = [0, 1] if ani[0] >= ani[1] else [1, 0]
     assert [int(g) for g in rows["genome"]] == want == [e.genome for e in exp]
     assert np.array_equal(rows["final_est_ani"], [ani[i] for i in want])
+
+
+def spec_id(v):
+    return "_".join(map(str, v[1:])) if isinstance(v, tuple) else str(v)
+
+
+@pytest.mark.parametrize("pseudotax", [False, True])
+@pytest.mark.parametrize("pin", T.MISROUNDED, ids=lambda m: "k%d_%s_%s" % (m[0], m[1][0], spec_id(m[1])))
+def test_ani_where_glibc_misrounds(ctx, formulation, pin, pseudotax):
+    """The device's ANI is the correctly rounded one; the glibc oracle's is one ulp away (the naive ANI too where it
+    is final)."""
+    k, spec, a_glibc, a_cr = pin
+    case = T.Case([spec])
+    rows, _ = run(ctx, case, k, pseudotax, minimum_ani=0.0)
+    ref = glibc_rows(case, k, pseudotax, minimum_ani=0.0)
+    assert len(rows) == len(ref) == 1
+    assert float(rows["final_est_ani"][0]) == a_cr and ref[0].final_est_ani == a_glibc != a_cr
+    if spec[0] == "naive":
+        assert float(rows["naive_ani"][0]) == a_cr and ref[0].naive_ani == a_glibc
+
+
+@pytest.mark.parametrize("pseudotax", [False, True])
+@pytest.mark.parametrize("gate", T.MISROUNDED_GATES, ids=lambda g: "k%d_%s_%s" % (g[0], g[1][0], spec_id(g[1])))
+def test_gate_where_glibc_misrounds(ctx, formulation, gate, pseudotax):
+    """-m p with RN(p / 100) == the correctly rounded ANI: the device keeps the row, the glibc oracle (whose ANI is
+    the double below) drops it."""
+    k, spec, p = gate
+    case = T.Case([spec])
+    rows, _ = run(ctx, case, k, pseudotax, minimum_ani=p)
+    assert len(rows) == 1 and float(rows["final_est_ani"][0]) == p / 100.0
+    assert glibc_rows(case, k, pseudotax, minimum_ani=p) == []
+
+
+@pytest.mark.parametrize("pair", T.MISROUNDED_WINNERS, ids=lambda w: "k%d_%s_%s" % (w[0], spec_id(w[1]), spec_id(w[2])))
+def test_winner_where_glibc_misrounds(ctx, formulation, pair):
+    """Genomes A (index 0) and B sharing SHARED hit k-mers whose ANIs are equal or adjacent doubles, where one glibc
+    misrounding reverses the order: in pass 2 the device gives the shared k-mers to the correctly rounded winner, the
+    glibc oracle to the other genome."""
+    k, a, b, win_glibc, win_cr = pair
+    case = T.Case([a, b], shared=SHARED)
+    rows, _ = run(ctx, case, k, True, minimum_ani=0.0)
+    lost = {int(r["genome"]): int(r["kmers_lost"]) for r in rows}
+    assert win_cr != win_glibc and lost == {win_cr: 0, 1 - win_cr: SHARED}
+    ref = glibc_rows(case, k, True, minimum_ani=0.0)
+    assert {e.genome: e.kmers_lost for e in ref} == {win_glibc: 0, 1 - win_glibc: SHARED}

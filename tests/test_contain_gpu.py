@@ -1,11 +1,11 @@
-"""GPU parity: containment query/profile vs the CPU oracle.
-Integers bit-exact, floats bit-exact except where the reference's glibc pow / exp misround (compare below)."""
+"""GPU parity: containment query/profile vs the CPU oracle in its correctly rounded mode, every field bit-exact
+(tests/contain_compare.py)."""
 import os
 
 import numpy as np
 import pytest
 
-from tests import ani_ties as T
+from tests.contain_compare import compare, cr_params, oracle_rows, sort_query_rows
 from tests.util import DATA, flatten, read_fastx
 
 pytestmark = [pytest.mark.gpu, pytest.mark.usefixtures("contain_mode")]
@@ -23,66 +23,6 @@ def contain_mode(request, monkeypatch):
     if request.param == "synchronous":
         monkeypatch.setenv("SYL_CONTAIN_CSR", "1")
     return request.param
-
-
-def oracle_rows(db, sample_hc, pseudotax, **kw):
-    from oracle import oracle as O
-    p = O.default_params(pseudotax=pseudotax, **kw)
-    smp = O.Sample(*sample_hc)
-    return O.contain_sample(p, db["kmers"], db["kmer_off"], db["tracked"], db["tracked_off"], db["gn_size"], smp)
-
-
-def naive_ani_matches(dev, exp):
-    """The device's pow is correctly rounded (crmath.cuh), the reference's is glibc's (0.52 ulp): they differ exactly
-    where glibc misrounds, and the device value must then be the correctly rounded one."""
-    if dev == exp.naive_ani:
-        return True
-    for k in (21, 31):
-        if T.glibc_naive(exp.contain, exp.glen, k) == exp.naive_ani:
-            return dev == T.cr_naive(exp.contain, exp.glen, k)
-    return False
-
-
-def within_one_ulp(a, b):
-    return a == b or np.nextafter(a, np.inf) == b or np.nextafter(a, -np.inf) == b
-
-
-def compare(rows, exp, pseudotax):
-    """Row by row against the oracle.  Integers, median, lambda, the coverages and the abundances bit-exact (IEEE
-    operations on equal integers, summed in the oracle's order).  naive_ani bit-exact, or the correctly rounded value
-    where glibc's pow misrounds; the adjusted final_est_ani (an exp inside the pow) and the bootstrap ANI percentiles
-    within one ulp, which only a glibc misrounding can use; the bootstrap lambda percentiles bit-exact."""
-    assert len(rows) == len(exp), (len(rows), len(exp))
-    for r, e in zip(rows, exp):
-        assert int(r["genome"]) == e.genome
-        assert int(r["contain"]) == e.contain and int(r["glen"]) == e.glen
-        assert int(r["lambda_status"]) == e.lambda_status
-        assert int(r["kmers_lost"]) == e.kmers_lost
-        assert float(r["median_cov"]) == e.median_cov
-        for f in ("final_est_cov", "mean_cov"):
-            assert float(r[f]) == getattr(e, f), (f, float(r[f]).hex(), getattr(e, f).hex())
-        assert naive_ani_matches(float(r["naive_ani"]), e), (float(r["naive_ani"]).hex(), e.naive_ani.hex())
-        if e.final_est_ani == e.naive_ani:
-            assert float(r["final_est_ani"]) == float(r["naive_ani"])
-        else:
-            assert within_one_ulp(float(r["final_est_ani"]), e.final_est_ani), (float(r["final_est_ani"]).hex(), e.final_est_ani.hex())
-        if e.lambda_status == 2:
-            assert float(r["lambda"]) == e.lambda_
-        assert int(r["ci_valid"]) == e.ci_valid
-        if e.ci_valid:
-            for i in range(2):
-                assert within_one_ulp(float(r["ci"][i]), e.ci[i]), ("ci", i)
-            for i in range(2, 4):
-                assert float(r["ci"][i]) == e.ci[i], ("ci", i)
-        if pseudotax:
-            assert float(r["rel_abund"]) == e.rel_abund
-            assert float(r["seq_abund"]) == e.seq_abund
-
-
-def sort_query_rows(rows):
-    """syl_query returns (sample, genome) order; the reference prints by ANI descending (stable)."""
-    order = sorted(range(len(rows)), key=lambda i: (-float(rows[i]["final_est_ani"]), i))
-    return rows[order]
 
 
 @pytest.fixture(scope="module")
@@ -271,7 +211,7 @@ def test_k21_scalar_semantics_end_to_end(ctx):
     db = ctx.build_db(g)
     for pt in (False, True):
         rows = ctx.profile(db, [smp], contain_params(k=21, pseudotax=True)) if pt else sort_query_rows(ctx.query(db, [smp], contain_params(k=21)))
-        p = O.default_params(k=21, pseudotax=pt)
+        p = cr_params(k=21, pseudotax=pt)
         exp = O.contain_sample(p, d["kmers"], d["kmer_off"], d["tracked"], d["tracked_off"], d["gn_size"], O.Sample(*hc))
         assert len(exp) > 5
         compare(rows, exp, pt)
@@ -310,9 +250,9 @@ def test_estimate_unknown_with_read_seq_id(ctx, pseudotax):
     db = ctx.build_db(g)
     P = contain_params(pseudotax=pseudotax, estimate_unknown=1, read_seq_id=98.0)
     rows = ctx.profile(db, [smp], P) if pseudotax else sort_query_rows(ctx.query(db, [smp], P))
-    exp = O.contain_sample(O.default_params(pseudotax=pseudotax), d["kmers"], d["kmer_off"], d["tracked"], d["tracked_off"], d["gn_size"],
+    exp = O.contain_sample(cr_params(pseudotax=pseudotax), d["kmers"], d["kmer_off"], d["tracked"], d["tracked_off"], d["gn_size"],
                            O.Sample(*hc), unknown=O.Unknown(98.0, smp.mean_read_length, 20))
-    plain = O.contain_sample(O.default_params(pseudotax=pseudotax), d["kmers"], d["kmer_off"], d["tracked"], d["tracked_off"], d["gn_size"],
+    plain = O.contain_sample(cr_params(pseudotax=pseudotax), d["kmers"], d["kmer_off"], d["tracked"], d["tracked_off"], d["gn_size"],
                              O.Sample(*hc))
     assert len(exp) > 5 and exp[0].final_est_cov > plain[0].final_est_cov
     compare(rows, exp, pseudotax)

@@ -12,7 +12,7 @@ import numpy as np
 import pytest
 
 from tests import contain_scripts as S
-from tests.test_contain_gpu import compare, sort_query_rows
+from tests.contain_compare import compare, cr_params, sort_query_rows
 
 pytestmark = pytest.mark.gpu
 
@@ -60,7 +60,7 @@ def oracle(name, pseudotax, pi, sel=None):
     w = S.world()
     d = w.db(sel)
     P = S.params_for(name)[pi]
-    return O.contain_sample(O.default_params(pseudotax=pseudotax, **P), d["kmers"], d["kmer_off"], d["tracked"],
+    return O.contain_sample(cr_params(pseudotax=pseudotax, **P), d["kmers"], d["kmer_off"], d["tracked"],
                             d["tracked_off"], d["gn_size"], O.Sample(*w.sample_arrays(name)))
 
 

@@ -11,7 +11,7 @@ import pytest
 
 from tests import ani_ties as T
 from tests import contain_scripts as S
-from tests.test_contain_gpu import compare
+from tests.contain_compare import compare, cr_params
 from tests.test_contain_scripts_gpu import check, same
 from tests.test_db_shards_gpu import PARAM_SETS, comm, community, world  # noqa: F401  (fixtures)
 from tests.test_sample_stream_gpu import pinned_copy
@@ -103,7 +103,7 @@ def test_near_tied_genomes_in_different_chunks(ctx, monkeypatch, formulation, pa
             for pseudotax in (False, True):
                 got = scan_build_one(ctx, monkeypatch, db, sh, [smp], pseudotax, {"k": k, "minimum_ani": 0.0}, "1")
                 if pseudotax:
-                    exp = O.contain_sample(O.default_params(k=k, pseudotax=True, minimum_ani=0.0), d["kmers"], d["kmer_off"],
+                    exp = O.contain_sample(cr_params(k=k, pseudotax=True, minimum_ani=0.0), d["kmers"], d["kmer_off"],
                                            d["tracked"], d["tracked_off"], d["gn_size"], O.Sample(case.hash, case.count))
                     compare(got, exp, True)
         finally:

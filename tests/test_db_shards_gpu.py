@@ -12,7 +12,7 @@ import pytest
 
 from tests import ani_ties as T
 from tests import contain_scripts as S
-from tests.test_contain_gpu import compare
+from tests.contain_compare import compare, cr_params
 from tests.test_contain_scripts_gpu import Gpu, check, same
 from tests.test_db_build_gpu import fracminhash_db
 
@@ -118,7 +118,7 @@ def test_near_tied_genomes_in_separate_shards(ctx, formulation, pair, swap):
             got = sh.profile([smp], p) if pseudotax else sh.query([smp], p)
             same(got, want, (pair, swap, pseudotax))
             if pseudotax:
-                exp = O.contain_sample(O.default_params(k=k, pseudotax=True, minimum_ani=0.0), d["kmers"], d["kmer_off"],
+                exp = O.contain_sample(cr_params(k=k, pseudotax=True, minimum_ani=0.0), d["kmers"], d["kmer_off"],
                                        d["tracked"], d["tracked_off"], d["gn_size"], O.Sample(case.hash, case.count))
                 compare(got, exp, True)
                 assert sorted(int(x) for x in got["kmers_lost"]) == [0, 3]

@@ -4,7 +4,7 @@
             state machine of src/sketch.rs:690-731 runs on ~4 M events) — the oracle sketches the same
             bytes with all host cores in a few seconds; hashes, counts and num_dup_removed must be equal.
   config 3: that sample against 10 000 synthetic 4 Mbp genome sketches — `query` and `profile` rows
-            field by field (integers exact, floats <= 1e-6).
+            field by field, bit for bit against the correctly rounded oracle (tests/contain_compare.py).
   config 5 shape: a batch of 4 Mbp genomes sketched in ONE call == the oracle's per-genome sketches.
 plus the size-independent properties (sortedness, conservation, determinism, host path == device path).
 """
@@ -14,7 +14,7 @@ from concurrent.futures import ThreadPoolExecutor
 import numpy as np
 import pytest
 
-from tests.test_contain_gpu import compare, sort_query_rows
+from tests.contain_compare import compare, cr_params, sort_query_rows
 
 pytestmark = pytest.mark.gpu
 
@@ -83,7 +83,7 @@ def test_config3_10k_genomes_query_and_profile_vs_oracle(ctx, gbp):
     db = ctx.build_db(genomes)
     smp = O.Sample(gbp["h"], gbp["c"])
     for pseudotax in (False, True):
-        exp = O.contain_sample(O.default_params(pseudotax=pseudotax), d["kmers"], d["kmer_off"], d["tracked"], d["tracked_off"],
+        exp = O.contain_sample(cr_params(pseudotax=pseudotax), d["kmers"], d["kmer_off"], d["tracked"], d["tracked_off"],
                                d["gn_size"], smp, nthreads=cores)
         rows = ctx.profile(db, [gbp["s"]]) if pseudotax else sort_query_rows(ctx.query(db, [gbp["s"]]))
         assert len(exp) >= 40

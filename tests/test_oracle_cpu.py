@@ -5,6 +5,7 @@
   * the committed oracle-generated regression fixture tests/golden/config1.json
 """
 import json
+import math
 import os
 import re
 
@@ -287,6 +288,81 @@ def test_contain_sample_vs_pyref(pseudotax):
             assert abs(r.rel_abund - e["rel_abund"]) < 1e-9 and abs(r.seq_abund - e["seq_abund"]) < 1e-9
     if pseudotax:
         assert sum(r.seq_abund for r in got_u) < 99.0 < sum(r.seq_abund for r in got) + 1e-6   # some reads are unexplained
+
+
+def cr_genomes(k, seed):
+    """small genomes of every lambda status (most of them ratio-lambda rows with a bootstrap interval), sharing some
+    hit k-mers, and the misrounding pins of this k (tests/ani_ties.py) -> (pyref genomes, sample dict, CSR arrays)"""
+    from tests import ani_ties as T
+    rng = np.random.default_rng(seed)
+    pool = iter(rng.permutation(np.unique(rng.integers(1, 2**63, size=40000, dtype=np.uint64))).tolist())
+    genomes, sample = [], {}
+    for i in range(10):
+        gl = int(rng.integers(50, 700))
+        kmers = [next(pool) for _ in range(gl)]
+        if i and i % 4 == 0:
+            kmers[:20] = genomes[i - 1]["kmers"][:20]      # shared with the previous genome: a pass-2 winner
+        lam = [0.3, 0.8, 1.5, 6.0, 0.05][i % 5]
+        for km in kmers[: int(gl * rng.uniform(0.5, 1.0))]:
+            c = int(rng.poisson(lam))
+            if c:
+                sample.setdefault(km, c)
+        genomes.append(dict(kmers=kmers, tracked=[next(pool)], gn_size=400000 + 1000 * i))
+    for kk, spec, *_ in T.MISROUNDED:
+        if kk != k:
+            continue
+        case = T.Case([spec], seed=len(genomes))
+        genomes.append(dict(kmers=case.db["kmers"].tolist(), tracked=case.db["tracked"].tolist(), gn_size=500000))
+        sample.update(case.sample)
+    d = dict(kmers=np.array([x for g in genomes for x in g["kmers"]], np.uint64),
+             kmer_off=np.cumsum([0] + [len(g["kmers"]) for g in genomes]).astype(np.uint64),
+             tracked=np.array([x for g in genomes for x in g["tracked"]], np.uint64),
+             tracked_off=np.cumsum([0] + [len(g["tracked"]) for g in genomes]).astype(np.uint64),
+             gn_size=np.array([g["gn_size"] for g in genomes], np.uint64))
+    return genomes, sample, d
+
+
+@pytest.mark.parametrize("pseudotax", [False, True])
+@pytest.mark.parametrize("k", [21, 31])
+def test_cr_math_c_quad_vs_pyref_decimal(k, pseudotax):
+    """The correctly rounded mode of both restatements: the C oracle's ANI pow / exp through libquadmath, pyref's
+    through 50-digit decimal.  Every field of every row bit-equal, the bootstrap percentiles included, on small genomes
+    of every lambda status and on the pins where glibc misrounds (where the glibc mode must differ)."""
+    genomes, sample, d = cr_genomes(k, 31 + k + int(pseudotax))
+    sh = np.array(list(sample), np.uint64)
+    sc = np.array(list(sample.values()), np.uint32)
+    got = O.contain_sample(O.default_params(k=k, pseudotax=pseudotax, minimum_ani=0.0, cr_math=1), d["kmers"],
+                           d["kmer_off"], d["tracked"], d["tracked_off"], d["gn_size"], O.Sample(sh, sc))
+    exp = R.contain_sample(genomes, sample, k=k, pseudotax=pseudotax, minimum_ani=0.0, cr_math=True)
+    assert [r.genome for r in got] == [e["genome"] for e in exp]
+    assert sum(r.ci_valid for r in got) >= 4 and {r.lambda_status for r in got} == {0, 1, 2}
+    for r, e in zip(got, exp):
+        for f in ("naive_ani", "final_est_ani", "final_est_cov", "mean_cov", "median_cov"):
+            assert getattr(r, f) == e[f], (r.genome, f)
+        assert (r.lambda_ if r.lambda_status == 2 else None) == e["lam"]
+        assert (tuple(r.ci) if r.ci_valid else None) == e["ci"], r.genome
+        if pseudotax:   # Python's sum() of floats is compensated, so the abundances' totals may differ in the last bits
+            assert r.kmers_lost == e["kmers_lost"]
+            assert abs(r.rel_abund - e["rel_abund"]) < 1e-9 and abs(r.seq_abund - e["seq_abund"]) < 1e-9
+    glibc = O.contain_sample(O.default_params(k=k, pseudotax=pseudotax, minimum_ani=0.0), d["kmers"], d["kmer_off"],
+                             d["tracked"], d["tracked_off"], d["gn_size"], O.Sample(sh, sc))
+    assert sum(a.final_est_ani != b.final_est_ani for a, b in zip(sorted(got, key=lambda r: r.genome),
+                                                                    sorted(glibc, key=lambda r: r.genome))) >= 4
+
+
+def test_cr_math_refuses_a_rounding_midpoint():
+    """pyref's decimal rounding refuses a value at a midpoint between two doubles (50 digits cannot decide it)."""
+    import decimal
+    from decimal import Decimal
+    y = 0.75
+    ctx = decimal.Context(prec=100)
+    mid = ctx.divide(ctx.add(Decimal(y), Decimal(math.nextafter(y, math.inf))), 2)
+    for v in (mid, ctx.add(mid, Decimal("1e-45")), ctx.subtract(mid, Decimal("1e-45"))):
+        with pytest.raises(ValueError):
+            R._nearest(v)
+    assert R._nearest(Decimal(y)) == y
+    assert R._nearest(ctx.add(mid, Decimal("1e-30"))) == math.nextafter(y, math.inf)
+    assert R._nearest(ctx.subtract(mid, Decimal("1e-30"))) == y
 
 
 @pytest.fixture(scope="module")

@@ -27,7 +27,7 @@ import pytest
 
 from tests import ani_ties as T
 from tests import contain_scripts as S
-from tests.test_contain_gpu import compare
+from tests.contain_compare import compare, cr_params
 from tests.test_contain_scripts_gpu import Gpu, check, same
 from tests.test_db_shards_gpu import PAIRS, PARAM_SETS, shards_of
 from tests.test_sample_stream_gpu import pinned_copy
@@ -253,7 +253,7 @@ def test_near_tied_pairs_streamed_over_shards(ctx, formulation, monkeypatch, pai
             got["sample"] = 0
             same(got, want, (pair, pseudotax))
             if pseudotax:
-                exp = O.contain_sample(O.default_params(k=k, pseudotax=True, minimum_ani=0.0), d["kmers"], d["kmer_off"],
+                exp = O.contain_sample(cr_params(k=k, pseudotax=True, minimum_ani=0.0), d["kmers"], d["kmer_off"],
                                        d["tracked"], d["tracked_off"], d["gn_size"], O.Sample(case.hash, case.count))
                 compare(got, exp, True)
                 assert sorted(int(x) for x in got["kmers_lost"]) == [0, 3]
@@ -347,7 +347,7 @@ def test_segment_sort_regimes(ctx, regime, monkeypatch, tmp_path):
     oracle; the call's H2D bytes are one copy of the batch"""
     from oracle import oracle as O
     from sylph_b200.api import contain_params
-    from tests.test_contain_gpu import sort_query_rows
+    from tests.contain_compare import sort_query_rows
     for k in HOOKS:
         monkeypatch.delenv(k, raising=False)
     d, samples, db, handles = regime
@@ -382,7 +382,7 @@ def test_segment_sort_regimes(ctx, regime, monkeypatch, tmp_path):
             sub["sample"] = 0
             if not pseudotax:
                 sub = sort_query_rows(sub)
-            exp = O.contain_sample(O.default_params(pseudotax=pseudotax, minimum_ani=0.0), d["kmers"], d["kmer_off"],
+            exp = O.contain_sample(cr_params(pseudotax=pseudotax, minimum_ani=0.0), d["kmers"], d["kmer_off"],
                                    d["tracked"], d["tracked_off"], d["gn_size"], O.Sample(*samples[i]))
             compare(sub, exp, pseudotax)
 
@@ -493,7 +493,7 @@ def test_device_memory_bounded_when_joins_outgrow_the_plan(ctx, monkeypatch, cas
     from oracle import oracle as O
     from sylph_b200 import _lib
     from sylph_b200.api import contain_params
-    from tests.test_contain_gpu import sort_query_rows
+    from tests.contain_compare import sort_query_rows
     for k in HOOKS:
         monkeypatch.delenv(k, raising=False)
     d, hs, cs = memory_world(deep=case == "deep")
@@ -538,7 +538,7 @@ def test_device_memory_bounded_when_joins_outgrow_the_plan(ctx, monkeypatch, cas
                 sub["sample"] = 0
                 if not pseudotax:
                     sub = sort_query_rows(sub)
-                exp = O.contain_sample(O.default_params(pseudotax=pseudotax), d["kmers"], d["kmer_off"], d["tracked"],
+                exp = O.contain_sample(cr_params(pseudotax=pseudotax), d["kmers"], d["kmer_off"], d["tracked"],
                                        d["tracked_off"], d["gn_size"], O.Sample(hs[i], cs[i]))
                 compare(sub, exp, pseudotax)
     finally:

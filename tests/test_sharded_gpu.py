@@ -20,7 +20,7 @@ import pytest
 
 from tests import ani_ties as T
 from tests import contain_scripts as S
-from tests.test_contain_gpu import compare, sort_query_rows
+from tests.contain_compare import compare, cr_params, sort_query_rows
 from tests.util import DATA, flatten, read_fastx
 
 pytestmark = pytest.mark.gpu
@@ -276,7 +276,7 @@ class Whole:
         if kw.pop("estimate_unknown", 0):
             unknown = O.Unknown(kw.pop("read_seq_id"), self.samples[si].mrl, self.samples[si].c)
         d = self.d
-        return O.contain_sample(O.default_params(pseudotax=pseudotax, **kw), d["kmers"], d["kmer_off"], d["tracked"],
+        return O.contain_sample(cr_params(pseudotax=pseudotax, **kw), d["kmers"], d["kmer_off"], d["tracked"],
                                 d["tracked_off"], d["gn_size"], O.Sample(*self.samples[si].hc), unknown=unknown)
 
     def check(self, got, kw=None):
